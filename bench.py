@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- DPFs/sec of the hot path on N B200s (one process per GPU).
+"""bench.py -- DPFs/sec of the hot path on N H100s (one process per GPU).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]          our engine
     python bench.py --impl reference [...]                       reference CPU path
@@ -16,6 +16,11 @@ so per-GPU work is fixed: weak scaling.
 Rank 0 prints ONE JSON line.  `value` is device-timed with keys resident in
 HBM; `e2e` goes through the public dpf-API call with pinned HOST keys, H2D and
 D2H inside the timed region.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step
+(rank 0's [B, E] result, as float64) to DIR/out.npy; inputs are seeded, so two
+builds run with the same arguments can be compared output for output.  Above
+64 MiB a fixed, seeded sample of rows is written, their indices in DIR/out_rows.npy.
 """
 import argparse
 import json
@@ -34,6 +39,8 @@ import gpu_dpf_b200  # noqa: E402,F401  (importable alias of gpu-dpf_b200/; make
 
 PRF_IDS = {"dummy": 0, "salsa20": 1, "chacha20": 2, "aes128": 3}
 KEY_BYTES = 2096
+HBM_GBS_DATASHEET = 3350.0   # H100 SXM HBM3, NVIDIA data sheet; used when MEASURED_PEAKS.json is absent
+DUMP_CAP_BYTES = 64 << 20    # --dump-outputs writes at most this much
 BASELINE_PUBLISHED = {  # BASELINE.md section 1 (reference README.md:129-146), V100, batch 512, entry 16
     ("aes128", 1 << 14): 52536, ("aes128", 1 << 16): 15392, ("aes128", 1 << 18): 3967, ("aes128", 1 << 20): 923,
     ("salsa20", 1 << 14): 145646, ("salsa20", 1 << 16): 54892, ("salsa20", 1 << 18): 16650, ("salsa20", 1 << 20): 3894,
@@ -60,7 +67,7 @@ def parse_args():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "reference-gpu"],
                     help="reference = the reference's CPU path on the host cores; reference-gpu = the reference's "
-                         "own GPU kernel compiled unmodified for sm_100a (oracle/_ref/ref_dpf_cpp.so), 1 GPU")
+                         "own GPU kernel compiled unmodified for sm_90a (oracle/_ref/ref_dpf_cpp.so), 1 GPU")
     ap.add_argument("--entries", "--n", dest="n", type=int, default=1 << 20, help="table size n (use --entries under torchrun: --n is ambiguous to its parser)")
     ap.add_argument("--entry", type=int, default=16)
     ap.add_argument("--prf", default="aes128", choices=sorted(PRF_IDS))
@@ -78,7 +85,28 @@ def parse_args():
     ap.add_argument("--no-parity", action="store_true", help="skip the post-timing parity check of the timed batch")
     ap.add_argument("--reduce", default="nccl", choices=["nccl", "fused"],
                     help="N>1: NCCL reduce of the partials, or the kernel's peer-memory red.add epilogue")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the last timed step to DIR/out.npy (float64)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs: the reference CPU arm evaluates a sample of indices per key and returns no [B, E] result")
+    return args
+
+
+def dump_outputs(dump_dir, result, cap_bytes=DUMP_CAP_BYTES):
+    """Write a [B, E] result as float64 to dump_dir/out.npy.  When that would exceed cap_bytes, a fixed,
+    seeded sample of rows is written instead, with their row indices in dump_dir/out_rows.npy."""
+    result = np.asarray(result)
+    os.makedirs(dump_dir, exist_ok=True)
+    rows_path = os.path.join(dump_dir, "out_rows.npy")
+    if os.path.exists(rows_path):
+        os.unlink(rows_path)
+    keep = max(1, cap_bytes // (8 * result.shape[1] + 8))      # each sampled row also stores its index
+    if result.shape[0] > keep:
+        rows = np.sort(np.random.RandomState(0).choice(result.shape[0], size=keep, replace=False))
+        np.save(rows_path, rows.astype(np.float64))
+        result = result[rows]
+    np.save(os.path.join(dump_dir, "out.npy"), result.astype(np.float64))
 
 
 def bytes_per_dpf(n, entry):
@@ -141,7 +169,7 @@ def load_peaks():
 
 
 # ---------------------------------------------------------------------------
-# clocks (B200_PROFILING.md recipe)
+# clocks: nvidia-smi sampled while the timed steps run
 # ---------------------------------------------------------------------------
 class ClockSampler:
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
@@ -299,49 +327,19 @@ def run_reference_gpu(args):
     emit({"impl": "reference-gpu", "metric": "DPFs/sec", "value": value, "unit": "DPFs/sec", "n_gpus": 1,
           "steps": args.steps, "warmup": max(args.warmup, 1), "ms_per_step": 1e3 * dt / args.steps,
           "higher_is_better": True, "dtype": "u128", "data": "synthetic",
-          "config": {"workload": "n=%d entry_size=%d %s batch=%d, reference dpf_hybrid_kernel compiled for sm_100a, "
+          "config": {"workload": "n=%d entry_size=%d %s batch=%d, reference dpf_hybrid_kernel compiled for sm_90a, "
                                  "wall clock incl. host marshalling (benchmark.py method)" % (n, entry, args.prf.upper(), batch),
                      "eval_init_s": t_init},
           "e2e": {"value": value, "unit": "DPFs/sec", "h2d_bytes_per_step": batch * 2080, "d2h_bytes_per_step": batch * 256},
           "checksum": int(out.to(torch.int64).sum().item())})
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out.numpy())
     ref.close()
 
 
 # ---------------------------------------------------------------------------
 # our engine
 # ---------------------------------------------------------------------------
-def pipe_roofline(prf_name, dpfs_per_s, n_local, sm_mhz):
-    """Integer-pipe roofline from MEASURED peaks (profiles/int_peaks.json, written by
-    tools/microbench/int_pipes.cu on a B200) and MEASURED per-node-pair instruction counts
-    (profiles/pipe_ops.json, from ncu sm__inst_executed_pipe_* / l1tex wavefront counters of the
-    evaluation kernel).  One node pair = one parent expanded into two children for a warp of 32
-    keys; a DPF over n_local leaves has n_local - 1 of them."""
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "profiles", "int_peaks.json")))
-        ops = json.load(open(os.path.join(ROOT, "profiles", "pipe_ops.json")))[prf_name]
-    except Exception:
-        return None
-    pipe = ops["binding_pipe"]                      # "alu" | "lsu"
-    per_pair = float(ops["warp_inst_per_node_pair"][pipe])
-    peak_per_clk_sm = float(peaks["peak_warp_inst_per_clk_sm"][pipe])
-    sms = int(peaks.get("sms", 148))
-    mhz = float(sm_mhz or peaks.get("sm_max_mhz", 1965.0))
-    pairs_per_s = dpfs_per_s / 32.0 * max(n_local - 1, 1)
-    achieved = pairs_per_s * per_pair                # warp-instructions (or wavefronts) per second
-    peak = peak_per_clk_sm * sms * mhz * 1e6
-    return {"pipe": ops.get("pipe_name", pipe), "warp_inst_per_node_pair": per_pair,
-            "achieved_ginst_s": achieved / 1e9, "peak_ginst_s": peak / 1e9, "frac": achieved / peak,
-            "peak_source": "profiles/int_peaks.json (tools/microbench/int_pipes.cu, %s/clk/SM) x %d SMs x %.0f MHz"
-                           % (peak_per_clk_sm, sms, mhz),
-            "ops_source": ops.get("source", "profiles/pipe_ops.json")}
-
-
-try:   # DRAM bytes per launch of the evaluation kernel, measured with ncu per configuration (tools/gpu_r2_final.sh)
-    TRAFFIC = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-except Exception:
-    TRAFFIC = {}
-
-
 class Harness:
     """torch / process-group state shared by every measurement of one bench.py run."""
 
@@ -360,7 +358,7 @@ class Harness:
             import datetime
             dist.init_process_group("nccl", device_id=self.dev, timeout=datetime.timedelta(seconds=600))
         assert self.world == args.gpus or self.world == 1, "launch with torchrun --nproc-per-node %d" % args.gpus
-        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=self.dev)   # > 126 MB L2
+        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=self.dev)   # > 50 MB L2 of an H100
         self.args = args
 
     def barrier(self, world=None):
@@ -410,7 +408,7 @@ def parity_check(h, d, world, prf, table, keys_a, keys_b, alphas, n_oracle=4):
 
 
 def measure(h, prf_name, n, entry, batch, steps, warmup, world=None, axis="entries", reduce="nccl",
-            e2e=True, parity=4, settle_s=0.0, subtree_log2=0, sampler=None):
+            e2e=True, parity=4, settle_s=0.0, subtree_log2=0, sampler=None, dump_dir=None):
     """One configuration: eval_init, warm-up, `steps` device-timed steps (CUDA events on the launching
     stream, max over ranks, L2 flushed before every step), optionally the end-to-end leg through the
     public host-buffer API, and the parity check of the timed batch.  world=1 on a multi-rank run
@@ -439,7 +437,7 @@ def measure(h, prf_name, n, entry, batch, steps, warmup, world=None, axis="entri
     out_dev = torch.empty((batch, entry), dtype=torch.int32, device=h.dev)
 
     def step_device():
-        d.eval_gpu_device(keys_dev, out_dev)
+        return d.eval_gpu_device(keys_dev, out_dev)
 
     nwarm = max(warmup, 3)
     t_warm = time.perf_counter()
@@ -468,14 +466,17 @@ def measure(h, prf_name, n, entry, batch, steps, warmup, world=None, axis="entri
     h.barrier(world)
     torch.cuda.synchronize()
     t_wall0 = time.perf_counter()
+    last = None
     for k in range(steps):
         h.flush.zero_()                       # cold L2 at the start of every timed step
         starts[k].record()
-        step_device()
+        last = step_device()
         ends[k].record()
     torch.cuda.synchronize()
     h.barrier(world)
     t_wall = time.perf_counter() - t_wall0
+    if dump_dir and last is not None and (world == 1 or h.rank == 0):   # only rank 0 holds the complete result
+        dump_outputs(dump_dir, last.cpu().numpy())
     clocks = sampler.stop() if sampler else None
     dev_ms = h.max_over_ranks(sum(s.elapsed_time(e) for s, e in zip(starts, ends)), world)
     # per-step times (max over ranks, step by step): the median is what the sub-millisecond extras report
@@ -526,7 +527,7 @@ def run_ours(args):
     axis = args.axis if (args.strong or args.axis != "auto") else "entries"
     m = measure(h, args.prf, n, entry, batch, args.steps, args.warmup, axis=axis, reduce=args.reduce,
                 e2e=not args.no_e2e, parity=0 if args.no_parity else 4, settle_s=0.5,
-                subtree_log2=args.subtree_log2, sampler=sampler)
+                subtree_log2=args.subtree_log2, sampler=sampler, dump_dir=args.dump_outputs)
     table = m.pop("table")
     value, clocks = m["value"], m["clocks"]
 
@@ -541,12 +542,8 @@ def run_ours(args):
                    "axis": r["axis"], "value": r["value"], "ms_per_step": r["ms_per_step"],
                    "ms_per_step_median": r["ms_per_step_median"],
                    "e2e": r["e2e"]["value"] if r["e2e"] else None, "launches_per_step": r["launches_per_step"],
-                   "frac": (alg / (r["ms_per_step"] / 1e3) / 1e9) / (float(load_peaks().get("hbm_gbs", 6650.0)) * ww),
+                   "frac": (alg / (r["ms_per_step"] / 1e3) / 1e9) / (float(load_peaks().get("hbm_gbs", HBM_GBS_DATASHEET)) * ww),
                    "parity_ok": r["parity_check"]["ok"] if r["parity_check"] else None}
-            shards_e = ww if r["axis"] == "entries" else 1
-            pr = pipe_roofline(prf_name, r["value"] / ww, nn // shards_e, (clocks or {}).get("sm_mhz")) if ee == 16 else None
-            out["pipe_frac"] = pr["frac"] if pr else None
-            out["traffic"] = TRAFFIC.get("%s_n%d_e%d_b%d_%dgpu" % (prf_name, nn, ee, bb, ww), {}).get("dram_bytes_per_launch")
             return out
         try:
             if world == 1:
@@ -595,23 +592,19 @@ def run_ours(args):
 
     if rank == 0:
         peaks = load_peaks()
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", HBM_GBS_DATASHEET))
+        peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet (3.35 TB/s HBM3)"
         # dominant kernel = the one evaluation kernel of a step; per launch it processes `batch`
         # keys over n/world leaves each
         shards = world if m["axis"] == "entries" else 1
         alg_bytes = batch * (n // shards * entry * 4 + KEY_BYTES + 4 * entry)
         launch_ms = m["ms_per_step"]
         achieved = alg_bytes / (launch_ms / 1e3) / 1e9
-        # measured with ncu (dram__bytes_read.sum + dram__bytes_write.sum), per launch
-        traffic = TRAFFIC.get("%s_n%d_e%d_b%d_%dgpu" % (args.prf, n, entry, batch, world), {}).get("dram_bytes_per_launch")
         roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": traffic, "peak_source": peak_kind,
-                    "pipe": pipe_roofline(args.prf, value / world, n // shards, (clocks or {}).get("sm_mhz")),
+                    "peak_source": peak_kind,
                     "note": "algorithmic bytes = batch*(n*E*4/ngpu + 2096 + 4E) per launch (table streamed once "
-                            "per key, SURVEY 8d); actual DRAM traffic is far lower because 32 keys share each row "
-                            "load and the table stays in L2, so the HBM fraction is nominal.  `pipe` is the roofline "
-                            "that binds: measured instruction count per node pair / measured pipe issue rate."}
+                            "per key, SURVEY 8d); actual DRAM traffic is lower because each row a warp loads serves "
+                            "its 32 keys, so the HBM fraction is nominal (DRAM traffic itself is not measured)."}
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
             kind, cores, sample, step = cpu_reference_runner(n, entry, prf, table)

@@ -1,6 +1,6 @@
 """In-tree build of the engine's two binaries.
 
-    libb200dpf.so                 CUDA kernels (sm_100a) + C ABI (include/b200dpf.h)
+    libb200dpf.so                 CUDA kernels (sm_90a) + C ABI (include/b200dpf.h)
     dpf_cpp.<abi>.so              the `dpf_cpp` PyTorch extension module (pybind shim
                                   over the C ABI; same surface as the reference's
                                   dpf_wrapper.cu)
@@ -22,11 +22,13 @@ LIB = os.path.join(HERE, "libb200dpf.so")
 EXT = os.path.join(HERE, "dpf_cpp" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 
 LIB_SOURCES = ["dpf_kernels.cu", "dpf_capi.cu", "dpf_keygen.cu", "dpf_host.cpp"]
-LIB_DEPS = LIB_SOURCES + ["dpf_core.cuh", "dpf_kernels.cuh", "dpf_host.h", os.path.join(INCLUDE, "b200dpf.h")]
+# this script is a dependency too: its flags (the target architecture among them) shape both binaries
+LIB_DEPS = LIB_SOURCES + ["dpf_core.cuh", "dpf_kernels.cuh", "dpf_host.h", os.path.join(INCLUDE, "b200dpf.h"),
+                          os.path.abspath(__file__)]
 EXT_SOURCES = ["dpf_cpp_ext.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unknown-pragmas",
 ]
@@ -51,19 +53,25 @@ def _stale(target, deps):
 
 
 def build_lib(force=False, verbose=False):
-    if not force and not _stale(LIB, LIB_DEPS):
-        return LIB
     extra = os.environ.get("B200DPF_EXTRA_NVCC_FLAGS", "").split()
     cmd = [_nvcc()] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + [
         "-shared", "-I", INCLUDE, "-o", LIB] + [os.path.join(CSRC, s) for s in LIB_SOURCES]
+    # the command of the last build sits next to the library: a build with other flags (say, extra
+    # ones from the environment) is not mistaken for an up-to-date one
+    stamp = LIB + ".cmd"
+    same_cmd = os.path.exists(stamp) and open(stamp).read() == " ".join(cmd)
+    if not force and same_cmd and not _stale(LIB, LIB_DEPS):
+        return LIB
     subprocess.run(cmd, check=True)
+    with open(stamp, "w") as f:
+        f.write(" ".join(cmd))
     return LIB
 
 
 def build_ext(force=False):
     """Compile the pybind shim with g++ against torch's headers (host-only C++)."""
     build_lib(force=False)
-    deps = EXT_SOURCES + [os.path.join(INCLUDE, "b200dpf.h")]
+    deps = EXT_SOURCES + [os.path.join(INCLUDE, "b200dpf.h"), os.path.abspath(__file__)]
     if not force and not _stale(EXT, deps):
         return EXT
     import torch

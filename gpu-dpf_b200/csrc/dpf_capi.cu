@@ -2,7 +2,7 @@
  * dpf_capi.cu -- implementation of the C ABI declared in include/b200dpf.h.
  *
  * Owns the device state of one table (or one entry-range shard of it) and
- * turns b200dpf_eval* calls into launches of the sm_100a kernel in
+ * turns b200dpf_eval* calls into launches of the sm_90a kernel in
  * dpf_kernels.cu.  The GPU entry points have no CPU fallback: without a usable
  * CUDA device they fail with B200DPF_ECUDA.
  */
@@ -132,8 +132,9 @@ struct b200dpf_ctx {
         int timing = 0;            /* B200DPF_TIMING         per-block phase time stamps (diagnostics)      */
         int top_log2 = 0;          /* B200DPF_TOP_LOG2       log2 leaves-of-the-frontier per tree-top item (0 = estimate) */
         int tma_rows = 0;          /* B200DPF_TMA_ROWS       fused kernel: stage each item's rows with cp.async.bulk
-                                                             (16-column tables, Salsa/ChaCha/dummy); measured slower than
-                                                             broadcast loads -- profiles/r2_tma_rows_ab.txt -- so off */
+                                                             (16-column tables, Salsa/ChaCha/dummy); on an H100 at n=2^20
+                                                             +4 % for Salsa20, -2 % for ChaCha20 against broadcast
+                                                             loads, other sizes unmeasured -- so off */
     } knobs;
     unsigned long long *d_timing = nullptr;   /* [timing_blocks][8] */
     int timing_blocks = 0;
@@ -334,19 +335,19 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     int64_t key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
 
     /* ---- work-item size s and the frontier depth --------------------------------
-     * measured on B200 (profiles/r1_sweeps.txt).  Without a frontier every item
-     * re-walks depth-s levels from the root, so items must be big; with one the
-     * walk is (almost) free and small items balance the tail. */
+     * Without a frontier every item re-walks depth-s levels from the root, so items
+     * must be big; with one the walk is (almost) free and small items balance the
+     * tail. */
     const bool want_frontier = K.frontier != 0;
     int s;
     if (K.subtree_log2 > 0) {
         s = std::min(K.subtree_log2, std::min(c->depth_local, L.s_max));
     } else {
-        /* B=512 E=16 1xB200, DPFs/s (profiles/r1_sweeps.txt):
-         *   AES n=2^20, frontier: s=4 23.99k, 5 24.83k, 6 25.03k, 7 25.01k, 8 24.92k; no frontier s=8 24.19k
-         *   AES n=2^16, frontier: s=4 372.7k, 5 366.4k, 6 351.7k; no frontier 340.3k
-         *   AES n=2^14, frontier: s=3 1.242M, 4 1.179M, 5 1.147M; no frontier 1.225M
-         *   ChaCha n=2^20, frontier: s=5 22.93k, 6 23.20k, 7 23.30k, 8 23.23k; no frontier 22.10k */
+        /* B=512 E=16, frontier on, 1x H100 SXM 80 GB at a 400 W power limit, DPFs/s (run-to-run
+         * spread about 3 %); the automatic choice is within the spread of the best fixed s:
+         *   AES n=2^20: auto 19.47k; s=4 19.39k, 5 19.77k, 6 19.56k, 7 20.01k, 8 19.56k
+         *   AES n=2^16: auto 319.3k; s=4 317.5k, 5 318.1k, 6 318.1k, 7 300.5k
+         *   ChaCha n=2^20: auto 19.18k; s=5 18.94k, 6 19.13k, 7 19.19k */
         const int s_cap = want_frontier ? 7 : ((prf == B200DPF_PRF_AES128) ? 8 : 10);
         const int s_floor = want_frontier ? 3 : 5;
         const int64_t items_per_warp = want_frontier ? 24 : 6;
@@ -713,7 +714,7 @@ static void multi_destroy(b200dpf_ctx *root);
 
 extern "C" {
 
-const char *b200dpf_version(void) { return "b200dpf 0.1.0 sm_100a"; }
+const char *b200dpf_version(void) { return "b200dpf 0.1.0 sm_90a"; }
 
 const char *b200dpf_last_error(void) { return g_err; }
 
@@ -993,7 +994,8 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     if (e == cudaSuccess) e = cudaMalloc(&c->d_table, table_bytes);
     if (e == cudaSuccess) e = cudaMemsetAsync(c->d_table, 0, table_bytes, c->stream);
     if (e == cudaSuccess)
-        e = launch_permute_table(d_stage, c->d_table, (uint64_t)c->n_local, c->depth_local, entry_size, c->entry_pad, c->stream);
+        e = launch_permute_table(d_stage, c->d_table, (uint64_t)c->n_local, c->depth_local, entry_size, c->entry_pad,
+                                 c->sm_count, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     cudaFree(d_stage);
     CTX_TRY(e);
@@ -1533,7 +1535,7 @@ static int multi_eval_host(b200dpf_ctx *root, const void *keys, size_t key_strid
             CUDA_TRY(cudaStreamWaitEvent(c0->stream, M->sub[(size_t)d]->ev_done, 0));
             parts.p[parts.n++] = reinterpret_cast<const uint32_t *>(M->sub[(size_t)d]->d_out);
         }
-        CUDA_TRY(launch_sum_partials(reinterpret_cast<uint32_t *>(c0->d_out), parts, out_elems, c0->stream));
+        CUDA_TRY(launch_sum_partials(reinterpret_cast<uint32_t *>(c0->d_out), parts, out_elems, c0->sm_count, c0->stream));
         int32_t *dst = out;
         if (!M->out_pinned) {
             rc = ensure_host_out(c0, out_elems);
@@ -1703,7 +1705,7 @@ int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const 
         e = cudaMemcpyAsync(d_stage, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream);
         if (e == cudaSuccess)
             e = launch_permute_table(d_stage, c->d_table + row0 * (uint64_t)c->entry_pad, (uint64_t)n[g], depth, entry_size,
-                                     c->entry_pad, c->stream);
+                                     c->entry_pad, c->sm_count, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);    /* the staging buffer is reused */
         row0 += (uint64_t)n[g];
     }

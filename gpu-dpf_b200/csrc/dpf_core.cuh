@@ -2,7 +2,7 @@
  * dpf_core.cuh -- arithmetic core of the DPF evaluation engine.
  *
  * Everything here is `host + device`: the same functions are compiled by nvcc
- * into the sm_100a kernels (dpf_kernels.cu) and by g++ into the host library
+ * into the sm_90a kernels (dpf_kernels.cu) and by g++ into the host library
  * (keygen / eval_cpu in dpf_host.cpp) and the CPU lane-emulator used by the
  * tests.  Device builds pick the hardware instruction (funnel shift, PRMT,
  * carry-chain adds, ld.shared with immediate offsets); host builds use a
@@ -71,7 +71,7 @@ DPF_HD uint32_t rotl(uint32_t v, int r)
  * split across its halves (low = x<<r, high = x>>(32-r)), which do not overlap.
  * One IMAD.WIDE + one add, no ALU-pipe slot: used for a fraction of the
  * Salsa/ChaCha rotates because those kernels saturate the ALU pipe (LOP3/SHF)
- * while the FMA pipe idles (profiles/r1_ncu_full_chacha20_*). */
+ * while the FMA pipe idles. */
 #ifndef DPF_FMA_ROT_MASK
 #define DPF_FMA_ROT_MASK 0
 #endif

@@ -1,10 +1,10 @@
 /*
- * dpf_kernels.cu -- sm_100a kernels of the DPF evaluation engine.
+ * dpf_kernels.cu -- sm_90a kernels of the DPF evaluation engine.
  *
  * One kernel does the whole hot path of the reference's dpf_hybrid_kernel
  * (dpf_gpu/dpf/dpf_hybrid.cu:38-256): GGM-tree expansion of every key over the
  * full domain, fused with the inner product against the table, plus the
- * reduction -- but organised for Blackwell rather than translated:
+ * reduction -- but organised for Hopper rather than translated:
  *
  *   work item   = (group of 32 keys) x (one 2^s-leaf subtree).  A warp owns a
  *                 work item; LANE = KEY.  All 32 lanes walk the same tree shape,
@@ -246,7 +246,7 @@ struct DevEnv {
  * threads fit the register file. */
 template <int PRF, int NV> struct KernelShape { enum { THREADS = (NV <= 8 ? 256 : 384), MIN_BLOCKS = (NV <= 8 ? 2 : 1) }; };
 #ifndef DPF_AES_THREADS
-#define DPF_AES_THREADS 384      /* 8 warps (256) measured against 12 (384): profiles/r2_aes_block_size_ab.txt */
+#define DPF_AES_THREADS 384      /* 12 warps: on an H100 1.5 % (n=2^20) and 3 % (n=2^16) faster than 8 (256) */
 #endif
 template <int NV> struct KernelShape<PRF_AES128, NV> { enum { THREADS = (NV <= 8 ? DPF_AES_THREADS : 256), MIN_BLOCKS = 1 }; };
 
@@ -392,13 +392,13 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
         /* SMALL items (<= 15 node pairs) draw their tickets one draw ahead, so the atomic's round trip
          * to L2 overlaps the items being expanded instead of stalling the warp between items.  Big items
          * draw when they are done: holding a ticket for the length of a 127-pair item makes the hand-out
-         * one item less adaptive at the end of a key group (measured: +0.6 % kernel time at n = 2^20,
-         * profiles/r2_kernel_regression_bisect.txt), and the atomic's latency is nothing against it.
+         * one item less adaptive at the end of a key group (slower at n = 2^20 when measured before the
+         * H100 port), and the atomic's latency is nothing against it.
          * A draw takes a CHUNK of consecutive items, sized from what is left: (remaining / 8x the
          * warps of the grid), between 1 and 8 -- guided self-scheduling: big early chunks when a key
          * group holds many more items than the grid has warps, single items at the end keep the tail
          * fine-grained.  (Cutting a group's tickets into several counters was tried for the case of
-         * one or two key groups per GPU and measured slower: profiles/r2_ticket_split_ab.txt.) */
+         * one or two key groups per GPU and measured slower.) */
         const uint32_t grid_warps = gridDim.x * (uint32_t)(THREADS / 32);
         const bool chunked = quota == 0xffffffffu;          /* the balanced top round counts single tickets */
         const bool ahead = g_s <= 4;
@@ -892,20 +892,20 @@ cudaError_t launch_mac(int nv, const MacParams &p, int grid, cudaStream_t stream
     return cudaGetLastError();
 }
 
-cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t words, cudaStream_t stream)
+cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t words, int sm_count, cudaStream_t stream)
 {
     if (parts.n <= 0 || words == 0) return cudaSuccess;
-    int grid = (int)std::min<size_t>((words / 4 + 255) / 256 + 1, 148 * 4);
+    int grid = (int)std::min<size_t>((words / 4 + 255) / 256 + 1, (size_t)std::max(sm_count, 1) * 4);
     sum_partials_kernel<<<grid, 256, 0, stream>>>(dst, parts, words);
     return cudaGetLastError();
 }
 
 cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
-                                 int cols, int stride, cudaStream_t stream)
+                                 int cols, int stride, int sm_count, cudaStream_t stream)
 {
     const uint64_t total = rows * (uint64_t)cols;
-    int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 16) grid = 148 * 16;
+    const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
+    int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
     if (grid < 1) grid = 1;
     permute_table_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, cols, stride);
     return cudaGetLastError();

@@ -1,6 +1,6 @@
 /*
  * dpf_kernels.cuh -- launch interface between the C-ABI layer (dpf_capi.cu)
- * and the sm_100a kernels (dpf_kernels.cu).  Plain structs, no torch.
+ * and the sm_90a kernels (dpf_kernels.cu).  Plain structs, no torch.
  */
 #pragma once
 
@@ -157,7 +157,7 @@ struct PeerParts {
     const uint32_t *p[15];
     int n;
 };
-cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t words, cudaStream_t stream);
+cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t words, int sm_count, cudaStream_t stream);
 
 /* Batched key generation on the device (dpf_keygen.cu): one thread per key pair, ChaCha20-DRBG draws
  * from 44 seed bytes per key; keys in the reference wire format, [count][131] 128-bit slots each. */
@@ -168,8 +168,9 @@ cudaError_t launch_keygen(int prf, const int64_t *alphas, const uint8_t *seeds44
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
 /* table[q][c] = stage[bitrev_bits(q)][c] for q < rows, c < cols; padded columns
- * [cols, stride) are left untouched (pre-zeroed). */
+ * [cols, stride) are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM
+ * count to cap their grids at a few waves. */
 cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
-                                 int cols, int stride, cudaStream_t stream);
+                                 int cols, int stride, int sm_count, cudaStream_t stream);
 
 }  // namespace b200dpf

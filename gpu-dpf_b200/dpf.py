@@ -1,4 +1,4 @@
-"""dpf.DPF -- the reference's Python API (dpf.py:35-137) on the B200-native engine.
+"""dpf.DPF -- the reference's Python API (dpf.py:35-137) on the H100-native engine.
 
 Same class, method names, argument meaning and exceptions as the reference, so
 `sample.py` and `benchmark.py` written against it keep working:
@@ -9,7 +9,7 @@ Same class, method names, argument meaning and exceptions as the reference, so
     shares = d.eval_gpu([k1, ...])  # server: int32 [len(keys), entry_size] on the CPU
 
 What differs is behind the boundary: `dpf_cpp` here is the pybind shim over
-include/b200dpf.h (hand-written sm_100a kernels), tables may have any entry
+include/b200dpf.h (hand-written sm_90a kernels), tables may have any entry
 size, batches may have any length (no pad-to-512 round trip, no pad-to-16
 columns), and one process can own an entry-range shard of the table
 (`DPF(prf, device=d, shard=(rank, count))`) whose partial results add mod 2^32.

@@ -1,5 +1,5 @@
 /*
- * b200dpf.h -- C ABI of the B200-native DPF evaluation engine.
+ * b200dpf.h -- C ABI of the H100-native DPF evaluation engine.
  *
  * This is the drop-in boundary for the ONE hot path of facebookresearch/GPU-DPF:
  * batched full-domain evaluation of log(n)-key distributed point functions
@@ -61,7 +61,7 @@ enum {
 
 typedef struct b200dpf_ctx b200dpf_ctx;
 
-/* Library identification: "b200dpf <semver> sm_100a". */
+/* Library identification: "b200dpf <semver> sm_90a". */
 const char *b200dpf_version(void);
 
 /* Thread-local description of the last failure on this thread. */
@@ -148,7 +148,7 @@ int64_t b200dpf_key_n(const int32_t *key);
 int b200dpf_key_depth(const int32_t *key);
 
 /* ------------------------------------------------------------------------- */
-/* Server side (GPU, sm_100a).                                                */
+/* Server side (GPU, sm_90a).                                                 */
 /* ------------------------------------------------------------------------- */
 
 /*

@@ -11,7 +11,7 @@ for sub in ("gpu-dpf_b200", "oracle", "tests"):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")

@@ -58,3 +58,31 @@ def test_key_slices_cover_batch():
             spans = [key_slice(nkeys, r, world) for r in range(world)]
             covered = [i for b, e in spans for i in range(b, e)]
             assert covered == list(range(nkeys))
+
+
+def test_dump_outputs_sample_is_seeded_and_capped(tmp_path):
+    """--dump-outputs: the whole [B, E] result as float64 under the cap; above it the same seeded sample of
+    rows every time, with their indices, within the cap."""
+    import numpy as np
+    sys.path.insert(0, ROOT)
+    import bench
+    result = (np.arange(40 * 16, dtype=np.int64).reshape(40, 16) * 2654435761 % 2**32 - 2**31).astype(np.int32)
+    bench.dump_outputs(str(tmp_path), result)
+    out = np.load(tmp_path / "out.npy")
+    assert out.dtype == np.float64 and np.array_equal(out, result) and not (tmp_path / "out_rows.npy").exists()
+    cap = 10 * (16 * 8 + 8)
+    for _ in range(2):
+        bench.dump_outputs(str(tmp_path), result, cap_bytes=cap)
+        out, rows = np.load(tmp_path / "out.npy"), np.load(tmp_path / "out_rows.npy")
+        assert out.nbytes + rows.nbytes <= cap and out.shape == (10, 16)
+        assert np.array_equal(out, result[rows.astype(np.int64)]) and np.all(np.diff(rows) > 0)
+        if _ == 0:
+            first = rows
+    assert np.array_equal(rows, first)
+
+
+def test_reference_arm_rejects_dump_outputs(tmp_path):
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--entries", "1024",
+                        "--steps", "1", "--warmup", "0", "--dump-outputs", str(tmp_path / "d")],
+                       capture_output=True, text=True, timeout=120)
+    assert r.returncode != 0 and "--dump-outputs" in r.stderr and not (tmp_path / "d").exists()

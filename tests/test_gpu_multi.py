@@ -144,8 +144,8 @@ def test_single_process_all_gpus():
 
 
 def test_python_api_devices_all():
-    """dpf.DPF(devices='all') and the B200DPF_DEVICES switch that lets the reference's unmodified
-    dpf.py / benchmark.py use every GPU."""
+    """dpf.DPF(devices='all'), and the B200DPF_DEVICES switch that lets callers of the reference's
+    pybind interface (eval_init(table) has no device argument) use every GPU."""
     devs = _devices()
     if len(devs) < 2:
         pytest.skip("needs >= 2 GPUs")
@@ -166,15 +166,20 @@ def test_python_api_devices_all():
     b = d.eval_gpu(torch.stack([k[1] for k in keys]))
     assert torch.equal(a - b, table[idx])
     d.close()
-    scripts = os.path.join(ROOT, "oracle", "_ref", "scripts")
-    if os.path.isfile(os.path.join(scripts, "sample.py")):
-        env = dict(os.environ, PYTHONPATH=os.path.join(ROOT, "gpu-dpf_b200"), B200DPF_DEVICES="all")
-        r = subprocess.run([sys.executable, "sample.py"], cwd=scripts, env=env, capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0 and r.stdout.strip().split()[-1] == "42", r.stdout + r.stderr
-        r = subprocess.run([sys.executable, "benchmark.py"], cwd=scripts, env=env, capture_output=True, text=True, timeout=1200)
-        assert r.returncode == 0 and r.stdout.count("dpfs/sec") == 12, r.stdout + r.stderr
-        try:
-            with open(os.path.join(ROOT, "gpurun_out", "r2_benchmark_py_unmodified_all_gpus.txt"), "w") as f:
-                f.write("B200DPF_DEVICES=all (%d GPUs), reference dpf.py + benchmark.py unmodified\n" % torch.cuda.device_count() + r.stdout)
-        except OSError:
-            pass
+    # the reference's calling convention (sample.py's query: entry 42 of a 2^14-row table, a batch of
+    # exactly 512 keys) in a fresh process whose environment asks for every GPU
+    script = (
+        "import torch, dpf_cpp\n"
+        "n = 16384\n"
+        "table = torch.randint(2**31, (n, 16), generator=torch.Generator().manual_seed(5)).int()\n"
+        "table[42] = 42\n"
+        "k1, k2 = dpf_cpp.gen(42, n, bytes(128), dpf_cpp.PRF_AES128)\n"
+        "buf = dpf_cpp.eval_init(table)\n"
+        "assert dpf_cpp.device_count(buf) == torch.cuda.device_count(), dpf_cpp.device_count(buf)\n"
+        "r = dpf_cpp.eval_gpu([k1, k2] + [k2] * 510, buf, n, dpf_cpp.PRF_AES128).cpu()\n"
+        "assert tuple(r.shape) == (512, 16) and torch.equal(r[0] - r[1], table[42]), r[:2]\n"
+        "dpf_cpp.eval_free(buf)\n"
+        "print('ok')\n")
+    env = dict(os.environ, PYTHONPATH=os.path.join(ROOT, "gpu-dpf_b200"), B200DPF_DEVICES="all")
+    r = subprocess.run([sys.executable, "-c", script], env=env, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout + r.stderr

@@ -1,10 +1,17 @@
-"""The CPU oracle against (a) the golden vectors produced by the real reference and
-(b) the real reference itself when oracle/_ref is built.  No GPU."""
+"""The CPU oracle against the golden vectors produced by the original project's CPU core.  No GPU."""
+import hashlib
+import os
 import random
 
 import numpy as np
+import pytest
 
 from common import dot_u32, formula_table
+
+
+@pytest.fixture(scope="module")
+def ref_checks():
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_checks_v1.npz"))
 
 # values printed by the unmodified reference for seed 0x0123456789abcdef_fedcba9876543210 (SURVEY.md section 8c)
 SURVEY_SEED = 0x0123456789ABCDEFFEDCBA9876543210
@@ -87,35 +94,52 @@ def test_dot_range_matches_full(oracle, golden):
     assert np.array_equal((a + b).astype(np.int32)[0], golden["dots_a"][ci])
 
 
-# ---- against the real reference (build container only) --------------------
+# ---- against the original project's CPU core (outputs stored by tests/golden/make_golden_ref_checks.py)
 
-def test_oracle_matches_reference_prf(oracle, ref):
+def _sha256(a):
+    return hashlib.sha256(np.ascontiguousarray(a, "<i4").tobytes()).digest()
+
+
+def _u128(lohi):
+    return int(lohi[0]) | (int(lohi[1]) << 64)
+
+
+def test_oracle_matches_reference_prf(oracle, ref_checks):
     r = random.Random(7)
-    for _ in range(200):
-        s = r.getrandbits(128)
-        for prf in range(4):
+    seeds = [r.getrandbits(128) for _ in range(200)]
+    for prf in range(4):
+        got = np.zeros((len(seeds), 2, 2), np.uint64)          # [seed][pos][lo, hi]
+        for si, s in enumerate(seeds):
             for pos in (0, 1):
-                assert oracle.prf(prf, s, pos) == ref.prf(prf, s, pos)
+                v = oracle.prf(prf, s, pos)
+                got[si, pos] = (v & (2**64 - 1), v >> 64)
+        assert hashlib.sha256(got.tobytes()).digest() == ref_checks["prf_out_sha256"][prf].tobytes(), prf
 
 
-def test_oracle_matches_reference_gen_and_eval(oracle, ref):
+def test_oracle_matches_reference_gen_and_eval(oracle, ref_checks):
     r = random.Random(11)
+    ci = 0
     for prf in range(4):
         for n in (2, 4, 256, 2048):
             for _ in range(3):
                 alpha, seed32 = r.randrange(n), r.getrandbits(32)
                 ka, kb = oracle.gen(alpha, n, seed32, prf)
-                ra, rb = ref.gen(alpha, n, seed32, prf)
-                assert np.array_equal(ka, ra) and np.array_equal(kb, rb)
-                assert np.array_equal(oracle.eval_full(ka, prf), ref.eval_full(ka, prf))
-                for idx in (0, alpha, n - 1):
-                    assert oracle.eval_flat(kb, idx, prf) == ref.eval_flat(kb, idx, prf)
+                assert _sha256(ka) == ref_checks["gen_keys_a_sha256"][ci].tobytes(), (prf, n, alpha)
+                assert _sha256(kb) == ref_checks["gen_keys_b_sha256"][ci].tobytes(), (prf, n, alpha)
+                assert _sha256(oracle.eval_full(ka, prf)) == ref_checks["gen_full_a_sha256"][ci].tobytes(), (prf, n, alpha)
+                for j, idx in enumerate((0, alpha, n - 1)):
+                    assert oracle.eval_flat(kb, idx, prf) == _u128(ref_checks["gen_flat_b"][ci, j]), (prf, n, idx)
+                ci += 1
+    assert ci == ref_checks["gen_keys_a_sha256"].shape[0]
 
 
-def test_reference_baseline_harness(oracle, ref):
-    """ref_eval_dot_mt (the --impl reference timing leg) computes the same inner product."""
+def test_reference_baseline_harness(oracle, ref_checks):
+    """ref_eval_dot_mt (the --impl reference timing leg) computes the same inner product as the oracle."""
     n = 512
     t = formula_table(n, 16)
     keys = np.stack([oracle.gen(i * 37 % n, n, 50 + i, 2)[0] for i in range(5)])
-    got = ref.eval_dot_mt(keys, 2, t, 0, n, 3)
-    assert np.array_equal(got, oracle.eval_dot(keys, 2, t))
+    assert _sha256(keys) == ref_checks["harness_keys_sha256"].tobytes()
+    assert np.array_equal(ref_checks["harness_dot"], oracle.eval_dot(keys, 2, t))
+    import oracle as O
+    if O.Ref.available():      # where the reference core was built, also run the code bench.py times
+        assert np.array_equal(O.Ref().eval_dot_mt(keys, 2, t, 0, n, 3), ref_checks["harness_dot"])

@@ -11,9 +11,9 @@
 //   quarter rounds: Salsa20 / ChaCha as the kernels write them, and variants that move some of
 //   the rotates to the fma pipe as IMAD.WIDE (x*2^r = {x<<r, x>>(32-r)}; the halves are disjoint,
 //   so  b ^ rotl(t,r) == lop3.xor(b, lo, hi)).
-// Which SASS instruction each PTX line became is checked with cuobjdump (profiles/r2_int_pipes_sass.txt).
+// Which SASS instruction each PTX line became can be checked with cuobjdump -sass.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bin/int_pipes int_pipes.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bin/int_pipes int_pipes.cu
 // Output: one JSON object per line on stdout.
 #include <cstdint>
 #include <cstdio>

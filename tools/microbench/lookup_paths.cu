@@ -4,7 +4,7 @@
 //   C: constant memory, per-lane (divergent) index
 //   G: global memory through L1 (1 KiB table, ld.global.nc), per-lane index
 //   T: texture object fetch (tex1Dfetch), per-lane index
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bin/lookup_paths lookup_paths.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bin/lookup_paths lookup_paths.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -75,7 +75,7 @@ int main()
     uint32_t *g_tab, *out;
     cudaMalloc(&g_tab, sizeof h);
     cudaMemcpy(g_tab, h, sizeof h, cudaMemcpyHostToDevice);
-    cudaMalloc(&out, 148 * 384 * 4 * 4);
+    cudaMalloc(&out, (size_t)p.multiProcessorCount * 384 * 4 * 4);
     cudaResourceDesc rd = {};
     rd.resType = cudaResourceTypeLinear;
     rd.res.linear.devPtr = g_tab;
