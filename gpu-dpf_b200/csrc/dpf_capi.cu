@@ -453,7 +453,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
                 const double quota = std::ceil(tickets / blocks_per_group);
                 const double steps = 0.55 * (c->shard_bits + f_rel - cand) + (double)((1 << cand) - 1);
                 const double full_rounds = std::floor(quota / nw), rest = quota - full_rounds * nw;
-                const double busy = 342.0, latency = 1500.0;        /* per node pair: pipe slots, dependent-chain latency */
+                const double busy = 330.0, latency = 1500.0;        /* per node pair: pipe slots, dependent-chain latency */
                 double t = full_rounds * steps * std::max(nw * busy, latency);
                 if (rest > 0) t += steps * std::max(rest * busy, latency);
                 if (t < best) {

@@ -13,8 +13,9 @@
  *   pos = 0 and pos = 1 of one GGM node at once, because they share work:
  *     - Salsa20/ChaCha12: three of the four first-round quarter rounds do not
  *       touch the position word and are common to both children;
- *     - AES-128: the key schedule (10 S-box rounds) is common, and the first
- *       cipher round of the second child differs in one table lookup.
+ *     - AES-128: the key schedule (10 S-box rounds) is common, the first
+ *       cipher round of the second child differs in one table lookup and its
+ *       second round in four.
  *   The LEAF flavour only produces the low 32 bits of each child: the fused
  *   inner product keeps nothing else (dpf_wrapper.cu:182), which lets the
  *   compiler drop the unused tail of the last round.
@@ -31,8 +32,10 @@
 
 #if defined(__CUDA_ARCH__)
 #define DPF_UNROLL _Pragma("unroll")
+#define DPF_NO_UNROLL _Pragma("unroll 1")
 #else
 #define DPF_UNROLL
+#define DPF_NO_UNROLL
 #endif
 
 #if defined(__CUDA_ARCH__)
@@ -328,6 +331,31 @@ DPF_HD void aes_first_round(const TA &ta, uint32_t pos, uint32_t &k0, uint32_t &
     col0_te0 = l00;
 }
 
+/*
+ * Round 2 of both children.  After round 1 they differ in column 0 alone (a0 vs
+ * b0; a1..a3 are shared), and ShiftRows sends exactly one byte of column 0 into
+ * each output column: byte 0 to column 0 (Te0), byte 3 to column 1 (Te3), byte 2
+ * to column 2 (Te2), byte 1 to column 3 (Te1).  So the second child's column c is
+ * the first child's with that one lookup swapped, t_c(b) = t_c(a) ^ L_c(a0) ^ L_c(b0):
+ * 4 lookups instead of 16.  In: a0..a3, b0 and rk2.  Out: both states after round 2.
+ */
+template <class TA>
+DPF_HD void aes_round2_pair(const TA &ta, uint32_t &a0, uint32_t &a1, uint32_t &a2, uint32_t &a3, uint32_t &b0,
+                            uint32_t &b1, uint32_t &b2, uint32_t &b3, uint32_t k0, uint32_t k1, uint32_t k2, uint32_t k3)
+{
+    const uint32_t x0 = ta.template te<0, 0>(a0), x1 = ta.template te<3, 3>(a0), x2 = ta.template te<2, 2>(a0), x3 = ta.template te<1, 1>(a0);
+    const uint32_t y0 = ta.template te<0, 0>(b0), y1 = ta.template te<3, 3>(b0), y2 = ta.template te<2, 2>(b0), y3 = ta.template te<1, 1>(b0);
+    const uint32_t t0 = x0 ^ ta.template te<1, 1>(a1) ^ ta.template te<2, 2>(a2) ^ ta.template te<3, 3>(a3) ^ k0;
+    const uint32_t t1 = ta.template te<0, 0>(a1) ^ ta.template te<1, 1>(a2) ^ ta.template te<2, 2>(a3) ^ x1 ^ k1;
+    const uint32_t t2 = ta.template te<0, 0>(a2) ^ ta.template te<1, 1>(a3) ^ x2 ^ ta.template te<3, 3>(a1) ^ k2;
+    const uint32_t t3 = ta.template te<0, 0>(a3) ^ x3 ^ ta.template te<2, 2>(a1) ^ ta.template te<3, 3>(a2) ^ k3;
+    b0 = t0 ^ x0 ^ y0;
+    b1 = t1 ^ x1 ^ y1;
+    b2 = t2 ^ x2 ^ y2;
+    b3 = t3 ^ x3 ^ y3;
+    a0 = t0; a1 = t1; a2 = t2; a3 = t3;
+}
+
 /* Both children of one node: AES_seed(0) and AES_seed(1).  LEAF: .x only. */
 template <bool LEAF, class TA>
 DPF_HD void aes128_pair(const TA &ta, const Seed &s, Seed &c0, Seed &c1)
@@ -338,10 +366,12 @@ DPF_HD void aes128_pair(const TA &ta, const Seed &s, Seed &c0, Seed &c1)
      * which after ShiftRows+MixColumns lands in output column 0 alone */
     const uint32_t sib = ta.template te<0, 0>(k0 ^ 1u);
     aes_first_round(ta, 0u, k0, k1, k2, k3, a0, a1, a2, a3, l00);
-    uint32_t b0 = a0 ^ l00 ^ sib, b1 = a1, b2 = a2, b3 = a3;
-    uint32_t rc = 2;
+    uint32_t b0 = a0 ^ l00 ^ sib, b1, b2, b3;
+    aes_next_rk(ta, k0, k1, k2, k3, 2u);
+    aes_round2_pair(ta, a0, a1, a2, a3, b0, b1, b2, b3, k0, k1, k2, k3);
+    uint32_t rc = 4;
 DPF_UNROLL
-    for (int r = 2; r <= 9; r++) {
+    for (int r = 3; r <= 9; r++) {
         aes_next_rk(ta, k0, k1, k2, k3, rc);
         rc = (rc << 1) ^ ((rc & 0x80u) ? 0x11bu : 0u);
         aes_round(ta, a0, a1, a2, a3, k0, k1, k2, k3);
@@ -464,6 +494,23 @@ DPF_HD int ctz32(uint32_t v)
 #endif
 }
 
+/* The two leaves (FULL: frontier nodes) below a node of height 1, at local
+ * positions pos and pos+1. */
+template <int PRF, bool FULL, class Env>
+DPF_HD void eval_leaf_pair(Env &env, const Seed &seed, uint32_t pos, int level_base)
+{
+    Seed l0, l1;
+    const uint32_t bank = seed.x & 1u;
+    if (FULL) {
+        expand_pair<PRF, false>(env.ta, seed, l0, l1);
+        env.node_pair(pos, add128(l0, env.cw(level_base, bank, 0)), add128(l1, env.cw(level_base, bank, 1)));
+    } else {
+        env.leaf_prefetch(pos);
+        expand_pair<PRF, true>(env.ta, seed, l0, l1);
+        env.leaf_pair(pos, l0.x + env.cw_lo(bank, 0), l1.x + env.cw_lo(bank, 1));
+    }
+}
+
 /*
  * Depth-first expansion of a complete subtree with 2^s leaves, one node pair at
  * a time, keeping only the pending right siblings (one per height).  A node of
@@ -477,9 +524,51 @@ DPF_HD int ctz32(uint32_t v)
  *   FULL = true : whole 128-bit seeds via env.node_pair(local_pos, c0, c1) --
  *                 used to materialise an interior frontier of the tree.
  */
+/* AES: the bottom of the walk goes by nodes of height 2, each expanded as a unit:
+ * one interior pair, then the leaf pairs of both its children.  The right child
+ * waits in registers, so the stack (shared memory on the device, the pipe AES
+ * binds) holds pending nodes of height 2 and up only.  Every interior pair,
+ * whatever its height, goes through the same code, and so do both leaf pairs: the
+ * loop body stays small enough for the instruction cache.  Requires s >= 2. */
+template <int PRF, bool FULL, class Env>
+DPF_HD void eval_subtree_by_quads(Env &env, Seed seed, int s, int level_base)
+{
+    int h = s;
+    const uint32_t nquads = 1u << (s - 2);
+    for (uint32_t i = 0;;) {
+        Seed c0, c1;
+        expand_pair<PRF, false>(env.ta, seed, c0, c1);
+        const uint32_t bank = seed.x & 1u;
+        const int level = level_base + h - 1;
+        c0 = add128(c0, env.cw(level, bank, 0));
+        c1 = add128(c1, env.cw(level, bank, 1));
+        if (h > 2) {
+            env.push(h - 1, c1);
+            seed = c0;
+            h--;
+            continue;
+        }
+DPF_NO_UNROLL
+        for (uint32_t k = 0; k < 2; k++) {
+            eval_leaf_pair<PRF, FULL>(env, c0, 4 * i + 2 * k, level_base);
+            c0 = c1;
+        }
+        if (++i == nquads) break;
+        h = ctz32(i) + 2;
+        seed = env.pop(h);
+    }
+}
+
+/* Salsa20 and ChaCha bind the integer ALU pipe, where the stack's shared-memory
+ * traffic costs nothing, and they keep the walk one node pair at a time (the
+ * height-2 unit measured about 3 % slower for ChaCha20 at n = 2^16 and 2^18). */
 template <int PRF, bool FULL, class Env>
 DPF_HD void eval_subtree(Env &env, Seed seed, int s, int level_base)
 {
+    if (PRF == PRF_AES128 && s >= 2) {
+        eval_subtree_by_quads<PRF, FULL>(env, seed, s, level_base);
+        return;
+    }
     int h = s;
     const uint32_t npairs = 1u << (s - 1);
     for (uint32_t i = 0; i < npairs; i++) {
@@ -493,16 +582,7 @@ DPF_HD void eval_subtree(Env &env, Seed seed, int s, int level_base)
             seed = add128(c0, env.cw(level, bank, 0));
             h--;
         }
-        Seed l0, l1;
-        const uint32_t bank = seed.x & 1u;
-        if (FULL) {
-            expand_pair<PRF, false>(env.ta, seed, l0, l1);
-            env.node_pair(2 * i, add128(l0, env.cw(level_base, bank, 0)), add128(l1, env.cw(level_base, bank, 1)));
-        } else {
-            env.leaf_prefetch(2 * i);
-            expand_pair<PRF, true>(env.ta, seed, l0, l1);
-            env.leaf_pair(2 * i, l0.x + env.cw_lo(bank, 0), l1.x + env.cw_lo(bank, 1));
-        }
+        eval_leaf_pair<PRF, FULL>(env, seed, 2 * i, level_base);
         h = ctz32(i + 1) + 1;
         if (h < s) seed = env.pop(h);
     }

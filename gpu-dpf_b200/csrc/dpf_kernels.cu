@@ -19,7 +19,8 @@
  *                 produced together in registers (shared AES key schedule /
  *                 shared first-round quarter rounds), the right child parks in a
  *                 per-thread shared-memory slot (one slot per tree height), the
- *                 left child is descended into.  No global scratch, no
+ *                 left child is descended into; below height 2 the right child
+ *                 waits in registers instead.  No global scratch, no
  *                 __syncthreads in the main loop (the reference ping-pongs two
  *                 global stacks with two barriers per step).
  *   MAC         = only the low 32 bits of a leaf survive (dpf_wrapper.cu:182),

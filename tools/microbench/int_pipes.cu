@@ -8,6 +8,9 @@
 //   fma pipe : IMAD (mad.lo), IMAD.WIDE (mul.wide), IMAD.HI (mul.hi)
 //   lsu      : conflict-free 32-bit shared-memory loads (the AES T-table access pattern)
 //   mixes    : LOP3+IMAD, LOP3+SHF+IMAD (can the two pipes issue in the same clock?), LDS+PRMT+LOP3
+//   lsu + ldg: the LDS steps plus 3 warp-uniform (broadcast) LDG.128 per 128 LDS, the ratio of the
+//              fused AES kernel's table-row loads (8 per leaf pair of ~300 lookups); each load hits
+//              one 64-byte row of a 4 MiB buffer (L2-resident), consumed by IMADs like the MAC
 //   quarter rounds: Salsa20 / ChaCha as the kernels write them, and variants that move some of
 //   the rotates to the fma pipe as IMAD.WIDE (x*2^r = {x<<r, x>>(32-r)}; the halves are disjoint,
 //   so  b ^ rotl(t,r) == lop3.xor(b, lo, hi)).
@@ -23,7 +26,7 @@
 #define UNROLL 16     // ops per chain per loop trip
 
 enum Op { OP_LOP3, OP_SHF, OP_PRMT, OP_IADD3, OP_IMAD, OP_IMADWIDE, OP_IMADHI, OP_LDS,
-          OP_MIX_LOP3_IMAD, OP_MIX_LOP3_SHF_IMAD, OP_MIX_LDS_PRMT_LOP3, OP_MIX_LOP3_IMADWIDE };
+          OP_MIX_LOP3_IMAD, OP_MIX_LOP3_SHF_IMAD, OP_MIX_LDS_PRMT_LOP3, OP_MIX_LOP3_IMADWIDE, OP_LDS_LDG };
 
 template <int OP>
 __device__ __forceinline__ void step(uint32_t &x, uint32_t y, uint32_t z, uint32_t smem_lane)
@@ -44,7 +47,7 @@ __device__ __forceinline__ void step(uint32_t &x, uint32_t y, uint32_t z, uint32
                      "lop3.b32 %0, lo, hi, %1, 0x96;\n\t}" : "+r"(x) : "r"(y));
     } else if (OP == OP_IMADHI) {
         asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(x) : "r"(y));
-    } else if (OP == OP_LDS) {
+    } else if (OP == OP_LDS || OP == OP_LDS_LDG) {
         uint32_t a;
         asm volatile("prmt.b32 %0, %1, %2, 0x7604;" : "=r"(a) : "r"(x), "r"(smem_lane));
         asm volatile("ld.shared.u32 %0, [%1];" : "=r"(x) : "r"(a));
@@ -74,7 +77,7 @@ __host__ __device__ constexpr Mix mix_of(int op)
     return op == OP_LOP3 || op == OP_SHF || op == OP_PRMT || op == OP_IADD3 ? Mix{1, 0, 0}
          : op == OP_IMAD || op == OP_IMADHI ? Mix{0, 1, 0}
          : op == OP_IMADWIDE ? Mix{1, 1, 0}
-         : op == OP_LDS ? Mix{1, 0, 1}
+         : op == OP_LDS || op == OP_LDS_LDG ? Mix{1, 0, 1}
          : op == OP_MIX_LOP3_IMAD ? Mix{1, 1, 0}
          : op == OP_MIX_LOP3_SHF_IMAD ? Mix{2, 1, 0}
          : op == OP_MIX_LDS_PRMT_LOP3 ? Mix{2, 0, 1}
@@ -87,7 +90,8 @@ extern __shared__ __align__(16) unsigned char s_raw[];
 #define TAB_SMEM (128 * 1024 + 16)
 
 template <int OP>
-__global__ void __launch_bounds__(512, 1) pipe_kernel(uint32_t *out, long long *cycles, int iters)
+#define ROWS_MASK 65535u   /* 64 KiB rows of 64 bytes = 4 MiB */
+__global__ void __launch_bounds__(512, 1) pipe_kernel(uint32_t *out, long long *cycles, int iters, const uint4 *rows)
 {
     const uint32_t base = (uint32_t)__cvta_generic_to_shared(s_raw);
     const uint32_t tab = (base + 65535u) & ~65535u;            /* 64 KiB-aligned window address inside the 128 KiB */
@@ -100,6 +104,8 @@ __global__ void __launch_bounds__(512, 1) pipe_kernel(uint32_t *out, long long *
 #pragma unroll
     for (int c = 0; c < CH; c++) x[c] = threadIdx.x * 2654435761u + c * 40503u + blockIdx.x;
     const uint32_t y = x[0] | 1u, z = x[1] ^ 0x5bd1e995u;
+    const uint32_t warp_id = blockIdx.x * 16u + (threadIdx.x >> 5);
+    uint32_t sink = 0;
     __syncthreads();
     const long long t0 = clock64();
     for (int it = 0; it < iters; it++) {
@@ -107,11 +113,15 @@ __global__ void __launch_bounds__(512, 1) pipe_kernel(uint32_t *out, long long *
         for (int u = 0; u < UNROLL; u++) {
 #pragma unroll
             for (int c = 0; c < CH; c++) step<OP>(x[c], y, z, smem_lane);
+            if (OP == OP_LDS_LDG && u % 5 == 2) {   /* u = 2, 7, 12: words 0..2 of this trip's row */
+                const uint4 r = __ldg(rows + (size_t)(((uint32_t)it * 2654435761u + warp_id) & ROWS_MASK) * 4 + u / 5);
+                sink += r.x * y + r.y * z + r.z * y + r.w * z;
+            }
         }
     }
     __syncthreads();
     const long long t1 = clock64();
-    uint32_t acc = 0;
+    uint32_t acc = sink;
 #pragma unroll
     for (int c = 0; c < CH; c++) acc ^= x[c];
     out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
@@ -210,6 +220,7 @@ __global__ void __launch_bounds__(512, 1) qr_kernel(uint32_t *out, long long *cy
 
 static uint32_t *g_out;
 static long long *g_cycles;
+static uint4 *g_rows;
 static int g_sms;
 
 static double max_cycles()
@@ -227,11 +238,11 @@ static void run_pipe(const char *name)
     auto k = pipe_kernel<OP>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TAB_SMEM);
     const int iters = 2000;
-    k<<<g_sms, 512, TAB_SMEM>>>(g_out, g_cycles, 50);
+    k<<<g_sms, 512, TAB_SMEM>>>(g_out, g_cycles, 50, g_rows);
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a);
-    k<<<g_sms, 512, TAB_SMEM>>>(g_out, g_cycles, iters);
+    k<<<g_sms, 512, TAB_SMEM>>>(g_out, g_cycles, iters, g_rows);
     cudaEventRecord(b);
     cudaEventSynchronize(b);
     float ms = 0;
@@ -281,6 +292,8 @@ int main()
            "\"chains_per_thread\": %d}\n", p.name, g_sms, khz / 1000.0, CH);
     cudaMalloc(&g_out, sizeof(uint32_t) * g_sms * 512);
     cudaMalloc(&g_cycles, sizeof(long long) * 1024);
+    cudaMalloc(&g_rows, sizeof(uint4) * 4 * (ROWS_MASK + 1));
+    cudaMemset(g_rows, 0x5a, sizeof(uint4) * 4 * (ROWS_MASK + 1));
     run_pipe<OP_LOP3>("LOP3");
     run_pipe<OP_SHF>("SHF");
     run_pipe<OP_PRMT>("PRMT");
@@ -289,6 +302,7 @@ int main()
     run_pipe<OP_IMADWIDE>("IMAD.WIDE+LOP3");
     run_pipe<OP_IMADHI>("IMAD.HI");
     run_pipe<OP_LDS>("PRMT+LDS.32 conflict-free");
+    run_pipe<OP_LDS_LDG>("PRMT+LDS.32 + 3 broadcast LDG.128 per 128 LDS");
     run_pipe<OP_MIX_LOP3_IMAD>("LOP3+IMAD");
     run_pipe<OP_MIX_LOP3_SHF_IMAD>("LOP3+SHF+IMAD");
     run_pipe<OP_MIX_LDS_PRMT_LOP3>("PRMT+LDS+LOP3");
