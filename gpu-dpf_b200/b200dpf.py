@@ -22,6 +22,7 @@ SYMBOLS = [
     "b200dpf_key_packed_size", "b200dpf_key_pack", "b200dpf_key_unpack", "b200dpf_key_n", "b200dpf_key_depth", "b200dpf_create", "b200dpf_destroy", "b200dpf_eval",
     "b200dpf_eval_packed", "b200dpf_eval_gather", "b200dpf_ctx_set_option", "b200dpf_create_multi", "b200dpf_ctx_device_count", "b200dpf_ctx_axis", "b200dpf_ctx_read_timing",
     "b200dpf_group_create", "b200dpf_group_eval", "b200dpf_group_bins", "b200dpf_ctx_last_device_ms",
+    "b200dpf_update_rows", "b200dpf_update_rows_device", "b200dpf_group_update_rows",
     "b200dpf_host_staging", "b200dpf_eval_device", "b200dpf_eval_device_acc", "b200dpf_expand_device", "b200dpf_ctx_n", "b200dpf_ctx_entry_size",
     "b200dpf_ctx_device", "b200dpf_ctx_last_launches", "b200dpf_ctx_set_subtree_log2",
 ]
@@ -65,6 +66,9 @@ def load():
     L.b200dpf_ctx_last_device_ms.restype = C.c_double
     L.b200dpf_ctx_read_timing.argtypes = [C.c_void_p, np.ctypeslib.ndpointer(dtype=np.uint64, flags="C_CONTIGUOUS"), C.c_int,
                                           C.POINTER(C.c_int)]
+    L.b200dpf_update_rows.argtypes = [C.c_void_p, _i64p, _i32p, C.c_int64]
+    L.b200dpf_update_rows_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    L.b200dpf_group_update_rows.argtypes = [C.c_void_p, _i32p, _i64p, _i32p, C.c_int64]
     L.b200dpf_destroy.argtypes = [C.c_void_p]
     L.b200dpf_eval.argtypes = [C.c_void_p, _i32p, C.c_int64, C.c_int, _i32p]
     L.b200dpf_eval_packed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int, _i32p]
@@ -232,6 +236,17 @@ class Context:
         _check(lib().b200dpf_eval_gather(self.handle, ptrs, len(arrs), prf, out), "b200dpf_eval_gather")
         return out
 
+    def update_rows(self, indices, rows):
+        """table[indices[j]] := rows[j] (natural indices, last occurrence wins); synchronous"""
+        indices = np.ascontiguousarray(indices, np.int64).reshape(-1)
+        rows = np.ascontiguousarray(rows, np.int32).reshape(len(indices), self.entry_size)
+        _check(lib().b200dpf_update_rows(self.handle, indices, rows, len(indices)), "b200dpf_update_rows")
+
+    def update_rows_device(self, idx_ptr, rows_ptr, count, stream=0):
+        """update_rows from device buffers (int64 [count], int32 [count, entry_size]), enqueued on `stream`"""
+        _check(lib().b200dpf_update_rows_device(self.handle, C.c_void_p(idx_ptr), C.c_void_p(rows_ptr), count,
+                                                C.c_void_p(stream)), "b200dpf_update_rows_device")
+
     def set_option(self, name, value):
         _check(lib().b200dpf_ctx_set_option(self.handle, name.encode(), int(value)), "b200dpf_ctx_set_option")
 
@@ -300,3 +315,11 @@ class GroupContext(Context):
         out = np.zeros((keys.shape[0], self.entry_size), np.int32)
         _check(lib().b200dpf_group_eval(self.handle, keys, bins, keys.shape[0], prf, out), "b200dpf_group_eval")
         return out
+
+    def update_rows(self, bins, indices, rows):
+        """row indices[j] of bin bins[j] := rows[j] (last occurrence wins); synchronous"""
+        bins = np.ascontiguousarray(bins, np.int32).reshape(-1)
+        indices = np.ascontiguousarray(indices, np.int64).reshape(-1)
+        assert bins.shape == indices.shape
+        rows = np.ascontiguousarray(rows, np.int32).reshape(len(indices), self.entry_size)
+        _check(lib().b200dpf_group_update_rows(self.handle, bins, indices, rows, len(indices)), "b200dpf_group_update_rows")

@@ -84,6 +84,7 @@ struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behi
     GroupDesc *h_descs = nullptr;      /* pinned */
     size_t h_descs_cap = 0;
     std::vector<int64_t> perm;         /* sorted position -> caller's index, of the last evaluation */
+    uint2 *d_bin_info = nullptr;       /* [nbins] (row_off, depth) for row updates, uploaded on first use */
 };
 
 struct b200dpf_ctx {
@@ -153,6 +154,10 @@ struct b200dpf_ctx {
      * want the kernel time next to their own wall clock */
     cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
     bool timed = false;
+    /* row updates (b200dpf_update_rows*): their own scratch, so an update never touches a buffer an
+     * evaluation in flight may read; layout at UpdateLayout */
+    void *d_update = nullptr;
+    size_t update_cap = 0;       /* bytes */
 };
 
 namespace {
@@ -1041,9 +1046,11 @@ int b200dpf_destroy(b200dpf_ctx *c)
     if (c->d_top_counters) cudaFree(c->d_top_counters);
     if (c->d_gridbar) cudaFree(c->d_gridbar);
     if (c->d_timing) cudaFree(c->d_timing);
+    if (c->d_update) cudaFree(c->d_update);
     if (c->bins) {
         if (c->bins->d_descs) cudaFree(c->bins->d_descs);
         if (c->bins->h_descs) cudaFreeHost(c->bins->h_descs);
+        if (c->bins->d_bin_info) cudaFree(c->bins->d_bin_info);
         delete c->bins;
     }
     if (c->ev_done) cudaEventDestroy(c->ev_done);
@@ -1875,6 +1882,223 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     for (int64_t pos = 0; pos < nkeys; pos++)       /* back to the caller's order */
         std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
+    return B200DPF_OK;
+}
+
+/* ------------------------------------------------------------------------------------------- */
+/* Row updates of a live table.                                                                  */
+/* ------------------------------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+
+constexpr int64_t kMaxUpdateCount = 0x7fffffff;   /* occurrence numbers are 32-bit, as is the sort's item count */
+
+/* Update scratch (one allocation, every section 256-byte aligned):
+ *   [idx int64 | bins int32 | rows int32 [count][entry_size]]   host paths only: the caller's rows copied in
+ *   pos_in | pos_out | ord_in | ord_out                          uint32 [count] each
+ *   sort temporary                                               cub::DeviceRadixSort::SortPairs */
+struct UpdateLayout {
+    size_t off_idx, off_bins, off_rows, off_work[4], off_temp, temp_bytes, total;
+    int end_bit;
+};
+
+size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+/* rows of the device table; also the skip marker of the update kernels (larger than every position) */
+uint64_t update_table_rows(const b200dpf_ctx *c)
+{
+    return c->bins ? c->bins->row_off.back() + (uint64_t)c->bins->n.back() : (uint64_t)c->n_local;
+}
+
+uint32_t bitrev_host(uint32_t v, int bits)
+{
+    uint32_t r = 0;
+    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
+    return r;
+}
+
+/* Grow the scratch for `count` rows (staged: the inputs are copied into it) and order everything that
+ * follows on `stream` after the context's previous evaluation or update: the update writes the table
+ * those read, and the scratch is the previous update's. */
+int update_begin(b200dpf_ctx *c, int64_t count, bool staged, bool with_bins, cudaStream_t stream, UpdateLayout *L)
+{
+    const uint64_t rows = update_table_rows(c);
+    if (rows >= 0xffffffffull) return fail(B200DPF_EINVAL, "table of %llu rows too large for row updates", (unsigned long long)rows);
+    L->end_bit = 1;
+    while (L->end_bit < 32 && (rows >> L->end_bit) != 0) L->end_bit++;
+    CUDA_TRY(update_temp_bytes(count, L->end_bit, &L->temp_bytes));
+    size_t off = 0;
+    L->off_idx = off;
+    if (staged) off = align256(off + (size_t)count * sizeof(int64_t));
+    L->off_bins = off;
+    if (staged && with_bins) off = align256(off + (size_t)count * sizeof(int32_t));
+    L->off_rows = off;
+    if (staged) off = align256(off + (size_t)count * (size_t)c->entry_size * sizeof(int32_t));
+    for (int k = 0; k < 4; k++) {
+        L->off_work[k] = off;
+        off = align256(off + (size_t)count * sizeof(uint32_t));
+    }
+    L->off_temp = off;
+    L->total = align256(off + L->temp_bytes);
+    const int rc = ensure_buffer(&c->d_update, &c->update_cap, L->total);
+    if (rc) return rc;
+    if (c->has_last && c->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, c->ev_done, 0));
+    return B200DPF_OK;
+}
+
+/* Enqueue the scatter (inputs in device memory) and record it as the context's last operation. */
+int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const int32_t *bins, const int32_t *rows,
+               int64_t count, cudaStream_t stream)
+{
+    char *s = static_cast<char *>(c->d_update);
+    UpdateParams u;
+    std::memset(&u, 0, sizeof u);
+    u.idx = idx;
+    u.bins = bins;
+    if (bins) {
+        u.bin_info = c->bins->d_bin_info;
+        u.nbins = (int)c->bins->n.size();
+    }
+    u.rows = rows;
+    u.count = count;
+    u.n = c->n;
+    u.own_mask = (uint32_t)c->shard_count - 1u;
+    u.own_val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
+    u.shift = c->shard_bits;
+    u.depth = c->depth_local;
+    u.table_rows = (uint32_t)update_table_rows(c);
+    u.table = c->d_table;
+    u.cols = c->entry_size;
+    u.stride = c->entry_pad;
+    UpdateWork w;
+    w.pos_in = reinterpret_cast<uint32_t *>(s + L.off_work[0]);
+    w.pos_out = reinterpret_cast<uint32_t *>(s + L.off_work[1]);
+    w.ord_in = reinterpret_cast<uint32_t *>(s + L.off_work[2]);
+    w.ord_out = reinterpret_cast<uint32_t *>(s + L.off_work[3]);
+    w.temp = s + L.off_temp;
+    w.temp_bytes = L.temp_bytes;
+    CUDA_TRY(launch_update_rows(u, w, L.end_bit, c->sm_count, stream));
+    CUDA_TRY(cudaEventRecord(c->ev_done, stream));
+    c->last_stream = stream;
+    c->has_last = true;
+    return B200DPF_OK;
+}
+
+/* Host path on one single-device context (device already current, inputs validated): copy the rows this
+ * context owns into the scratch and enqueue the scatter on the context's stream.  The caller synchronises. */
+int update_host_enqueue(b200dpf_ctx *c, const int64_t *idx, const int32_t *bins, const int32_t *rows, int64_t count)
+{
+    std::vector<int64_t> own_idx;
+    std::vector<int32_t> own_rows;
+    if (c->shard_count > 1) {             /* a shard copies only its own rows */
+        const uint32_t mask = (uint32_t)c->shard_count - 1u, val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
+        for (int64_t j = 0; j < count; j++)
+            if (((uint32_t)idx[j] & mask) == val) {
+                own_idx.push_back(idx[j]);
+                own_rows.insert(own_rows.end(), rows + j * c->entry_size, rows + (j + 1) * c->entry_size);
+            }
+        idx = own_idx.data();
+        rows = own_rows.data();
+        count = (int64_t)own_idx.size();
+    }
+    if (count == 0) return B200DPF_OK;
+    UpdateLayout L;
+    int rc = update_begin(c, count, true, bins != nullptr, c->stream, &L);
+    if (rc) return rc;
+    char *s = static_cast<char *>(c->d_update);
+    CUDA_TRY(cudaMemcpyAsync(s + L.off_idx, idx, (size_t)count * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
+    if (bins) CUDA_TRY(cudaMemcpyAsync(s + L.off_bins, bins, (size_t)count * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(s + L.off_rows, rows, (size_t)count * (size_t)c->entry_size * sizeof(int32_t),
+                             cudaMemcpyHostToDevice, c->stream));
+    return update_run(c, L, reinterpret_cast<const int64_t *>(s + L.off_idx),
+                      bins ? reinterpret_cast<const int32_t *>(s + L.off_bins) : nullptr,
+                      reinterpret_cast<const int32_t *>(s + L.off_rows), count, c->stream);
+}
+
+int check_update_args(const b200dpf_ctx *c, const void *idx, const void *rows, int64_t count)
+{
+    if (!c) return fail(B200DPF_EINVAL, "null context");
+    if (count < 0 || count > kMaxUpdateCount) return fail(B200DPF_EINVAL, "update count=%lld out of range [0, 2^31)", (long long)count);
+    if (count > 0 && (!idx || !rows)) return fail(B200DPF_EINVAL, "null buffer");
+    return B200DPF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200dpf_update_rows(b200dpf_ctx *c, const int64_t *indices, const int32_t *rows, int64_t count)
+{
+    int rc = check_update_args(c, indices, rows, count);
+    if (rc) return rc;
+    if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_update_rows");
+    if (!c->d_table && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
+    for (int64_t j = 0; j < count; j++)
+        if (indices[j] < 0 || indices[j] >= c->n)
+            return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld)", (long long)j, (long long)indices[j],
+                        (long long)c->n);
+    if (count == 0) return B200DPF_OK;
+    std::vector<b200dpf_ctx *> subs = c->multi ? c->multi->sub : std::vector<b200dpf_ctx *>{c};
+    /* every device's copies and kernels are issued before the first synchronisation */
+    for (b200dpf_ctx *s : subs) {
+        DeviceGuard guard(s->device);
+        if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", s->device);
+        rc = update_host_enqueue(s, indices, nullptr, rows, count);
+        if (rc) return rc;
+    }
+    for (b200dpf_ctx *s : subs) {
+        DeviceGuard guard(s->device);
+        CUDA_TRY(cudaStreamSynchronize(s->stream));
+    }
+    return B200DPF_OK;
+}
+
+int b200dpf_update_rows_device(b200dpf_ctx *c, const int64_t *indices_dev, const int32_t *rows_dev, int64_t count,
+                               void *cuda_stream)
+{
+    int rc = check_update_args(c, indices_dev, rows_dev, count);
+    if (rc) return rc;
+    if (c->multi) return fail(B200DPF_EINVAL, "multi-device contexts take host buffers (b200dpf_update_rows)");
+    if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_update_rows");
+    if (!c->d_table) return fail(B200DPF_ESTATE, "context has no table");
+    if (count == 0) return B200DPF_OK;
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    UpdateLayout L;
+    rc = update_begin(c, count, false, false, stream, &L);
+    if (rc) return rc;
+    return update_run(c, L, indices_dev, nullptr, rows_dev, count, stream);
+}
+
+int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t *indices, const int32_t *rows, int64_t count)
+{
+    int rc = check_update_args(c, indices, rows, count);
+    if (rc) return rc;
+    if (!c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
+    if (count > 0 && !bins) return fail(B200DPF_EINVAL, "null buffer");
+    GroupBins *B = c->bins;
+    const int nbins = (int)B->n.size();
+    for (int64_t j = 0; j < count; j++) {
+        if (bins[j] < 0 || bins[j] >= nbins)
+            return fail(B200DPF_EINVAL, "update %lld: bin %d out of range [0,%d)", (long long)j, bins[j], nbins);
+        if (indices[j] < 0 || indices[j] >= B->n[(size_t)bins[j]])
+            return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld) of bin %d", (long long)j,
+                        (long long)indices[j], (long long)B->n[(size_t)bins[j]], bins[j]);
+    }
+    if (count == 0) return B200DPF_OK;
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    if (!B->d_bin_info) {
+        std::vector<uint2> info((size_t)nbins);
+        for (int g = 0; g < nbins; g++) info[(size_t)g] = make_uint2((uint32_t)B->row_off[(size_t)g], (uint32_t)B->depth[(size_t)g]);
+        CUDA_TRY(cudaMalloc(&B->d_bin_info, info.size() * sizeof(uint2)));
+        CUDA_TRY(cudaMemcpy(B->d_bin_info, info.data(), info.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    }
+    rc = update_host_enqueue(c, indices, bins, rows, count);
+    if (rc) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
     return B200DPF_OK;
 }
 

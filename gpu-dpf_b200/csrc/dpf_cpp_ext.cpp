@@ -13,7 +13,7 @@
  *   - errors surface as Python exceptions (RuntimeError) instead of assert /
  *     exit (dpf_wrapper.cu:7-15);
  *   - extra entry points: gen_batch, eval_gpu_packed, eval_init_sharded,
- *     expand_gpu, version; attribute NATIVE_SHAPES = 1 advertises them.
+ *     expand_gpu, update_rows, version; attribute NATIVE_SHAPES = 1 advertises them.
  */
 #include <torch/extension.h>
 #include <torch/csrc/autograd/python_variable.h>
@@ -201,6 +201,46 @@ at::Tensor group_eval(const at::Tensor &keys, const at::Tensor &bins, const std:
               "group_eval");
     }
     return result;
+}
+
+/* row updates of a live table (b200dpf_update_rows): indices int64 [count] natural, rows int32 [count, E],
+ * both CPU tensors; synchronous */
+void update_rows(const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
+{
+    b200dpf_ctx *ctx = ctx_of(buffers);
+    TORCH_CHECK(indices.device().is_cpu() && indices.scalar_type() == at::kLong && indices.dim() == 1 && indices.is_contiguous(),
+                "update_rows: indices must be a contiguous CPU int64 tensor [count]");
+    TORCH_CHECK(rows.device().is_cpu() && rows.scalar_type() == at::kInt && rows.dim() == 2 && rows.is_contiguous() &&
+                    rows.size(0) == indices.size(0) && rows.size(1) == b200dpf_ctx_entry_size(ctx),
+                "update_rows: rows must be a contiguous CPU int32 tensor [count, entry_size]");
+    py::gil_scoped_release nogil;
+    check(b200dpf_update_rows(ctx, indices.data_ptr<int64_t>(), rows.data_ptr<int32_t>(), indices.size(0)), "update_rows");
+}
+
+/* the same from device buffers, enqueued on the stream handle passed as an integer */
+void update_rows_device(int64_t idx_ptr, int64_t rows_ptr, int64_t count, const std::vector<void *> &buffers, int64_t stream)
+{
+    check(b200dpf_update_rows_device(ctx_of(buffers), reinterpret_cast<const int64_t *>(idx_ptr),
+                                     reinterpret_cast<const int32_t *>(rows_ptr), count, reinterpret_cast<void *>(stream)),
+          "update_rows_device");
+}
+
+/* grouped context: row indices[j] of bin bins[j] := rows[j]; CPU tensors, synchronous */
+void group_update_rows(const at::Tensor &bins, const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
+{
+    b200dpf_ctx *ctx = ctx_of(buffers);
+    TORCH_CHECK(bins.device().is_cpu() && bins.scalar_type() == at::kInt && bins.dim() == 1 && bins.is_contiguous(),
+                "group_update_rows: bins must be a contiguous CPU int32 tensor [count]");
+    TORCH_CHECK(indices.device().is_cpu() && indices.scalar_type() == at::kLong && indices.sizes() == bins.sizes() &&
+                    indices.is_contiguous(),
+                "group_update_rows: indices must be a contiguous CPU int64 tensor [count]");
+    TORCH_CHECK(rows.device().is_cpu() && rows.scalar_type() == at::kInt && rows.dim() == 2 && rows.is_contiguous() &&
+                    rows.size(0) == indices.size(0) && rows.size(1) == b200dpf_ctx_entry_size(ctx),
+                "group_update_rows: rows must be a contiguous CPU int32 tensor [count, entry_size]");
+    py::gil_scoped_release nogil;
+    check(b200dpf_group_update_rows(ctx, bins.data_ptr<int32_t>(), indices.data_ptr<int64_t>(), rows.data_ptr<int32_t>(),
+                                    indices.size(0)),
+          "group_update_rows");
 }
 
 /* "all" / "" -> every visible device; "0,2,3" -> that list */
@@ -409,6 +449,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("group_eval", &group_eval, "batch PIR: evaluate (bin, key) pairs in one launch");
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),
           py::arg("devices"), py::arg("axis") = 0);
+    m.def("update_rows", &update_rows, "table[indices[j]] := rows[j] on a live context (CPU tensors)");
+    m.def("update_rows_device", &update_rows_device, "row update from device buffers, enqueued on a stream",
+          py::arg("idx_ptr"), py::arg("rows_ptr"), py::arg("count"), py::arg("buffers"), py::arg("stream"));
+    m.def("group_update_rows", &group_update_rows, "batch PIR: row indices[j] of bin bins[j] := rows[j]");
     m.def("parse_devices", &parse_devices, "'all' or '0,1,2' -> device list");
     m.def("device_count", [](const std::vector<void *> &b) { return b200dpf_ctx_device_count(ctx_of(b)); });
     m.def("axis", [](const std::vector<void *> &b) { return b200dpf_ctx_axis(ctx_of(b)); });

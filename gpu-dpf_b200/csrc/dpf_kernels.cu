@@ -58,6 +58,8 @@
 #include <algorithm>
 #include <atomic>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include "dpf_core.cuh"
 
 namespace b200dpf {
@@ -739,6 +741,54 @@ __global__ void permute_table_kernel(const int32_t *__restrict__ stage, int32_t 
     }
 }
 
+__device__ __forceinline__ uint32_t bitrev_bits(uint32_t v, int bits) { return bits ? __brev(v) >> (32 - bits) : 0u; }
+
+/* row update, step 1: natural index -> table row (or the skip marker), occurrence number j */
+__global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
+                                                         uint32_t *__restrict__ ord)
+{
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = u.idx[j];
+        uint32_t p = u.table_rows;
+        if (u.bins) {
+            const int32_t g = u.bins[j];
+            if (g >= 0 && g < u.nbins) {
+                const uint2 info = u.bin_info[g];
+                if (i >= 0 && i < ((int64_t)1 << info.y)) p = info.x + bitrev_bits((uint32_t)i, (int)info.y);
+            }
+        } else if (i >= 0 && i < u.n && ((uint32_t)i & u.own_mask) == u.own_val) {
+            p = bitrev_bits((uint32_t)(i >> u.shift), u.depth);
+        }
+        pos[j] = p;
+        ord[j] = (uint32_t)j;
+    }
+}
+
+/* row update, step 3: positions sorted stably, so the last occurrence of a position ends its run;
+ * one warp copies that occurrence's row, 16 bytes per lane and step when the rows allow it.  (Scalar
+ * arguments: reading them out of the UpdateParams struct costs this loop a spill.) */
+__global__ void __launch_bounds__(256) update_scatter_kernel(const int32_t *__restrict__ rows, int32_t *__restrict__ table,
+                                                             const uint32_t *__restrict__ pos, const uint32_t *__restrict__ ord,
+                                                             int64_t count, uint32_t skip, int cols, int stride, int vec4)
+{
+    const int lane = (int)(threadIdx.x & 31u);
+    const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x / 32);
+    for (int64_t k = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; k < count; k += nwarps) {
+        const uint32_t p = pos[k];
+        if (p == skip) break;                               /* skipped entries sort last */
+        if (k + 1 < count && pos[k + 1] == p) continue;     /* a later occurrence wins  */
+        const int32_t *src = rows + (size_t)ord[k] * (size_t)cols;
+        int32_t *dst = table + (size_t)p * (size_t)stride;
+        if (vec4) {
+            const int4 *s4 = reinterpret_cast<const int4 *>(src);
+            int4 *d4 = reinterpret_cast<int4 *>(dst);
+            for (int c = lane; c < cols / 4; c += 32) d4[c] = s4[c];
+        } else {
+            for (int c = lane; c < cols; c += 32) dst[c] = src[c];
+        }
+    }
+}
+
 template <int PRF, int NV, int MODE>
 cudaError_t launch_one(const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
 {
@@ -909,6 +959,32 @@ cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t 
     int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
     if (grid < 1) grid = 1;
     permute_table_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, cols, stride);
+    return cudaGetLastError();
+}
+
+cudaError_t update_temp_bytes(int64_t count, int end_bit, size_t *bytes)
+{
+    *bytes = 0;
+    return cub::DeviceRadixSort::SortPairs(nullptr, *bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
+                                           (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)count, 0, end_bit);
+}
+
+cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int end_bit, int sm_count, cudaStream_t stream)
+{
+    if (u.count <= 0) return cudaSuccess;
+    const int64_t cap = (int64_t)std::max(sm_count, 1) * 16;
+    const int grid_map = (int)std::max<int64_t>(1, std::min<int64_t>((u.count + 255) / 256, cap));
+    update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    size_t temp_bytes = w.temp_bytes;
+    e = cub::DeviceRadixSort::SortPairs(w.temp, temp_bytes, w.pos_in, w.pos_out, w.ord_in, w.ord_out, (int)u.count, 0,
+                                        end_bit, stream);
+    if (e != cudaSuccess) return e;
+    const bool vec4 = (u.cols & 3) == 0 && (reinterpret_cast<uintptr_t>(u.rows) & 15u) == 0;
+    const int grid_scatter = (int)std::max<int64_t>(1, std::min<int64_t>((u.count + 7) / 8, cap));
+    update_scatter_kernel<<<grid_scatter, 256, 0, stream>>>(u.rows, u.table, w.pos_out, w.ord_out, u.count, u.table_rows,
+                                                            u.cols, u.stride, vec4 ? 1 : 0);
     return cudaGetLastError();
 }
 

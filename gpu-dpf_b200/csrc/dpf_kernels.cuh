@@ -173,4 +173,38 @@ cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
                                  int cols, int stride, int sm_count, cudaStream_t stream);
 
+/* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
+ * j < count, the last occurrence of a position winning.  Position of natural index i:
+ *   bins == null   skip unless 0 <= i < n and (i & own_mask) == own_val;
+ *                  else bitrev_depth(i >> shift)                      (whole table or one shard)
+ *   bins != null   bin g = bins[j] (skip unless 0 <= g < nbins); skip unless 0 <= i < 2^bin_info[g].y;
+ *                  else bin_info[g].x + bitrev_{bin_info[g].y}(i)     (grouped context)
+ * Skipped entries are never written. */
+struct UpdateParams {
+    const int64_t *idx;       /* [count] natural indices                                      */
+    const int32_t *bins;      /* [count] bin ids, or null                                     */
+    const uint2 *bin_info;    /* [nbins] (first row, depth)                                   */
+    int nbins;
+    const int32_t *rows;      /* [count][cols] new rows                                       */
+    int64_t count;            /* <= 2^31 - 1                                                  */
+    int64_t n;
+    uint32_t own_mask, own_val;
+    int shift, depth;
+    uint32_t table_rows;      /* rows of the device table: the skip marker, larger than every position */
+    int32_t *table;           /* [table_rows][stride], 64-byte rows; pad columns are not touched */
+    int cols, stride;
+};
+/* Device scratch of one update: positions and occurrence numbers before and after the sort, then
+ * the sort's temporary storage (update_temp_bytes). */
+struct UpdateWork {
+    uint32_t *pos_in, *pos_out, *ord_in, *ord_out;
+    void *temp;
+    size_t temp_bytes;
+};
+/* Bytes of temporary storage the stable sort of `count` positions below 2^end_bit needs. */
+cudaError_t update_temp_bytes(int64_t count, int end_bit, size_t *bytes);
+/* map -> stable radix sort of (position, occurrence) -> one warp per surviving row; enqueued on
+ * `stream`, no host synchronisation. */
+cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int end_bit, int sm_count, cudaStream_t stream);
+
 }  // namespace b200dpf

@@ -77,6 +77,7 @@ class DPF(object):
         self.table_num_entries = None
         self.table_effective_entry_size = None
         self.table = None
+        self.table_rows = None
         self.device = device
         self.shard = tuple(shard)
         self.prf_method = prf if prf is not None else self.DEFAULT_PRF
@@ -137,10 +138,15 @@ class DPF(object):
             self.buffers = None
         if table.shape[0] < 128:
             raise Exception("Table (%d) must have at least 128 elements" % table.shape[0])
+        # the caller's row count: with allow_non_pow2 the rows beyond it are zero padding that updates may not touch
+        self.table_rows = table.shape[0]
+        # eval_cpu reads self.table; update_rows copies it before the first write, never writing the caller's tensor
+        self._table_is_callers = True
         if table.shape[0] & (table.shape[0] - 1) != 0:
             if not self.allow_non_pow2:
                 raise Exception("Table num entries (%d) must be a power of two" % (table.shape[0]))
             table = _pad_rows_to_pow2(table)
+            self._table_is_callers = False
         self.table = table
         self.table_num_entries = table.shape[0]
         self.table_effective_entry_size = table.shape[1]
@@ -148,6 +154,45 @@ class DPF(object):
             self.buffers = dpf_cpp.eval_init_multi(table, self.devices, {"auto": 0, "entries": 1, "keys": 2}[self.axis])
         else:
             self.buffers = dpf_cpp.eval_init_sharded(table, self.device, self.shard[0], self.shard[1])
+
+    def update_rows(self, indices, rows):
+        """Replace rows of the uploaded table in place: table[indices[j]] := rows[j] for natural indices (the
+        numbering keys use); when an index repeats, its last row wins.  `rows` [count, entry_size] is cast to
+        int32 like eval_init's table.  Only the touched rows move: no re-upload, and `buffers` stays valid.
+
+        CPU tensors (or lists) are applied synchronously.  CUDA tensors on the context's device are applied on
+        the current torch stream, after every evaluation issued before and before every one issued after,
+        without the host waiting for the update itself; the index range check before it does synchronise
+        (one reduction read back), and so does keeping self.table in step when it lives on the CPU.
+        self.table (what eval_cpu multiplies with) follows every update; the tensor passed to eval_init is
+        copied on the first update and never written."""
+        if self.buffers is None:
+            raise Exception("Must call `eval_init` before `update_rows`")
+        idx, rows = _update_args(indices, rows, self.table_effective_entry_size)
+        if idx.is_cuda != rows.is_cuda or (idx.is_cuda and (idx.device.index != self.device or rows.device.index != self.device)):
+            raise Exception("indices and rows must both be CPU tensors or both CUDA tensors on cuda:%d" % self.device)
+        if idx.is_cuda and self.devices:
+            raise Exception("a multi-device DPF takes host rows (CPU tensors); device-resident updates are per GPU "
+                            "(DPF(device=d, shard=(rank, count)) or sharded.ShardedDPF)")
+        if idx.numel() and not bool(((idx >= 0) & (idx < self.table_rows)).all()):
+            raise Exception("update index out of range [0, %d)" % self.table_rows)
+        idx = idx.to(torch.int64).contiguous()
+        rows = rows.to(torch.int32).contiguous()
+        if idx.numel() == 0:
+            return
+        if idx.is_cuda:
+            stream = torch.cuda.current_stream(idx.device).cuda_stream
+            dpf_cpp.update_rows_device(idx.data_ptr(), rows.data_ptr(), idx.numel(), self.buffers, stream)
+        else:
+            dpf_cpp.update_rows(idx, rows, self.buffers)
+        if self.table is not None:
+            if self._table_is_callers:
+                self.table = self.table.clone()
+                self._table_is_callers = False
+            uniq, inverse = torch.unique(idx, return_inverse=True)
+            last = torch.full((uniq.numel(),), -1, dtype=torch.int64, device=idx.device).scatter_reduce_(
+                0, inverse, torch.arange(idx.numel(), device=idx.device), "amax")
+            self.table[uniq.to(self.table.device)] = rows[last].to(self.table.device, self.table.dtype)
 
     def eval_gpu(self, keys):
         """Evaluate a batch on the GPU (dpf.py:115-131): int32 [len(keys), entry_size] on the CPU.
@@ -315,6 +360,18 @@ class BinnedDPF(DPF):
             keys = torch.stack(list(keys))
         return dpf_cpp.group_eval(keys.contiguous(), torch.as_tensor(bins), self.buffers, self.prf_method)
 
+    def update_rows(self, bins, indices, rows):
+        """Replace rows of live bins: row indices[j] of bin bins[j] := rows[j] (the last occurrence of a
+        (bin, index) pair wins); synchronous.  A bin or index out of range raises, and nothing is applied."""
+        if self.buffers is None:
+            raise Exception("Must call `eval_init` before `update_rows`")
+        idx, rows = _update_args(indices, rows, self.table_effective_entry_size)
+        bins = torch.as_tensor(bins)
+        if bins.dim() != 1 or bins.numel() != idx.numel() or bins.is_floating_point() or bins.dtype == torch.bool:
+            raise Exception("bins must be a 1-D integer tensor with one bin per index")
+        dpf_cpp.group_update_rows(bins.to(torch.int32).cpu().contiguous(), idx.to(torch.int64).cpu().contiguous(),
+                                  rows.to(torch.int32).cpu().contiguous(), self.buffers)
+
     def __repr__(self):
         if self.buffers is None:
             return "BinnedDPF(_uninitialized_, prf_method=%s)" % self.prf_method_string
@@ -324,6 +381,20 @@ class BinnedDPF(DPF):
 
 def _next_pow2(n):
     return 1 << max(1, (n - 1).bit_length())
+
+
+def _update_args(indices, rows, entry_size):
+    """Shape and dtype checks of an update, before anything reaches the extension."""
+    idx = torch.as_tensor(indices)
+    rows = torch.as_tensor(rows)
+    if idx.dim() != 1 or idx.is_floating_point() or idx.is_complex() or idx.dtype == torch.bool:
+        raise Exception("indices must be a 1-D integer tensor")
+    if rows.dim() != 2 or rows.shape[0] != idx.shape[0] or rows.shape[1] != entry_size:
+        raise Exception("rows must be [%d, %d] (one row of entry_size columns per index), got %s"
+                        % (idx.shape[0], entry_size, list(rows.shape)))
+    if rows.is_complex() or rows.dtype == torch.bool:
+        raise Exception("rows must be a real-valued tensor (cast to int32 like eval_init's table)")
+    return idx, rows
 
 
 def _pad_rows_to_pow2(table):

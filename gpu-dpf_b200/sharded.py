@@ -90,6 +90,13 @@ class ShardedDPF(object):
         self._dpf.eval_init(table)
         return self
 
+    def update_rows(self, indices, rows):
+        """table[indices[j]] := rows[j] on every rank (dpf.DPF.update_rows).  Every rank passes the same list,
+        as with eval_init: an entry-range shard applies the rows it owns, a keys-axis replica applies all."""
+        if self._dpf is None:
+            raise Exception("Must call `eval_init` before `update_rows`")
+        self._dpf.update_rows(indices, rows)
+
     # -- fused reduction plumbing ------------------------------------------------
     def _symm_buffer(self, nkeys):
         import torch.distributed._symmetric_memory as symm_mem

@@ -211,6 +211,49 @@ int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bin
                        int32_t *out);
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
 
+/*
+ * Row updates of a live table (no counterpart in the reference, whose only way to change a row is a
+ * new eval_init).  table[indices[j]] := rows[j] for j = 0 .. count-1, with NATURAL indices (the
+ * numbering keys use); rows: int32 [count][entry_size].  Only the touched rows move: nothing else is
+ * uploaded, re-permuted or reallocated, and every buffer and handle of the context stays valid.
+ *   - Duplicates in one call: the LAST occurrence wins, on every path.
+ *   - Ordering: an evaluation enqueued on the context before the update, on any stream, sees only old
+ *     rows; one enqueued after it sees only new rows; none sees a mix.  The update joins the context's
+ *     one-operation-in-flight chain exactly like an evaluation (see "Threading" above).
+ *   - Only the entry_size live columns of a row are written; the padding of device rows stays zero.
+ *   - 0 <= count < 2^31.  count == 0 is a no-op.
+ *   - Scratch: the update has its own device buffer, grown on demand and kept until b200dpf_destroy
+ *     (it never touches the key / result buffers or the b200dpf_host_staging memory an evaluation in
+ *     flight may still read): 16 bytes per row + the temporary storage of a CUB radix sort of `count`
+ *     32-bit keys, plus a copy of the list itself (12 + 4*entry_size bytes per row) on the host paths.
+ *     Memory is O(count), independent of n (no n-sized claim array).
+ * How each kind of context applies the list:
+ *   whole table         every entry.
+ *   shard (r, G)        index i is owned iff (i & (G-1)) == bitrev_g(r); every shard takes the FULL
+ *                       list (as b200dpf_create takes the full table) and ignores rows it does not own;
+ *                       the host path does not copy those to the GPU.
+ *   b200dpf_create_multi  ENTRIES: each device applies its shard's rows; KEYS: every replica applies
+ *                       every row.  All devices' copies and kernels are issued before the first
+ *                       synchronisation.  Host buffers only: b200dpf_update_rows_device returns EINVAL.
+ *   grouped             use b200dpf_group_update_rows; the two other entry points return ESTATE there,
+ *                       and b200dpf_group_update_rows returns ESTATE on any other context.
+ */
+
+/* Host buffers, synchronous.  Every index is validated before anything is copied: EINVAL (an index
+ * outside [0, n), a negative count, a null buffer) means nothing was applied. */
+int b200dpf_update_rows(b200dpf_ctx *ctx, const int64_t *indices, const int32_t *rows, int64_t count);
+
+/* Device buffers on the context's GPU, enqueued on `cuda_stream` (NULL: the default stream) with no
+ * host synchronisation; the buffers must stay valid until the stream reaches the update.  Entries
+ * with an index outside [0, n) are skipped (never written); the others are applied. */
+int b200dpf_update_rows_device(b200dpf_ctx *ctx, const int64_t *indices_dev, const int32_t *rows_dev, int64_t count,
+                               void *cuda_stream);
+
+/* Grouped (batch-PIR) context: row indices[j] of bin bins[j] := rows[j].  Host buffers, synchronous.  A
+ * bin id outside [0, nbins) or an index >= n[bin] is EINVAL, and nothing is applied. */
+int b200dpf_group_update_rows(b200dpf_ctx *ctx, const int32_t *bins, const int64_t *indices, const int32_t *rows,
+                              int64_t count);
+
 /* Replaces: dpf_cpp.eval_free -> eval_free()               dpf_wrapper.cu:86-91. */
 int b200dpf_destroy(b200dpf_ctx *ctx);
 
