@@ -17,10 +17,13 @@
 #include <cstring>
 #include <atomic>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "dpf_host.h"
@@ -56,6 +59,13 @@ int ilog2(int64_t v)
     return b;
 }
 
+uint32_t bitrev_host(uint32_t v, int bits)
+{
+    uint32_t r = 0;
+    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
+    return r;
+}
+
 struct DeviceGuard {
     int prev = -1;
     bool ok = false;
@@ -70,6 +80,40 @@ struct DeviceGuard {
     }
 };
 
+/* A grow-only allocation of device memory (cudaMalloc) or, if Pinned, page-locked host memory
+ * (cudaMallocHost), freed by its destructor. */
+template <class T, bool Pinned>
+struct Buffer {
+    T *ptr = nullptr;
+    size_t cap = 0;   /* bytes */
+    Buffer() = default;
+    Buffer(Buffer &&o) noexcept : ptr(std::exchange(o.ptr, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    ~Buffer() { release(); }
+    void release()
+    {
+        if (ptr && Pinned) cudaFreeHost(ptr);
+        else if (ptr) cudaFree(ptr);
+        ptr = nullptr;
+        cap = 0;
+    }
+    /* at least `bytes`; a smaller buffer is replaced (its contents are lost) and *grown says so */
+    int reserve(size_t bytes, bool *grown = nullptr)
+    {
+        if (grown) *grown = false;
+        if (bytes <= cap) return B200DPF_OK;
+        release();
+        if (Pinned) CUDA_TRY(cudaMallocHost(&ptr, bytes));
+        else CUDA_TRY(cudaMalloc(&ptr, bytes));
+        cap = bytes;
+        if (grown) *grown = true;
+        return B200DPF_OK;
+    }
+};
+template <class T> using DeviceBuffer = Buffer<T, false>;
+template <class T> using PinnedBuffer = Buffer<T, true>;
+
+constexpr size_t kKeyBytes = host::KEY_WORDS * sizeof(int32_t);   /* one key in the wire format */
+
 }  // namespace
 
 struct SmemLayoutCache;   /* per (prf, nv, mode) launch layouts, filled on first use */
@@ -79,18 +123,16 @@ struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behi
     std::vector<int64_t> n;
     std::vector<int> depth;
     std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
-    GroupDesc *d_descs = nullptr;
-    size_t descs_cap = 0;              /* descriptors */
-    GroupDesc *h_descs = nullptr;      /* pinned */
-    size_t h_descs_cap = 0;
+    DeviceBuffer<GroupDesc> d_descs;   /* both hold at least 1,024 descriptors */
+    PinnedBuffer<GroupDesc> h_descs;
     std::vector<int64_t> perm;         /* sorted position -> caller's index, of the last evaluation */
-    uint2 *d_bin_info = nullptr;       /* [nbins] (row_off, depth) for row updates, uploaded on first use */
+    DeviceBuffer<uint2> d_bin_info;    /* [nbins] (row_off, depth) for row updates, uploaded on first use */
 };
 
 struct b200dpf_ctx {
-    MultiState *multi = nullptr;   /* non-null: this context only fans out to multi->sub[] */
-    GroupBins *bins = nullptr;     /* non-null: grouped (batch-PIR) context, use b200dpf_group_eval */
-    SmemLayoutCache *layouts = nullptr;
+    std::unique_ptr<MultiState> multi;   /* non-null: this context only fans out to multi->sub[] */
+    std::unique_ptr<GroupBins> bins;     /* non-null: grouped (batch-PIR) context, use b200dpf_group_eval */
+    std::unique_ptr<SmemLayoutCache> layouts;
     int device = 0;
     int64_t n = 0;
     int depth = 0;
@@ -99,22 +141,15 @@ struct b200dpf_ctx {
     int shard_rank = 0, shard_count = 1, shard_bits = 0;
     int64_t n_local = 0;
     int depth_local = 0;
-    int32_t *d_table = nullptr;
+    DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
-    int32_t *d_keys = nullptr;
-    size_t keys_cap = 0;     /* keys */
-    int32_t *d_out = nullptr;
-    size_t out_cap = 0;      /* int32 elements */
-    uint32_t *d_counters = nullptr;
-    size_t counters_cap = 0;  /* bytes */
-    void *d_frontier = nullptr;
-    size_t frontier_cap = 0;  /* bytes */
-    void *d_leaf_cache = nullptr;
-    size_t leaf_cache_cap = 0;  /* bytes */
-    int32_t *h_keys = nullptr;  /* pinned staging */
-    size_t h_keys_cap = 0;      /* keys */
-    int32_t *h_out = nullptr;   /* pinned staging */
-    size_t h_out_cap = 0;       /* int32 elements */
+    DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
+    DeviceBuffer<int32_t> d_out;
+    DeviceBuffer<uint32_t> d_counters;
+    DeviceBuffer<void> d_frontier;
+    DeviceBuffer<uint32_t> d_leaf_cache;
+    PinnedBuffer<int32_t> h_keys;     /* staging: whole wire-format keys, at least 512 */
+    PinnedBuffer<int32_t> h_out;      /* staging: at least 8,192 int32 */
     int sm_count = 0;
     uint32_t smem_base = 0;
     int last_launches = 0;
@@ -137,12 +172,10 @@ struct b200dpf_ctx {
                                                              +4 % for Salsa20, -2 % for ChaCha20 against broadcast
                                                              loads, other sizes unmeasured -- so off */
     } knobs;
-    unsigned long long *d_timing = nullptr;   /* [timing_blocks][8] */
-    int timing_blocks = 0;
+    DeviceBuffer<unsigned long long> d_timing;   /* [blocks][8] */
     int coop_ok = 0;               /* device supports cooperative launches                                 */
-    uint32_t *d_top_counters = nullptr;   /* top-phase tickets: zero between launches (self re-arming)     */
-    size_t top_counters_cap = 0;          /* bytes                                                          */
-    uint32_t *d_gridbar = nullptr;        /* monotonic arrival counter of the in-kernel grid barrier        */
+    DeviceBuffer<uint32_t> d_top_counters;  /* top-phase tickets: zero between launches (self re-arming)   */
+    DeviceBuffer<uint32_t> d_gridbar;       /* monotonic arrival counter of the in-kernel grid barrier      */
     uint32_t bar_epoch = 0;               /* value d_gridbar holds when no launch is in flight              */
     bool coop_state_dirty = true;         /* top tickets / barrier counter must be cleared before use       */
     /* one evaluation in flight per context: launches on a different stream than the previous
@@ -156,8 +189,8 @@ struct b200dpf_ctx {
     bool timed = false;
     /* row updates (b200dpf_update_rows*): their own scratch, so an update never touches a buffer an
      * evaluation in flight may read; layout at UpdateLayout */
-    void *d_update = nullptr;
-    size_t update_cap = 0;       /* bytes */
+    DeviceBuffer<char> d_update;
+    ~b200dpf_ctx();   /* the members free the buffers; this destroys the stream and events */
 };
 
 namespace {
@@ -186,7 +219,7 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
 int smem_layout(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L)
 {
     const int ni = nv == 4 ? 0 : (nv == 8 ? 1 : 2);
-    if (!c->layouts) c->layouts = new (std::nothrow) SmemLayoutCache();
+    if (!c->layouts) c->layouts.reset(new (std::nothrow) SmemLayoutCache());
     if (c->layouts && c->layouts->valid[prf][ni][mode]) {
         *L = c->layouts->entry[prf][ni][mode];
         return B200DPF_OK;
@@ -259,7 +292,7 @@ void fill_common(const b200dpf_ctx *c, const SmemLayout &L, int s, int64_t nkeys
     p->nkeys = (int)nkeys;
     p->kpw_log2 = kpw_log2;
     p->key_groups = (int)((nkeys + (1 << kpw_log2) - 1) >> kpw_log2);
-    p->table = reinterpret_cast<const uint4 *>(c->d_table);
+    p->table = reinterpret_cast<const uint4 *>(c->d_table.ptr);
     p->row_stride_v = (uint32_t)c->entry_pad / 4u;
     p->out_stride = (uint32_t)c->entry_size;
     p->n = (uint64_t)c->n;
@@ -279,15 +312,39 @@ int env_int(const char *name, int dflt)
     return (v && *v) ? std::atoi(v) : dflt;
 }
 
-int ensure_buffer(void **ptr, size_t *cap, size_t bytes)
+/* One operation in flight per context: its scratch buffers are shared.  Work about to be enqueued on
+ * `stream` first waits for the context's last operation when that ran on another stream. */
+int wait_last(b200dpf_ctx *c, cudaStream_t stream)
 {
-    if (bytes <= *cap) return B200DPF_OK;
-    if (*ptr) cudaFree(*ptr);
-    *ptr = nullptr;
-    *cap = 0;
-    CUDA_TRY(cudaMalloc(ptr, bytes));
-    *cap = bytes;
+    if (c->has_last && c->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, c->ev_done, 0));
     return B200DPF_OK;
+}
+
+/* The work enqueued on `stream` so far becomes the context's last operation. */
+int mark_last(b200dpf_ctx *c, cudaStream_t stream)
+{
+    CUDA_TRY(cudaEventRecord(c->ev_done, stream));
+    c->last_stream = stream;
+    c->has_last = true;
+    return B200DPF_OK;
+}
+
+/* Pinned staging never shrinks below 512 keys or 8,192 result elements. */
+int reserve_host_keys(b200dpf_ctx *c, size_t key_bytes)
+{
+    return c->h_keys.reserve(std::max<size_t>((key_bytes + kKeyBytes - 1) / kKeyBytes, 512) * kKeyBytes);
+}
+
+int reserve_host_out(b200dpf_ctx *c, size_t out_elems)
+{
+    return c->h_out.reserve(std::max<size_t>(out_elems, 8192) * sizeof(int32_t));
+}
+
+/* device key / result buffers of the host-buffer entry points */
+int reserve_device_io(b200dpf_ctx *c, size_t key_bytes, size_t out_elems)
+{
+    const int rc = c->d_keys.reserve((key_bytes + kKeyBytes - 1) / kKeyBytes * kKeyBytes);
+    return rc ? rc : c->d_out.reserve(out_elems * sizeof(int32_t));
 }
 
 /* Where the kernel finds the live parts of a key. */
@@ -297,6 +354,30 @@ struct KeyLayout {
 };
 KeyLayout reference_layout() { return KeyLayout{131u, 129u, 0}; }                       /* dpf_wrapper.cu:26-46 */
 KeyLayout compact_layout(int depth) { return KeyLayout{2u + 4u * (uint32_t)depth, 1u, 1}; }   /* b200dpf_key_pack */
+
+/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks) */
+inline void pack_compact(const int32_t *key, uint8_t *dst, int depth)
+{
+    const uint8_t *k = reinterpret_cast<const uint8_t *>(key);
+    std::memset(dst, 0, 16);
+    std::memcpy(dst, "DPF2", 4);
+    dst[4] = (uint8_t)depth;
+    std::memcpy(dst + 16, k + 16 * host::SLOT_ROOT, 16);
+    uint8_t *o = dst + 32;
+    const uint8_t *c1 = k + 16 * host::SLOT_CW1, *c2 = k + 16 * host::SLOT_CW2;
+    for (int L = 0; L < depth; L++, o += 64) {
+        std::memcpy(o, c1 + 32 * L, 32);
+        std::memcpy(o + 32, c2 + 32 * L, 32);
+    }
+}
+
+/* key number `b` of a batch (null: none) must have been generated for the table's n */
+inline int check_key_n(const int32_t *key, int64_t b, int64_t n)
+{
+    const int64_t kn = key ? host::key_n(key) : -1;
+    if (kn == n) return B200DPF_OK;
+    return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b, (long long)kn, (long long)n);
+}
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
 {
@@ -394,32 +475,30 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
 
     const bool one_launch = K.one_launch != 0 && c->coop_ok != 0;
     const size_t n_main_counters = (size_t)passes * (size_t)key_groups;
-    rc = ensure_buffer(reinterpret_cast<void **>(&c->d_counters), &c->counters_cap, n_main_counters * sizeof(uint32_t));
+    rc = c->d_counters.reserve(n_main_counters * sizeof(uint32_t));
     if (rc) return rc;
     {
-        const size_t before = c->top_counters_cap;
-        rc = ensure_buffer(reinterpret_cast<void **>(&c->d_top_counters), &c->top_counters_cap,
-                           std::max<size_t>((size_t)key_groups, 64) * sizeof(uint32_t));
+        bool grown = false;
+        rc = c->d_top_counters.reserve(std::max<size_t>((size_t)key_groups, 64) * sizeof(uint32_t), &grown);
         if (rc) return rc;
-        if (c->top_counters_cap != before) c->coop_state_dirty = true;
+        if (grown) c->coop_state_dirty = true;
     }
     if (f_rel > 0) {
-        rc = ensure_buffer(reinterpret_cast<void **>(&c->d_frontier), &c->frontier_cap,
-                           ((size_t)key_groups * (16 << kpw_log2)) << f_rel);
+        rc = c->d_frontier.reserve(((size_t)key_groups * (16 << kpw_log2)) << f_rel);
         if (rc) return rc;
     }
 
-    /* one evaluation in flight per context (shared scratch): order after the previous one */
-    if (c->has_last && c->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, c->ev_done, 0));
+    rc = wait_last(c, stream);
+    if (rc) return rc;
 
     if (!one_launch || c->coop_state_dirty) {
-        CUDA_TRY(cudaMemsetAsync(c->d_top_counters, 0, c->top_counters_cap, stream));
-        CUDA_TRY(cudaMemsetAsync(c->d_gridbar, 0, sizeof(uint32_t), stream));
+        CUDA_TRY(cudaMemsetAsync(c->d_top_counters.ptr, 0, c->d_top_counters.cap, stream));
+        CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), stream));
         c->bar_epoch = 0;
         c->coop_state_dirty = false;
     }
     if (!one_launch) {
-        CUDA_TRY(cudaMemsetAsync(c->d_counters, 0, n_main_counters * sizeof(uint32_t), stream));
+        CUDA_TRY(cudaMemsetAsync(c->d_counters.ptr, 0, n_main_counters * sizeof(uint32_t), stream));
         if (mode_main == MODE_FUSED && clear_out)
             CUDA_TRY(cudaMemsetAsync(out_dev, 0, (size_t)nkeys * c->entry_size * sizeof(int32_t), stream));
         c->coop_state_dirty = true;     /* the stand-alone frontier kernel leaves its tickets used */
@@ -473,14 +552,14 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         top.walk_first_level = c->depth - 1;
         top.walk_steps = c->shard_bits + f_rel - s_top;
         top.level_base = c->depth_local - f_rel;
-        top.counters = c->d_top_counters;
+        top.counters = c->d_top_counters.ptr;
         if (!one_launch) {
             fill_common(c, LF, s_top, nkeys, kpw_log2, &p, &smem);
             p.keys = reinterpret_cast<const uint4 *>(keys_dev);
             p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
             p.main = top;
             p.nfront = (uint32_t)1 << f_rel;
-            p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier);
+            p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier.ptr);
             CUDA_TRY(launch_eval(prf, 4, MODE_FRONTIER, p, LF.grid, smem, stream));
             c->last_launches++;
         }
@@ -499,7 +578,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     p.main.nsub = (uint32_t)1 << rel;
     p.main.sub_first = (uint32_t)c->shard_rank << rel;
     if (f_rel > 0) {
-        p.main.frontier_in = reinterpret_cast<const uint4 *>(c->d_frontier);
+        p.main.frontier_in = reinterpret_cast<const uint4 *>(c->d_frontier.ptr);
         p.nfront = (uint32_t)1 << f_rel;
         p.main.front_shift = rel - f_rel;
         p.main.walk_first_level = c->depth_local - f_rel - 1;
@@ -508,18 +587,18 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         p.main.walk_first_level = c->depth - 1;
         p.main.walk_steps = c->depth - s;
     }
-    p.main.counters = c->d_counters;
+    p.main.counters = c->d_counters.ptr;
     if (one_launch) {
         p.fuse_top = 1;
         p.top = top;                      /* nsub == 0: no frontier, the top phase only clears */
-        p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier);
+        p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier.ptr);
         if (mode_main == MODE_FUSED && clear_out) {
             p.zero_a = reinterpret_cast<uint32_t *>(out_dev);
             p.zero_a_words = (uint64_t)nkeys * (uint64_t)c->entry_size;
         }
-        p.zero_b = c->d_counters;
+        p.zero_b = c->d_counters.ptr;
         p.zero_b_words = n_main_counters;
-        p.rearm = c->d_top_counters;
+        p.rearm = c->d_top_counters.ptr;
         p.rearm_words = (uint32_t)key_groups;
         {
             const uint64_t items = (uint64_t)key_groups * (uint64_t)(top.nsub >> spw_log2);
@@ -527,22 +606,12 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
                                               : 0x7fffffffu;
         }
         if (K.timing) {
-            if (c->timing_blocks < L.grid) {
-                if (c->d_timing) cudaFree(c->d_timing);
-    if (c->bins) {
-        if (c->bins->d_descs) cudaFree(c->bins->d_descs);
-        if (c->bins->h_descs) cudaFreeHost(c->bins->h_descs);
-        delete c->bins;
-    }
-                c->d_timing = nullptr;
-                c->timing_blocks = 0;
-                CUDA_TRY(cudaMalloc(&c->d_timing, (size_t)L.grid * 8 * sizeof(unsigned long long)));
-                c->timing_blocks = L.grid;
-            }
-            CUDA_TRY(cudaMemsetAsync(c->d_timing, 0, (size_t)c->timing_blocks * 8 * sizeof(unsigned long long), stream));
-            p.timing = c->d_timing;
+            rc = c->d_timing.reserve((size_t)L.grid * 8 * sizeof(unsigned long long));
+            if (rc) return rc;
+            CUDA_TRY(cudaMemsetAsync(c->d_timing.ptr, 0, c->d_timing.cap, stream));
+            p.timing = c->d_timing.ptr;
         }
-        p.grid_bar = c->d_gridbar;
+        p.grid_bar = c->d_gridbar.ptr;
         c->bar_epoch += (uint32_t)L.grid;
         p.grid_bar_target = c->bar_epoch;
     }
@@ -571,9 +640,9 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     p.out = reinterpret_cast<uint32_t *>(out_dev);
     if (want_cache) {
         const size_t cache_bytes = (size_t)key_groups * 32u * (size_t)c->n_local * sizeof(uint32_t);
-        rc = ensure_buffer(&c->d_leaf_cache, &c->leaf_cache_cap, cache_bytes);
+        rc = c->d_leaf_cache.reserve(cache_bytes);
         if (rc) return rc;
-        p.leaf_cache = reinterpret_cast<uint32_t *>(c->d_leaf_cache);
+        p.leaf_cache = c->d_leaf_cache.ptr;
         p.n_local = (uint64_t)c->n_local;
         p.col_off_v = 0;
         p.col_off = 0;
@@ -621,7 +690,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         p.col_off = (uint32_t)(pass * 4 * nv);
         p.ncols = (uint32_t)std::max(0, std::min(4 * nv, c->entry_size - pass * 4 * nv));
         if (p.ncols == 0) break;
-        p.main.counters = c->d_counters + (size_t)pass * key_groups;
+        p.main.counters = c->d_counters.ptr + (size_t)pass * key_groups;
         rc = launch_main(nv, mode_kernel);
         if (rc) return rc;
     }
@@ -663,12 +732,7 @@ int run_pipeline(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int6
         }
     }
     c->last_launches = launches;
-    if (rc == B200DPF_OK) {
-        CUDA_TRY(cudaEventRecord(c->ev_done, stream));
-        c->last_stream = stream;
-        c->has_last = true;
-    }
-    return rc;
+    return rc ? rc : mark_last(c, stream);
 }
 
 int run_eval(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, int prf, void *out_dev, cudaStream_t stream)
@@ -684,27 +748,114 @@ bool is_pinned_host(const void *ptr)
     return yes;
 }
 
-int ensure_host_keys(b200dpf_ctx *c, int64_t nkeys)
+/* Copy `elems` results from the context's d_out into the caller's host buffer `out` and wait for them;
+ * pageable memory is staged through the pinned h_out so the copy is a real asynchronous DMA. */
+int download_out(b200dpf_ctx *c, int32_t *out, bool out_pinned, size_t elems)
 {
-    if ((size_t)nkeys <= c->h_keys_cap) return B200DPF_OK;
-    if (c->h_keys) cudaFreeHost(c->h_keys);
-    c->h_keys = nullptr;
-    c->h_keys_cap = 0;
-    const size_t cap = std::max<size_t>((size_t)nkeys, 512);
-    CUDA_TRY(cudaMallocHost(&c->h_keys, cap * host::KEY_WORDS * sizeof(int32_t)));
-    c->h_keys_cap = cap;
+    int32_t *dst = out;
+    if (!out_pinned) {
+        const int rc = reserve_host_out(c, elems);
+        if (rc) return rc;
+        dst = c->h_out.ptr;
+    }
+    CUDA_TRY(cudaMemcpyAsync(dst, c->d_out.ptr, elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (dst != out) std::memcpy(out, dst, elems * sizeof(int32_t));
     return B200DPF_OK;
+}
+
+/* The evaluation of keys already enqueued for upload into d_keys, timed, and its results into `out`. */
+int eval_tail(b200dpf_ctx *c, const KeyLayout &kl, int64_t nkeys, int prf, int32_t *out)
+{
+    CUDA_TRY(cudaEventRecord(c->ev_t0, c->stream));
+    const int rc = run_pipeline(c, c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, c->stream);
+    if (rc) return rc;
+    CUDA_TRY(cudaEventRecord(c->ev_t1, c->stream));
+    c->timed = true;
+    return download_out(c, out, is_pinned_host(out), (size_t)nkeys * c->entry_size);
 }
 
 int check_eval_args(const b200dpf_ctx *c, const void *keys, int64_t nkeys, int prf, const void *out)
 {
     if (!c) return fail(B200DPF_EINVAL, "null context");
-    if (!c->d_table && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
+    if (!c->d_table.ptr && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
     if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_eval");
     if (!keys || !out) return fail(B200DPF_EINVAL, "null buffer");
     if (nkeys < 1 || nkeys > (int64_t)1 << 24) return fail(B200DPF_EINVAL, "nkeys=%lld out of range", (long long)nkeys);
     if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
     return B200DPF_OK;
+}
+
+/* Check that `device` exists and make it current for as long as `guard` lives; `cpu_hint` completes the
+ * message on a machine without CUDA devices. */
+int open_device(int device, const char *cpu_hint, std::optional<DeviceGuard> *guard)
+{
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return fail(B200DPF_ECUDA, "no CUDA device available (%s)", cpu_hint);
+    if (device < 0 || device >= ndev) return fail(B200DPF_EINVAL, "device %d out of range (have %d)", device, ndev);
+    guard->emplace(device);
+    if (!(*guard)->ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", device);
+    return B200DPF_OK;
+}
+
+/* The set-up both create functions share: a context on `device`, current while `guard` lives, with the
+ * device's properties, its stream and events, the grid-barrier word, the shared-memory base and the AES
+ * tables.  With `read_env` the tuning knobs start from the B200DPF_* environment variables. */
+int ctx_open(int device, bool read_env, std::optional<DeviceGuard> *guard, std::unique_ptr<b200dpf_ctx> *out)
+{
+    int rc = open_device(device, "this engine has no CPU fallback", guard);
+    if (rc) return rc;
+    std::unique_ptr<b200dpf_ctx> c(new (std::nothrow) b200dpf_ctx());
+    if (!c) return fail(B200DPF_ENOMEM, "out of host memory");
+    c->device = device;
+    CUDA_TRY(cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device));
+    CUDA_TRY(cudaDeviceGetAttribute(&c->coop_ok, cudaDevAttrCooperativeLaunch, device));
+    CUDA_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreate(&c->ev_t0));
+    CUDA_TRY(cudaEventCreate(&c->ev_t1));
+    rc = c->d_gridbar.reserve(sizeof(uint32_t));
+    if (rc) return rc;
+    if (read_env) {
+        /* the environment is consulted here and nowhere else (b200dpf_ctx_set_option changes a
+         * live context) */
+        b200dpf_ctx::Knobs &K = c->knobs;
+        K.leaf_cache = env_int("B200DPF_LEAF_CACHE", K.leaf_cache);
+        K.leaf_cache_mb = env_int("B200DPF_LEAF_CACHE_MB", K.leaf_cache_mb);
+        K.lane_split = env_int("B200DPF_LANE_SPLIT", K.lane_split);
+        K.frontier = env_int("B200DPF_FRONTIER", K.frontier);
+        K.frontier_mb = env_int("B200DPF_FRONTIER_MB", K.frontier_mb);
+        K.subtree_log2 = env_int("B200DPF_S", K.subtree_log2);
+        K.mac_tma = env_int("B200DPF_MAC_TMA", K.mac_tma);
+        K.one_launch = env_int("B200DPF_ONE_LAUNCH", K.one_launch);
+        K.balance_top = env_int("B200DPF_BALANCE_TOP", K.balance_top);
+        K.timing = env_int("B200DPF_TIMING", K.timing);
+        K.top_log2 = env_int("B200DPF_TOP_LOG2", K.top_log2);
+        K.tma_rows = env_int("B200DPF_TMA_ROWS", K.tma_rows);
+    }
+    CUDA_TRY(probe_dynamic_smem_base(&c->smem_base, c->stream));
+    CUDA_TRY(upload_aes_table(host::aes_te0()));
+    *out = std::move(c);
+    return B200DPF_OK;
+}
+
+/* Run gen_one(i) for every i < count on `nthreads` threads (0: one per hardware thread); false when any
+ * call failed. */
+template <class GenOne>
+bool gen_parallel(int64_t count, int nthreads, GenOne gen_one)
+{
+    if (nthreads <= 0) nthreads = (int)std::max(1u, std::thread::hardware_concurrency());
+    nthreads = (int)std::min<int64_t>(nthreads, std::max<int64_t>(count, 1));
+    std::vector<int> rcs((size_t)nthreads, 0);
+    auto work = [&](int t) {
+        for (int64_t i = t; i < count; i += nthreads)
+            if (gen_one(i)) rcs[(size_t)t] = -1;
+    };
+    std::vector<std::thread> pool;
+    for (int t = 1; t < nthreads; t++) pool.emplace_back(work, t);
+    work(0);
+    for (auto &th : pool) th.join();
+    return std::find(rcs.begin(), rcs.end(), -1) == rcs.end();
 }
 
 }  // namespace
@@ -715,7 +866,6 @@ static int multi_last_launches(const b200dpf_ctx *root);
 static int multi_set_option(b200dpf_ctx *root, const char *name, int value);
 static int multi_eval_host(b200dpf_ctx *root, const void *keys, size_t key_stride_bytes, const KeyLayout &kl, int64_t nkeys,
                            int prf, int32_t *out);
-static void multi_destroy(b200dpf_ctx *root);
 
 extern "C" {
 
@@ -750,20 +900,10 @@ int b200dpf_gen_batch(const int64_t *alphas, const uint32_t *seeds32, int64_t co
                       int nthreads, int32_t *keys_a, int32_t *keys_b)
 {
     if (!alphas || !seeds32 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch argument");
-    if (nthreads <= 0) nthreads = (int)std::max(1u, std::thread::hardware_concurrency());
-    nthreads = (int)std::min<int64_t>(nthreads, std::max<int64_t>(count, 1));
-    std::vector<int> rcs((size_t)nthreads, 0);
-    auto work = [&](int t) {
-        for (int64_t i = t; i < count; i += nthreads)
-            if (host::gen(alphas[i], n, seeds32[i], prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS))
-                rcs[(size_t)t] = -1;
-    };
-    std::vector<std::thread> pool;
-    for (int t = 1; t < nthreads; t++) pool.emplace_back(work, t);
-    work(0);
-    for (auto &th : pool) th.join();
-    for (int r : rcs)
-        if (r) return fail(B200DPF_EINVAL, "gen_batch: invalid alpha/n/prf in batch");
+    if (!gen_parallel(count, nthreads, [&](int64_t i) {
+            return host::gen(alphas[i], n, seeds32[i], prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
+        }))
+        return fail(B200DPF_EINVAL, "gen_batch: invalid alpha/n/prf in batch");
     return B200DPF_OK;
 }
 
@@ -771,20 +911,10 @@ int b200dpf_gen_batch_secure(const int64_t *alphas, const uint8_t *seeds44, int6
                              int nthreads, int32_t *keys_a, int32_t *keys_b)
 {
     if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_secure argument");
-    if (nthreads <= 0) nthreads = (int)std::max(1u, std::thread::hardware_concurrency());
-    nthreads = (int)std::min<int64_t>(nthreads, std::max<int64_t>(count, 1));
-    std::vector<int> rcs((size_t)nthreads, 0);
-    auto work = [&](int t) {
-        for (int64_t i = t; i < count; i += nthreads)
-            if (host::gen_secure(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS))
-                rcs[(size_t)t] = -1;
-    };
-    std::vector<std::thread> pool;
-    for (int t = 1; t < nthreads; t++) pool.emplace_back(work, t);
-    work(0);
-    for (auto &th : pool) th.join();
-    for (int r : rcs)
-        if (r) return fail(B200DPF_EINVAL, "gen_batch_secure: invalid alpha/n/prf in batch");
+    if (!gen_parallel(count, nthreads, [&](int64_t i) {
+            return host::gen_secure(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
+        }))
+        return fail(B200DPF_EINVAL, "gen_batch_secure: invalid alpha/n/prf in batch");
     return B200DPF_OK;
 }
 
@@ -797,33 +927,27 @@ int b200dpf_gen_batch_gpu(const int64_t *alphas, const uint8_t *seeds44, int64_t
     for (int64_t i = 0; i < count; i++)
         if (alphas[i] < 0 || alphas[i] >= n) return fail(B200DPF_EINVAL, "gen_batch_gpu: alpha[%lld]=%lld out of range", (long long)i, (long long)alphas[i]);
     if (count == 0) return B200DPF_OK;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return fail(B200DPF_ECUDA, "no CUDA device available (use b200dpf_gen_batch_secure on the CPU)");
-    if (device < 0 || device >= ndev) return fail(B200DPF_EINVAL, "device %d out of range (have %d)", device, ndev);
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", device);
-    const size_t key_bytes = (size_t)count * host::KEY_WORDS * sizeof(int32_t);
-    int64_t *d_alphas = nullptr;
-    uint8_t *d_seeds = nullptr;
-    uint32_t *d_te0 = nullptr;
-    uint4 *d_a = nullptr, *d_b = nullptr;
-    cudaError_t e = cudaMalloc(&d_alphas, (size_t)count * sizeof(int64_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_seeds, (size_t)count * 44);
-    if (e == cudaSuccess) e = cudaMalloc(&d_te0, 256 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_a, key_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_b, key_bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(d_alphas, alphas, (size_t)count * sizeof(int64_t), cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(d_seeds, seeds44, (size_t)count * 44, cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(d_te0, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = launch_keygen(prf, d_alphas, d_seeds, count, ilog2(n), (uint64_t)n, d_te0, d_a, d_b, nullptr);
-    if (e == cudaSuccess) e = cudaMemcpy(keys_a, d_a, key_bytes, cudaMemcpyDefault);      /* host or device destination */
-    if (e == cudaSuccess) e = cudaMemcpy(keys_b, d_b, key_bytes, cudaMemcpyDefault);
-    cudaFree(d_alphas);
-    cudaFree(d_seeds);
-    cudaFree(d_te0);
-    cudaFree(d_a);
-    cudaFree(d_b);
+    std::optional<DeviceGuard> guard;
+    int rc = open_device(device, "use b200dpf_gen_batch_secure on the CPU", &guard);
+    if (rc) return rc;
+    const size_t key_bytes = (size_t)count * kKeyBytes;
+    DeviceBuffer<int64_t> d_alphas;
+    DeviceBuffer<uint8_t> d_seeds;
+    DeviceBuffer<uint32_t> d_te0;
+    DeviceBuffer<uint4> d_a, d_b;
+    rc = d_alphas.reserve((size_t)count * sizeof(int64_t));
+    if (!rc) rc = d_seeds.reserve((size_t)count * 44);
+    if (!rc) rc = d_te0.reserve(256 * sizeof(uint32_t));
+    if (!rc) rc = d_a.reserve(key_bytes);
+    if (!rc) rc = d_b.reserve(key_bytes);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(d_alphas.ptr, alphas, (size_t)count * sizeof(int64_t), cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(d_seeds.ptr, seeds44, (size_t)count * 44, cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess)
+        e = launch_keygen(prf, d_alphas.ptr, d_seeds.ptr, count, ilog2(n), (uint64_t)n, d_te0.ptr, d_a.ptr, d_b.ptr, nullptr);
+    if (e == cudaSuccess) e = cudaMemcpy(keys_a, d_a.ptr, key_bytes, cudaMemcpyDefault);      /* host or device destination */
+    if (e == cudaSuccess) e = cudaMemcpy(keys_b, d_b.ptr, key_bytes, cudaMemcpyDefault);
     if (e != cudaSuccess) return fail(B200DPF_ECUDA, "gen_batch_gpu: %s", cudaGetErrorString(e));
     return B200DPF_OK;
 }
@@ -844,16 +968,7 @@ int b200dpf_key_pack(const int32_t *key, uint8_t *out, size_t out_cap, size_t *w
     if (depth < 1 || host::key_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack: malformed key");
     const size_t need = b200dpf_key_packed_size(depth);
     if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack: need %zu bytes, have %zu", need, out_cap);
-    const uint8_t *k = reinterpret_cast<const uint8_t *>(key);
-    std::memset(out, 0, 16);
-    std::memcpy(out, "DPF2", 4);
-    out[4] = (uint8_t)depth;
-    std::memcpy(out + 16, k + 16 * host::SLOT_ROOT, 16);
-    for (int L = 0; L < depth; L++) {
-        uint8_t *o = out + 32 + 64 * L;
-        std::memcpy(o, k + 16 * (host::SLOT_CW1 + 2 * L), 32);
-        std::memcpy(o + 32, k + 16 * (host::SLOT_CW2 + 2 * L), 32);
-    }
+    pack_compact(key, out, depth);
     if (written) *written = need;
     return B200DPF_OK;
 }
@@ -897,16 +1012,10 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
         shard_rank < 0 || shard_rank >= shard_count)
         return fail(B200DPF_EINVAL, "bad shard %d of %d for n=%lld", shard_rank, shard_count, (long long)n);
 
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return fail(B200DPF_ECUDA, "no CUDA device available (this engine has no CPU fallback)");
-    if (device < 0 || device >= ndev) return fail(B200DPF_EINVAL, "device %d out of range (have %d)", device, ndev);
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", device);
-
-    b200dpf_ctx *c = new (std::nothrow) b200dpf_ctx();
-    if (!c) return fail(B200DPF_ENOMEM, "out of host memory");
-    c->device = device;
+    std::optional<DeviceGuard> guard;
+    std::unique_ptr<b200dpf_ctx> c;
+    int rc = ctx_open(device, true, &guard, &c);
+    if (rc) return rc;
     c->n = n;
     c->depth = ilog2(n);
     c->entry_size = entry_size;
@@ -917,40 +1026,6 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     c->shard_bits = ilog2(shard_count);
     c->n_local = n / shard_count;
     c->depth_local = c->depth - c->shard_bits;
-
-#define CTX_TRY(expr)                                                                          \
-    do {                                                                                       \
-        cudaError_t e__ = (expr);                                                              \
-        if (e__ != cudaSuccess) {                                                              \
-            fail(B200DPF_ECUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            b200dpf_destroy(c);                                                                \
-            return B200DPF_ECUDA;                                                              \
-        }                                                                                      \
-    } while (0)
-
-    CTX_TRY(cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device));
-    CTX_TRY(cudaDeviceGetAttribute(&c->coop_ok, cudaDevAttrCooperativeLaunch, device));
-    CTX_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CTX_TRY(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
-    CTX_TRY(cudaEventCreate(&c->ev_t0));
-    CTX_TRY(cudaEventCreate(&c->ev_t1));
-    CTX_TRY(cudaMalloc(&c->d_gridbar, sizeof(uint32_t)));
-    /* the environment is consulted here and nowhere else (b200dpf_ctx_set_option changes a
-     * live context) */
-    c->knobs.leaf_cache = env_int("B200DPF_LEAF_CACHE", c->knobs.leaf_cache);
-    c->knobs.leaf_cache_mb = env_int("B200DPF_LEAF_CACHE_MB", c->knobs.leaf_cache_mb);
-    c->knobs.lane_split = env_int("B200DPF_LANE_SPLIT", c->knobs.lane_split);
-    c->knobs.frontier = env_int("B200DPF_FRONTIER", c->knobs.frontier);
-    c->knobs.frontier_mb = env_int("B200DPF_FRONTIER_MB", c->knobs.frontier_mb);
-    c->knobs.subtree_log2 = env_int("B200DPF_S", c->knobs.subtree_log2);
-    c->knobs.mac_tma = env_int("B200DPF_MAC_TMA", c->knobs.mac_tma);
-    c->knobs.one_launch = env_int("B200DPF_ONE_LAUNCH", c->knobs.one_launch);
-    c->knobs.balance_top = env_int("B200DPF_BALANCE_TOP", c->knobs.balance_top);
-    c->knobs.timing = env_int("B200DPF_TIMING", c->knobs.timing);
-    c->knobs.top_log2 = env_int("B200DPF_TOP_LOG2", c->knobs.top_log2);
-    c->knobs.tma_rows = env_int("B200DPF_TMA_ROWS", c->knobs.tma_rows);
-    CTX_TRY(probe_dynamic_smem_base(&c->smem_base, c->stream));
-    CTX_TRY(upload_aes_table(host::aes_te0()));
 
     /* Table: gather this shard's rows (natural indices j*G + bitrev_g(rank)),
      * then permute on the device into breadth-first leaf order, padded to
@@ -965,141 +1040,71 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
             if (attr.device != device) cudaSetDevice(attr.device);
             const cudaError_t es = cudaDeviceSynchronize();
             if (attr.device != device) cudaSetDevice(device);
-            CTX_TRY(es);
+            CUDA_TRY(es);
         }
         cudaGetLastError();
     }
     const size_t row_bytes = (size_t)entry_size * sizeof(int32_t);
     const size_t stage_bytes = (size_t)c->n_local * row_bytes;
     const size_t table_bytes = (size_t)c->n_local * (size_t)c->entry_pad * sizeof(int32_t);
-    int32_t *d_stage = nullptr;
-    CTX_TRY(cudaMalloc(&d_stage, stage_bytes));
+    DeviceBuffer<int32_t> d_stage;
+    rc = d_stage.reserve(stage_bytes);
+    if (rc) return rc;
     cudaError_t e = cudaSuccess;
     if (shard_count == 1) {
-        e = cudaMemcpyAsync(d_stage, table, stage_bytes, cudaMemcpyDefault, c->stream);
+        e = cudaMemcpyAsync(d_stage.ptr, table, stage_bytes, cudaMemcpyDefault, c->stream);
     } else {
-        uint32_t rr = 0;
-        for (int i = 0; i < c->shard_bits; i++) rr |= (((uint32_t)shard_rank >> i) & 1u) << (c->shard_bits - 1 - i);
-        const int32_t *src = table + (size_t)rr * entry_size;
+        const int32_t *src = table + (size_t)bitrev_host((uint32_t)shard_rank, c->shard_bits) * entry_size;
         cudaPointerAttributes attr;
         const bool on_device = cudaPointerGetAttributes(&attr, table) == cudaSuccess &&
                                (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
         cudaGetLastError();
         if (on_device) {
-            e = cudaMemcpy2DAsync(d_stage, row_bytes, src, row_bytes * shard_count, row_bytes, (size_t)c->n_local,
+            e = cudaMemcpy2DAsync(d_stage.ptr, row_bytes, src, row_bytes * shard_count, row_bytes, (size_t)c->n_local,
                                   cudaMemcpyDefault, c->stream);
         } else {
             std::vector<int32_t> gathered((size_t)c->n_local * entry_size);
             for (int64_t j = 0; j < c->n_local; j++)
                 std::memcpy(gathered.data() + (size_t)j * entry_size, src + (size_t)j * shard_count * entry_size, row_bytes);
-            e = cudaMemcpyAsync(d_stage, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
+            e = cudaMemcpyAsync(d_stage.ptr, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         }
     }
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_table, table_bytes);
-    if (e == cudaSuccess) e = cudaMemsetAsync(c->d_table, 0, table_bytes, c->stream);
-    if (e == cudaSuccess)
-        e = launch_permute_table(d_stage, c->d_table, (uint64_t)c->n_local, c->depth_local, entry_size, c->entry_pad,
-                                 c->sm_count, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d_stage);
-    CTX_TRY(e);
+    CUDA_TRY(e);
+    rc = c->d_table.reserve(table_bytes);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
+    CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size, c->entry_pad,
+                                  c->sm_count, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    d_stage.release();
 
     /* Like the reference's eval_init (dpf_wrapper.cu:120-129), set up everything a default batch
      * (512 keys) needs now, so the first evaluation pays neither allocations nor lazy module
      * loading: device key/result/ticket buffers, pinned staging, launch layouts of every PRF. */
-    {
-        const int64_t b0 = B200DPF_DEFAULT_BATCH_SIZE;
-        CTX_TRY(cudaMalloc(&c->d_keys, (size_t)b0 * host::KEY_WORDS * sizeof(int32_t)));
-        c->keys_cap = (size_t)b0;
-        CTX_TRY(cudaMalloc(&c->d_out, (size_t)b0 * entry_size * sizeof(int32_t)));
-        c->out_cap = (size_t)b0 * entry_size;
-        if (ensure_host_keys(c, b0) != B200DPF_OK) { b200dpf_destroy(c); return B200DPF_ECUDA; }
-        CTX_TRY(cudaMallocHost(&c->h_out, std::max<size_t>((size_t)b0 * entry_size, 8192) * sizeof(int32_t)));
-        c->h_out_cap = std::max<size_t>((size_t)b0 * entry_size, 8192);
-        const int nv0 = c->entry_pad <= 16 ? 4 : (c->entry_pad <= 32 ? 8 : 4);
-        SmemLayout tmp;
-        for (int prf = 0; prf < 4; prf++) {
-            smem_layout(c, prf, nv0, MODE_FUSED, &tmp);
-            smem_layout(c, prf, 4, MODE_FRONTIER, &tmp);
-        }
+    const size_t b0 = B200DPF_DEFAULT_BATCH_SIZE;
+    rc = reserve_device_io(c.get(), b0 * kKeyBytes, b0 * entry_size);
+    if (!rc) rc = reserve_host_keys(c.get(), b0 * kKeyBytes);
+    if (!rc) rc = reserve_host_out(c.get(), b0 * entry_size);
+    if (rc) return rc;
+    const int nv0 = c->entry_pad <= 16 ? 4 : (c->entry_pad <= 32 ? 8 : 4);
+    SmemLayout tmp;
+    for (int prf = 0; prf < 4; prf++) {
+        smem_layout(c.get(), prf, nv0, MODE_FUSED, &tmp);
+        smem_layout(c.get(), prf, 4, MODE_FRONTIER, &tmp);
     }
-#undef CTX_TRY
-    *out = c;
+    *out = c.release();
     return B200DPF_OK;
 }
 
 int b200dpf_destroy(b200dpf_ctx *c)
 {
     if (!c) return B200DPF_OK;
-    if (c->multi) {
-        multi_destroy(c);
-        delete c;
-        return B200DPF_OK;
-    }
     DeviceGuard guard(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->d_table) cudaFree(c->d_table);
-    if (c->d_keys) cudaFree(c->d_keys);
-    if (c->d_out) cudaFree(c->d_out);
-    if (c->d_counters) cudaFree(c->d_counters);
-    if (c->d_top_counters) cudaFree(c->d_top_counters);
-    if (c->d_gridbar) cudaFree(c->d_gridbar);
-    if (c->d_timing) cudaFree(c->d_timing);
-    if (c->d_update) cudaFree(c->d_update);
-    if (c->bins) {
-        if (c->bins->d_descs) cudaFree(c->bins->d_descs);
-        if (c->bins->h_descs) cudaFreeHost(c->bins->h_descs);
-        if (c->bins->d_bin_info) cudaFree(c->bins->d_bin_info);
-        delete c->bins;
-    }
-    if (c->ev_done) cudaEventDestroy(c->ev_done);
-    if (c->ev_t0) cudaEventDestroy(c->ev_t0);
-    if (c->ev_t1) cudaEventDestroy(c->ev_t1);
-    if (c->d_frontier) cudaFree(c->d_frontier);
-    if (c->d_leaf_cache) cudaFree(c->d_leaf_cache);
-    if (c->h_keys) cudaFreeHost(c->h_keys);
-    if (c->h_out) cudaFreeHost(c->h_out);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c->layouts;
     delete c;
     return B200DPF_OK;
 }
-
-/* device key / result buffers of the host-buffer entry points, grown on demand */
-static int ensure_device_io(b200dpf_ctx *c, size_t key_bytes, size_t out_elems)
-{
-    const size_t key_unit = host::KEY_WORDS * sizeof(int32_t);
-    if (key_bytes > c->keys_cap * key_unit) {
-        if (c->d_keys) cudaFree(c->d_keys);
-        c->d_keys = nullptr;
-        c->keys_cap = 0;
-        const size_t cap_keys = (key_bytes + key_unit - 1) / key_unit;
-        CUDA_TRY(cudaMalloc(&c->d_keys, cap_keys * key_unit));
-        c->keys_cap = cap_keys;
-    }
-    if (out_elems > c->out_cap) {
-        if (c->d_out) cudaFree(c->d_out);
-        c->d_out = nullptr;
-        c->out_cap = 0;
-        CUDA_TRY(cudaMalloc(&c->d_out, out_elems * sizeof(int32_t)));
-        c->out_cap = out_elems;
-    }
-    return B200DPF_OK;
-}
-
-static int ensure_host_out(b200dpf_ctx *c, size_t out_elems)
-{
-    if (out_elems <= c->h_out_cap) return B200DPF_OK;
-    if (c->h_out) cudaFreeHost(c->h_out);
-    c->h_out = nullptr;
-    c->h_out_cap = 0;
-    const size_t cap = std::max<size_t>(out_elems, 8192);
-    CUDA_TRY(cudaMallocHost(&c->h_out, cap * sizeof(int32_t)));
-    c->h_out_cap = cap;
-    return B200DPF_OK;
-}
-
 
 /* Host buffers in and out: keys (either layout) -> pinned staging if pageable -> H2D, the
  * evaluation, D2H, one stream synchronisation. */
@@ -1108,37 +1113,23 @@ static int eval_host(b200dpf_ctx *c, const void *keys, size_t key_bytes, const K
 {
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    const size_t out_elems = (size_t)nkeys * c->entry_size;
-    int rc = ensure_device_io(c, key_bytes, out_elems);
+    int rc = reserve_device_io(c, key_bytes, (size_t)nkeys * c->entry_size);
     if (rc) return rc;
     /* pageable host memory goes through the context's pinned staging so both copies are real
      * asynchronous DMA transfers; already-pinned buffers (ours or the caller's) are used as is */
     const void *src = keys;
     if (!is_pinned_host(keys)) {
-        rc = ensure_host_keys(c, (int64_t)((key_bytes + host::KEY_WORDS * sizeof(int32_t) - 1) / (host::KEY_WORDS * sizeof(int32_t))));
+        rc = reserve_host_keys(c, key_bytes);
         if (rc) return rc;
-        std::memcpy(c->h_keys, keys, key_bytes);
-        src = c->h_keys;
-    }
-    int32_t *dst = out;
-    if (!is_pinned_host(out)) {
-        rc = ensure_host_out(c, out_elems);
-        if (rc) return rc;
-        dst = c->h_out;
+        std::memcpy(c->h_keys.ptr, keys, key_bytes);
+        src = c->h_keys.ptr;
     }
     /* the previous evaluation may have run on a caller's stream: the staging copy below must not
      * overtake it (run_pipeline orders the kernels, this orders the H2D) */
-    if (c->has_last && c->last_stream != c->stream) CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_done, 0));
-    CUDA_TRY(cudaMemcpyAsync(c->d_keys, src, key_bytes, cudaMemcpyHostToDevice, c->stream));
-    CUDA_TRY(cudaEventRecord(c->ev_t0, c->stream));
-    rc = run_pipeline(c, c->d_keys, kl, nkeys, prf, MODE_FUSED, c->d_out, c->stream);
+    rc = wait_last(c, c->stream);
     if (rc) return rc;
-    CUDA_TRY(cudaEventRecord(c->ev_t1, c->stream));
-    c->timed = true;
-    CUDA_TRY(cudaMemcpyAsync(dst, c->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
-    if (dst != out) std::memcpy(out, dst, out_elems * sizeof(int32_t));
-    return B200DPF_OK;
+    CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, src, key_bytes, cudaMemcpyHostToDevice, c->stream));
+    return eval_tail(c, kl, nkeys, prf, out);
 }
 
 static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t nkeys, int prf, int32_t *out, bool validate);
@@ -1148,9 +1139,7 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     int rc = check_eval_args(c, keys, nkeys, prf, out);
     if (rc) return rc;
     for (int64_t b = 0; b < nkeys; b++)
-        if (host::key_n(keys + b * host::KEY_WORDS) != c->n)
-            return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b,
-                        (long long)host::key_n(keys + b * host::KEY_WORDS), (long long)c->n);
+        if ((rc = check_key_n(keys + b * host::KEY_WORDS, b, c->n))) return rc;
     if (!is_pinned_host(keys)) {
         /* pageable keys have to be staged by the CPU anyway: stage only their live 32 + 64*depth bytes
          * (44 % of a key at n = 2^14, 63 % at 2^20) and let the DMA of a chunk overlap the next one */
@@ -1162,80 +1151,42 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     return eval_host(c, keys, (size_t)nkeys * host::KEY_WORDS * sizeof(int32_t), reference_layout(), nkeys, prf, out);
 }
 
-/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks) */
-static inline void pack_compact(const int32_t *key, uint8_t *dst, int depth)
-{
-    const uint8_t *k = reinterpret_cast<const uint8_t *>(key);
-    std::memset(dst, 0, 16);
-    std::memcpy(dst, "DPF2", 4);
-    dst[4] = (uint8_t)depth;
-    std::memcpy(dst + 16, k + 16 * host::SLOT_ROOT, 16);
-    uint8_t *o = dst + 32;
-    const uint8_t *c1 = k + 16 * host::SLOT_CW1, *c2 = k + 16 * host::SLOT_CW2;
-    for (int L = 0; L < depth; L++, o += 64) {
-        std::memcpy(o, c1 + 32 * L, 32);
-        std::memcpy(o + 32, c2 + 32 * L, 32);
-    }
-}
-
-/* keys given as pointers (already validated): gather the live parts into pinned staging in the compact
- * layout, upload chunk by chunk while gathering, evaluate, copy back */
+/* keys given as pointers: gather the live parts into pinned staging in the compact layout (validating them
+ * if asked), upload chunk by chunk while gathering, evaluate, copy back */
 static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t nkeys, int prf, int32_t *out, bool validate)
 {
-    int rc;
     b200dpf_ctx *c0 = c->multi ? multi_first(c) : c;
     DeviceGuard guard(c0->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c0->device);
     const size_t stride = b200dpf_key_packed_size(c->depth);
     const size_t key_bytes = (size_t)nkeys * stride;
-    const size_t unit = host::KEY_WORDS * sizeof(int32_t);
-    rc = ensure_host_keys(c0, (int64_t)((key_bytes + unit - 1) / unit));
+    int rc = reserve_host_keys(c0, key_bytes);
     if (rc) return rc;
-    uint8_t *stage = reinterpret_cast<uint8_t *>(c0->h_keys);
-    if (c->multi) {
-        for (int64_t b = 0; b < nkeys; b++) {
-            if (validate && (!keys[b] || host::key_n(keys[b]) != c->n))
-                return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b,
-                            (long long)(keys[b] ? host::key_n(keys[b]) : -1), (long long)c->n);
-            pack_compact(keys[b], stage + (size_t)b * stride, c->depth);
-        }
-        return multi_eval_host(c, stage, stride, compact_layout(c->depth), nkeys, prf, out);
+    uint8_t *stage = reinterpret_cast<uint8_t *>(c0->h_keys.ptr);
+    if (!c->multi) {
+        rc = reserve_device_io(c, key_bytes, (size_t)nkeys * c->entry_size);
+        if (rc) return rc;
+        rc = wait_last(c, c->stream);
+        if (rc) return rc;
     }
     /* pack a chunk into pinned staging, start its DMA, pack the next: the copy engine works while
-     * the host gathers (the reference converts all 512 keys, then issues one blocking cudaMemcpy) */
-    const size_t out_elems = (size_t)nkeys * c->entry_size;
-    rc = ensure_device_io(c, key_bytes, out_elems);
-    if (rc) return rc;
-    if (c->has_last && c->last_stream != c->stream) CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_done, 0));
+     * the host gathers (the reference converts all 512 keys, then issues one blocking cudaMemcpy);
+     * a multi-device context uploads from the whole staged batch instead */
     const int64_t chunk = 64;
     for (int64_t b0 = 0; b0 < nkeys; b0 += chunk) {
         const int64_t b1 = std::min(nkeys, b0 + chunk);
         for (int64_t b = b0; b < b1; b++) {
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
-            if (validate && (!keys[b] || host::key_n(keys[b]) != c->n))
-                return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b,
-                            (long long)(keys[b] ? host::key_n(keys[b]) : -1), (long long)c->n);
+            if (validate && (rc = check_key_n(keys[b], b, c->n))) return rc;
             pack_compact(keys[b], stage + (size_t)b * stride, c->depth);
         }
-        CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
-                                 (size_t)(b1 - b0) * stride, cudaMemcpyHostToDevice, c->stream));
+        if (!c->multi)
+            CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys.ptr) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
+                                     (size_t)(b1 - b0) * stride, cudaMemcpyHostToDevice, c->stream));
     }
-    CUDA_TRY(cudaEventRecord(c->ev_t0, c->stream));
-    rc = run_pipeline(c, c->d_keys, compact_layout(c->depth), nkeys, prf, MODE_FUSED, c->d_out, c->stream);
-    if (rc) return rc;
-    CUDA_TRY(cudaEventRecord(c->ev_t1, c->stream));
-    c->timed = true;
-    int32_t *dst = out;
-    if (!is_pinned_host(out)) {
-        rc = ensure_host_out(c, out_elems);
-        if (rc) return rc;
-        dst = c->h_out;
-    }
-    CUDA_TRY(cudaMemcpyAsync(dst, c->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
-    if (dst != out) std::memcpy(out, dst, out_elems * sizeof(int32_t));
-    return B200DPF_OK;
+    if (c->multi) return multi_eval_host(c, stage, stride, compact_layout(c->depth), nkeys, prf, out);
+    return eval_tail(c, compact_layout(c->depth), nkeys, prf, out);
 }
 
 int b200dpf_eval_gather(b200dpf_ctx *c, const int32_t *const *keys, int64_t nkeys, int prf, int32_t *out)
@@ -1266,9 +1217,9 @@ int b200dpf_host_staging(b200dpf_ctx *c, int64_t nkeys, int32_t **keys_pinned)
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
     if (c->multi) c = multi_first(c);
-    const int rc = ensure_host_keys(c, nkeys);
+    const int rc = reserve_host_keys(c, (size_t)nkeys * kKeyBytes);
     if (rc) return rc;
-    *keys_pinned = c->h_keys;
+    *keys_pinned = c->h_keys.ptr;
     return B200DPF_OK;
 }
 
@@ -1380,7 +1331,26 @@ struct MultiState {
     std::vector<int64_t> k0, k1;      /* KEYS axis: slice of the batch per device */
     std::vector<int> rc;
     std::vector<std::string> err;
+
+    ~MultiState()   /* the workers stop before the sub-contexts they use go */
+    {
+        {
+            std::lock_guard<std::mutex> lk(m);
+            quit.store(true, std::memory_order_release);
+        }
+        cv.notify_all();
+        for (auto &t : workers) t.join();
+        for (b200dpf_ctx *c : sub) b200dpf_destroy(c);
+    }
 };
+
+b200dpf_ctx::~b200dpf_ctx()
+{
+    if (ev_done) cudaEventDestroy(ev_done);
+    if (ev_t0) cudaEventDestroy(ev_t0);
+    if (ev_t1) cudaEventDestroy(ev_t1);
+    if (stream) cudaStreamDestroy(stream);
+}
 
 static inline void cpu_relax()
 {
@@ -1404,27 +1374,19 @@ static int multi_device_part(MultiState *M, int d)
     const int64_t nk = e - b;
     const size_t key_bytes = (size_t)nk * M->key_stride_bytes;
     const size_t out_elems = (size_t)nk * c->entry_size;
-    int rc = ensure_device_io(c, key_bytes, out_elems);
+    int rc = reserve_device_io(c, key_bytes, out_elems);
     if (rc) return rc;
-    if (c->has_last && c->last_stream != c->stream) CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_done, 0));
-    CUDA_TRY(cudaMemcpyAsync(c->d_keys, static_cast<const char *>(M->keys) + (size_t)b * M->key_stride_bytes, key_bytes,
+    rc = wait_last(c, c->stream);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, static_cast<const char *>(M->keys) + (size_t)b * M->key_stride_bytes, key_bytes,
                              cudaMemcpyHostToDevice, c->stream));
-    rc = run_pipeline(c, c->d_keys, M->kl, nk, M->prf, MODE_FUSED, c->d_out, c->stream);
+    rc = run_pipeline(c, c->d_keys.ptr, M->kl, nk, M->prf, MODE_FUSED, c->d_out.ptr, c->stream);
     if (rc) return rc;
-    if (M->axis == B200DPF_AXIS_KEYS) {
-        int32_t *dst = M->out + (size_t)b * c->entry_size;
-        if (!M->out_pinned) {
-            rc = ensure_host_out(c, out_elems);
-            if (rc) return rc;
-            dst = c->h_out;
-        }
-        CUDA_TRY(cudaMemcpyAsync(dst, c->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_TRY(cudaStreamSynchronize(c->stream));
-        if (!M->out_pinned) std::memcpy(M->out + (size_t)b * c->entry_size, dst, out_elems * sizeof(int32_t));
-    } else if (!M->peer) {
-        rc = ensure_host_out(c, out_elems);
+    if (M->axis == B200DPF_AXIS_KEYS) return download_out(c, M->out + (size_t)b * c->entry_size, M->out_pinned, out_elems);
+    if (!M->peer) {
+        rc = reserve_host_out(c, out_elems);
         if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaMemcpyAsync(c->h_out.ptr, c->d_out.ptr, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
     /* ENTRIES + peer: run_pipeline recorded c->ev_done on c->stream; device 0 waits for it */
@@ -1472,37 +1434,21 @@ static int multi_set_option(b200dpf_ctx *root, const char *name, int value)
     return B200DPF_OK;
 }
 
-static void multi_destroy(b200dpf_ctx *root)
-{
-    MultiState *M = root->multi;
-    {
-        std::lock_guard<std::mutex> lk(M->m);
-        M->quit.store(true, std::memory_order_release);
-    }
-    M->cv.notify_all();
-    for (auto &t : M->workers) t.join();
-    for (b200dpf_ctx *c : M->sub) b200dpf_destroy(c);
-    delete M;
-    root->multi = nullptr;
-}
-
 static int multi_eval_host(b200dpf_ctx *root, const void *keys, size_t key_stride_bytes, const KeyLayout &kl, int64_t nkeys,
                            int prf, int32_t *out)
 {
-    MultiState *M = root->multi;
+    MultiState *M = root->multi.get();
     b200dpf_ctx *c0 = M->sub[0];
     DeviceGuard guard(c0->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c0->device);
     /* every device DMA-reads the keys from the same host buffer: it has to be pinned */
     const size_t key_bytes = (size_t)nkeys * key_stride_bytes;
     const void *src = keys;
-    int rc;
     if (!is_pinned_host(keys)) {
-        const size_t unit = host::KEY_WORDS * sizeof(int32_t);
-        rc = ensure_host_keys(c0, (int64_t)((key_bytes + unit - 1) / unit));
+        const int rc = reserve_host_keys(c0, key_bytes);
         if (rc) return rc;
-        std::memcpy(c0->h_keys, keys, key_bytes);
-        src = c0->h_keys;
+        std::memcpy(c0->h_keys.ptr, keys, key_bytes);
+        src = c0->h_keys.ptr;
     }
     const size_t out_elems = (size_t)nkeys * root->entry_size;
     M->keys = src;
@@ -1540,27 +1486,18 @@ static int multi_eval_host(b200dpf_ctx *root, const void *keys, size_t key_strid
         parts.n = 0;
         for (int d = 1; d < M->ndev; d++) {
             CUDA_TRY(cudaStreamWaitEvent(c0->stream, M->sub[(size_t)d]->ev_done, 0));
-            parts.p[parts.n++] = reinterpret_cast<const uint32_t *>(M->sub[(size_t)d]->d_out);
+            parts.p[parts.n++] = reinterpret_cast<const uint32_t *>(M->sub[(size_t)d]->d_out.ptr);
         }
-        CUDA_TRY(launch_sum_partials(reinterpret_cast<uint32_t *>(c0->d_out), parts, out_elems, c0->sm_count, c0->stream));
-        int32_t *dst = out;
-        if (!M->out_pinned) {
-            rc = ensure_host_out(c0, out_elems);
-            if (rc) return rc;
-            dst = c0->h_out;
-        }
-        CUDA_TRY(cudaMemcpyAsync(dst, c0->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c0->stream));
-        CUDA_TRY(cudaStreamSynchronize(c0->stream));
-        if (dst != out) std::memcpy(out, dst, out_elems * sizeof(int32_t));
-    } else {
-        /* no peer access between these devices: every shard already copied its partial to pinned
-         * host memory; wrapping 32-bit adds on the host */
-        uint32_t *o = reinterpret_cast<uint32_t *>(out);
-        std::memcpy(o, c0->h_out, out_elems * sizeof(int32_t));
-        for (int d = 1; d < M->ndev; d++) {
-            const uint32_t *part = reinterpret_cast<const uint32_t *>(M->sub[(size_t)d]->h_out);
-            for (size_t i = 0; i < out_elems; i++) o[i] += part[i];
-        }
+        CUDA_TRY(launch_sum_partials(reinterpret_cast<uint32_t *>(c0->d_out.ptr), parts, out_elems, c0->sm_count, c0->stream));
+        return download_out(c0, out, M->out_pinned, out_elems);
+    }
+    /* no peer access between these devices: every shard already copied its partial to pinned
+     * host memory; wrapping 32-bit adds on the host */
+    uint32_t *o = reinterpret_cast<uint32_t *>(out);
+    std::memcpy(o, c0->h_out.ptr, out_elems * sizeof(int32_t));
+    for (int d = 1; d < M->ndev; d++) {
+        const uint32_t *part = reinterpret_cast<const uint32_t *>(M->sub[(size_t)d]->h_out.ptr);
+        for (size_t i = 0; i < out_elems; i++) o[i] += part[i];
     }
     return B200DPF_OK;
 }
@@ -1584,14 +1521,10 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
     if (axis == B200DPF_AXIS_ENTRIES && (!pow2 || (int64_t)ndev > n / 2))
         return fail(B200DPF_EINVAL, "entry-range sharding needs a power-of-two device count <= n/2 (got %d)", ndev);
 
-    b200dpf_ctx *root = new (std::nothrow) b200dpf_ctx();
-    MultiState *M = new (std::nothrow) MultiState();
-    if (!root || !M) {
-        delete root;
-        delete M;
-        return fail(B200DPF_ENOMEM, "out of host memory");
-    }
-    root->multi = M;
+    std::unique_ptr<b200dpf_ctx> root(new (std::nothrow) b200dpf_ctx());
+    if (root) root->multi.reset(new (std::nothrow) MultiState());
+    if (!root || !root->multi) return fail(B200DPF_ENOMEM, "out of host memory");
+    MultiState *M = root->multi.get();
     root->n = n;
     root->depth = ilog2(n);
     root->entry_size = entry_size;
@@ -1606,12 +1539,7 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
         b200dpf_ctx *c = nullptr;
         const int rc = axis == B200DPF_AXIS_ENTRIES ? b200dpf_create(&c, table, n, entry_size, devices[d], d, ndev)
                                                     : b200dpf_create(&c, table, n, entry_size, devices[d], 0, 1);
-        if (rc) {
-            for (b200dpf_ctx *s : M->sub) b200dpf_destroy(s);
-            delete M;
-            delete root;
-            return rc;     /* message already set by b200dpf_create */
-        }
+        if (rc) return rc;     /* message already set by b200dpf_create; the root destroys the sub-contexts made */
         M->sub.push_back(c);
     }
     /* device 0 reads the other shards' partial results in place: NVLink peer mappings */
@@ -1629,7 +1557,7 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
         cudaGetLastError();
     }
     for (int d = 1; d < ndev; d++) M->workers.emplace_back(multi_worker, M, d);
-    *out = root;
+    *out = root.release();
     return B200DPF_OK;
 }
 
@@ -1651,75 +1579,42 @@ int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const 
         n_max = std::max(n_max, n[g]);
         rows += n[g];
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1)
-        return fail(B200DPF_ECUDA, "no CUDA device available (this engine has no CPU fallback)");
-    if (device < 0 || device >= ndev) return fail(B200DPF_EINVAL, "device %d out of range (have %d)", device, ndev);
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", device);
-
-    b200dpf_ctx *c = new (std::nothrow) b200dpf_ctx();
-    GroupBins *B = new (std::nothrow) GroupBins();
-    if (!c || !B) {
-        delete c;
-        delete B;
-        return fail(B200DPF_ENOMEM, "out of host memory");
-    }
-    c->bins = B;
-    c->device = device;
-    c->n = n_max;                       /* the launch plan (shared memory for correction words) is sized by the deepest bin */
+    std::optional<DeviceGuard> guard;
+    std::unique_ptr<b200dpf_ctx> c;
+    int rc = ctx_open(device, false, &guard, &c);     /* grouped contexts keep the default knobs */
+    if (rc) return rc;
+    c->bins.reset(new (std::nothrow) GroupBins());
+    if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
+    GroupBins *B = c->bins.get();
+    c->n = n_max;                      /* the launch plan (shared memory for correction words) is sized by the deepest bin */
     c->depth = ilog2(n_max);
     c->entry_size = entry_size;
     c->entry_pad = (entry_size + 15) & ~15;       /* 16 columns per pass */
     c->n_local = n_max;
     c->depth_local = c->depth;
-#define GRP_TRY(expr)                                                                          \
-    do {                                                                                       \
-        cudaError_t e__ = (expr);                                                              \
-        if (e__ != cudaSuccess) {                                                              \
-            fail(B200DPF_ECUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-            b200dpf_destroy(c);                                                                \
-            return B200DPF_ECUDA;                                                              \
-        }                                                                                      \
-    } while (0)
-    GRP_TRY(cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device));
-    GRP_TRY(cudaDeviceGetAttribute(&c->coop_ok, cudaDevAttrCooperativeLaunch, device));
-    GRP_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    GRP_TRY(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
-    GRP_TRY(cudaEventCreate(&c->ev_t0));
-    GRP_TRY(cudaEventCreate(&c->ev_t1));
-    GRP_TRY(cudaMalloc(&c->d_gridbar, sizeof(uint32_t)));
-    GRP_TRY(cudaMemsetAsync(c->d_gridbar, 0, sizeof(uint32_t), c->stream));
-    GRP_TRY(probe_dynamic_smem_base(&c->smem_base, c->stream));
-    GRP_TRY(upload_aes_table(host::aes_te0()));
-    if (!c->coop_ok) {
-        b200dpf_destroy(c);
-        return fail(B200DPF_ECUDA, "grouped evaluation needs cooperative launch support");
-    }
+    CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), c->stream));
+    if (!c->coop_ok) return fail(B200DPF_ECUDA, "grouped evaluation needs cooperative launch support");
     const size_t table_bytes = (size_t)rows * (size_t)c->entry_pad * sizeof(int32_t);
-    GRP_TRY(cudaMalloc(&c->d_table, table_bytes));
-    GRP_TRY(cudaMemsetAsync(c->d_table, 0, table_bytes, c->stream));
-    int32_t *d_stage = nullptr;
-    GRP_TRY(cudaMalloc(&d_stage, (size_t)n_max * entry_size * sizeof(int32_t)));
+    rc = c->d_table.reserve(table_bytes);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
+    DeviceBuffer<int32_t> d_stage;
+    rc = d_stage.reserve((size_t)n_max * entry_size * sizeof(int32_t));
+    if (rc) return rc;
     uint64_t row0 = 0;
-    cudaError_t e = cudaSuccess;
-    for (int g = 0; g < nbins && e == cudaSuccess; g++) {
+    for (int g = 0; g < nbins; g++) {
         /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows */
         const int depth = ilog2(n[g]);
         B->n.push_back(n[g]);
         B->depth.push_back(depth);
         B->row_off.push_back(row0);
-        e = cudaMemcpyAsync(d_stage, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream);
-        if (e == cudaSuccess)
-            e = launch_permute_table(d_stage, c->d_table + row0 * (uint64_t)c->entry_pad, (uint64_t)n[g], depth, entry_size,
-                                     c->entry_pad, c->sm_count, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);    /* the staging buffer is reused */
+        CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
+        CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr + row0 * (uint64_t)c->entry_pad, (uint64_t)n[g], depth,
+                                      entry_size, c->entry_pad, c->sm_count, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
         row0 += (uint64_t)n[g];
     }
-    cudaFree(d_stage);
-    GRP_TRY(e);
-#undef GRP_TRY
-    *out = c;
+    *out = c.release();
     return B200DPF_OK;
 }
 
@@ -1729,7 +1624,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     if (!keys || !bins || !out) return fail(B200DPF_EINVAL, "null buffer");
     if (nkeys < 1 || nkeys > (int64_t)1 << 24) return fail(B200DPF_EINVAL, "nkeys=%lld out of range", (long long)nkeys);
     if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
-    GroupBins *B = c->bins;
+    GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
     /* counting sort by bin: a key group must not mix bins */
     std::vector<int64_t> count((size_t)nbins + 1, 0);
@@ -1749,14 +1644,13 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     const KeyLayout kl = compact_layout(c->depth);
     const size_t stride = (size_t)kl.stride_v * 16u;
     const size_t key_bytes = (size_t)nkeys * stride;
-    const size_t unit = host::KEY_WORDS * sizeof(int32_t);
-    int rc = ensure_host_keys(c, (int64_t)((key_bytes + unit - 1) / unit));
+    int rc = reserve_host_keys(c, key_bytes);
     if (rc) return rc;
     B->perm.assign((size_t)nkeys, 0);
     {
         std::vector<int64_t> next(count.begin(), count.end() - 1);
         for (int64_t b = 0; b < nkeys; b++) B->perm[(size_t)(next[(size_t)bins[b]]++)] = b;
-        uint8_t *stage = reinterpret_cast<uint8_t *>(c->h_keys);
+        uint8_t *stage = reinterpret_cast<uint8_t *>(c->h_keys.ptr);
         auto pack_range = [&](int64_t p0, int64_t p1) {
             for (int64_t pos = p0; pos < p1; pos++) {
                 const int64_t b = B->perm[(size_t)pos];
@@ -1789,17 +1683,10 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             if (items >= 2 * warps) break;
         }
     }
-    if ((size_t)ngroups > B->h_descs_cap) {
-        if (B->h_descs) cudaFreeHost(B->h_descs);
-        if (B->d_descs) cudaFree(B->d_descs);
-        B->h_descs = nullptr;
-        B->d_descs = nullptr;
-        B->h_descs_cap = B->descs_cap = 0;
-        const size_t cap = std::max<size_t>((size_t)ngroups, 1024);
-        CUDA_TRY(cudaMallocHost(&B->h_descs, cap * sizeof(GroupDesc)));
-        CUDA_TRY(cudaMalloc(&B->d_descs, cap * sizeof(GroupDesc)));
-        B->h_descs_cap = B->descs_cap = cap;
-    }
+    const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
+    rc = B->h_descs.reserve(descs_bytes);
+    if (!rc) rc = B->d_descs.reserve(descs_bytes);
+    if (rc) return rc;
     int s_max = 1;
     {
         int64_t gi = 0;
@@ -1807,7 +1694,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             const int depth = B->depth[(size_t)g];
             const int s = std::max(1, std::min(depth, s_target));
             for (int64_t k = count[(size_t)g]; k < count[(size_t)g + 1]; k += 32, gi++) {
-                GroupDesc &d = B->h_descs[gi];
+                GroupDesc &d = B->h_descs.ptr[gi];
                 d.key_first = (uint32_t)k;
                 d.nkeys = (uint32_t)std::min<int64_t>(32, count[(size_t)g + 1] - k);
                 d.depth = depth;
@@ -1821,18 +1708,17 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     }
     const int passes = c->entry_pad / 16;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
-    rc = ensure_device_io(c, key_bytes, out_elems);
-    if (rc) return rc;
-    rc = ensure_host_out(c, out_elems);
+    rc = reserve_device_io(c, key_bytes, out_elems);
+    if (!rc) rc = reserve_host_out(c, out_elems);
     if (rc) return rc;
     const size_t n_counters = (size_t)passes * (size_t)ngroups;
-    rc = ensure_buffer(reinterpret_cast<void **>(&c->d_counters), &c->counters_cap, n_counters * sizeof(uint32_t));
+    rc = c->d_counters.reserve(n_counters * sizeof(uint32_t));
+    if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
-    if (c->has_last && c->last_stream != c->stream) CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_done, 0));
-    CUDA_TRY(cudaMemcpyAsync(c->d_keys, c->h_keys, key_bytes, cudaMemcpyHostToDevice, c->stream));
-    CUDA_TRY(cudaMemcpyAsync(B->d_descs, B->h_descs, (size_t)ngroups * sizeof(GroupDesc), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, B->h_descs.ptr, (size_t)ngroups * sizeof(GroupDesc), cudaMemcpyHostToDevice, c->stream));
     if (c->coop_state_dirty) {
-        CUDA_TRY(cudaMemsetAsync(c->d_gridbar, 0, sizeof(uint32_t), c->stream));
+        CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), c->stream));
         c->bar_epoch = 0;
         c->coop_state_dirty = false;
     }
@@ -1840,17 +1726,17 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     size_t smem;
     fill_common(c, L, s_max, nkeys, 5, &p, &smem);
     p.key_groups = (int)ngroups;
-    p.keys = reinterpret_cast<const uint4 *>(c->d_keys);
+    p.keys = reinterpret_cast<const uint4 *>(c->d_keys.ptr);
     p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
-    p.groups = B->d_descs;
+    p.groups = B->d_descs.ptr;
     fill_phase(L, s_max, &p.main);
-    p.main.counters = c->d_counters;
-    p.out = reinterpret_cast<uint32_t *>(c->d_out);
+    p.main.counters = c->d_counters.ptr;
+    p.out = reinterpret_cast<uint32_t *>(c->d_out.ptr);
     /* one cooperative launch per 16 columns; the first one clears the result and every pass's tickets */
     p.fuse_top = 1;
     p.zero_a = p.out;
     p.zero_a_words = out_elems;
-    p.zero_b = c->d_counters;
+    p.zero_b = c->d_counters.ptr;
     p.zero_b_words = n_counters;
     c->last_launches = 0;
     CUDA_TRY(cudaEventRecord(c->ev_t0, c->stream));
@@ -1859,9 +1745,9 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         p.col_off = (uint32_t)(pass * 16);
         p.ncols = (uint32_t)std::max(0, std::min(16, c->entry_size - pass * 16));
         if (p.ncols == 0) break;
-        p.main.counters = c->d_counters + (size_t)pass * (size_t)ngroups;
+        p.main.counters = c->d_counters.ptr + (size_t)pass * (size_t)ngroups;
         if (p.fuse_top) {
-            p.grid_bar = c->d_gridbar;
+            p.grid_bar = c->d_gridbar.ptr;
             c->bar_epoch += (uint32_t)L.grid;
             p.grid_bar_target = c->bar_epoch;
         }
@@ -1875,13 +1761,12 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     }
     CUDA_TRY(cudaEventRecord(c->ev_t1, c->stream));
     c->timed = true;
-    CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaEventRecord(c->ev_done, c->stream));
-    c->last_stream = c->stream;
-    c->has_last = true;
+    CUDA_TRY(cudaMemcpyAsync(c->h_out.ptr, c->d_out.ptr, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    rc = mark_last(c, c->stream);
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     for (int64_t pos = 0; pos < nkeys; pos++)       /* back to the caller's order */
-        std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
+        std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out.ptr + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
     return B200DPF_OK;
 }
 
@@ -1911,13 +1796,6 @@ uint64_t update_table_rows(const b200dpf_ctx *c)
     return c->bins ? c->bins->row_off.back() + (uint64_t)c->bins->n.back() : (uint64_t)c->n_local;
 }
 
-uint32_t bitrev_host(uint32_t v, int bits)
-{
-    uint32_t r = 0;
-    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
-    return r;
-}
-
 /* Grow the scratch for `count` rows (staged: the inputs are copied into it) and order everything that
  * follows on `stream` after the context's previous evaluation or update: the update writes the table
  * those read, and the scratch is the previous update's. */
@@ -1941,23 +1819,21 @@ int update_begin(b200dpf_ctx *c, int64_t count, bool staged, bool with_bins, cud
     }
     L->off_temp = off;
     L->total = align256(off + L->temp_bytes);
-    const int rc = ensure_buffer(&c->d_update, &c->update_cap, L->total);
-    if (rc) return rc;
-    if (c->has_last && c->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, c->ev_done, 0));
-    return B200DPF_OK;
+    const int rc = c->d_update.reserve(L->total);
+    return rc ? rc : wait_last(c, stream);
 }
 
 /* Enqueue the scatter (inputs in device memory) and record it as the context's last operation. */
 int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const int32_t *bins, const int32_t *rows,
                int64_t count, cudaStream_t stream)
 {
-    char *s = static_cast<char *>(c->d_update);
+    char *s = c->d_update.ptr;
     UpdateParams u;
     std::memset(&u, 0, sizeof u);
     u.idx = idx;
     u.bins = bins;
     if (bins) {
-        u.bin_info = c->bins->d_bin_info;
+        u.bin_info = c->bins->d_bin_info.ptr;
         u.nbins = (int)c->bins->n.size();
     }
     u.rows = rows;
@@ -1968,7 +1844,7 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     u.shift = c->shard_bits;
     u.depth = c->depth_local;
     u.table_rows = (uint32_t)update_table_rows(c);
-    u.table = c->d_table;
+    u.table = c->d_table.ptr;
     u.cols = c->entry_size;
     u.stride = c->entry_pad;
     UpdateWork w;
@@ -1979,10 +1855,7 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     w.temp = s + L.off_temp;
     w.temp_bytes = L.temp_bytes;
     CUDA_TRY(launch_update_rows(u, w, L.end_bit, c->sm_count, stream));
-    CUDA_TRY(cudaEventRecord(c->ev_done, stream));
-    c->last_stream = stream;
-    c->has_last = true;
-    return B200DPF_OK;
+    return mark_last(c, stream);
 }
 
 /* Host path on one single-device context (device already current, inputs validated): copy the rows this
@@ -2006,7 +1879,7 @@ int update_host_enqueue(b200dpf_ctx *c, const int64_t *idx, const int32_t *bins,
     UpdateLayout L;
     int rc = update_begin(c, count, true, bins != nullptr, c->stream, &L);
     if (rc) return rc;
-    char *s = static_cast<char *>(c->d_update);
+    char *s = c->d_update.ptr;
     CUDA_TRY(cudaMemcpyAsync(s + L.off_idx, idx, (size_t)count * sizeof(int64_t), cudaMemcpyHostToDevice, c->stream));
     if (bins) CUDA_TRY(cudaMemcpyAsync(s + L.off_bins, bins, (size_t)count * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(s + L.off_rows, rows, (size_t)count * (size_t)c->entry_size * sizeof(int32_t),
@@ -2033,7 +1906,7 @@ int b200dpf_update_rows(b200dpf_ctx *c, const int64_t *indices, const int32_t *r
     int rc = check_update_args(c, indices, rows, count);
     if (rc) return rc;
     if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_update_rows");
-    if (!c->d_table && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
+    if (!c->d_table.ptr && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
     for (int64_t j = 0; j < count; j++)
         if (indices[j] < 0 || indices[j] >= c->n)
             return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld)", (long long)j, (long long)indices[j],
@@ -2061,7 +1934,7 @@ int b200dpf_update_rows_device(b200dpf_ctx *c, const int64_t *indices_dev, const
     if (rc) return rc;
     if (c->multi) return fail(B200DPF_EINVAL, "multi-device contexts take host buffers (b200dpf_update_rows)");
     if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_update_rows");
-    if (!c->d_table) return fail(B200DPF_ESTATE, "context has no table");
+    if (!c->d_table.ptr) return fail(B200DPF_ESTATE, "context has no table");
     if (count == 0) return B200DPF_OK;
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
@@ -2078,7 +1951,7 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     if (rc) return rc;
     if (!c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
     if (count > 0 && !bins) return fail(B200DPF_EINVAL, "null buffer");
-    GroupBins *B = c->bins;
+    GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
     for (int64_t j = 0; j < count; j++) {
         if (bins[j] < 0 || bins[j] >= nbins)
@@ -2090,11 +1963,12 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     if (count == 0) return B200DPF_OK;
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    if (!B->d_bin_info) {
+    if (!B->d_bin_info.ptr) {
         std::vector<uint2> info((size_t)nbins);
         for (int g = 0; g < nbins; g++) info[(size_t)g] = make_uint2((uint32_t)B->row_off[(size_t)g], (uint32_t)B->depth[(size_t)g]);
-        CUDA_TRY(cudaMalloc(&B->d_bin_info, info.size() * sizeof(uint2)));
-        CUDA_TRY(cudaMemcpy(B->d_bin_info, info.data(), info.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+        rc = B->d_bin_info.reserve(info.size() * sizeof(uint2));
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpy(B->d_bin_info.ptr, info.data(), info.size() * sizeof(uint2), cudaMemcpyHostToDevice));
     }
     rc = update_host_enqueue(c, indices, bins, rows, count);
     if (rc) return rc;
@@ -2124,11 +1998,11 @@ int b200dpf_ctx_read_timing(b200dpf_ctx *c, uint64_t *stamps, int max_blocks, in
     if (!c || !stamps || !nblocks) return fail(B200DPF_EINVAL, "null argument");
     if (c->multi) c = multi_first(c);
     *nblocks = 0;
-    if (!c->d_timing) return B200DPF_OK;
+    if (!c->d_timing.ptr) return B200DPF_OK;
     DeviceGuard guard(c->device);
-    const int nb = std::min(max_blocks, c->timing_blocks);
+    const int nb = std::min(max_blocks, (int)(c->d_timing.cap / (8 * sizeof(unsigned long long))));
     CUDA_TRY(cudaDeviceSynchronize());
-    CUDA_TRY(cudaMemcpy(stamps, c->d_timing, (size_t)nb * 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(stamps, c->d_timing.ptr, (size_t)nb * 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     *nblocks = nb;
     return B200DPF_OK;
 }
