@@ -25,6 +25,8 @@ SYMBOLS = [
     "b200dpf_update_rows", "b200dpf_update_rows_device", "b200dpf_group_update_rows",
     "b200dpf_host_staging", "b200dpf_eval_device", "b200dpf_eval_device_acc", "b200dpf_expand_device", "b200dpf_ctx_n", "b200dpf_ctx_entry_size",
     "b200dpf_ctx_device", "b200dpf_ctx_last_launches", "b200dpf_ctx_set_subtree_log2",
+    "b200dpf_gen_et", "b200dpf_gen_batch_et", "b200dpf_eval_cpu_et", "b200dpf_key_pack_et", "b200dpf_key_unpack_et",
+    "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf",
 ]
 
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
@@ -84,6 +86,13 @@ def load():
     L.b200dpf_ctx_device.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_launches.argtypes = [C.c_void_p]
     L.b200dpf_ctx_set_subtree_log2.argtypes = [C.c_void_p, C.c_int]
+    L.b200dpf_gen_et.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
+    L.b200dpf_gen_batch_et.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
+    L.b200dpf_eval_cpu_et.argtypes = [_i32p, C.c_int, _i32p]
+    L.b200dpf_key_pack_et.argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.b200dpf_key_unpack_et.argtypes = [C.c_char_p, C.c_size_t, _i32p]
+    L.b200dpf_create_et.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
     return L
 
 
@@ -176,16 +185,70 @@ def eval_cpu(key, prf):
     return out
 
 
-class Context:
-    """One table (or one entry-range shard of it) resident on one GPU."""
+def _et_key_n(key):
+    """rows of an early-terminated key (slot 0 = (d, 2, 0, 0), slot 130 = 4 * 2^d), or -1"""
+    d, w = int(key[0]), int(key[1])
+    if w != 2 or key[2] or key[3] or not 1 <= d <= 29:
+        return -1
+    n = int(np.uint32(key[130 * 4]))
+    return n if n == 4 << d and not key[130 * 4 + 1:130 * 4 + 4].any() else -1
 
-    def __init__(self, table, device=0, shard_rank=0, shard_count=1):
+
+def gen_et(alpha, n, seed_bytes, prf):
+    """early-terminated key pair for row alpha of an n-row table (DESIGN.md section 9); >= 44 seed bytes"""
+    a = np.zeros(KEY_WORDS, np.int32)
+    b = np.zeros(KEY_WORDS, np.int32)
+    _check(lib().b200dpf_gen_et(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), "b200dpf_gen_et")
+    return a, b
+
+
+def gen_batch_et(alphas, n, seed_bytes, prf, nthreads=0):
+    """seed_bytes: 44 bytes of entropy per key, concatenated"""
+    alphas = np.ascontiguousarray(alphas, np.int64)
+    if len(seed_bytes) != 44 * len(alphas):
+        raise ValueError("gen_batch_et needs 44 seed bytes per key (%d keys, %d bytes)" % (len(alphas), len(seed_bytes)))
+    a = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    b = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    _check(lib().b200dpf_gen_batch_et(alphas, bytes(seed_bytes), len(alphas), n, prf, nthreads, a, b), "b200dpf_gen_batch_et")
+    return a, b
+
+
+def eval_cpu_et(key, prf):
+    key = np.ascontiguousarray(key, np.int32)
+    n = _et_key_n(key)
+    if n < 0:
+        raise B200DPFError("not an early-terminated key")
+    out = np.zeros(n, np.int32)
+    _check(lib().b200dpf_eval_cpu_et(key, prf, out), "b200dpf_eval_cpu_et")
+    return out
+
+
+def key_pack_et(key):
+    key = np.ascontiguousarray(key, np.int32)
+    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
+    n = C.c_size_t()
+    _check(lib().b200dpf_key_pack_et(key, buf, len(buf), C.byref(n)), "b200dpf_key_pack_et")
+    return buf.raw[:n.value]
+
+
+def key_unpack_et(packed):
+    key = np.zeros(KEY_WORDS, np.int32)
+    _check(lib().b200dpf_key_unpack_et(bytes(packed), len(packed), key), "b200dpf_key_unpack_et")
+    return key
+
+
+class Context:
+    """One table (or one entry-range shard of it) resident on one GPU.  early_termination=True makes a
+    context for early-terminated keys (b200dpf_create_et): four table rows per tree leaf."""
+
+    def __init__(self, table, device=0, shard_rank=0, shard_count=1, early_termination=False):
         table = np.ascontiguousarray(table, np.int32)
         assert table.ndim == 2
         self.n, self.entry_size = table.shape
         self.handle = C.c_void_p()
-        _check(lib().b200dpf_create(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
-                                    device, shard_rank, shard_count), "b200dpf_create")
+        create = lib().b200dpf_create_et if early_termination else lib().b200dpf_create
+        _check(create(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
+                      device, shard_rank, shard_count), "b200dpf_create_et" if early_termination else "b200dpf_create")
 
     @classmethod
     def multi(cls, table, devices, axis=0):
@@ -276,6 +339,10 @@ class Context:
     @property
     def last_launches(self):
         return lib().b200dpf_ctx_last_launches(self.handle)
+
+    @property
+    def rows_per_leaf(self):
+        return lib().b200dpf_ctx_rows_per_leaf(self.handle)
 
     def close(self):
         if self.handle:

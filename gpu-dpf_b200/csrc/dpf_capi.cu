@@ -141,6 +141,10 @@ struct b200dpf_ctx {
     int shard_rank = 0, shard_count = 1, shard_bits = 0;
     int64_t n_local = 0;
     int depth_local = 0;
+    /* log2 table rows per tree leaf: 0, or 2 on an early-terminated context (b200dpf_create_et).  n,
+     * n_local, the table, the leaf cache and the results count rows; depth, depth_local, the shards,
+     * the work items and the frontier count leaves. */
+    int lane_bits = 0;
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
     DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
@@ -206,8 +210,8 @@ struct SmemLayout {
 }  // namespace
 
 struct SmemLayoutCache {
-    SmemLayout entry[4][3][5];
-    bool valid[4][3][5] = {};
+    SmemLayout entry[4][3][MODE_COUNT];
+    bool valid[4][3][MODE_COUNT] = {};
 };
 
 namespace {
@@ -355,12 +359,15 @@ struct KeyLayout {
 KeyLayout reference_layout() { return KeyLayout{131u, 129u, 0}; }                       /* dpf_wrapper.cu:26-46 */
 KeyLayout compact_layout(int depth) { return KeyLayout{2u + 4u * (uint32_t)depth, 1u, 1}; }   /* b200dpf_key_pack */
 
-/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks) */
-inline void pack_compact(const int32_t *key, uint8_t *dst, int depth)
+/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks); the magic is
+ * "DPF2", or "DPE4" for an early-terminated key */
+constexpr char kMagic[] = "DPF2", kMagicEt[] = "DPE4";
+
+inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char *magic = kMagic)
 {
     const uint8_t *k = reinterpret_cast<const uint8_t *>(key);
     std::memset(dst, 0, 16);
-    std::memcpy(dst, "DPF2", 4);
+    std::memcpy(dst, magic, 4);
     dst[4] = (uint8_t)depth;
     std::memcpy(dst + 16, k + 16 * host::SLOT_ROOT, 16);
     uint8_t *o = dst + 32;
@@ -377,6 +384,22 @@ inline int check_key_n(const int32_t *key, int64_t b, int64_t n)
     const int64_t kn = key ? host::key_n(key) : -1;
     if (kn == n) return B200DPF_OK;
     return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b, (long long)kn, (long long)n);
+}
+
+/* key number `b` of a batch must be of the context's kind (standard or early-terminated) and n */
+inline int check_key(const b200dpf_ctx *c, const int32_t *key, int64_t b)
+{
+    if (!c->lane_bits) {
+        if (key && host::key_et_n(key) >= 0)
+            return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this context takes standard keys", (long long)b);
+        return check_key_n(key, b, c->n);
+    }
+    const int64_t kn = key ? host::key_et_n(key) : -1;
+    if (kn == c->n) return B200DPF_OK;
+    if (key && host::key_n(key) >= 0)
+        return fail(B200DPF_EINVAL, "key %lld is a standard key; this early-terminated context takes keys of b200dpf_gen_et", (long long)b);
+    return fail(B200DPF_EINVAL, "key %lld is not an early-terminated key for n=%lld (its n: %lld)", (long long)b, (long long)c->n,
+                (long long)kn);
 }
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
@@ -403,12 +426,16 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
      * columns, NV = 4), which also caches each leaf's low word; every other column is produced by
      * MAC-only passes over that cache.  Without the cache (disabled or lane-split batches) wide
      * entries use one tree expansion per 64 columns. */
-    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache) ? 4 : (c->entry_pad <= 32 ? 8 : 16);
+    const bool et = c->lane_bits != 0;   /* early-terminated: 32 columns per pass at most */
+    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache) ? 4 : (c->entry_pad <= 32 || et ? 8 : 16);
     const int passes = mode_main == MODE_FUSED ? (want_cache ? 1 : c->entry_pad / (4 * nv)) : 1;
+    /* the kernel modes of this context's kind */
+    const int mode_fused = et ? MODE_FUSED_ET : MODE_FUSED, mode_expand = et ? MODE_EXPAND_ET : MODE_EXPAND;
     /* optional variant: the rows of each work item staged into shared memory by cp.async.bulk */
     bool tma_rows = K.tma_rows != 0 && K.one_launch != 0 && c->coop_ok != 0 && mode_main == MODE_FUSED && c->entry_pad == 16 &&
-                    prf != B200DPF_PRF_AES128 && nkeys >= 17;
-    int mode_kernel = tma_rows ? MODE_FUSED_TMA : mode_main;
+                    prf != B200DPF_PRF_AES128 && nkeys >= 17 && !et;
+    const int mode_plain = mode_main == MODE_FUSED ? mode_fused : mode_expand;
+    int mode_kernel = tma_rows ? MODE_FUSED_TMA : mode_plain;
     SmemLayout L;
     int rc = smem_layout(c, prf, nv, mode_kernel, &L);
     if (rc) return rc;
@@ -451,7 +478,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         tile_bytes = (size_t)warps_blk * ((size_t)64 << s) + 8u * (size_t)warps_blk + 16u;
         if ((size_t)L.off_lo + (size_t)(std::max(s, 7) - 1) * L.level_bytes + tile_bytes > (size_t)L.budget) {
             tma_rows = false;               /* does not fit beside correction words and stack: broadcast loads */
-            mode_kernel = mode_main;
+            mode_kernel = mode_plain;
             tile_bytes = 0;
             rc = smem_layout(c, prf, nv, mode_kernel, &L);
             if (rc) return rc;
@@ -635,7 +662,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     };
     if (mode_main == MODE_EXPAND) {
         p.shares = reinterpret_cast<uint32_t *>(out_dev);
-        return launch_main(4, MODE_EXPAND);
+        return launch_main(4, mode_expand);
     }
     p.out = reinterpret_cast<uint32_t *>(out_dev);
     if (want_cache) {
@@ -647,7 +674,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         p.col_off_v = 0;
         p.col_off = 0;
         p.ncols = (uint32_t)std::min(16, c->entry_size);
-        rc = launch_main(4, MODE_FUSED);
+        rc = launch_main(4, mode_fused);
         if (rc) return rc;
         MacParams m;
         std::memset(&m, 0, sizeof m);
@@ -999,16 +1026,87 @@ int b200dpf_key_unpack(const uint8_t *in, size_t in_len, int32_t *key)
 int64_t b200dpf_key_n(const int32_t *key) { return key ? host::key_n(key) : -1; }
 int b200dpf_key_depth(const int32_t *key) { return key ? host::key_depth(key) : -1; }
 
-int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
-                   int shard_rank, int shard_count)
+/* ---- early-terminated keys ---- */
+
+int b200dpf_gen_et(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf, int32_t *key_a, int32_t *key_b)
+{
+    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
+    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "gen_et needs at least 44 bytes of seed (got %zu)", seed_len);
+    if (host::gen_et(alpha, n, seed, prf, key_a, key_b) != 0)
+        return fail(B200DPF_EINVAL, "gen_et: need power-of-two n in [8, 2^31], 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
+                    (long long)alpha, (long long)n, prf);
+    return B200DPF_OK;
+}
+
+int b200dpf_gen_batch_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int nthreads,
+                         int32_t *keys_a, int32_t *keys_b)
+{
+    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_et argument");
+    if (!gen_parallel(count, nthreads, [&](int64_t i) {
+            return host::gen_et(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
+        }))
+        return fail(B200DPF_EINVAL, "gen_batch_et: invalid alpha/n/prf in batch");
+    return B200DPF_OK;
+}
+
+int b200dpf_eval_cpu_et(const int32_t *key, int prf, int32_t *out_n)
+{
+    if (!key || !out_n) return fail(B200DPF_EINVAL, "null buffer");
+    if (host::key_et_n(key) < 0) return fail(B200DPF_EINVAL, "eval_cpu_et: not an early-terminated key");
+    if (host::eval_cpu_et(key, prf, out_n) != 0) return fail(B200DPF_EINVAL, "eval_cpu_et: unknown prf id %d", prf);
+    return B200DPF_OK;
+}
+
+int b200dpf_key_pack_et(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
+{
+    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
+    const int depth = host::key_et_depth(key);
+    if (depth < 1 || host::key_et_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack_et: not an early-terminated key");
+    const size_t need = b200dpf_key_packed_size(depth);
+    if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack_et: need %zu bytes, have %zu", need, out_cap);
+    pack_compact(key, out, depth, kMagicEt);
+    if (written) *written = need;
+    return B200DPF_OK;
+}
+
+int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key)
+{
+    if (!in || !key) return fail(B200DPF_EINVAL, "null buffer");
+    if (in_len < 32 || std::memcmp(in, kMagicEt, 4) != 0) return fail(B200DPF_EINVAL, "key_unpack_et: bad header");
+    const int depth = in[4];
+    bool pad_zero = true;
+    for (int i = 5; i < 16; i++) pad_zero = pad_zero && in[i] == 0;
+    if (depth < 1 || depth > host::ET_MAX_DEPTH || !pad_zero || in_len != b200dpf_key_packed_size(depth))
+        return fail(B200DPF_EINVAL, "key_unpack_et: depth %d does not match %zu bytes", depth, in_len);
+    std::memset(key, 0, sizeof(int32_t) * host::KEY_WORDS);
+    uint8_t *k = reinterpret_cast<uint8_t *>(key);
+    k[16 * host::SLOT_DEPTH] = (uint8_t)depth;
+    k[16 * host::SLOT_DEPTH + 4] = (uint8_t)host::ET_LOG2_ROWS_PER_LEAF;
+    std::memcpy(k + 16 * host::SLOT_ROOT, in + 16, 16);
+    for (int L = 0; L < depth; L++) {
+        const uint8_t *o = in + 32 + 64 * L;
+        std::memcpy(k + 16 * (host::SLOT_CW1 + 2 * L), o, 32);
+        std::memcpy(k + 16 * (host::SLOT_CW2 + 2 * L), o + 32, 32);
+    }
+    const uint64_t n = (uint64_t)1 << (depth + host::ET_LOG2_ROWS_PER_LEAF);
+    std::memcpy(k + 16 * host::SLOT_N, &n, 8);
+    return B200DPF_OK;
+}
+
+}  // extern "C"
+
+/* b200dpf_create (lane_bits = 0) and b200dpf_create_et (lane_bits = 2: 2^lane_bits rows per leaf) */
+static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int shard_rank,
+                       int shard_count, int lane_bits)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!table) return fail(B200DPF_EINVAL, "null table");
-    if (n < 2 || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0)
-        return fail(B200DPF_EINVAL, "table size n=%lld must be a power of two in [2, 2^31]", (long long)n);
+    const int64_t n_min = (int64_t)2 << lane_bits;
+    if (n < n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0)
+        return fail(B200DPF_EINVAL, "table size n=%lld must be a power of two in [%lld, 2^31]", (long long)n, (long long)n_min);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
-    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 || (int64_t)shard_count > n / 2 ||
+    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 || (int64_t)shard_count > n / n_min ||
         shard_rank < 0 || shard_rank >= shard_count)
         return fail(B200DPF_EINVAL, "bad shard %d of %d for n=%lld", shard_rank, shard_count, (long long)n);
 
@@ -1017,7 +1115,8 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     int rc = ctx_open(device, true, &guard, &c);
     if (rc) return rc;
     c->n = n;
-    c->depth = ilog2(n);
+    c->lane_bits = lane_bits;
+    c->depth = ilog2(n) - lane_bits;   /* the tree is over leaves */
     c->entry_size = entry_size;
     /* rows padded to what one pass reads: 16, 32 or a multiple of 64 int32 */
     c->entry_pad = entry_size <= 16 ? 16 : (entry_size <= 32 ? 32 : ((entry_size + 63) & ~63));
@@ -1030,7 +1129,8 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     /* Table: gather this shard's rows (natural indices j*G + bitrev_g(rank)),
      * then permute on the device into breadth-first leaf order, padded to
      * 64-byte rows.  dpf_wrapper.cu:103-115 does the analogous reorder on the
-     * host with one ATen call per element. */
+     * host with one ATen call per element.  On an early-terminated context the
+     * same is done to runs of 2^lane_bits rows, one leaf each. */
     {   /* a device-resident table may still be being written on the caller's stream (e.g. a dtype
          * cast enqueued just before this call): our copy runs on a private non-blocking stream,
          * so wait for the producing device first */
@@ -1046,6 +1146,8 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     }
     const size_t row_bytes = (size_t)entry_size * sizeof(int32_t);
     const size_t stage_bytes = (size_t)c->n_local * row_bytes;
+    const size_t leaf_bytes = row_bytes << lane_bits;            /* one leaf's rows */
+    const int64_t leaves_local = c->n_local >> lane_bits;
     const size_t table_bytes = (size_t)c->n_local * (size_t)c->entry_pad * sizeof(int32_t);
     DeviceBuffer<int32_t> d_stage;
     rc = d_stage.reserve(stage_bytes);
@@ -1054,18 +1156,19 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     if (shard_count == 1) {
         e = cudaMemcpyAsync(d_stage.ptr, table, stage_bytes, cudaMemcpyDefault, c->stream);
     } else {
-        const int32_t *src = table + (size_t)bitrev_host((uint32_t)shard_rank, c->shard_bits) * entry_size;
+        const int32_t *src = table + ((size_t)bitrev_host((uint32_t)shard_rank, c->shard_bits) << lane_bits) * entry_size;
         cudaPointerAttributes attr;
         const bool on_device = cudaPointerGetAttributes(&attr, table) == cudaSuccess &&
                                (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
         cudaGetLastError();
         if (on_device) {
-            e = cudaMemcpy2DAsync(d_stage.ptr, row_bytes, src, row_bytes * shard_count, row_bytes, (size_t)c->n_local,
+            e = cudaMemcpy2DAsync(d_stage.ptr, leaf_bytes, src, leaf_bytes * shard_count, leaf_bytes, (size_t)leaves_local,
                                   cudaMemcpyDefault, c->stream);
         } else {
             std::vector<int32_t> gathered((size_t)c->n_local * entry_size);
-            for (int64_t j = 0; j < c->n_local; j++)
-                std::memcpy(gathered.data() + (size_t)j * entry_size, src + (size_t)j * shard_count * entry_size, row_bytes);
+            const size_t leaf_words = (size_t)entry_size << lane_bits;
+            for (int64_t j = 0; j < leaves_local; j++)
+                std::memcpy(gathered.data() + (size_t)j * leaf_words, src + (size_t)j * shard_count * leaf_words, leaf_bytes);
             e = cudaMemcpyAsync(d_stage.ptr, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         }
@@ -1074,8 +1177,12 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size, c->entry_pad,
-                                  c->sm_count, c->stream));
+    if (lane_bits)
+        CUDA_TRY(launch_permute_table_et(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size,
+                                         c->entry_pad, c->sm_count, c->stream));
+    else
+        CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size,
+                                      c->entry_pad, c->sm_count, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     d_stage.release();
 
@@ -1090,12 +1197,28 @@ int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry
     const int nv0 = c->entry_pad <= 16 ? 4 : (c->entry_pad <= 32 ? 8 : 4);
     SmemLayout tmp;
     for (int prf = 0; prf < 4; prf++) {
-        smem_layout(c.get(), prf, nv0, MODE_FUSED, &tmp);
+        smem_layout(c.get(), prf, nv0, lane_bits ? MODE_FUSED_ET : MODE_FUSED, &tmp);
         smem_layout(c.get(), prf, 4, MODE_FRONTIER, &tmp);
     }
     *out = c.release();
     return B200DPF_OK;
 }
+
+extern "C" {
+
+int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
+                   int shard_rank, int shard_count)
+{
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, 0);
+}
+
+int b200dpf_create_et(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
+                      int shard_rank, int shard_count)
+{
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::ET_LOG2_ROWS_PER_LEAF);
+}
+
+int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *c) { return c ? 1 << c->lane_bits : -1; }
 
 int b200dpf_destroy(b200dpf_ctx *c)
 {
@@ -1139,7 +1262,7 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     int rc = check_eval_args(c, keys, nkeys, prf, out);
     if (rc) return rc;
     for (int64_t b = 0; b < nkeys; b++)
-        if ((rc = check_key_n(keys + b * host::KEY_WORDS, b, c->n))) return rc;
+        if ((rc = check_key(c, keys + b * host::KEY_WORDS, b))) return rc;
     if (!is_pinned_host(keys)) {
         /* pageable keys have to be staged by the CPU anyway: stage only their live 32 + 64*depth bytes
          * (44 % of a key at n = 2^14, 63 % at 2^20) and let the DMA of a chunk overlap the next one */
@@ -1178,8 +1301,8 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
         for (int64_t b = b0; b < b1; b++) {
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
-            if (validate && (rc = check_key_n(keys[b], b, c->n))) return rc;
-            pack_compact(keys[b], stage + (size_t)b * stride, c->depth);
+            if (validate && (rc = check_key(c, keys[b], b))) return rc;
+            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, c->lane_bits ? kMagicEt : kMagic);
         }
         if (!c->multi)
             CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys.ptr) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
@@ -1203,7 +1326,7 @@ int b200dpf_eval_packed(b200dpf_ctx *c, const uint8_t *packed, int64_t nkeys, in
     const size_t stride = b200dpf_key_packed_size(c->depth);
     for (int64_t b = 0; b < nkeys; b++) {
         const uint8_t *k = packed + (size_t)b * stride;
-        if (std::memcmp(k, "DPF2", 4) != 0 || k[4] != (uint8_t)c->depth)
+        if (std::memcmp(k, c->lane_bits ? kMagicEt : kMagic, 4) != 0 || k[4] != (uint8_t)c->depth)
             return fail(B200DPF_EINVAL, "packed key %lld: bad header or depth %d, table has depth %d (n=%lld)", (long long)b,
                         (int)k[4], c->depth, (long long)c->n);
     }
@@ -1844,6 +1967,7 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     u.shift = c->shard_bits;
     u.depth = c->depth_local;
     u.table_rows = (uint32_t)update_table_rows(c);
+    u.lane_bits = c->lane_bits;
     u.table = c->d_table.ptr;
     u.cols = c->entry_size;
     u.stride = c->entry_pad;
@@ -1867,7 +1991,7 @@ int update_host_enqueue(b200dpf_ctx *c, const int64_t *idx, const int32_t *bins,
     if (c->shard_count > 1) {             /* a shard copies only its own rows */
         const uint32_t mask = (uint32_t)c->shard_count - 1u, val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
         for (int64_t j = 0; j < count; j++)
-            if (((uint32_t)idx[j] & mask) == val) {
+            if (((uint32_t)(idx[j] >> c->lane_bits) & mask) == val) {
                 own_idx.push_back(idx[j]);
                 own_rows.insert(own_rows.end(), rows + j * c->entry_size, rows + (j + 1) * c->entry_size);
             }

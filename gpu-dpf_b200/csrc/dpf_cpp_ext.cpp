@@ -150,6 +150,72 @@ std::vector<void *> eval_init_sharded(const at::Tensor &table, int device, int s
     return {static_cast<void *>(ctx)};
 }
 
+/* ---- early-terminated keys: four table rows per tree leaf (include/b200dpf.h, b200dpf_gen_et) ---- */
+
+std::vector<at::Tensor> gen_et(int64_t k, int64_t n, const std::string &seed, int prf)
+{
+    at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
+    at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
+    check(b200dpf_gen_et(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf, a.data_ptr<int32_t>(),
+                         b.data_ptr<int32_t>()),
+          "gen_et");
+    return {a, b};
+}
+
+std::vector<at::Tensor> gen_batch_et(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
+{
+    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
+    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), "gen_batch_et: need 44 seed bytes per key");
+    const int64_t count = al.numel();
+    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
+    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
+    {
+        py::gil_scoped_release nogil;
+        check(b200dpf_gen_batch_et(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf,
+                                   nthreads, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
+              "gen_batch_et");
+    }
+    return {a, b};
+}
+
+at::Tensor eval_cpu_et(const at::Tensor &key, int prf)
+{
+    const int32_t *k = key_ptr(key);
+    /* slot 0 = (d, 2, 0, 0), slot 130 = n = 4 * 2^d; b200dpf_eval_cpu_et checks the rest */
+    const uint32_t d = (uint32_t)k[0];
+    TORCH_CHECK(k[1] == 2 && d >= 1 && d <= 29, "eval_cpu_et: not an early-terminated key");
+    at::Tensor result = torch::empty({(int64_t)4 << d}, at::kInt);
+    check(b200dpf_eval_cpu_et(k, prf, result.data_ptr<int32_t>()), "eval_cpu_et");
+    return result;
+}
+
+py::bytes key_pack_et(const at::Tensor &key)
+{
+    const int32_t *k = key_ptr(key);
+    std::string buf(b200dpf_key_packed_size(32), '\0');
+    size_t written = 0;
+    check(b200dpf_key_pack_et(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), "key_pack_et");
+    return py::bytes(buf.data(), written);
+}
+
+at::Tensor key_unpack_et(const std::string &packed)
+{
+    at::Tensor key = torch::zeros({kKeyWords}, at::kInt);
+    check(b200dpf_key_unpack_et(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()),
+          "key_unpack_et");
+    return key;
+}
+
+std::vector<void *> eval_init_et(const at::Tensor &table, int device, int shard_rank, int shard_count)
+{
+    TORCH_CHECK(table.dim() == 2, "eval_init_et: table must be [num_entries, entry_size]");
+    at::Tensor t = table.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    check(b200dpf_create_et(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count),
+          "eval_init_et");
+    return {static_cast<void *>(ctx)};
+}
+
 /* one table on several GPUs of this process (b200dpf_create_multi); axis: 0 auto, 1 entries, 2 keys */
 std::vector<void *> eval_init_multi(const at::Tensor &table, const std::vector<int> &devices, int axis)
 {
@@ -309,8 +375,8 @@ at::Tensor eval_gpu_compact(const at::Tensor &packed, int64_t nkeys, const std::
     b200dpf_ctx *ctx = ctx_of(buffers);
     TORCH_CHECK(packed.device().is_cpu() && packed.scalar_type() == at::kByte && packed.is_contiguous(),
                 "eval_gpu_compact: packed keys must be a contiguous CPU uint8 tensor");
-    int depth = 0;
-    for (int64_t n = b200dpf_ctx_n(ctx); n > 1; n >>= 1) depth++;
+    int depth = 0;   /* of the tree: over leaves, which are rows_per_leaf rows each */
+    for (int64_t n = b200dpf_ctx_n(ctx) / b200dpf_ctx_rows_per_leaf(ctx); n > 1; n >>= 1) depth++;
     TORCH_CHECK(nkeys >= 1 && (int64_t)packed.numel() == nkeys * (int64_t)b200dpf_key_packed_size(depth),
                 "eval_gpu_compact: expected ", nkeys, " keys of ", b200dpf_key_packed_size(depth), " bytes");
     at::Tensor result = torch::empty({nkeys, (int64_t)b200dpf_ctx_entry_size(ctx)}, at::kInt);
@@ -467,4 +533,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("set_option", &set_option, "tuning knob of a live context (include/b200dpf.h: b200dpf_ctx_set_option)");
     m.def("eval_gpu_compact", &eval_gpu_compact, "eval_gpu with keys in the compact wire form (uint8 tensor)");
     m.def("key_packed_size", [](int depth) { return (int64_t)b200dpf_key_packed_size(depth); });
+    m.def("gen_et", &gen_et, "early-terminated key pair for row k of an n-row table (seed: >= 44 bytes)");
+    m.def("gen_batch_et", &gen_batch_et, "batched early-terminated keygen (44 seed bytes per key)", py::arg("alphas"),
+          py::arg("n"), py::arg("seeds"), py::arg("prf"), py::arg("nthreads") = 0);
+    m.def("eval_cpu_et", &eval_cpu_et, "share of every row of an early-terminated key on the CPU");
+    m.def("key_pack_et", &key_pack_et, "compact wire form (\"DPE4\") of an early-terminated key");
+    m.def("key_unpack_et", &key_unpack_et, "restore an early-terminated int32[524] key from its compact form");
+    m.def("eval_init_et", &eval_init_et, "eval_init for early-terminated keys (four rows per leaf)", py::arg("table"),
+          py::arg("device") = 0, py::arg("shard_rank") = 0, py::arg("shard_count") = 1);
+    m.def("rows_per_leaf", [](const std::vector<void *> &b) { return b200dpf_ctx_rows_per_leaf(ctx_of(b)); });
 }

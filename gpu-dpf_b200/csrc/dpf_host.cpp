@@ -138,6 +138,21 @@ u128 random128_odd(Rng &g)
     return k;
 }
 
+/* Lane-wise arithmetic in (Z/2^32)^4: the payload level of an early-terminated key. */
+u128 lanes_add(u128 a, u128 b)
+{
+    u128 r = 0;
+    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)((uint32_t)(a >> (32 * l)) + (uint32_t)(b >> (32 * l))) << (32 * l);
+    return r;
+}
+
+u128 lanes_neg(u128 a)
+{
+    u128 r = 0;
+    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)(0u - (uint32_t)(a >> (32 * l))) << (32 * l);
+    return r;
+}
+
 template <class Rng>
 struct KeyBuilder {
     int depth;
@@ -146,6 +161,10 @@ struct KeyBuilder {
     Rng &g;
     u128 cw1[64], cw2[64];
     u128 root_a, root_b;
+    bool lanes = false;   /* early-terminated key: level 0 adds and subtracts lane-wise */
+
+    u128 add(int L, u128 a, u128 b) const { return (lanes && L == 0) ? lanes_add(a, b) : a + b; }
+    u128 sub(int L, u128 a, u128 b) const { return (lanes && L == 0) ? lanes_add(a, lanes_neg(b)) : a - b; }
 
     /* Builds flat level L (domain 2^(depth-L)) for payload `beta` and returns
      * the two servers' seeds on the alpha path just below this level. */
@@ -162,12 +181,12 @@ struct KeyBuilder {
             root_b = kb;
             u128 delta[2];
             for (int i = 0; i < 2; i++) {
-                delta[i] = prf128(prf_id, ka, (uint32_t)i) - prf128(prf_id, kb, (uint32_t)i);
-                if (i == row) delta[i] -= beta;
+                delta[i] = sub(L, prf128(prf_id, ka, (uint32_t)i), prf128(prf_id, kb, (uint32_t)i));
+                if (i == row) delta[i] = sub(L, delta[i], beta);
             }
             for (int i = 0; i < 2; i++) {
                 cw1[2 * L + i] = g.draw128();
-                cw2[2 * L + i] = cw1[2 * L + i] + delta[i];
+                cw2[2 * L + i] = add(L, cw1[2 * L + i], delta[i]);
             }
             up_a = ka;
             up_b = kb;
@@ -178,11 +197,11 @@ struct KeyBuilder {
             up_b = below.second;
             const bool a_even = (up_a & 1) == 0;
             for (int i = 0; i < 2; i++) {
-                u128 d = prf128(prf_id, up_b, (uint32_t)i) - prf128(prf_id, up_a, (uint32_t)i);
-                if (a_even) d = (u128)0 - d;
+                u128 d = sub(L, prf128(prf_id, up_b, (uint32_t)i), prf128(prf_id, up_a, (uint32_t)i));
+                if (a_even) d = sub(L, 0, d);
                 cw1[2 * L + i] = g.draw_upper_cw();   /* reference: a 32-bit draw, dpf.h:450 */
-                cw2[2 * L + i] = cw1[2 * L + i] + d;
-                if (i == row) cw1[2 * L + i] += a_even ? beta : (u128)0 - beta;
+                cw2[2 * L + i] = add(L, cw1[2 * L + i], d);
+                if (i == row) cw1[2 * L + i] = a_even ? add(L, cw1[2 * L + i], beta) : sub(L, cw1[2 * L + i], beta);
             }
         }
         const u128 *bank_a = (up_a & 1) ? cw2 : cw1;
@@ -235,6 +254,22 @@ int64_t key_n(const int32_t *key)
     return n;
 }
 
+int key_et_depth(const int32_t *key)
+{
+    const Seed d = key_slot(key, SLOT_DEPTH);
+    if (d.y != (uint32_t)ET_LOG2_ROWS_PER_LEAF || d.z || d.w || d.x < 1 || d.x > ET_MAX_DEPTH) return -1;
+    return (int)d.x;
+}
+
+int64_t key_et_n(const int32_t *key)
+{
+    const Seed v = key_slot(key, SLOT_N);
+    const int depth = key_et_depth(key);
+    if (depth < 0 || v.y || v.z || v.w) return -1;
+    if ((int64_t)v.x != ((int64_t)1 << (depth + ET_LOG2_ROWS_PER_LEAF))) return -1;
+    return (int64_t)v.x;
+}
+
 namespace {
 
 template <class Rng>
@@ -279,6 +314,34 @@ int gen_secure(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int
     return gen_with(rng, alpha, n, prf_id, key_a, key_b);
 }
 
+int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
+{
+    if (n < 8 || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0 || alpha < 0 || alpha >= n) return -1;
+    if (prf_id < PRF_DUMMY || prf_id > PRF_AES128) return -1;
+    int depth = 0;
+    while (((int64_t)1 << (depth + ET_LOG2_ROWS_PER_LEAF)) < n) depth++;
+
+    ChaCha20Rng rng(seed, seed + 32);
+    KeyBuilder<ChaCha20Rng> kb{depth, alpha >> ET_LOG2_ROWS_PER_LEAF, prf_id, rng, {}, {}, 0, 0};
+    kb.lanes = true;
+    std::memset(kb.cw1, 0, sizeof kb.cw1);
+    std::memset(kb.cw2, 0, sizeof kb.cw2);
+    kb.build(0, (u128)1 << (32 * (alpha & 3)));   /* beta = unit vector of lane alpha & 3 */
+
+    for (int srv = 0; srv < 2; srv++) {
+        int32_t *key = srv ? key_b : key_a;
+        std::memset(key, 0, sizeof(int32_t) * KEY_WORDS);
+        set_slot(key, SLOT_DEPTH, (u128)depth | ((u128)ET_LOG2_ROWS_PER_LEAF << 32));
+        for (int i = 0; i < 64; i++) {
+            set_slot(key, SLOT_CW1 + i, kb.cw1[i]);
+            set_slot(key, SLOT_CW2 + i, kb.cw2[i]);
+        }
+        set_slot(key, SLOT_ROOT, srv ? kb.root_b : kb.root_a);
+        set_slot(key, SLOT_N, (u128)n);
+    }
+    return 0;
+}
+
 namespace {
 
 /* per-key storage for the CPU traversal */
@@ -311,9 +374,17 @@ struct CpuEnv {
         out[bitrev(base_pos + local_pos, depth)] = (int32_t)v0;
         out[bitrev(base_pos + local_pos + 1, depth)] = (int32_t)v1;
     }
+    void leaf_quads(uint32_t local_pos, const Seed &w0, const Seed &w1)
+    {
+        /* early-terminated: leaf position p holds leaf bitrev_depth(p), whose word l is row 4 * leaf + l */
+        int32_t *o0 = out + 4 * (size_t)bitrev(base_pos + local_pos, depth);
+        int32_t *o1 = out + 4 * (size_t)bitrev(base_pos + local_pos + 1, depth);
+        o0[0] = (int32_t)w0.x; o0[1] = (int32_t)w0.y; o0[2] = (int32_t)w0.z; o0[3] = (int32_t)w0.w;
+        o1[0] = (int32_t)w1.x; o1[1] = (int32_t)w1.y; o1[2] = (int32_t)w1.z; o1[3] = (int32_t)w1.w;
+    }
 };
 
-template <int PRF>
+template <int PRF, bool ET = false>
 void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
 {
     CpuEnv env;
@@ -327,7 +398,7 @@ void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
     for (uint32_t q = 0; q < nsub; q++) {
         env.base_pos = q << s;
         const Seed r = walk_down<PRF>(env, key_slot(key, SLOT_ROOT), depth - 1, depth - s, q);
-        eval_subtree<PRF, false>(env, r, s, 0);
+        eval_subtree<PRF, false, CpuEnv, ET>(env, r, s, 0);
     }
 }
 
@@ -342,6 +413,20 @@ int eval_cpu(const int32_t *key, int prf_id, int32_t *out_n)
     case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20>(key, depth, out_n); break;
     case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20>(key, depth, out_n); break;
     case PRF_AES128: eval_cpu_impl<PRF_AES128>(key, depth, out_n); break;
+    default: return -1;
+    }
+    return 0;
+}
+
+int eval_cpu_et(const int32_t *key, int prf_id, int32_t *out_n)
+{
+    const int depth = key_et_depth(key);
+    if (depth < 1 || key_et_n(key) < 0) return -1;
+    switch (prf_id) {
+    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, true>(key, depth, out_n); break;
+    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, true>(key, depth, out_n); break;
+    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, true>(key, depth, out_n); break;
+    case PRF_AES128: eval_cpu_impl<PRF_AES128, true>(key, depth, out_n); break;
     default: return -1;
     }
     return 0;

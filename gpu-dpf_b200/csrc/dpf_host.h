@@ -34,10 +34,21 @@ inline Seed key_slot(const int32_t *key, int slot)
 int key_depth(const int32_t *key);
 int64_t key_n(const int32_t *key);
 
+/* Early-terminated keys (DESIGN.md section 9): a tree of 2^depth leaves over n = 4 * 2^depth
+ * table rows, slot 0 = (depth, 2, 0, 0), slot 130 = n.  These return the tree depth (1..29)
+ * or n, or -1 for anything else -- a standard key included. */
+enum : int { ET_LOG2_ROWS_PER_LEAF = 2, ET_MAX_DEPTH = 29 };
+int key_et_depth(const int32_t *key);
+int64_t key_et_n(const int32_t *key);
+
 int gen(int64_t alpha, int64_t n, uint32_t seed32, int prf_id, int32_t *key_a, int32_t *key_b);
 /* ChaCha20-DRBG variant: key = seed[0..31], nonce = seed[32..43] */
 int gen_secure(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b);
 int eval_cpu(const int32_t *key, int prf_id, int32_t *out_n);
+/* Early-terminated key for row alpha of an n-row table (8 <= n <= 2^31, a power of two), drawn
+ * from the ChaCha20 DRBG like gen_secure; eval_cpu_et writes its share of all n rows. */
+int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b);
+int eval_cpu_et(const int32_t *key, int prf_id, int32_t *out_n);
 
 }  // namespace host
 }  // namespace b200dpf

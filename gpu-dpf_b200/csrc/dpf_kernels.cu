@@ -170,7 +170,12 @@ struct DevEnv {
         const uint4 v = *slot(h);
         return make_seed(v.x, v.y, v.z, v.w);
     }
-    static constexpr bool MAC = (MODE == MODE_FUSED || MODE == MODE_GROUPED || MODE == MODE_FUSED_TMA);   /* leaves feed the inner product */
+    static constexpr bool MAC = (MODE == MODE_FUSED || MODE == MODE_GROUPED || MODE == MODE_FUSED_TMA ||
+                                 MODE == MODE_FUSED_ET);   /* leaves feed the inner product */
+    static constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);   /* four rows per leaf */
+    /* ET prefetches the first row pair before the leaf expansion at 16 columns only: at 32, rows held
+     * across the full-width expansion (or two rows in flight beside the next two) spill */
+    static constexpr bool ET_PREFETCH = ET && NV == 4;
     static constexpr bool STAGED = (MODE == MODE_FUSED_TMA);
     /* STAGED: the work item's 2^s rows were requested with one cp.async.bulk when the item was drawn;
      * they are first needed s-1 node expansions later, which hides the copy */
@@ -192,12 +197,90 @@ struct DevEnv {
             for (int j = 0; j < 4; j++) ra[j] = r[j];
 #pragma unroll
             for (int j = 0; j < 4; j++) rb[j] = r[4 + j];
-        } else if (MAC) {
+        } else if (MAC && ET_PREFETCH) {
+            /* the first 64 bytes of the two rows multiplied first: lane 0 of both leaves */
+            const uint4 *r = rows + (size_t)local_pos * 4 * row_stride_v;
+#pragma unroll
+            for (int j = 0; j < 4; j++) ra[j] = __ldg(r + j);
+#pragma unroll
+            for (int j = 0; j < 4; j++) rb[j] = __ldg(r + 4 * row_stride_v + j);
+        } else if (MAC && !ET) {
             const uint4 *r = rows + (size_t)local_pos * row_stride_v;
 #pragma unroll
             for (int j = 0; j < 4; j++) ra[j] = __ldg(r + j);
 #pragma unroll
             for (int j = 0; j < 4; j++) rb[j] = __ldg(r + row_stride_v + j);
+        }
+    }
+    /* ET: leaves local_pos and local_pos + 1 with their four row shares each, against rows 4 local_pos ..
+     * 4 local_pos + 7 */
+    __device__ __forceinline__ void leaf_quads(uint32_t local_pos, const Seed &w0, const Seed &w1)
+    {
+        const uint32_t a[4] = {w0.x, w0.y, w0.z, w0.w}, b[4] = {w1.x, w1.y, w1.z, w1.w};
+        if (MAC) {
+            if (leaf_out != nullptr) {   /* coalesced: 32 keys x 4 bytes per row */
+#pragma unroll
+                for (int l = 0; l < 4; l++) {
+                    leaf_out[((size_t)local_pos * 4 + l) * 32] = a[l];
+                    leaf_out[((size_t)local_pos * 4 + 4 + l) * 32] = b[l];
+                }
+            }
+            const uint4 *r0 = rows + (size_t)local_pos * 4 * row_stride_v;
+            if constexpr (ET_PREFETCH) {
+                /* 16 columns: rows in pairs (4 local_pos + l, 4 local_pos + 4 + l), the first pair prefetched
+                 * by leaf_prefetch, the next pair's loads issued before the current one is multiplied */
+#pragma unroll
+                for (int l = 0; l < 4; l++) {
+                    uint4 na[4], nb[4];
+                    if (l + 1 < 4) {
+                        const uint4 *r = r0 + (size_t)(l + 1) * row_stride_v;
+#pragma unroll
+                        for (int j = 0; j < 4; j++) na[j] = __ldg(r + j);
+#pragma unroll
+                        for (int j = 0; j < 4; j++) nb[j] = __ldg(r + 4 * row_stride_v + j);
+                    }
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        acc[4 * j + 0] += a[l] * ra[j].x + b[l] * rb[j].x;
+                        acc[4 * j + 1] += a[l] * ra[j].y + b[l] * rb[j].y;
+                        acc[4 * j + 2] += a[l] * ra[j].z + b[l] * rb[j].z;
+                        acc[4 * j + 3] += a[l] * ra[j].w + b[l] * rb[j].w;
+                    }
+                    if (l + 1 < 4) {
+#pragma unroll
+                        for (int j = 0; j < 4; j++) { ra[j] = na[j]; rb[j] = nb[j]; }
+                    }
+                }
+            } else {
+                /* 32 columns: one whole row per step, the row loop kept rolled (unrolled, the compiler
+                 * hoists the loads of several rows and spills) */
+#pragma unroll 1
+                for (int row = 0; row < 8; row++) {
+                    const uint4 *r = r0 + (size_t)row * row_stride_v;
+                    uint4 t[NV];
+#pragma unroll
+                    for (int j = 0; j < NV; j++) t[j] = __ldg(r + j);
+                    const uint32_t v = row == 0 ? a[0] : row == 1 ? a[1] : row == 2 ? a[2] : row == 3 ? a[3]
+                                     : row == 4 ? b[0] : row == 5 ? b[1] : row == 6 ? b[2] : b[3];
+#pragma unroll
+                    for (int j = 0; j < NV; j++) {
+                        acc[4 * j + 0] += v * t[j].x;
+                        acc[4 * j + 1] += v * t[j].y;
+                        acc[4 * j + 2] += v * t[j].z;
+                        acc[4 * j + 3] += v * t[j].w;
+                    }
+                }
+            }
+        } else if (MODE == MODE_EXPAND_ET && key_valid) {
+            /* leaf position p holds leaf bitrev_depth(p), whose word l is the share of row 4 * leaf + l */
+            const uint32_t p = pos_base + local_pos;
+            uint32_t *o0 = share_row + 4 * (size_t)(__brev(p) >> (32 - depth));
+            uint32_t *o1 = share_row + 4 * (size_t)(__brev(p + 1) >> (32 - depth));
+#pragma unroll
+            for (int l = 0; l < 4; l++) {   /* the caller's buffer need not be 16-byte aligned */
+                o0[l] = a[l];
+                o1[l] = b[l];
+            }
         }
     }
     __device__ __forceinline__ void leaf_pair(uint32_t local_pos, uint32_t v0, uint32_t v1)
@@ -330,6 +413,9 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
     }
 
     constexpr bool GROUPED = (MODE == MODE_GROUPED);
+    constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);
+    constexpr bool FUSED = (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || MODE == MODE_FUSED_ET || GROUPED);
+    constexpr int ROW_SHIFT = ET ? 2 : 0;   /* log2 table rows per leaf */
     uint32_t taken = 0;
     for (int j = 0; j < p.key_groups; j++) {
         const int kg = (int)((blockIdx.x + (unsigned)j) % (unsigned)p.key_groups);
@@ -383,10 +469,10 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 
         const int key = g_key_first + kslot;
         env.key_valid = key <= g_key_last;
-        if (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || GROUPED) {
+        if (FUSED) {
 #pragma unroll
             for (int e = 0; e < 4 * NV; e++) env.acc[e] = 0;
-        } else if (MODE == MODE_EXPAND) {
+        } else if (MODE == MODE_EXPAND || MODE == MODE_EXPAND_ET) {
             env.share_row = p.shares + (size_t)(env.key_valid ? key : 0) * p.n;
         }
         const uint4 rv = root_s[kslot];
@@ -432,7 +518,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                 env.front_out = p.frontier_out + ((size_t)kg * p.nfront + ((size_t)q << g_s)) * kpw + kslot;
                 eval_subtree<PRF, true>(env, r, g_s, ph.level_base);
             } else {
-                env.rows = g_table + ((size_t)q << g_s) * p.row_stride_v + p.col_off_v;
+                env.rows = g_table + ((size_t)q << (g_s + ROW_SHIFT)) * p.row_stride_v + p.col_off_v;
                 if constexpr (MODE == MODE_FUSED_TMA) {
                     /* the item's rows are one contiguous run (64-byte rows, breadth-first leaf order) */
                     __syncwarp();                                   /* every lane is done with the previous tile */
@@ -445,15 +531,15 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                     env.tile_pending = true;
                 }
                 env.pos_base = (ph.sub_first + q) << g_s;
-                env.leaf_out = (!GROUPED && p.leaf_cache) ? p.leaf_cache + ((size_t)kg * p.n_local + ((size_t)q << g_s)) * 32 + lane
+                env.leaf_out = (!GROUPED && p.leaf_cache) ? p.leaf_cache + ((size_t)kg * p.n_local + ((size_t)q << (g_s + ROW_SHIFT))) * 32 + lane
                                                           : nullptr;
-                eval_subtree<PRF, false>(env, r, g_s, 0);
+                eval_subtree<PRF, false, decltype(env), ET>(env, r, g_s, 0);
             }
           }
             if (!ahead && draw && lane == 0) t_raw = atomicAdd(ph.counters + kg, chunk);
         }
 
-        if (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || GROUPED) {
+        if (FUSED) {
             /* lanes that hold the same key (different subtree slots) fold their partial sums
              * first, so every key receives one red.add per warp and column, not 32/kpw */
             for (int off = kpw; off < 32; off <<= 1) {
@@ -743,6 +829,37 @@ __global__ void permute_table_kernel(const int32_t *__restrict__ stage, int32_t 
 
 __device__ __forceinline__ uint32_t bitrev_bits(uint32_t v, int bits) { return bits ? __brev(v) >> (32 - bits) : 0u; }
 
+/* early-terminated table: runs of four rows (one leaf) move together, table[4q + l] = stage[4 bitrev(q) + l] */
+__global__ void permute_table_et_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table,
+                                        uint64_t rows, int bits, int cols, int stride)
+{
+    const uint64_t total = rows * (uint64_t)cols;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+         i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t q = i / (uint64_t)cols;
+        const int c = (int)(i - q * (uint64_t)cols);
+        const uint64_t src = ((uint64_t)bitrev_bits((uint32_t)(q >> 2), bits) << 2) | (q & 3u);
+        table[q * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
+    }
+}
+
+/* row update of an early-terminated context, step 1 (UpdateParams::lane_bits = 2) */
+__global__ void __launch_bounds__(256) update_map_et_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
+                                                            uint32_t *__restrict__ ord)
+{
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = u.idx[j];
+        uint32_t p = u.table_rows;
+        if (i >= 0 && i < u.n) {
+            const uint32_t leaf = (uint32_t)(i >> u.lane_bits);
+            if ((leaf & u.own_mask) == u.own_val)
+                p = (bitrev_bits(leaf >> u.shift, u.depth) << u.lane_bits) | ((uint32_t)i & ((1u << u.lane_bits) - 1u));
+        }
+        pos[j] = p;
+        ord[j] = (uint32_t)j;
+    }
+}
+
 /* row update, step 1: natural index -> table row (or the skip marker), occurrence number j */
 __global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
                                                          uint32_t *__restrict__ ord)
@@ -829,12 +946,18 @@ cudaError_t max_smem_one(int *bytes)
     return cudaSuccess;
 }
 
-/* (prf, nv, mode) -> instantiation; modes 1 and 2 never touch the table, so NV = 4 only; grouped
- * evaluation takes 16 columns per pass */
+/* (prf, nv, mode) -> instantiation; modes 1, 2 and 6 never touch the table, so NV = 4 only; grouped
+ * evaluation takes 16 columns per pass, early-terminated evaluation 16 or 32 */
 template <int PRF>
 cudaError_t launch_prf(int nv, int mode, const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
 {
     if (mode == MODE_EXPAND) return launch_one<PRF, 4, MODE_EXPAND>(p, grid, smem, stream);
+    if (mode == MODE_EXPAND_ET) return launch_one<PRF, 4, MODE_EXPAND_ET>(p, grid, smem, stream);
+    if (mode == MODE_FUSED_ET) {
+        if (nv == 4) return launch_one<PRF, 4, MODE_FUSED_ET>(p, grid, smem, stream);
+        if (nv == 8) return launch_one<PRF, 8, MODE_FUSED_ET>(p, grid, smem, stream);
+        return cudaErrorInvalidValue;
+    }
     if (mode == MODE_FRONTIER) return launch_one<PRF, 4, MODE_FRONTIER>(p, grid, smem, stream);
     if (mode == MODE_GROUPED) return launch_one<PRF, 4, MODE_GROUPED>(p, grid, smem, stream);
     if (mode == MODE_FUSED_TMA) {
@@ -851,6 +974,12 @@ template <int PRF>
 cudaError_t max_smem_prf(int nv, int mode, int *bytes)
 {
     if (mode == MODE_EXPAND) return max_smem_one<PRF, 4, MODE_EXPAND>(bytes);
+    if (mode == MODE_EXPAND_ET) return max_smem_one<PRF, 4, MODE_EXPAND_ET>(bytes);
+    if (mode == MODE_FUSED_ET) {
+        if (nv == 4) return max_smem_one<PRF, 4, MODE_FUSED_ET>(bytes);
+        if (nv == 8) return max_smem_one<PRF, 8, MODE_FUSED_ET>(bytes);
+        return cudaErrorInvalidValue;
+    }
     if (mode == MODE_FRONTIER) return max_smem_one<PRF, 4, MODE_FRONTIER>(bytes);
     if (mode == MODE_GROUPED) return max_smem_one<PRF, 4, MODE_GROUPED>(bytes);
     if (mode == MODE_FUSED_TMA) {
@@ -962,6 +1091,17 @@ cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t 
     return cudaGetLastError();
 }
 
+cudaError_t launch_permute_table_et(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
+                                    int cols, int stride, int sm_count, cudaStream_t stream)
+{
+    const uint64_t total = rows * (uint64_t)cols;
+    const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
+    int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
+    if (grid < 1) grid = 1;
+    permute_table_et_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, cols, stride);
+    return cudaGetLastError();
+}
+
 cudaError_t update_temp_bytes(int64_t count, int end_bit, size_t *bytes)
 {
     *bytes = 0;
@@ -974,7 +1114,8 @@ cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int e
     if (u.count <= 0) return cudaSuccess;
     const int64_t cap = (int64_t)std::max(sm_count, 1) * 16;
     const int grid_map = (int)std::max<int64_t>(1, std::min<int64_t>((u.count + 255) / 256, cap));
-    update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    if (u.lane_bits) update_map_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    else update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     size_t temp_bytes = w.temp_bytes;

@@ -110,8 +110,14 @@ struct EvalParams {
 
 /* Kernel modes. */
 enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3,
-       MODE_FUSED_TMA = 4 /* MODE_FUSED with each work item's table rows staged into shared memory by
-                             cp.async.bulk (16-column tables, non-AES PRFs, whole-warp key groups) */ };
+       MODE_FUSED_TMA = 4, /* MODE_FUSED with each work item's table rows staged into shared memory by
+                             cp.async.bulk (16-column tables, non-AES PRFs, whole-warp key groups) */
+       /* early-terminated keys (four table rows per leaf): the tree is over leaves, the table, the
+        * leaf cache (EvalParams::n_local), the result and the shares (EvalParams::n) over rows; leaf
+        * position p owns rows 4p..4p+3 of the device table */
+       MODE_FUSED_ET = 5,  /* MODE_FUSED, nv = 4 or 8 */
+       MODE_EXPAND_ET = 6, /* MODE_EXPAND: shares[key][4 * leaf + lane] */
+       MODE_COUNT = 7 };
 
 /* Threads per block / minimum blocks per SM of the kernel instantiated for
  * (prf, nv) where nv = uint4 (4 int32 columns) of a table row handled per pass:
@@ -169,9 +175,12 @@ cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
 /* table[q][c] = stage[bitrev_bits(q)][c] for q < rows, c < cols; padded columns
  * [cols, stride) are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM
- * count to cap their grids at a few waves. */
+ * count to cap their grids at a few waves.  With lane_bits = 2 (early-terminated contexts) rows
+ * move in runs of four: table[4q + l] = stage[4 bitrev_bits(q) + l], rows = 4 * 2^bits. */
 cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
                                  int cols, int stride, int sm_count, cudaStream_t stream);
+cudaError_t launch_permute_table_et(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
+                                    int cols, int stride, int sm_count, cudaStream_t stream);
 
 /* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
  * j < count, the last occurrence of a position winning.  Position of natural index i:
@@ -191,6 +200,11 @@ struct UpdateParams {
     uint32_t own_mask, own_val;
     int shift, depth;
     uint32_t table_rows;      /* rows of the device table: the skip marker, larger than every position */
+    int lane_bits;            /* log2 rows per leaf: 0, or 2 on an early-terminated context, where
+                                 row i < n belongs to leaf v = i >> 2, is owned when (v & own_mask)
+                                 == own_val and goes to row 4 bitrev_depth(v >> shift) + (i & 3).
+                                 (It fills the alignment gap before `table`: the struct's layout is
+                                 that of the update kernels without it.)                          */
     int32_t *table;           /* [table_rows][stride], 64-byte rows; pad columns are not touched */
     int cols, stride;
 };

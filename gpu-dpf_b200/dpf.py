@@ -56,7 +56,8 @@ class DPF(object):
         dpf_cpp.PRF_AES128: "AES128",
     }
 
-    def __init__(self, prf=None, device=0, shard=(0, 1), allow_non_pow2=False, devices=None, axis="auto"):
+    def __init__(self, prf=None, device=0, shard=(0, 1), allow_non_pow2=False, devices=None, axis="auto",
+                 early_termination=False):
         # devices: None (one GPU: `device`), "all", or a list of device ids -- one process drives them all
         # (b200dpf_create_multi); axis "auto" | "entries" | "keys".  B200DPF_DEVICES / B200DPF_AXIS in the
         # environment set the defaults, so an unchanged `dpf.DPF()` caller (benchmark.py) can scale too.
@@ -82,6 +83,12 @@ class DPF(object):
         self.shard = tuple(shard)
         self.prf_method = prf if prf is not None else self.DEFAULT_PRF
         self.prf_method_string = self._PRF_NAMES[self.prf_method]
+        # early_termination: keys whose leaves carry four table rows each (include/b200dpf.h, b200dpf_gen_et):
+        # about a quarter of the tree to expand.  Keys of the two kinds are not interchangeable.
+        self.early_termination = bool(early_termination)
+        if self.early_termination and self.devices:
+            raise Exception("early_termination=True has no multi-device variant: use one device per DPF "
+                            "(DPF(device=d, shard=(rank, count), early_termination=True))")
 
     # ---- client -----------------------------------------------------------
     def gen(self, k, n, seed=None, secure=None):
@@ -93,6 +100,8 @@ class DPF(object):
         generator states of a key it holds and recover the index: that generator is kept only
         for callers that pass an explicit `seed` (deterministic keys, bit-identical to the
         reference's for the same seed: golden and parity tests) and do not ask for secure=True."""
+        if self.early_termination:
+            return self._gen_et(k, n, seed, secure)
         if secure is None:
             secure = seed is None
         if seed is None:
@@ -107,10 +116,35 @@ class DPF(object):
             return dpf_cpp.gen_secure(k, n, seed, self.prf_method)
         return dpf_cpp.gen(k, n, seed, self.prf_method)
 
+    def _gen_et(self, k, n, seed, secure):
+        # early-terminated keys draw from the ChaCha20 DRBG only: explicit seeds are >= 44 bytes
+        if secure is False:
+            raise Exception("early-terminated keys have no secure=False generator: pass >= 44 seed bytes or none")
+        if seed is None:
+            seed = os.urandom(44)
+        if not isinstance(seed, (bytes, bytearray)) or len(seed) < 44:
+            raise Exception("early-terminated keys take a seed of at least 44 bytes")
+        if n & (n - 1) != 0 and not self.allow_non_pow2:
+            raise Exception("Table num entries (%d) must be a power of two" % (n))
+        if k >= n:
+            raise Exception("k (%d), the selected element, must be less than n (%d), the number of entries in the table"
+                            % (k, n))
+        return dpf_cpp.gen_et(k, _next_pow2(n), bytes(seed), self.prf_method)
+
     def gen_batch(self, indices, n, seeds=None, nthreads=0):
         """Keys for many indices at once: two int32 [B, 524] tensors (multi-threaded keygen).
         seeds=None: ChaCha20-DRBG keys from os.urandom entropy (44 bytes per key); explicit integer
-        seeds select the reference's 32-bit mt19937 generator (deterministic, for tests)."""
+        seeds select the reference's 32-bit mt19937 generator (deterministic, for tests).  With
+        early_termination, explicit seeds are bytes: 44 per key, concatenated."""
+        if self.early_termination:
+            if n & (n - 1) != 0:
+                raise Exception("Table num entries (%d) must be a power of two" % (n))
+            idx = torch.as_tensor(list(indices), dtype=torch.int64)
+            if seeds is None:
+                seeds = os.urandom(44 * idx.numel())
+            if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * idx.numel():
+                raise Exception("early-terminated gen_batch takes seeds as bytes, 44 per key")
+            return dpf_cpp.gen_batch_et(idx, n, bytes(seeds), self.prf_method, nthreads)
         if n & (n - 1) != 0:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
         idx = torch.as_tensor(list(indices), dtype=torch.int64)
@@ -124,11 +158,12 @@ class DPF(object):
     # ---- server -----------------------------------------------------------
     def eval_cpu(self, keys, one_hot_only=False):
         """CPU evaluation (dpf.py:76-86): share vectors, or shares @ table."""
+        eval_one = dpf_cpp.eval_cpu_et if self.early_termination else dpf_cpp.eval_cpu
         if one_hot_only:
-            return torch.stack([dpf_cpp.eval_cpu(k, self.prf_method) for k in keys])
+            return torch.stack([eval_one(k, self.prf_method) for k in keys])
         if self.table is None:
             raise Exception("Must call `eval_init` before `eval_cpu` with one_hot_only=False")
-        one_hots = torch.stack([dpf_cpp.eval_cpu(k, self.prf_method) for k in keys])
+        one_hots = torch.stack([eval_one(k, self.prf_method) for k in keys])
         return torch.matmul(one_hots, self.table)
 
     def eval_init(self, table):
@@ -150,7 +185,9 @@ class DPF(object):
         self.table = table
         self.table_num_entries = table.shape[0]
         self.table_effective_entry_size = table.shape[1]
-        if self.devices:
+        if self.early_termination:
+            self.buffers = dpf_cpp.eval_init_et(table, self.device, self.shard[0], self.shard[1])
+        elif self.devices:
             self.buffers = dpf_cpp.eval_init_multi(table, self.devices, {"auto": 0, "entries": 1, "keys": 2}[self.axis])
         else:
             self.buffers = dpf_cpp.eval_init_sharded(table, self.device, self.shard[0], self.shard[1])
@@ -211,7 +248,8 @@ class DPF(object):
     def pack_keys(self, keys):
         """Compact wire form of a batch (24% to 56% smaller than int32[524] keys, depending on n): one
         contiguous uint8 tensor [B, 32 + 64*depth], pinned when CUDA is available, for eval_gpu_compact."""
-        blobs = [dpf_cpp.key_pack(k) for k in keys]
+        pack = dpf_cpp.key_pack_et if self.early_termination else dpf_cpp.key_pack
+        blobs = [pack(k) for k in keys]
         t = torch.frombuffer(bytearray(b"".join(blobs)), dtype=torch.uint8).reshape(len(blobs), -1)
         return t.pin_memory() if torch.cuda.is_available() else t
 
@@ -333,6 +371,11 @@ class BinnedDPF(DPF):
         k1, k2 = d.gen_in_bin(g, index)          # keys for entry `index` of bin g
         shares = d.eval_gpu(keys, bins)          # int32 [len(keys), entry_size]
     """
+
+    def __init__(self, *args, **kwargs):
+        if kwargs.get("early_termination"):
+            raise Exception("BinnedDPF has no early-terminated variant (early_termination=True)")
+        super().__init__(*args, **kwargs)
 
     def eval_init(self, tables):
         if self.buffers is not None:

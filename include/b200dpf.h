@@ -368,6 +368,56 @@ int b200dpf_ctx_set_option(b200dpf_ctx *ctx, const char *name, int value);
  */
 int b200dpf_ctx_read_timing(b200dpf_ctx *ctx, uint64_t *stamps, int max_blocks, int *nblocks);
 
+/* ------------------------------------------------------------------------------------------- */
+/* Early-terminated keys: four table rows per GGM leaf (DESIGN.md section 9).                   */
+/* ------------------------------------------------------------------------------------------- */
+/*
+ * A leaf's 128-bit output is four 32-bit shares, one per table row, so a DPF over n rows walks a
+ * tree of n/4 leaves: about a quarter of the PRF work of a standard key.  Row i is word (i & 3) of
+ * leaf i >> 2.  The result is defined as for standard keys: out[b][e] = sum_i share_b[i] *
+ * table[i][e] mod 2^32, so the two servers' results differ by table[alpha].
+ *
+ * The key is the int32[524] wire format with slot 0 = (d, 2, 0, 0) (d = log2(n) - 2 tree levels;
+ * word 1 = log2 rows per leaf) and slot 130 = n.  Level-0 correction words are added lane-wise in
+ * (Z/2^32)^4.  Every standard entry point refuses such a key (b200dpf_key_n / _key_depth return
+ * -1, the others EINVAL), and the functions below refuse standard keys.  Evaluation uses the
+ * standard entry points on a context made by b200dpf_create_et.
+ */
+
+/* Keys for row alpha of an n-row table, 8 <= n <= 2^31 a power of two.  Every draw comes from the
+ * ChaCha20 DRBG of b200dpf_gen_secure; seed_len must be >= 44. */
+int b200dpf_gen_et(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf,
+                   int32_t *key_a, int32_t *key_b);
+
+/* Batched b200dpf_gen_et on `nthreads` host threads (0 = one per hardware thread): seeds44 = count x
+ * 44 bytes; keys_a/keys_b: int32[count][524].  Identical keys for any nthreads. */
+int b200dpf_gen_batch_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
+                         int nthreads, int32_t *keys_a, int32_t *keys_b);
+
+/* One server's share of every row on the CPU, natural order: out[i], i < n (n read from the key). */
+int b200dpf_eval_cpu_et(const int32_t *key, int prf, int32_t *out_n);
+
+/* Compact form: the layout and size (b200dpf_key_packed_size(d) = 32 + 64*d) of b200dpf_key_pack,
+ * magic "DPE4".  b200dpf_key_unpack and b200dpf_eval_packed on a standard context refuse it. */
+int b200dpf_key_pack_et(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written);
+int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key);
+
+/*
+ * A context for early-terminated keys, arguments as b200dpf_create with n >= 8 and shard_count a
+ * power of two <= n/8.  The device table keeps each leaf's four rows together: row 4p + l holds
+ * natural row 4*bitrev(p) + l.  Shard (r, G) owns the leaves of breadth-first subtree r, i.e. row i
+ * iff ((i >> 2) & (G-1)) == bitrev_g(r).  b200dpf_eval, _eval_gather, _eval_packed ("DPE4" keys),
+ * _host_staging, _eval_device, _eval_device_acc, _expand_device, _update_rows, _update_rows_device,
+ * _ctx_set_option and the introspection functions work on it as on a standard context (ctx_n counts
+ * rows); the host paths return EINVAL for a standard key before copying anything.  The "tma_rows"
+ * option has no effect here.  There is no multi-device or grouped variant.
+ */
+int b200dpf_create_et(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
+                      int device, int shard_rank, int shard_count);
+
+/* Table rows per tree leaf: 4 on a context of b200dpf_create_et, 1 otherwise; -1 for null. */
+int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *ctx);
+
 #ifdef __cplusplus
 }
 #endif
