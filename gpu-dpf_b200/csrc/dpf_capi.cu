@@ -203,7 +203,9 @@ struct SmemLayout {
     int threads, blocks_per_sm, grid;
     int budget;               /* dynamic shared memory one block may use */
     size_t smem_fixed;        /* AES: whole budget; others: computed from s */
-    uint32_t off_meta, off_lo, off_hi, off_tab, meta_cw, level_bytes;
+    uint32_t off_meta;        /* correction words, meta_cw bytes                          */
+    uint32_t off_small;       /* level-0 low words, root seeds and flag (kMetaSmall bytes) */
+    uint32_t off_lo, off_hi, off_tab, meta_cw, level_bytes;
     int cap_lo, cap_hi, s_max;
 };
 
@@ -252,7 +254,8 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
     L->budget = budget;
 
     L->meta_cw = (uint32_t)c->depth * 4u * 32u * 16u;
-    const uint32_t meta = L->meta_cw + 512u + 512u + 16u;
+    const uint32_t kMetaSmall = 512u + 512u + 16u;
+    const uint32_t meta = L->meta_cw + kMetaSmall;
     L->level_bytes = (uint32_t)L->threads * 16u;
     if (prf == B200DPF_PRF_AES128) {
         /* tables: 128 KiB whose shared-window address is 64 KiB aligned */
@@ -264,8 +267,13 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
         const uint32_t b_size = (uint32_t)budget - b_off;
         L->off_tab = off_tab;
         uint32_t a_used = 0, b_used = 0;
-        if (meta <= a_size) { L->off_meta = 0; a_used = meta; }
-        else if (meta <= b_size) { L->off_meta = b_off; b_used = meta; }
+        if (meta <= a_size) { L->off_meta = 0; L->off_small = L->meta_cw; a_used = meta; }
+        else if (meta <= b_size) { L->off_meta = b_off; L->off_small = b_off + L->meta_cw; b_used = meta; }
+        else if (L->meta_cw <= a_size && kMetaSmall <= b_size) {
+            /* depth 31: the correction words alone fill region A, so the rest goes after the tables */
+            L->off_meta = 0; a_used = L->meta_cw;
+            L->off_small = b_off; b_used = kMetaSmall;
+        }
         else return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->depth);
         a_used = (a_used + 15u) & ~15u;
         b_used = (b_used + 15u) & ~15u;
@@ -276,6 +284,7 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
         L->smem_fixed = (size_t)budget;
     } else {
         L->off_meta = 0;
+        L->off_small = L->meta_cw;
         L->off_lo = (meta + 15u) & ~15u;
         if ((int64_t)budget < (int64_t)L->off_lo) return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->depth);
         L->cap_lo = (int)(((uint32_t)budget - L->off_lo) / L->level_bytes);
@@ -301,7 +310,7 @@ void fill_common(const b200dpf_ctx *c, const SmemLayout &L, int s, int64_t nkeys
     p->out_stride = (uint32_t)c->entry_size;
     p->n = (uint64_t)c->n;
     p->off_cw = L.off_meta;
-    p->off_cwlo = L.off_meta + L.meta_cw;
+    p->off_cwlo = L.off_small;
     p->off_root = p->off_cwlo + 512u;
     p->off_flag = p->off_root + 512u;
     p->off_stack_lo = L.off_lo;

@@ -11,6 +11,7 @@
  */
 #include "dpf_oracle.h"
 
+#include <pthread.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -256,6 +257,86 @@ void orc_eval_flat(const int32_t *key, int64_t idx, int prf,
     u128 r = eval_flat(key, idx, prf);
     *out_lo = (uint64_t)r;
     *out_hi = (uint64_t)(r >> 64);
+}
+
+/* An early-terminated key (slot 0 = (d, 2, 0, 0)): the same walk over the d levels of leaf `leaf`,
+ * except that the level-0 correction word is added lane-wise in (Z/2^32)^4 (DESIGN.md section 9). */
+static void eval_flat_et(const int32_t *key, int64_t leaf, int prf, uint32_t out[4])
+{
+    int depth = key[0];
+    u128 s = key_slot(key, SLOT_ROOT);
+    for (int level = depth - 1; level >= 0; level--) {
+        int bit = (int)(leaf & 1);
+        int bank = (s & 1) ? SLOT_CW2 : SLOT_CW1;
+        u128 v = prf_eval(prf, s, (uint32_t)bit), cw = key_slot(key, bank + 2 * level + bit);
+        if (level > 0) {
+            s = v + cw;
+        } else {
+            s = 0;
+            for (int l = 0; l < 4; l++)
+                s |= (u128)(uint32_t)((uint32_t)(v >> (32 * l)) + (uint32_t)(cw >> (32 * l))) << (32 * l);
+        }
+        leaf >>= 1;
+    }
+    for (int l = 0; l < 4; l++) out[l] = (uint32_t)(s >> (32 * l));
+}
+
+typedef struct {
+    const int32_t *keys;
+    int64_t nkeys, npoints;
+    int prf, et, nthreads, t;
+    const int64_t *points;
+    int32_t *out;
+} points_job;
+
+static void *points_worker(void *arg)
+{
+    const points_job *j = (const points_job *)arg;
+    const int64_t total = j->nkeys * j->npoints;
+    for (int64_t w = j->t; w < total; w += j->nthreads) {
+        const int32_t *key = j->keys + (w / j->npoints) * ORC_KEY_WORDS;
+        const int64_t x = j->points[w % j->npoints];
+        if (j->et) {
+            eval_flat_et(key, x, j->prf, (uint32_t *)j->out + 4 * w);
+        } else {
+            j->out[w] = (int32_t)(uint32_t)eval_flat(key, x, j->prf);
+        }
+    }
+    return NULL;
+}
+
+static int eval_points(const int32_t *keys, int64_t nkeys, int prf, const int64_t *points, int64_t npoints,
+                       int nthreads, int et, int32_t *out)
+{
+    if (nkeys < 0 || npoints < 0 || prf < 0 || prf > 3) return -1;
+    if (nthreads < 1) nthreads = 1;
+    if (nthreads > 256) nthreads = 256;
+    sbox_init();   /* once, before the threads share it */
+    pthread_t th[256];
+    points_job jobs[256];
+    int started = 0, rc = 0;
+    for (int t = 0; t < nthreads; t++) {
+        jobs[t] = (points_job){ keys, nkeys, npoints, prf, et, nthreads, t, points, out };
+        if (t == 0) continue;
+        if (pthread_create(&th[t], NULL, points_worker, &jobs[t]) != 0) { rc = -3; break; }
+        started = t;
+    }
+    points_worker(&jobs[0]);
+    for (int t = 1; t <= started; t++) pthread_join(th[t], NULL);
+    if (rc) return rc;   /* some share of the work was never done */
+    return 0;
+}
+
+int orc_eval_points(const int32_t *keys, int64_t nkeys, int prf, const int64_t *idx, int64_t nidx,
+                    int nthreads, int32_t *out)
+{
+    return eval_points(keys, nkeys, prf, idx, nidx, nthreads, 0, out);
+}
+
+int orc_eval_points_et(const int32_t *keys, int64_t nkeys, int prf, const int64_t *leaves, int64_t nleaves,
+                       int nthreads, int32_t *out)
+{
+    return eval_points(keys, nkeys, prf, leaves, nleaves, nthreads, 1, out);
 }
 
 int orc_eval_full_flat(const int32_t *key, int prf, int32_t *out_n)

@@ -46,6 +46,19 @@ void orc_aes128_encrypt(const uint8_t key[16], const uint8_t in[16], uint8_t out
 void orc_eval_flat(const int32_t *key, int64_t idx, int prf,
                    uint64_t *out_lo, uint64_t *out_hi);
 
+/* Batched per-index walks for sparse checks at any n: out[b][j] = low32(EvaluateFlat(keys[b], idx[j]))
+ * for nkeys keys (int32[nkeys][524]) and nidx indices, spread over `nthreads` host threads.  Each value
+ * is one root-to-leaf walk (the loop of orc_eval_flat), so the cost is O(nkeys * nidx * depth),
+ * independent of n.  Returns 0, or a negative code (bad argument, a thread that could not start). */
+int orc_eval_points(const int32_t *keys, int64_t nkeys, int prf, const int64_t *idx, int64_t nidx,
+                    int nthreads, int32_t *out);
+
+/* The same for early-terminated keys (slot 0 = (d, 2, 0, 0); DESIGN.md section 9): out[b][j][0..3] =
+ * the four 32-bit words of leaf leaves[j], i.e. the shares of rows 4*leaves[j] .. 4*leaves[j]+3.  Not
+ * pinned against the reference, which has no such keys; tests/et_oracle.py states the same walk. */
+int orc_eval_points_et(const int32_t *keys, int64_t nkeys, int prf, const int64_t *leaves, int64_t nleaves,
+                       int nthreads, int32_t *out);
+
 /* dpf_wrapper.cu:70-84 (eval_dpf_cpu): low 32 bits of EvaluateFlat for every
  * index, natural order, via per-index root-to-leaf walks (n*log n PRFs). */
 int orc_eval_full_flat(const int32_t *key, int prf, int32_t *out_n);

@@ -24,6 +24,7 @@ PRF_DUMMY, PRF_SALSA20, PRF_CHACHA20, PRF_AES128 = 0, 1, 2, 3
 PRF_NAMES = {0: "DUMMY", 1: "SALSA20", 2: "CHACHA20", 3: "AES128"}
 
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
+_i64p = np.ctypeslib.ndpointer(dtype=np.int64, flags="C_CONTIGUOUS")
 
 
 def build(ref=True):
@@ -40,11 +41,18 @@ def _u128(lo, hi):
 class Oracle:
     """Our C restatement."""
 
+    # the newest entry points: a library without them was built from older sources
+    REQUIRED = ("orc_eval_points", "orc_eval_points_et")
+
     def __init__(self):
         path = os.path.join(HERE, "libdpforacle.so")
         if not os.path.exists(path):
             build(ref=False)
         L = self.lib = C.CDLL(path)
+        missing = [s for s in self.REQUIRED if not hasattr(L, s)]
+        if missing:
+            raise RuntimeError("%s is stale (no %s): rebuild it with `make -C %s oracle`"
+                               % (path, ", ".join(missing), HERE))
         u64p = C.POINTER(C.c_uint64)
         L.orc_prf.argtypes = [C.c_int, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
         L.orc_aes128_encrypt.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p]
@@ -58,6 +66,26 @@ class Oracle:
         L.orc_gen.argtypes = [C.c_int64, C.c_int64, C.c_uint32, C.c_int, _i32p, _i32p]
         L.orc_bitrev.argtypes = [C.c_uint32, C.c_int]
         L.orc_bitrev.restype = C.c_uint32
+        for name in self.REQUIRED:
+            getattr(L, name).argtypes = [_i32p, C.c_int64, C.c_int, _i64p, C.c_int64, C.c_int, _i32p]
+
+    def _points(self, fn, keys, prf, points, width, nthreads):
+        keys = np.ascontiguousarray(keys, np.int32).reshape(-1, KEY_WORDS)
+        points = np.ascontiguousarray(points, np.int64).reshape(-1)
+        out = np.zeros((keys.shape[0], points.size * width), np.int32)
+        rc = fn(keys, keys.shape[0], prf, points, points.size, nthreads or os.cpu_count() or 1, out)
+        assert rc == 0, rc
+        return out
+
+    def eval_points(self, keys, prf, idx, nthreads=0):
+        """int32 [B, len(idx)]: low 32 bits of EvaluateFlat(keys[b], idx[j]), one walk per value,
+        on `nthreads` host threads (0 = every core)"""
+        return self._points(self.lib.orc_eval_points, keys, prf, idx, 1, nthreads)
+
+    def eval_points_et(self, keys, prf, leaves, nthreads=0):
+        """early-terminated keys: int32 [B, 4 * len(leaves)], the four words of each leaf in turn
+        (the shares of rows 4 * leaf .. 4 * leaf + 3)"""
+        return self._points(self.lib.orc_eval_points_et, keys, prf, leaves, 4, nthreads)
 
     def prf(self, prf, seed, pos):
         lo, hi = C.c_uint64(), C.c_uint64()
