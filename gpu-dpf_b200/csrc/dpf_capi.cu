@@ -241,7 +241,7 @@ int smem_layout(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L)
 int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L)
 {
     std::memset(L, 0, sizeof *L);
-    L->threads = eval_threads(prf, nv);
+    L->threads = eval_threads(prf, nv, mode);
     L->blocks_per_sm = eval_min_blocks(prf, nv);
     L->grid = c->sm_count * L->blocks_per_sm;
     int max_smem = 0;
@@ -445,16 +445,22 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
                     prf != B200DPF_PRF_AES128 && nkeys >= 17 && !et;
     const int mode_plain = mode_main == MODE_FUSED ? mode_fused : mode_expand;
     int mode_kernel = tma_rows ? MODE_FUSED_TMA : mode_plain;
-    SmemLayout L;
-    int rc = smem_layout(c, prf, nv, mode_kernel, &L);
-    if (rc) return rc;
-    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
     /* keys per warp: a full warp of keys when the batch allows; for small batches the
      * spare lanes take adjacent subtrees of the same keys (single-query latency mode) */
     int kpw_log2 = 5;
     if (K.lane_split != 0)
         while (kpw_log2 > 0 && ((int64_t)1 << (kpw_log2 - 1)) >= nkeys) kpw_log2--;
     int64_t key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
+    /* AES binds the shared-memory data pipe, and a broadcast row load is charged for every lane's copy
+     * of the row: with at least 4 keys per warp, each lane of a key quad loads a quarter of the row and
+     * the quad trades leaf values by SHFL instead (DESIGN.md section 3).  Decided before the layout: the
+     * kernel runs more threads, so its stack holds fewer levels (s_max).  kpw_log2 only grows below. */
+    if (mode_kernel == MODE_FUSED && prf == B200DPF_PRF_AES128 && nv == 4 && kpw_log2 >= 2)
+        mode_kernel = MODE_FUSED_COLSPLIT;
+    SmemLayout L;
+    int rc = smem_layout(c, prf, nv, mode_kernel, &L);
+    if (rc) return rc;
+    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
 
     /* ---- work-item size s and the frontier depth --------------------------------
      * Without a frontier every item re-walks depth-s levels from the root, so items

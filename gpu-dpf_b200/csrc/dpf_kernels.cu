@@ -171,7 +171,10 @@ struct DevEnv {
         return make_seed(v.x, v.y, v.z, v.w);
     }
     static constexpr bool MAC = (MODE == MODE_FUSED || MODE == MODE_GROUPED || MODE == MODE_FUSED_TMA ||
-                                 MODE == MODE_FUSED_ET);   /* leaves feed the inner product */
+                                 MODE == MODE_FUSED_ET || MODE == MODE_FUSED_COLSPLIT);   /* leaves feed the inner product */
+    /* rows points at this lane's 16 bytes of the row; acc[4 j + c] is column 4 (lane & 3) + c of key
+     * kslot ^ j, whose leaf values come from lane ^ j */
+    static constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
     static constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);   /* four rows per leaf */
     /* ET prefetches the first row pair before the leaf expansion at 16 columns only: at 32, rows held
      * across the full-width expansion (or two rows in flight beside the next two) spill */
@@ -197,6 +200,9 @@ struct DevEnv {
             for (int j = 0; j < 4; j++) ra[j] = r[j];
 #pragma unroll
             for (int j = 0; j < 4; j++) rb[j] = r[4 + j];
+        } else if (COLSPLIT) {
+            ra[0] = __ldg(rows + (size_t)local_pos * row_stride_v);
+            rb[0] = __ldg(rows + (size_t)(local_pos + 1) * row_stride_v);
         } else if (MAC && ET_PREFETCH) {
             /* the first 64 bytes of the two rows multiplied first: lane 0 of both leaves */
             const uint4 *r = rows + (size_t)local_pos * 4 * row_stride_v;
@@ -290,6 +296,24 @@ struct DevEnv {
                 leaf_out[(size_t)local_pos * 32] = v0;
                 leaf_out[(size_t)(local_pos + 1) * 32] = v1;
             }
+            if constexpr (COLSPLIT) {
+                uint32_t u0[4], u1[4];
+                u0[0] = v0;
+                u1[0] = v1;
+#pragma unroll
+                for (int j = 1; j < 4; j++) {
+                    u0[j] = __shfl_xor_sync(0xffffffffu, v0, j);
+                    u1[j] = __shfl_xor_sync(0xffffffffu, v1, j);
+                }
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    acc[4 * j + 0] += u0[j] * ra[0].x + u1[j] * rb[0].x;
+                    acc[4 * j + 1] += u0[j] * ra[0].y + u1[j] * rb[0].y;
+                    acc[4 * j + 2] += u0[j] * ra[0].z + u1[j] * rb[0].z;
+                    acc[4 * j + 3] += u0[j] * ra[0].w + u1[j] * rb[0].w;
+                }
+                return;
+            }
             const uint4 *r = rows + (size_t)local_pos * row_stride_v;
 #pragma unroll
             for (int c = 0; c < NV / 4; c++) {
@@ -335,6 +359,9 @@ template <int PRF, int NV> struct KernelShape { enum { THREADS = (NV <= 8 ? 256 
 #define DPF_AES_THREADS 384      /* 12 warps: on an H100 1.5 % (n=2^20) and 3 % (n=2^16) faster than 8 (256) */
 #endif
 template <int NV> struct KernelShape<PRF_AES128, NV> { enum { THREADS = (NV <= 8 ? DPF_AES_THREADS : 256), MIN_BLOCKS = 1 }; };
+/* the column-split AES kernel holds 4 row words per leaf instead of 16 and fits 128 registers: 16 warps */
+template <int PRF, int NV, int MODE> struct EvalShape : KernelShape<PRF, NV> {};
+template <> struct EvalShape<PRF_AES128, 4, MODE_FUSED_COLSPLIT> { enum { THREADS = 512, MIN_BLOCKS = 1 }; };
 
 extern __shared__ __align__(16) unsigned char g_dyn_smem[];
 
@@ -414,7 +441,8 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 
     constexpr bool GROUPED = (MODE == MODE_GROUPED);
     constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);
-    constexpr bool FUSED = (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || MODE == MODE_FUSED_ET || GROUPED);
+    constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
+    constexpr bool FUSED = (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || MODE == MODE_FUSED_ET || GROUPED || COLSPLIT);
     constexpr int ROW_SHIFT = ET ? 2 : 0;   /* log2 table rows per leaf */
     uint32_t taken = 0;
     for (int j = 0; j < p.key_groups; j++) {
@@ -518,7 +546,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                 env.front_out = p.frontier_out + ((size_t)kg * p.nfront + ((size_t)q << g_s)) * kpw + kslot;
                 eval_subtree<PRF, true>(env, r, g_s, ph.level_base);
             } else {
-                env.rows = g_table + ((size_t)q << (g_s + ROW_SHIFT)) * p.row_stride_v + p.col_off_v;
+                env.rows = g_table + ((size_t)q << (g_s + ROW_SHIFT)) * p.row_stride_v + p.col_off_v + (COLSPLIT ? (lane & 3) : 0);
                 if constexpr (MODE == MODE_FUSED_TMA) {
                     /* the item's rows are one contiguous run (64-byte rows, breadth-first leaf order) */
                     __syncwarp();                                   /* every lane is done with the previous tile */
@@ -546,7 +574,21 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 #pragma unroll
                 for (int e = 0; e < 4 * NV; e++) env.acc[e] += __shfl_xor_sync(0xffffffffu, env.acc[e], off);
             }
-            if (env.key_valid && sslot == 0) {
+            if (COLSPLIT) {
+                if (sslot == 0) {
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        const int kj = g_key_first + (kslot ^ j);
+                        if (kj > g_key_last) continue;
+                        uint32_t *o = p.out + (size_t)kj * p.out_stride + p.col_off;
+#pragma unroll
+                        for (int c = 0; c < 4; c++) {
+                            const uint32_t e = 4u * (uint32_t)(lane & 3) + (uint32_t)c;
+                            if (e < p.ncols) atomicAdd(o + e, env.acc[4 * j + c]);
+                        }
+                    }
+                }
+            } else if (env.key_valid && sslot == 0) {
                 uint32_t *o = p.out + (size_t)key * p.out_stride + p.col_off;
 #pragma unroll
                 for (int e = 0; e < 4 * NV; e++)
@@ -558,10 +600,10 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 }
 
 template <int PRF, int NV, int MODE>
-__global__ void __launch_bounds__((KernelShape<PRF, NV>::THREADS), (KernelShape<PRF, NV>::MIN_BLOCKS))
+__global__ void __launch_bounds__((EvalShape<PRF, NV, MODE>::THREADS), (EvalShape<PRF, NV, MODE>::MIN_BLOCKS))
 dpf_eval_kernel(const __grid_constant__ EvalParams p)
 {
-    constexpr int THREADS = KernelShape<PRF, NV>::THREADS;
+    constexpr int THREADS = EvalShape<PRF, NV, MODE>::THREADS;
     const int tid = threadIdx.x;
     unsigned long long *stamp = (p.timing != nullptr && tid == 0) ? p.timing + (size_t)blockIdx.x * 8 : nullptr;
     if (stamp) stamp[0] = global_ns();
@@ -927,9 +969,9 @@ cudaError_t launch_one(const EvalParams &p, int grid, size_t smem, cudaStream_t 
     if (p.fuse_top) {
         void *args[] = {const_cast<EvalParams *>(&p)};
         return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3((unsigned)grid),
-                                           dim3((unsigned)(KernelShape<PRF, NV>::THREADS)), args, smem, stream);
+                                           dim3((unsigned)(EvalShape<PRF, NV, MODE>::THREADS)), args, smem, stream);
     }
-    kern<<<grid, (KernelShape<PRF, NV>::THREADS), smem, stream>>>(p);
+    kern<<<grid, (EvalShape<PRF, NV, MODE>::THREADS), smem, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -959,6 +1001,10 @@ cudaError_t launch_prf(int nv, int mode, const EvalParams &p, int grid, size_t s
         return cudaErrorInvalidValue;
     }
     if (mode == MODE_FRONTIER) return launch_one<PRF, 4, MODE_FRONTIER>(p, grid, smem, stream);
+    if (mode == MODE_FUSED_COLSPLIT) {
+        if constexpr (PRF == PRF_AES128) return launch_one<PRF, 4, MODE_FUSED_COLSPLIT>(p, grid, smem, stream);
+        else return cudaErrorInvalidValue;   /* Salsa/ChaCha bind the ALU pipe, not the data pipe */
+    }
     if (mode == MODE_GROUPED) return launch_one<PRF, 4, MODE_GROUPED>(p, grid, smem, stream);
     if (mode == MODE_FUSED_TMA) {
         if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;    /* no shared memory left beside the tables */
@@ -981,6 +1027,10 @@ cudaError_t max_smem_prf(int nv, int mode, int *bytes)
         return cudaErrorInvalidValue;
     }
     if (mode == MODE_FRONTIER) return max_smem_one<PRF, 4, MODE_FRONTIER>(bytes);
+    if (mode == MODE_FUSED_COLSPLIT) {
+        if constexpr (PRF == PRF_AES128) return max_smem_one<PRF, 4, MODE_FUSED_COLSPLIT>(bytes);
+        else return cudaErrorInvalidValue;
+    }
     if (mode == MODE_GROUPED) return max_smem_one<PRF, 4, MODE_GROUPED>(bytes);
     if (mode == MODE_FUSED_TMA) {
         if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;
@@ -994,8 +1044,9 @@ cudaError_t max_smem_prf(int nv, int mode, int *bytes)
 
 }  // namespace
 
-int eval_threads(int prf, int nv)
+int eval_threads(int prf, int nv, int mode)
 {
+    if (prf == PRF_AES128 && mode == MODE_FUSED_COLSPLIT) return 512;
     if (prf == PRF_AES128) return nv <= 8 ? DPF_AES_THREADS : 256;
     return nv <= 8 ? 256 : 384;
 }

@@ -117,12 +117,16 @@ enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3,
         * position p owns rows 4p..4p+3 of the device table */
        MODE_FUSED_ET = 5,  /* MODE_FUSED, nv = 4 or 8 */
        MODE_EXPAND_ET = 6, /* MODE_EXPAND: shares[key][4 * leaf + lane] */
-       MODE_COUNT = 7 };
+       /* MODE_FUSED for AES at 16 columns with >= 4 keys per warp: the four lanes of a key quad split
+        * each table row, lane L loading columns 4 (L & 3) .. +3, and the quad's leaf values travel by
+        * SHFL instead, so a row costs the shared-memory data pipe one 16-byte load per lane, not four */
+       MODE_FUSED_COLSPLIT = 7,
+       MODE_COUNT = 8 };
 
-/* Threads per block / minimum blocks per SM of the kernel instantiated for
+/* Threads per block (for a kernel mode: the column-split AES kernel runs 16 warps) / minimum blocks per SM of the kernel instantiated for
  * (prf, nv) where nv = uint4 (4 int32 columns) of a table row handled per pass:
  * 4, 8 or 16. */
-int eval_threads(int prf, int nv);
+int eval_threads(int prf, int nv, int mode);
 int eval_min_blocks(int prf, int nv);
 
 /* Shared-window address of the first dynamic shared memory byte (probed). */

@@ -10,7 +10,12 @@
 //   mixes    : LOP3+IMAD, LOP3+SHF+IMAD (can the two pipes issue in the same clock?), LDS+PRMT+LOP3
 //   lsu + ldg: the LDS steps plus 3 warp-uniform (broadcast) LDG.128 per 128 LDS, the ratio of the
 //              fused AES kernel's table-row loads (8 per leaf pair of ~300 lookups); each load hits
-//              one 64-byte row of a 4 MiB buffer (L2-resident), consumed by IMADs like the MAC
+//              one 64-byte row of a 4 MiB buffer (L2-resident), consumed by IMADs like the MAC.  That
+//              ratio holds inside a leaf pair only; per AES height-2 unit (4 leaves: 1,268 lookups, 4
+//              rows) it is 16 per 1,268, the "16 per 1280 LDS" line
+//   tensor-core inner product: the LDS steps plus, per 1280 LDS, what an 8-key x 4-subtree lane
+//              mapping with the inner product on IMMA would issue per unit: 4 LDG.64 (no broadcast),
+//              24 PRMT and 10 IMMA.16816.U8.U8; and the same without the IMMA as a control
 //   quarter rounds: Salsa20 / ChaCha as the kernels write them, and variants that move some of
 //   the rotates to the fma pipe as IMAD.WIDE (x*2^r = {x<<r, x>>(32-r)}; the halves are disjoint,
 //   so  b ^ rotl(t,r) == lop3.xor(b, lo, hi)).
@@ -26,7 +31,8 @@
 #define UNROLL 16     // ops per chain per loop trip
 
 enum Op { OP_LOP3, OP_SHF, OP_PRMT, OP_IADD3, OP_IMAD, OP_IMADWIDE, OP_IMADHI, OP_LDS,
-          OP_MIX_LOP3_IMAD, OP_MIX_LOP3_SHF_IMAD, OP_MIX_LDS_PRMT_LOP3, OP_MIX_LOP3_IMADWIDE, OP_LDS_LDG };
+          OP_MIX_LOP3_IMAD, OP_MIX_LOP3_SHF_IMAD, OP_MIX_LDS_PRMT_LOP3, OP_MIX_LOP3_IMADWIDE, OP_LDS_LDG,
+          OP_LDS_LDG_UNIT, OP_LDS_MMA_UNIT, OP_LDS_LDG64_UNIT };
 
 template <int OP>
 __device__ __forceinline__ void step(uint32_t &x, uint32_t y, uint32_t z, uint32_t smem_lane)
@@ -47,7 +53,7 @@ __device__ __forceinline__ void step(uint32_t &x, uint32_t y, uint32_t z, uint32
                      "lop3.b32 %0, lo, hi, %1, 0x96;\n\t}" : "+r"(x) : "r"(y));
     } else if (OP == OP_IMADHI) {
         asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(x) : "r"(y));
-    } else if (OP == OP_LDS || OP == OP_LDS_LDG) {
+    } else if (OP == OP_LDS || OP == OP_LDS_LDG || OP == OP_LDS_LDG_UNIT || OP == OP_LDS_MMA_UNIT || OP == OP_LDS_LDG64_UNIT) {
         uint32_t a;
         asm volatile("prmt.b32 %0, %1, %2, 0x7604;" : "=r"(a) : "r"(x), "r"(smem_lane));
         asm volatile("ld.shared.u32 %0, [%1];" : "=r"(x) : "r"(a));
@@ -77,7 +83,7 @@ __host__ __device__ constexpr Mix mix_of(int op)
     return op == OP_LOP3 || op == OP_SHF || op == OP_PRMT || op == OP_IADD3 ? Mix{1, 0, 0}
          : op == OP_IMAD || op == OP_IMADHI ? Mix{0, 1, 0}
          : op == OP_IMADWIDE ? Mix{1, 1, 0}
-         : op == OP_LDS || op == OP_LDS_LDG ? Mix{1, 0, 1}
+         : op == OP_LDS || op == OP_LDS_LDG || op == OP_LDS_LDG_UNIT || op == OP_LDS_MMA_UNIT || op == OP_LDS_LDG64_UNIT ? Mix{1, 0, 1}
          : op == OP_MIX_LOP3_IMAD ? Mix{1, 1, 0}
          : op == OP_MIX_LOP3_SHF_IMAD ? Mix{2, 1, 0}
          : op == OP_MIX_LDS_PRMT_LOP3 ? Mix{2, 0, 1}
@@ -106,22 +112,55 @@ __global__ void __launch_bounds__(512, 1) pipe_kernel(uint32_t *out, long long *
     const uint32_t y = x[0] | 1u, z = x[1] ^ 0x5bd1e995u;
     const uint32_t warp_id = blockIdx.x * 16u + (threadIdx.x >> 5);
     uint32_t sink = 0;
+    uint32_t d0 = 0, d1 = 0, d2 = 0, d3 = 0, a0 = y, a1 = z, bp = 0;
+    uint2 ga = make_uint2(0, 0), gb = make_uint2(0, 0);
     __syncthreads();
     const long long t0 = clock64();
     for (int it = 0; it < iters; it++) {
+        /* the *_UNIT mixes repeat every 5 trips = 640 LDS, half of an AES height-2 unit's 1,268 lookups */
+        const int ph = it % 5;
+        const uint32_t row = ((uint32_t)it * 2654435761u + warp_id) & ROWS_MASK;
 #pragma unroll
         for (int u = 0; u < UNROLL; u++) {
 #pragma unroll
             for (int c = 0; c < CH; c++) step<OP>(x[c], y, z, smem_lane);
             if (OP == OP_LDS_LDG && u % 5 == 2) {   /* u = 2, 7, 12: words 0..2 of this trip's row */
-                const uint4 r = __ldg(rows + (size_t)(((uint32_t)it * 2654435761u + warp_id) & ROWS_MASK) * 4 + u / 5);
+                const uint4 r = __ldg(rows + (size_t)row * 4 + u / 5);
                 sink += r.x * y + r.y * z + r.z * y + r.w * z;
+            }
+            /* the fused kernel's row loads: 16 broadcast LDG.128 (4 rows x 64 bytes) per unit = 8 per 5 trips */
+            if (OP == OP_LDS_LDG_UNIT && (u == 2 || (u == 9 && ph < 3))) {
+                const uint4 r = __ldg(rows + (size_t)row * 4 + (u == 2 ? 0 : 1));
+                sink += r.x * y + r.y * z + r.z * y + r.w * z;
+            }
+            /* inner product on the tensor cores (8 keys x 4 subtrees per warp): per unit 4 LDG.64 (lane L:
+             * row of subtree slot L & 3, columns 2 (L >> 2) and +1), 24 PRMT byte-plane splits and 10
+             * IMMA.16816.U8.U8 = per 5 trips 2 / 12 / 5.  LDG64_UNIT: the same without the IMMA (its
+             * operands are folded into the sink instead) */
+            if (OP == OP_LDS_MMA_UNIT || OP == OP_LDS_LDG64_UNIT) {
+                if (u == 2 && ph == 0) {
+                    const uint2 *r = reinterpret_cast<const uint2 *>(rows) + ((threadIdx.x >> 2) & 7);
+                    ga = __ldg(r + (size_t)((row + (threadIdx.x & 3)) & ROWS_MASK) * 8);
+                    gb = __ldg(r + (size_t)((row + 4 + (threadIdx.x & 3)) & ROWS_MASK) * 8);
+                }
+                if (u == 5) {
+                    bp = __byte_perm(x[0], x[1], 0x5140);
+                    bp = __byte_perm(bp, x[2], 0x5410);
+                }
+                if (u == 11 && ph == 0) {
+                    a0 = __byte_perm(ga.x, gb.x, 0x5140);
+                    a1 = __byte_perm(ga.y, gb.y, 0x7362);
+                }
+                if (u == 13 && OP == OP_LDS_LDG64_UNIT) sink ^= a0 ^ a1 ^ bp;
+                if (u == 13 && OP == OP_LDS_MMA_UNIT)
+                    asm volatile("mma.sync.aligned.m16n8k16.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                                 : "+r"(d0), "+r"(d1), "+r"(d2), "+r"(d3) : "r"(a0), "r"(a1), "r"(bp));
             }
         }
     }
     __syncthreads();
     const long long t1 = clock64();
-    uint32_t acc = sink;
+    uint32_t acc = sink ^ d0 ^ d1 ^ d2 ^ d3;
 #pragma unroll
     for (int c = 0; c < CH; c++) acc ^= x[c];
     out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
@@ -233,11 +272,10 @@ static double max_cycles()
 }
 
 template <int OP>
-static void run_pipe(const char *name)
+static void run_pipe(const char *name, int iters = 2000)
 {
     auto k = pipe_kernel<OP>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TAB_SMEM);
-    const int iters = 2000;
     k<<<g_sms, 512, TAB_SMEM>>>(g_out, g_cycles, 50, g_rows);
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
@@ -303,6 +341,16 @@ int main()
     run_pipe<OP_IMADHI>("IMAD.HI");
     run_pipe<OP_LDS>("PRMT+LDS.32 conflict-free");
     run_pipe<OP_LDS_LDG>("PRMT+LDS.32 + 3 broadcast LDG.128 per 128 LDS");
+    run_pipe<OP_LDS_LDG_UNIT>("PRMT+LDS.32 + 16 broadcast LDG.128 per 1280 LDS");
+    run_pipe<OP_LDS_MMA_UNIT>("PRMT+LDS.32 + 4 LDG.64, 24 PRMT, 10 IMMA.16816.U8 per 1280 LDS");
+    run_pipe<OP_LDS_LDG64_UNIT>("PRMT+LDS.32 + 4 LDG.64, 24 PRMT, no IMMA per 1280 LDS");
+    /* the same mixes 10x longer (about 22 ms), alternating: the rates are per SM clock, but what a
+     * kernel costs is time, and sm_mhz_effective shows whether the clock moves with the mix */
+    run_pipe<OP_LDS>("PRMT+LDS.32 conflict-free (long)", 20000);
+    run_pipe<OP_LDS_LDG_UNIT>("PRMT+LDS.32 + 16 broadcast LDG.128 per 1280 LDS (long)", 20000);
+    run_pipe<OP_LDS_MMA_UNIT>("PRMT+LDS.32 + 4 LDG.64, 24 PRMT, 10 IMMA.16816.U8 per 1280 LDS (long)", 20000);
+    run_pipe<OP_LDS_LDG64_UNIT>("PRMT+LDS.32 + 4 LDG.64, 24 PRMT, no IMMA per 1280 LDS (long)", 20000);
+    run_pipe<OP_LDS_LDG_UNIT>("PRMT+LDS.32 + 16 broadcast LDG.128 per 1280 LDS (long, again)", 20000);
     run_pipe<OP_MIX_LOP3_IMAD>("LOP3+IMAD");
     run_pipe<OP_MIX_LOP3_SHF_IMAD>("LOP3+SHF+IMAD");
     run_pipe<OP_MIX_LDS_PRMT_LOP3>("PRMT+LDS+LOP3");
