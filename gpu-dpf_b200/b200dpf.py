@@ -26,7 +26,7 @@ SYMBOLS = [
     "b200dpf_host_staging", "b200dpf_eval_device", "b200dpf_eval_device_acc", "b200dpf_expand_device", "b200dpf_ctx_n", "b200dpf_ctx_entry_size",
     "b200dpf_ctx_device", "b200dpf_ctx_last_launches", "b200dpf_ctx_set_subtree_log2",
     "b200dpf_gen_et", "b200dpf_gen_batch_et", "b200dpf_eval_cpu_et", "b200dpf_key_pack_et", "b200dpf_key_unpack_et",
-    "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf",
+    "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf", "b200dpf_group_create_et",
 ]
 
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
@@ -93,6 +93,7 @@ def load():
     L.b200dpf_key_unpack_et.argtypes = [C.c_char_p, C.c_size_t, _i32p]
     L.b200dpf_create_et.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
+    L.b200dpf_group_create_et.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
     return L
 
 
@@ -358,9 +359,10 @@ class Context:
 
 class GroupContext(Context):
     """Many tables ("bins") of one entry size behind one context: the batch-PIR front end
-    (b200dpf_group_create / b200dpf_group_eval)."""
+    (b200dpf_group_create / b200dpf_group_eval).  early_termination=True makes the context for
+    early-terminated keys (b200dpf_group_create_et): bins of >= 8 rows, four rows per tree leaf."""
 
-    def __init__(self, tables, device=0):
+    def __init__(self, tables, device=0, early_termination=False):
         self.tables = [np.ascontiguousarray(t, np.int32) for t in tables]
         assert all(t.ndim == 2 and t.shape[1] == self.tables[0].shape[1] for t in self.tables)
         self.entry_size = self.tables[0].shape[1]
@@ -368,8 +370,8 @@ class GroupContext(Context):
         sizes = np.array([t.shape[0] for t in self.tables], np.int64)
         ptrs = (C.c_void_p * len(self.tables))(*[t.ctypes.data for t in self.tables])
         self.handle = C.c_void_p()
-        _check(lib().b200dpf_group_create(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size, device),
-               "b200dpf_group_create")
+        name = "b200dpf_group_create_et" if early_termination else "b200dpf_group_create"
+        _check(getattr(lib(), name)(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size, device), name)
 
     @property
     def nbins(self):

@@ -395,6 +395,17 @@ inline int check_key_n(const int32_t *key, int64_t b, int64_t n)
     return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b, (long long)kn, (long long)n);
 }
 
+/* key number `b` of a batch must be an early-terminated key for n rows */
+inline int check_key_et_n(const int32_t *key, int64_t b, int64_t n)
+{
+    const int64_t kn = key ? host::key_et_n(key) : -1;
+    if (kn == n) return B200DPF_OK;
+    if (key && host::key_n(key) >= 0)
+        return fail(B200DPF_EINVAL, "key %lld is a standard key; this early-terminated context takes keys of b200dpf_gen_et", (long long)b);
+    return fail(B200DPF_EINVAL, "key %lld is not an early-terminated key for n=%lld (its n: %lld)", (long long)b, (long long)n,
+                (long long)kn);
+}
+
 /* key number `b` of a batch must be of the context's kind (standard or early-terminated) and n */
 inline int check_key(const b200dpf_ctx *c, const int32_t *key, int64_t b)
 {
@@ -403,12 +414,7 @@ inline int check_key(const b200dpf_ctx *c, const int32_t *key, int64_t b)
             return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this context takes standard keys", (long long)b);
         return check_key_n(key, b, c->n);
     }
-    const int64_t kn = key ? host::key_et_n(key) : -1;
-    if (kn == c->n) return B200DPF_OK;
-    if (key && host::key_n(key) >= 0)
-        return fail(B200DPF_EINVAL, "key %lld is a standard key; this early-terminated context takes keys of b200dpf_gen_et", (long long)b);
-    return fail(B200DPF_EINVAL, "key %lld is not an early-terminated key for n=%lld (its n: %lld)", (long long)b, (long long)c->n,
-                (long long)kn);
+    return check_key_et_n(key, b, c->n);
 }
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
@@ -1702,18 +1708,22 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
 /* ------------------------------------------------------------------------------------------- */
 /* Grouped evaluation: the batch-PIR front end (SURVEY.md section 8(f) rank 4).                  */
 /* ------------------------------------------------------------------------------------------- */
-int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
-                         int device)
+/* b200dpf_group_create (lane_bits = 0) and b200dpf_group_create_et (lane_bits = 2: 2^lane_bits rows per
+ * leaf).  n and the row offsets count rows, the depths (per bin and the context's deepest) leaves. */
+static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                             int device, int lane_bits)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!tables || !n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
+    const int64_t n_min = (int64_t)2 << lane_bits;
     int64_t n_max = 0, rows = 0;
     for (int g = 0; g < nbins; g++) {
         if (!tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
-        if (n[g] < 2 || n[g] > ((int64_t)1 << 31) || (n[g] & (n[g] - 1)) != 0)
-            return fail(B200DPF_EINVAL, "bin %d: size n=%lld must be a power of two in [2, 2^31]", g, (long long)n[g]);
+        if (n[g] < n_min || n[g] > ((int64_t)1 << 31) || (n[g] & (n[g] - 1)) != 0)
+            return fail(B200DPF_EINVAL, "bin %d: size n=%lld must be a power of two in [%lld, 2^31]", g, (long long)n[g],
+                        (long long)n_min);
         n_max = std::max(n_max, n[g]);
         rows += n[g];
     }
@@ -1725,7 +1735,8 @@ int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const 
     if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
     GroupBins *B = c->bins.get();
     c->n = n_max;                      /* the launch plan (shared memory for correction words) is sized by the deepest bin */
-    c->depth = ilog2(n_max);
+    c->lane_bits = lane_bits;
+    c->depth = ilog2(n_max) - lane_bits;
     c->entry_size = entry_size;
     c->entry_pad = (entry_size + 15) & ~15;       /* 16 columns per pass */
     c->n_local = n_max;
@@ -1741,19 +1752,37 @@ int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const 
     if (rc) return rc;
     uint64_t row0 = 0;
     for (int g = 0; g < nbins; g++) {
-        /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows */
-        const int depth = ilog2(n[g]);
+        /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows; a
+         * leaf's 2^lane_bits rows stay adjacent */
+        const int depth = ilog2(n[g]) - lane_bits;
         B->n.push_back(n[g]);
         B->depth.push_back(depth);
         B->row_off.push_back(row0);
         CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
-        CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr + row0 * (uint64_t)c->entry_pad, (uint64_t)n[g], depth,
-                                      entry_size, c->entry_pad, c->sm_count, c->stream));
+        int32_t *dst = c->d_table.ptr + row0 * (uint64_t)c->entry_pad;
+        if (lane_bits)
+            CUDA_TRY(launch_permute_table_et(d_stage.ptr, dst, (uint64_t)n[g], depth, entry_size, c->entry_pad, c->sm_count,
+                                             c->stream));
+        else
+            CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, entry_size, c->entry_pad, c->sm_count,
+                                          c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
         row0 += (uint64_t)n[g];
     }
     *out = c.release();
     return B200DPF_OK;
+}
+
+int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                         int device)
+{
+    return group_create_impl(out, tables, n, nbins, entry_size, device, 0);
+}
+
+int b200dpf_group_create_et(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                            int device)
+{
+    return group_create_impl(out, tables, n, nbins, entry_size, device, host::ET_LOG2_ROWS_PER_LEAF);
 }
 
 int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
@@ -1769,7 +1798,10 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     for (int64_t b = 0; b < nkeys; b++) {
         const int g = bins[b];
         if (g < 0 || g >= nbins) return fail(B200DPF_EINVAL, "key %lld: bin %d out of range [0,%d)", (long long)b, g, nbins);
-        if (host::key_n(keys + b * host::KEY_WORDS) != B->n[(size_t)g])
+        if (c->lane_bits) {
+            const int rc = check_key_et_n(keys + b * host::KEY_WORDS, b, B->n[(size_t)g]);
+            if (rc) return rc;
+        } else if (host::key_n(keys + b * host::KEY_WORDS) != B->n[(size_t)g])
             return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, bin %d has n=%lld", (long long)b,
                         (long long)host::key_n(keys + b * host::KEY_WORDS), g, (long long)B->n[(size_t)g]);
         count[(size_t)g + 1]++;
@@ -1778,8 +1810,10 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
     /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
-     * 2^10-entry bin has 672 live bytes of its 2096 */
+     * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
     const KeyLayout kl = compact_layout(c->depth);
+    const int mode = c->lane_bits ? MODE_GROUPED_ET : MODE_GROUPED;
+    const char *magic = c->lane_bits ? kMagicEt : kMagic;
     const size_t stride = (size_t)kl.stride_v * 16u;
     const size_t key_bytes = (size_t)nkeys * stride;
     int rc = reserve_host_keys(c, key_bytes);
@@ -1792,7 +1826,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         auto pack_range = [&](int64_t p0, int64_t p1) {
             for (int64_t pos = p0; pos < p1; pos++) {
                 const int64_t b = B->perm[(size_t)pos];
-                pack_compact(keys + b * host::KEY_WORDS, stage + (size_t)pos * stride, B->depth[(size_t)bins[b]]);
+                pack_compact(keys + b * host::KEY_WORDS, stage + (size_t)pos * stride, B->depth[(size_t)bins[b]], magic);
             }
         };
         const int nthr = (int)std::min<int64_t>(std::min<int64_t>(8, std::max(1u, std::thread::hardware_concurrency())), nkeys / 2048 + 1);
@@ -1804,7 +1838,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     /* key groups and their work-item size: big items amortise the root-to-subtree walk every item
      * pays (there is no frontier: bins are small), small items keep every warp busy */
     SmemLayout L;
-    rc = smem_layout(c, prf, 4, MODE_GROUPED, &L);
+    rc = smem_layout(c, prf, 4, mode, &L);
     if (rc) return rc;
     const int64_t warps = (int64_t)L.grid * (L.threads / 32);
     int64_t ngroups = 0;
@@ -1889,7 +1923,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             c->bar_epoch += (uint32_t)L.grid;
             p.grid_bar_target = c->bar_epoch;
         }
-        const cudaError_t e = launch_eval(prf, 4, MODE_GROUPED, p, L.grid, smem, c->stream);
+        const cudaError_t e = launch_eval(prf, 4, mode, p, L.grid, smem, c->stream);
         if (e != cudaSuccess) {
             c->coop_state_dirty = true;
             return fail(B200DPF_ECUDA, "grouped evaluation launch: %s", cudaGetErrorString(e));

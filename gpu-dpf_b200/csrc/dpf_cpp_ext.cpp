@@ -232,23 +232,30 @@ std::vector<void *> eval_init_multi(const at::Tensor &table, const std::vector<i
     return {static_cast<void *>(ctx)};
 }
 
-/* batch PIR: many tables ("bins") of one entry size behind one context (b200dpf_group_create) */
-std::vector<void *> group_init(const std::vector<at::Tensor> &tables, int device)
+/* batch PIR: many tables ("bins") of one entry size behind one context (b200dpf_group_create, or
+ * b200dpf_group_create_et for early-terminated keys) */
+std::vector<void *> group_init_kind(const std::vector<at::Tensor> &tables, int device, bool et)
 {
-    TORCH_CHECK(!tables.empty(), "group_init: no tables");
+    const char *what = et ? "group_init_et" : "group_init";
+    TORCH_CHECK(!tables.empty(), what, ": no tables");
     std::vector<at::Tensor> keep;
     std::vector<const int32_t *> ptrs;
     std::vector<int64_t> sizes;
     for (const at::Tensor &t : tables) {
-        TORCH_CHECK(t.dim() == 2 && t.size(1) == tables[0].size(1), "group_init: tables must be [n_g, entry_size] with one entry_size");
+        TORCH_CHECK(t.dim() == 2 && t.size(1) == tables[0].size(1), what, ": tables must be [n_g, entry_size] with one entry_size");
         keep.push_back(t.to(at::kInt).contiguous().cpu());
         ptrs.push_back(keep.back().data_ptr<int32_t>());
         sizes.push_back(keep.back().size(0));
     }
     b200dpf_ctx *ctx = nullptr;
-    check(b200dpf_group_create(&ctx, ptrs.data(), sizes.data(), (int)ptrs.size(), (int)tables[0].size(1), device), "group_init");
+    auto create = et ? b200dpf_group_create_et : b200dpf_group_create;
+    check(create(&ctx, ptrs.data(), sizes.data(), (int)ptrs.size(), (int)tables[0].size(1), device), what);
     return {static_cast<void *>(ctx)};
 }
+
+std::vector<void *> group_init(const std::vector<at::Tensor> &tables, int device) { return group_init_kind(tables, device, false); }
+
+std::vector<void *> group_init_et(const std::vector<at::Tensor> &tables, int device) { return group_init_kind(tables, device, true); }
 
 /* keys int32 [B,524], bins int32/int64 [B] -> int32 [B, E]: key b evaluated on table bins[b] */
 at::Tensor group_eval(const at::Tensor &keys, const at::Tensor &bins, const std::vector<void *> &buffers, int prf)
@@ -512,6 +519,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("eval_init_sharded", &eval_init_sharded, "eval_init for one entry-range shard", py::arg("table"),
           py::arg("device"), py::arg("shard_rank"), py::arg("shard_count"));
     m.def("group_init", &group_init, "batch PIR: one context over many tables (bins)", py::arg("tables"), py::arg("device") = 0);
+    m.def("group_init_et", &group_init_et, "batch PIR for early-terminated keys (four rows per leaf)", py::arg("tables"),
+          py::arg("device") = 0);
     m.def("group_eval", &group_eval, "batch PIR: evaluate (bin, key) pairs in one launch");
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),
           py::arg("devices"), py::arg("axis") = 0);

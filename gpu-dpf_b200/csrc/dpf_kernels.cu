@@ -171,11 +171,12 @@ struct DevEnv {
         return make_seed(v.x, v.y, v.z, v.w);
     }
     static constexpr bool MAC = (MODE == MODE_FUSED || MODE == MODE_GROUPED || MODE == MODE_FUSED_TMA ||
-                                 MODE == MODE_FUSED_ET || MODE == MODE_FUSED_COLSPLIT);   /* leaves feed the inner product */
+                                 MODE == MODE_FUSED_ET || MODE == MODE_FUSED_COLSPLIT ||
+                                 MODE == MODE_GROUPED_ET);   /* leaves feed the inner product */
     /* rows points at this lane's 16 bytes of the row; acc[4 j + c] is column 4 (lane & 3) + c of key
      * kslot ^ j, whose leaf values come from lane ^ j */
     static constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
-    static constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);   /* four rows per leaf */
+    static constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET || MODE == MODE_GROUPED_ET);   /* four rows per leaf */
     /* ET prefetches the first row pair before the leaf expansion at 16 columns only: at 32, rows held
      * across the full-width expansion (or two rows in flight beside the next two) spill */
     static constexpr bool ET_PREFETCH = ET && NV == 4;
@@ -439,8 +440,8 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
         __syncwarp();
     }
 
-    constexpr bool GROUPED = (MODE == MODE_GROUPED);
-    constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET);
+    constexpr bool GROUPED = (MODE == MODE_GROUPED || MODE == MODE_GROUPED_ET);
+    constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET || MODE == MODE_GROUPED_ET);
     constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
     constexpr bool FUSED = (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || MODE == MODE_FUSED_ET || GROUPED || COLSPLIT);
     constexpr int ROW_SHIFT = ET ? 2 : 0;   /* log2 table rows per leaf */
@@ -902,6 +903,25 @@ __global__ void __launch_bounds__(256) update_map_et_kernel(const UpdateParams u
     }
 }
 
+/* row update of an early-terminated grouped context, step 1 (UpdateParams::bins set, lane_bits = 2): row i
+ * of bin g is word i & 3 of the bin's leaf i >> 2 */
+__global__ void __launch_bounds__(256) update_map_group_et_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
+                                                                  uint32_t *__restrict__ ord)
+{
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = u.idx[j];
+        const int32_t g = u.bins[j];
+        uint32_t p = u.table_rows;
+        if (g >= 0 && g < u.nbins) {
+            const uint2 info = u.bin_info[g];
+            if (i >= 0 && i < ((int64_t)4 << info.y))
+                p = info.x + ((bitrev_bits((uint32_t)(i >> 2), (int)info.y) << 2) | ((uint32_t)i & 3u));
+        }
+        pos[j] = p;
+        ord[j] = (uint32_t)j;
+    }
+}
+
 /* row update, step 1: natural index -> table row (or the skip marker), occurrence number j */
 __global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
                                                          uint32_t *__restrict__ ord)
@@ -989,7 +1009,7 @@ cudaError_t max_smem_one(int *bytes)
 }
 
 /* (prf, nv, mode) -> instantiation; modes 1, 2 and 6 never touch the table, so NV = 4 only; grouped
- * evaluation takes 16 columns per pass, early-terminated evaluation 16 or 32 */
+ * evaluation (both kinds of key) takes 16 columns per pass, early-terminated evaluation 16 or 32 */
 template <int PRF>
 cudaError_t launch_prf(int nv, int mode, const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
 {
@@ -1006,6 +1026,7 @@ cudaError_t launch_prf(int nv, int mode, const EvalParams &p, int grid, size_t s
         else return cudaErrorInvalidValue;   /* Salsa/ChaCha bind the ALU pipe, not the data pipe */
     }
     if (mode == MODE_GROUPED) return launch_one<PRF, 4, MODE_GROUPED>(p, grid, smem, stream);
+    if (mode == MODE_GROUPED_ET) return launch_one<PRF, 4, MODE_GROUPED_ET>(p, grid, smem, stream);
     if (mode == MODE_FUSED_TMA) {
         if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;    /* no shared memory left beside the tables */
         else return launch_one<PRF, 4, MODE_FUSED_TMA>(p, grid, smem, stream);
@@ -1032,6 +1053,7 @@ cudaError_t max_smem_prf(int nv, int mode, int *bytes)
         else return cudaErrorInvalidValue;
     }
     if (mode == MODE_GROUPED) return max_smem_one<PRF, 4, MODE_GROUPED>(bytes);
+    if (mode == MODE_GROUPED_ET) return max_smem_one<PRF, 4, MODE_GROUPED_ET>(bytes);
     if (mode == MODE_FUSED_TMA) {
         if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;
         else return max_smem_one<PRF, 4, MODE_FUSED_TMA>(bytes);
@@ -1165,7 +1187,8 @@ cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int e
     if (u.count <= 0) return cudaSuccess;
     const int64_t cap = (int64_t)std::max(sm_count, 1) * 16;
     const int grid_map = (int)std::max<int64_t>(1, std::min<int64_t>((u.count + 255) / 256, cap));
-    if (u.lane_bits) update_map_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    if (u.lane_bits && u.bins) update_map_group_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    else if (u.lane_bits) update_map_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
     else update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;

@@ -34,7 +34,7 @@ struct PhaseParams {
 struct GroupDesc {
     uint32_t key_first;       /* first key of the group in the (bin-sorted) key array       */
     uint32_t nkeys;           /* 1..32                                                      */
-    int32_t depth;            /* log2 of the bin's table size                               */
+    int32_t depth;            /* log2 of the bin's table size (MODE_GROUPED_ET: of its leaves) */
     int32_t s;                /* log2 leaves per work item for this group                   */
     uint32_t nsub;            /* work items (2^s-leaf subtrees) = 2^(depth - s)             */
     uint32_t pad;
@@ -62,7 +62,7 @@ struct EvalParams {
     uint32_t col_off;         /* first int32 column of this pass                        */
     uint32_t ncols;           /* valid int32 columns in this pass (<= 4*NV)             */
     int depth;                /* log2 n                                                 */
-    const GroupDesc *groups;  /* MODE_GROUPED: [key_groups] descriptors (else null)      */
+    const GroupDesc *groups;  /* MODE_GROUPED(_ET): [key_groups] descriptors (else null)  */
     PhaseParams main;         /* the phase that produces the result (or, in the stand-alone
                                  frontier kernel, the frontier)                          */
     /* single-launch pipeline: the launch first clears its own accumulators and ticket
@@ -121,7 +121,10 @@ enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3,
         * each table row, lane L loading columns 4 (L & 3) .. +3, and the quad's leaf values travel by
         * SHFL instead, so a row costs the shared-memory data pipe one 16-byte load per lane, not four */
        MODE_FUSED_COLSPLIT = 7,
-       MODE_COUNT = 8 };
+       /* MODE_GROUPED for early-terminated keys, nv = 4: GroupDesc::depth is the bin's leaf depth and
+        * the bin's leaf position p owns its rows 4p..4p+3 */
+       MODE_GROUPED_ET = 8,
+       MODE_COUNT = 9 };
 
 /* Threads per block (for a kernel mode: the column-split AES kernel runs 16 warps) / minimum blocks per SM of the kernel instantiated for
  * (prf, nv) where nv = uint4 (4 int32 columns) of a table row handled per pass:
@@ -192,6 +195,9 @@ cudaError_t launch_permute_table_et(const int32_t *stage, int32_t *table, uint64
  *                  else bitrev_depth(i >> shift)                      (whole table or one shard)
  *   bins != null   bin g = bins[j] (skip unless 0 <= g < nbins); skip unless 0 <= i < 2^bin_info[g].y;
  *                  else bin_info[g].x + bitrev_{bin_info[g].y}(i)     (grouped context)
+ *   bins != null and lane_bits = 2 (early-terminated grouped context, .y = the bin's leaf depth):
+ *                  skip unless 0 <= i < 4 << bin_info[g].y;
+ *                  else bin_info[g].x + (bitrev_{bin_info[g].y}(i >> 2) << 2 | (i & 3))
  * Skipped entries are never written. */
 struct UpdateParams {
     const int64_t *idx;       /* [count] natural indices                                      */

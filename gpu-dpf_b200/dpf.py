@@ -374,7 +374,8 @@ class BinnedDPF(DPF):
 
     def __init__(self, *args, **kwargs):
         if kwargs.get("early_termination"):
-            raise Exception("BinnedDPF has no early-terminated variant (early_termination=True)")
+            raise Exception("BinnedDPF has no early-terminated variant (early_termination=True): use "
+                            "dpf_cpp.group_init_et or b200dpf.GroupContext(early_termination=True)")
         super().__init__(*args, **kwargs)
 
     def eval_init(self, tables):

@@ -204,9 +204,17 @@ int b200dpf_ctx_axis(const b200dpf_ctx *ctx);
  * so many small bins fill the GPU the way one big table does.
  *   out[b][e] = the same inner product b200dpf_eval would give for key b on table bins[b].
  * tables[g]: int32 [n[g]][entry_size], host or device.  keys: int32[nkeys][524]; bins: int32[nkeys].
+ * b200dpf_group_create_et makes the same context for early-terminated keys (b200dpf_gen_et, see
+ * below): every n[g] a power of two in [8, 2^31], each bin laid out as by b200dpf_create_et.  There
+ * b200dpf_group_eval takes only keys of b200dpf_gen_et for n[bins[b]] rows (a standard key is EINVAL
+ * before anything is copied), out[b][e] is what b200dpf_eval on b200dpf_create_et(table bins[b]) gives,
+ * b200dpf_group_update_rows works as on a standard grouped context and b200dpf_ctx_rows_per_leaf is 4.
+ * A standard grouped context refuses early-terminated keys (EINVAL).
  */
 int b200dpf_group_create(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
                          int entry_size, int device);
+int b200dpf_group_create_et(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
+                            int entry_size, int device);
 int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf,
                        int32_t *out);
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
@@ -410,12 +418,14 @@ int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key);
  * _host_staging, _eval_device, _eval_device_acc, _expand_device, _update_rows, _update_rows_device,
  * _ctx_set_option and the introspection functions work on it as on a standard context (ctx_n counts
  * rows); the host paths return EINVAL for a standard key before copying anything.  The "tma_rows"
- * option has no effect here.  There is no multi-device or grouped variant.
+ * option has no effect here.  There is no multi-device variant; the grouped (batch-PIR) variant is
+ * b200dpf_group_create_et.
  */
 int b200dpf_create_et(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
                       int device, int shard_rank, int shard_count);
 
-/* Table rows per tree leaf: 4 on a context of b200dpf_create_et, 1 otherwise; -1 for null. */
+/* Table rows per tree leaf: 4 on a context of b200dpf_create_et or b200dpf_group_create_et, 1 otherwise;
+ * -1 for null. */
 int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *ctx);
 
 #ifdef __cplusplus
