@@ -241,8 +241,9 @@ int smem_layout(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L)
 int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L)
 {
     std::memset(L, 0, sizeof *L);
-    L->threads = eval_threads(prf, nv, mode);
-    L->blocks_per_sm = eval_min_blocks(prf, nv);
+    const BlockShape shape = eval_block_shape(prf, nv, mode);
+    L->threads = shape.threads;
+    L->blocks_per_sm = shape.min_blocks;
     L->grid = c->sm_count * L->blocks_per_sm;
     int max_smem = 0;
     CUDA_TRY(eval_max_smem(prf, nv, mode, &max_smem));
@@ -1198,12 +1199,8 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    if (lane_bits)
-        CUDA_TRY(launch_permute_table_et(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size,
-                                         c->entry_pad, c->sm_count, c->stream));
-    else
-        CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, entry_size,
-                                      c->entry_pad, c->sm_count, c->stream));
+    CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, lane_bits, entry_size,
+                                  c->entry_pad, c->sm_count, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     d_stage.release();
 
@@ -1760,12 +1757,8 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         B->row_off.push_back(row0);
         CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
         int32_t *dst = c->d_table.ptr + row0 * (uint64_t)c->entry_pad;
-        if (lane_bits)
-            CUDA_TRY(launch_permute_table_et(d_stage.ptr, dst, (uint64_t)n[g], depth, entry_size, c->entry_pad, c->sm_count,
-                                             c->stream));
-        else
-            CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, entry_size, c->entry_pad, c->sm_count,
-                                          c->stream));
+        CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, lane_bits, entry_size, c->entry_pad,
+                                      c->sm_count, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
         row0 += (uint64_t)n[g];
     }

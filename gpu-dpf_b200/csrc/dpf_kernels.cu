@@ -170,19 +170,13 @@ struct DevEnv {
         const uint4 v = *slot(h);
         return make_seed(v.x, v.y, v.z, v.w);
     }
-    static constexpr bool MAC = (MODE == MODE_FUSED || MODE == MODE_GROUPED || MODE == MODE_FUSED_TMA ||
-                                 MODE == MODE_FUSED_ET || MODE == MODE_FUSED_COLSPLIT ||
-                                 MODE == MODE_GROUPED_ET);   /* leaves feed the inner product */
-    /* rows points at this lane's 16 bytes of the row; acc[4 j + c] is column 4 (lane & 3) + c of key
-     * kslot ^ j, whose leaf values come from lane ^ j */
-    static constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
-    static constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET || MODE == MODE_GROUPED_ET);   /* four rows per leaf */
-    /* ET prefetches the first row pair before the leaf expansion at 16 columns only: at 32, rows held
-     * across the full-width expansion (or two rows in flight beside the next two) spill */
-    static constexpr bool ET_PREFETCH = ET && NV == 4;
-    static constexpr bool STAGED = (MODE == MODE_FUSED_TMA);
-    /* STAGED: the work item's 2^s rows were requested with one cp.async.bulk when the item was drawn;
-     * they are first needed s-1 node expansions later, which hides the copy */
+    static constexpr ModeTraits M = mode_traits(MODE);
+    /* early-terminated keys (four rows per leaf) prefetch the first row pair before the leaf expansion
+     * at 16 columns only: at 32, rows held across the full-width expansion (or two rows in flight
+     * beside the next two) spill */
+    static constexpr bool ET_PREFETCH = M.row_shift != 0 && NV == 4;
+    /* ROWS_STAGED: the work item's 2^s rows were requested with one cp.async.bulk when the item was
+     * drawn; they are first needed s-1 node expansions later, which hides the copy */
     const uint4 *tile;          /* this warp's staged rows (shared memory) */
     uint32_t tile_bar;          /* shared-window address of this warp's mbarrier */
     uint32_t tile_phase;
@@ -190,7 +184,7 @@ struct DevEnv {
 
     __device__ __forceinline__ void leaf_prefetch(uint32_t local_pos)
     {
-        if (STAGED) {
+        if (M.row_load == ROWS_STAGED) {
             if (tile_pending) {
                 tma::mbar_wait(tile_bar, tile_phase);
                 tile_phase ^= 1u;
@@ -201,17 +195,17 @@ struct DevEnv {
             for (int j = 0; j < 4; j++) ra[j] = r[j];
 #pragma unroll
             for (int j = 0; j < 4; j++) rb[j] = r[4 + j];
-        } else if (COLSPLIT) {
+        } else if (M.row_load == ROWS_COLSPLIT) {
             ra[0] = __ldg(rows + (size_t)local_pos * row_stride_v);
             rb[0] = __ldg(rows + (size_t)(local_pos + 1) * row_stride_v);
-        } else if (MAC && ET_PREFETCH) {
+        } else if (M.feeds == FEEDS_MAC && ET_PREFETCH) {
             /* the first 64 bytes of the two rows multiplied first: lane 0 of both leaves */
             const uint4 *r = rows + (size_t)local_pos * 4 * row_stride_v;
 #pragma unroll
             for (int j = 0; j < 4; j++) ra[j] = __ldg(r + j);
 #pragma unroll
             for (int j = 0; j < 4; j++) rb[j] = __ldg(r + 4 * row_stride_v + j);
-        } else if (MAC && !ET) {
+        } else if (M.feeds == FEEDS_MAC && M.row_shift == 0) {
             const uint4 *r = rows + (size_t)local_pos * row_stride_v;
 #pragma unroll
             for (int j = 0; j < 4; j++) ra[j] = __ldg(r + j);
@@ -219,12 +213,12 @@ struct DevEnv {
             for (int j = 0; j < 4; j++) rb[j] = __ldg(r + row_stride_v + j);
         }
     }
-    /* ET: leaves local_pos and local_pos + 1 with their four row shares each, against rows 4 local_pos ..
-     * 4 local_pos + 7 */
+    /* early-terminated keys: leaves local_pos and local_pos + 1 with their four row shares each, against
+     * rows 4 local_pos .. 4 local_pos + 7 */
     __device__ __forceinline__ void leaf_quads(uint32_t local_pos, const Seed &w0, const Seed &w1)
     {
         const uint32_t a[4] = {w0.x, w0.y, w0.z, w0.w}, b[4] = {w1.x, w1.y, w1.z, w1.w};
-        if (MAC) {
+        if (M.feeds == FEEDS_MAC) {
             if (leaf_out != nullptr) {   /* coalesced: 32 keys x 4 bytes per row */
 #pragma unroll
                 for (int l = 0; l < 4; l++) {
@@ -278,7 +272,7 @@ struct DevEnv {
                     }
                 }
             }
-        } else if (MODE == MODE_EXPAND_ET && key_valid) {
+        } else if (M.feeds == FEEDS_SHARES && key_valid) {
             /* leaf position p holds leaf bitrev_depth(p), whose word l is the share of row 4 * leaf + l */
             const uint32_t p = pos_base + local_pos;
             uint32_t *o0 = share_row + 4 * (size_t)(__brev(p) >> (32 - depth));
@@ -292,12 +286,14 @@ struct DevEnv {
     }
     __device__ __forceinline__ void leaf_pair(uint32_t local_pos, uint32_t v0, uint32_t v1)
     {
-        if (MAC) {
+        if (M.feeds == FEEDS_MAC) {
             if (leaf_out != nullptr) {   /* coalesced: 32 keys x 4 bytes per leaf */
                 leaf_out[(size_t)local_pos * 32] = v0;
                 leaf_out[(size_t)(local_pos + 1) * 32] = v1;
             }
-            if constexpr (COLSPLIT) {
+            if constexpr (M.row_load == ROWS_COLSPLIT) {
+                /* rows points at this lane's 16 bytes of the row; acc[4 j + c] is column 4 (lane & 3) + c of
+                 * key kslot ^ j, whose leaf values come from lane ^ j */
                 uint32_t u0[4], u1[4];
                 u0[0] = v0;
                 u1[0] = v1;
@@ -337,32 +333,20 @@ struct DevEnv {
                     for (int j = 0; j < 4; j++) { ra[j] = na[j]; rb[j] = nb[j]; }
                 }
             }
-        } else if (MODE == MODE_EXPAND && key_valid) {
+        } else if (M.feeds == FEEDS_SHARES && key_valid) {
             /* leaf position p holds index bitrev_depth(p) */
             const uint32_t p = pos_base + local_pos;
             share_row[__brev(p) >> (32 - depth)] = v0;
             share_row[__brev(p + 1) >> (32 - depth)] = v1;
         }
     }
-    /* MODE_FRONTIER: whole seeds of two adjacent frontier nodes */
+    /* FEEDS_FRONTIER: whole seeds of two adjacent frontier nodes */
     __device__ __forceinline__ void node_pair(uint32_t local_pos, const Seed &c0, const Seed &c1)
     {
         front_out[(size_t)local_pos * kpw] = make_uint4(c0.x, c0.y, c0.z, c0.w);
         front_out[(size_t)(local_pos + 1) * kpw] = make_uint4(c1.x, c1.y, c1.z, c1.w);
     }
 };
-
-/* Block shape per (PRF, NV).  AES needs 128 KiB of the SM's shared memory for its
- * tables, so one block per SM; accumulators (4*NV registers) decide how many
- * threads fit the register file. */
-template <int PRF, int NV> struct KernelShape { enum { THREADS = (NV <= 8 ? 256 : 384), MIN_BLOCKS = (NV <= 8 ? 2 : 1) }; };
-#ifndef DPF_AES_THREADS
-#define DPF_AES_THREADS 384      /* 12 warps: on an H100 1.5 % (n=2^20) and 3 % (n=2^16) faster than 8 (256) */
-#endif
-template <int NV> struct KernelShape<PRF_AES128, NV> { enum { THREADS = (NV <= 8 ? DPF_AES_THREADS : 256), MIN_BLOCKS = 1 }; };
-/* the column-split AES kernel holds 4 row words per leaf instead of 16 and fits 128 registers: 16 warps */
-template <int PRF, int NV, int MODE> struct EvalShape : KernelShape<PRF, NV> {};
-template <> struct EvalShape<PRF_AES128, 4, MODE_FUSED_COLSPLIT> { enum { THREADS = 512, MIN_BLOCKS = 1 }; };
 
 extern __shared__ __align__(16) unsigned char g_dyn_smem[];
 
@@ -402,6 +386,7 @@ template <int PRF, int NV, int THREADS, int MODE>
 __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams &ph,
                                           const typename TablePolicy<PRF>::type &ta, uint32_t quota = 0xffffffffu)
 {
+    constexpr ModeTraits M = mode_traits(MODE);
     const int tid = threadIdx.x;
     const int lane = tid & 31;
 
@@ -427,7 +412,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
     env.stack_split = ph.stack_split;
     env.row_stride_v = p.row_stride_v;
     env.depth = p.depth;
-    if constexpr (MODE == MODE_FUSED_TMA) {
+    if constexpr (M.row_load == ROWS_STAGED) {
         const int w = tid >> 5;
         env.tile = reinterpret_cast<const uint4 *>(g_dyn_smem + p.off_tile + ((size_t)w << (ph.s + 6)));
         env.tile_bar = (uint32_t)__cvta_generic_to_shared(g_dyn_smem + p.off_tile_bar + 8 * w);
@@ -440,11 +425,6 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
         __syncwarp();
     }
 
-    constexpr bool GROUPED = (MODE == MODE_GROUPED || MODE == MODE_GROUPED_ET);
-    constexpr bool ET = (MODE == MODE_FUSED_ET || MODE == MODE_EXPAND_ET || MODE == MODE_GROUPED_ET);
-    constexpr bool COLSPLIT = (MODE == MODE_FUSED_COLSPLIT);
-    constexpr bool FUSED = (MODE == MODE_FUSED || MODE == MODE_FUSED_TMA || MODE == MODE_FUSED_ET || GROUPED || COLSPLIT);
-    constexpr int ROW_SHIFT = ET ? 2 : 0;   /* log2 table rows per leaf */
     uint32_t taken = 0;
     for (int j = 0; j < p.key_groups; j++) {
         const int kg = (int)((blockIdx.x + (unsigned)j) % (unsigned)p.key_groups);
@@ -454,7 +434,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
         int g_key_first = kg * kpw, g_key_last = p.nkeys - 1;
         uint32_t g_tickets = ntickets;
         const uint4 *g_table = p.table;
-        if (GROUPED) {
+        if (M.grouped) {
             const GroupDesc g = p.groups[kg];
             g_depth = g.depth;
             g_s = g.s;
@@ -498,10 +478,10 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 
         const int key = g_key_first + kslot;
         env.key_valid = key <= g_key_last;
-        if (FUSED) {
+        if (M.feeds == FEEDS_MAC) {
 #pragma unroll
             for (int e = 0; e < 4 * NV; e++) env.acc[e] = 0;
-        } else if (MODE == MODE_EXPAND || MODE == MODE_EXPAND_ET) {
+        } else if (M.feeds == FEEDS_SHARES) {
             env.share_row = p.shares + (size_t)(env.key_valid ? key : 0) * p.n;
         }
         const uint4 rv = root_s[kslot];
@@ -543,12 +523,13 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                 start = make_seed(fv.x, fv.y, fv.z, fv.w);
             }
             const Seed r = walk_down<PRF>(env, start, g_walk_first, g_walk_steps, ph.sub_first + q);
-            if (MODE == MODE_FRONTIER) {
+            if (M.feeds == FEEDS_FRONTIER) {
                 env.front_out = p.frontier_out + ((size_t)kg * p.nfront + ((size_t)q << g_s)) * kpw + kslot;
                 eval_subtree<PRF, true>(env, r, g_s, ph.level_base);
             } else {
-                env.rows = g_table + ((size_t)q << (g_s + ROW_SHIFT)) * p.row_stride_v + p.col_off_v + (COLSPLIT ? (lane & 3) : 0);
-                if constexpr (MODE == MODE_FUSED_TMA) {
+                env.rows = g_table + ((size_t)q << (g_s + M.row_shift)) * p.row_stride_v + p.col_off_v +
+                           (M.row_load == ROWS_COLSPLIT ? (lane & 3) : 0);
+                if constexpr (M.row_load == ROWS_STAGED) {
                     /* the item's rows are one contiguous run (64-byte rows, breadth-first leaf order) */
                     __syncwarp();                                   /* every lane is done with the previous tile */
                     if (lane == 0) {
@@ -560,22 +541,23 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                     env.tile_pending = true;
                 }
                 env.pos_base = (ph.sub_first + q) << g_s;
-                env.leaf_out = (!GROUPED && p.leaf_cache) ? p.leaf_cache + ((size_t)kg * p.n_local + ((size_t)q << (g_s + ROW_SHIFT))) * 32 + lane
-                                                          : nullptr;
-                eval_subtree<PRF, false, decltype(env), ET>(env, r, g_s, 0);
+                env.leaf_out = (!M.grouped && p.leaf_cache)
+                                   ? p.leaf_cache + ((size_t)kg * p.n_local + ((size_t)q << (g_s + M.row_shift))) * 32 + lane
+                                   : nullptr;
+                eval_subtree<PRF, false, decltype(env), M.row_shift != 0>(env, r, g_s, 0);
             }
           }
             if (!ahead && draw && lane == 0) t_raw = atomicAdd(ph.counters + kg, chunk);
         }
 
-        if (FUSED) {
+        if (M.feeds == FEEDS_MAC) {
             /* lanes that hold the same key (different subtree slots) fold their partial sums
              * first, so every key receives one red.add per warp and column, not 32/kpw */
             for (int off = kpw; off < 32; off <<= 1) {
 #pragma unroll
                 for (int e = 0; e < 4 * NV; e++) env.acc[e] += __shfl_xor_sync(0xffffffffu, env.acc[e], off);
             }
-            if (COLSPLIT) {
+            if (M.row_load == ROWS_COLSPLIT) {
                 if (sslot == 0) {
 #pragma unroll
                     for (int j = 0; j < 4; j++) {
@@ -601,10 +583,10 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 }
 
 template <int PRF, int NV, int MODE>
-__global__ void __launch_bounds__((EvalShape<PRF, NV, MODE>::THREADS), (EvalShape<PRF, NV, MODE>::MIN_BLOCKS))
+__global__ void __launch_bounds__(eval_block_shape(PRF, NV, MODE).threads, eval_block_shape(PRF, NV, MODE).min_blocks)
 dpf_eval_kernel(const __grid_constant__ EvalParams p)
 {
-    constexpr int THREADS = EvalShape<PRF, NV, MODE>::THREADS;
+    constexpr int THREADS = eval_block_shape(PRF, NV, MODE).threads;
     const int tid = threadIdx.x;
     unsigned long long *stamp = (p.timing != nullptr && tid == 0) ? p.timing + (size_t)blockIdx.x * 8 : nullptr;
     if (stamp) stamp[0] = global_ns();
@@ -625,7 +607,7 @@ dpf_eval_kernel(const __grid_constant__ EvalParams p)
         ta.lanebase = tab + (tid & 31) * 4;
     }
 
-    if constexpr (MODE != MODE_FRONTIER) {
+    if constexpr (mode_traits(MODE).feeds != FEEDS_FRONTIER) {
         if (p.fuse_top) {
             /* single-launch pipeline: clear this launch's accumulators and main-phase tickets,
              * expand the top of every key's tree into the frontier, meet at the grid barrier */
@@ -857,86 +839,43 @@ __global__ void probe_smem_kernel(uint32_t *out)
     if (threadIdx.x == 0) *out = (uint32_t)__cvta_generic_to_shared(g_dyn_smem);
 }
 
-__global__ void permute_table_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table,
-                                     uint64_t rows, int bits, int cols, int stride)
-{
-    const uint64_t total = rows * (uint64_t)cols;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-         i += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t q = i / (uint64_t)cols;
-        const int c = (int)(i - q * (uint64_t)cols);
-        const uint64_t src = bits ? (uint64_t)(__brev((uint32_t)q) >> (32 - bits)) : 0;
-        table[q * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
-    }
-}
-
 __device__ __forceinline__ uint32_t bitrev_bits(uint32_t v, int bits) { return bits ? __brev(v) >> (32 - bits) : 0u; }
 
-/* early-terminated table: runs of four rows (one leaf) move together, table[4q + l] = stage[4 bitrev(q) + l] */
-__global__ void permute_table_et_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table,
-                                        uint64_t rows, int bits, int cols, int stride)
+/* runs of 2^lane_bits rows (one leaf) move together: table[q] = stage[(bitrev_bits(q >> lane_bits) << lane_bits)
+ * | (q & (2^lane_bits - 1))] */
+__global__ void permute_table_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table,
+                                     uint64_t rows, int bits, int lane_bits, int cols, int stride)
 {
     const uint64_t total = rows * (uint64_t)cols;
+    const uint64_t lane_mask = (1u << lane_bits) - 1u;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t q = i / (uint64_t)cols;
         const int c = (int)(i - q * (uint64_t)cols);
-        const uint64_t src = ((uint64_t)bitrev_bits((uint32_t)(q >> 2), bits) << 2) | (q & 3u);
+        const uint64_t src = ((uint64_t)bitrev_bits((uint32_t)(q >> lane_bits), bits) << lane_bits) | (q & lane_mask);
         table[q * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
     }
 }
 
-/* row update of an early-terminated context, step 1 (UpdateParams::lane_bits = 2) */
-__global__ void __launch_bounds__(256) update_map_et_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
-                                                            uint32_t *__restrict__ ord)
-{
-    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t i = u.idx[j];
-        uint32_t p = u.table_rows;
-        if (i >= 0 && i < u.n) {
-            const uint32_t leaf = (uint32_t)(i >> u.lane_bits);
-            if ((leaf & u.own_mask) == u.own_val)
-                p = (bitrev_bits(leaf >> u.shift, u.depth) << u.lane_bits) | ((uint32_t)i & ((1u << u.lane_bits) - 1u));
-        }
-        pos[j] = p;
-        ord[j] = (uint32_t)j;
-    }
-}
-
-/* row update of an early-terminated grouped context, step 1 (UpdateParams::bins set, lane_bits = 2): row i
- * of bin g is word i & 3 of the bin's leaf i >> 2 */
-__global__ void __launch_bounds__(256) update_map_group_et_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
-                                                                  uint32_t *__restrict__ ord)
-{
-    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t i = u.idx[j];
-        const int32_t g = u.bins[j];
-        uint32_t p = u.table_rows;
-        if (g >= 0 && g < u.nbins) {
-            const uint2 info = u.bin_info[g];
-            if (i >= 0 && i < ((int64_t)4 << info.y))
-                p = info.x + ((bitrev_bits((uint32_t)(i >> 2), (int)info.y) << 2) | ((uint32_t)i & 3u));
-        }
-        pos[j] = p;
-        ord[j] = (uint32_t)j;
-    }
-}
-
-/* row update, step 1: natural index -> table row (or the skip marker), occurrence number j */
+/* row update, step 1: natural index -> table row (the mapping documented on UpdateParams) or the skip
+ * marker, occurrence number j */
 __global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
                                                          uint32_t *__restrict__ ord)
 {
+    const uint32_t lane_mask = (1u << u.lane_bits) - 1u;
     for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = u.idx[j];
+        const uint32_t leaf = (uint32_t)(i >> u.lane_bits), lane = (uint32_t)i & lane_mask;
         uint32_t p = u.table_rows;
         if (u.bins) {
             const int32_t g = u.bins[j];
             if (g >= 0 && g < u.nbins) {
                 const uint2 info = u.bin_info[g];
-                if (i >= 0 && i < ((int64_t)1 << info.y)) p = info.x + bitrev_bits((uint32_t)i, (int)info.y);
+                if (i >= 0 && i < ((int64_t)1 << (info.y + u.lane_bits)))
+                    p = info.x + ((bitrev_bits(leaf, (int)info.y) << u.lane_bits) | lane);
             }
-        } else if (i >= 0 && i < u.n && ((uint32_t)i & u.own_mask) == u.own_val) {
-            p = bitrev_bits((uint32_t)(i >> u.shift), u.depth);
+        } else if (i >= 0 && i < u.n && (leaf & u.own_mask) == u.own_val) {
+            p = (bitrev_bits(leaf >> u.shift, u.depth) << u.lane_bits) | lane;
         }
         pos[j] = p;
         ord[j] = (uint32_t)j;
@@ -968,116 +907,66 @@ __global__ void __launch_bounds__(256) update_scatter_kernel(const int32_t *__re
     }
 }
 
-template <int PRF, int NV, int MODE>
-cudaError_t launch_one(const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
-{
-    auto kern = dpf_eval_kernel<PRF, NV, MODE>;
-    /* function attributes are per device and sticky: set them once per (device, size); contexts
-     * on different host threads may race here, hence the atomics (a duplicate set is harmless) */
-    static std::atomic<int> configured[64];   /* smem bytes + 1 last configured on each device, 0 = never */
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64 || configured[dev].load(std::memory_order_acquire) != (int)smem + 1) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        /* the kernels live in shared memory; L1 only sees broadcast table rows */
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) configured[dev].store((int)smem + 1, std::memory_order_release);
-    }
-    if (p.fuse_top) {
-        void *args[] = {const_cast<EvalParams *>(&p)};
-        return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3((unsigned)grid),
-                                           dim3((unsigned)(EvalShape<PRF, NV, MODE>::THREADS)), args, smem, stream);
-    }
-    kern<<<grid, (EvalShape<PRF, NV, MODE>::THREADS), smem, stream>>>(p);
-    return cudaGetLastError();
-}
+/* An instantiated evaluation kernel: its entry point, and the dynamic shared memory size last configured
+ * for it on each device (bytes + 1, 0 = never).  Function attributes are per device and sticky, so
+ * they are set once per (device, size); contexts on different host threads may race there, hence the
+ * atomics (a duplicate set is harmless). */
+struct EvalKernel {
+    const void *fn;
+    std::atomic<int> *configured;   /* [64] */
+};
 
 template <int PRF, int NV, int MODE>
-cudaError_t max_smem_one(int *bytes)
+EvalKernel eval_kernel()
 {
-    cudaFuncAttributes a;
-    cudaError_t e = cudaFuncGetAttributes(&a, dpf_eval_kernel<PRF, NV, MODE>);
-    if (e != cudaSuccess) return e;
-    int dev = 0, optin = 0;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-    if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
-    *bytes = optin - (int)a.sharedSizeBytes;
-    return cudaSuccess;
+    static std::atomic<int> configured[64];
+    return EvalKernel{reinterpret_cast<const void *>(dpf_eval_kernel<PRF, NV, MODE>), configured};
 }
 
-/* (prf, nv, mode) -> instantiation; modes 1, 2 and 6 never touch the table, so NV = 4 only; grouped
- * evaluation (both kinds of key) takes 16 columns per pass, early-terminated evaluation 16 or 32 */
+/* The instantiated kernels of one PRF.  Every mode runs at 16 columns per pass (nv = 4); the fused
+ * modes also at 32, the standard one at 64 as well.  Grouped evaluation (both kinds of key) takes 16
+ * columns per pass, and the modes that never touch the table need no other width. */
 template <int PRF>
-cudaError_t launch_prf(int nv, int mode, const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
+EvalKernel eval_kernel_of(int nv, int mode)
 {
-    if (mode == MODE_EXPAND) return launch_one<PRF, 4, MODE_EXPAND>(p, grid, smem, stream);
-    if (mode == MODE_EXPAND_ET) return launch_one<PRF, 4, MODE_EXPAND_ET>(p, grid, smem, stream);
-    if (mode == MODE_FUSED_ET) {
-        if (nv == 4) return launch_one<PRF, 4, MODE_FUSED_ET>(p, grid, smem, stream);
-        if (nv == 8) return launch_one<PRF, 8, MODE_FUSED_ET>(p, grid, smem, stream);
-        return cudaErrorInvalidValue;
+    if (nv == 4) {
+        switch (mode) {
+        case MODE_FUSED: return eval_kernel<PRF, 4, MODE_FUSED>();
+        case MODE_EXPAND: return eval_kernel<PRF, 4, MODE_EXPAND>();
+        case MODE_FRONTIER: return eval_kernel<PRF, 4, MODE_FRONTIER>();
+        case MODE_GROUPED: return eval_kernel<PRF, 4, MODE_GROUPED>();
+        case MODE_FUSED_ET: return eval_kernel<PRF, 4, MODE_FUSED_ET>();
+        case MODE_EXPAND_ET: return eval_kernel<PRF, 4, MODE_EXPAND_ET>();
+        case MODE_GROUPED_ET: return eval_kernel<PRF, 4, MODE_GROUPED_ET>();
+        case MODE_FUSED_TMA:        /* AES: no shared memory left beside the tables */
+            if constexpr (PRF != PRF_AES128) return eval_kernel<PRF, 4, MODE_FUSED_TMA>();
+            break;
+        case MODE_FUSED_COLSPLIT:   /* Salsa/ChaCha bind the ALU pipe, not the data pipe */
+            if constexpr (PRF == PRF_AES128) return eval_kernel<PRF, 4, MODE_FUSED_COLSPLIT>();
+            break;
+        }
+    } else if (nv == 8) {
+        if (mode == MODE_FUSED) return eval_kernel<PRF, 8, MODE_FUSED>();
+        if (mode == MODE_FUSED_ET) return eval_kernel<PRF, 8, MODE_FUSED_ET>();
+    } else if (nv == 16) {
+        if (mode == MODE_FUSED) return eval_kernel<PRF, 16, MODE_FUSED>();
     }
-    if (mode == MODE_FRONTIER) return launch_one<PRF, 4, MODE_FRONTIER>(p, grid, smem, stream);
-    if (mode == MODE_FUSED_COLSPLIT) {
-        if constexpr (PRF == PRF_AES128) return launch_one<PRF, 4, MODE_FUSED_COLSPLIT>(p, grid, smem, stream);
-        else return cudaErrorInvalidValue;   /* Salsa/ChaCha bind the ALU pipe, not the data pipe */
-    }
-    if (mode == MODE_GROUPED) return launch_one<PRF, 4, MODE_GROUPED>(p, grid, smem, stream);
-    if (mode == MODE_GROUPED_ET) return launch_one<PRF, 4, MODE_GROUPED_ET>(p, grid, smem, stream);
-    if (mode == MODE_FUSED_TMA) {
-        if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;    /* no shared memory left beside the tables */
-        else return launch_one<PRF, 4, MODE_FUSED_TMA>(p, grid, smem, stream);
-    }
-    if (nv == 4) return launch_one<PRF, 4, MODE_FUSED>(p, grid, smem, stream);
-    if (nv == 8) return launch_one<PRF, 8, MODE_FUSED>(p, grid, smem, stream);
-    if (nv == 16) return launch_one<PRF, 16, MODE_FUSED>(p, grid, smem, stream);
-    return cudaErrorInvalidValue;
+    return EvalKernel{nullptr, nullptr};
 }
 
-template <int PRF>
-cudaError_t max_smem_prf(int nv, int mode, int *bytes)
+/* (prf, nv, mode) -> its kernel, or {nullptr} when it is not instantiated */
+EvalKernel find_eval_kernel(int prf, int nv, int mode)
 {
-    if (mode == MODE_EXPAND) return max_smem_one<PRF, 4, MODE_EXPAND>(bytes);
-    if (mode == MODE_EXPAND_ET) return max_smem_one<PRF, 4, MODE_EXPAND_ET>(bytes);
-    if (mode == MODE_FUSED_ET) {
-        if (nv == 4) return max_smem_one<PRF, 4, MODE_FUSED_ET>(bytes);
-        if (nv == 8) return max_smem_one<PRF, 8, MODE_FUSED_ET>(bytes);
-        return cudaErrorInvalidValue;
+    switch (prf) {
+    case PRF_DUMMY: return eval_kernel_of<PRF_DUMMY>(nv, mode);
+    case PRF_SALSA20: return eval_kernel_of<PRF_SALSA20>(nv, mode);
+    case PRF_CHACHA20: return eval_kernel_of<PRF_CHACHA20>(nv, mode);
+    case PRF_AES128: return eval_kernel_of<PRF_AES128>(nv, mode);
+    default: return EvalKernel{nullptr, nullptr};
     }
-    if (mode == MODE_FRONTIER) return max_smem_one<PRF, 4, MODE_FRONTIER>(bytes);
-    if (mode == MODE_FUSED_COLSPLIT) {
-        if constexpr (PRF == PRF_AES128) return max_smem_one<PRF, 4, MODE_FUSED_COLSPLIT>(bytes);
-        else return cudaErrorInvalidValue;
-    }
-    if (mode == MODE_GROUPED) return max_smem_one<PRF, 4, MODE_GROUPED>(bytes);
-    if (mode == MODE_GROUPED_ET) return max_smem_one<PRF, 4, MODE_GROUPED_ET>(bytes);
-    if (mode == MODE_FUSED_TMA) {
-        if constexpr (PRF == PRF_AES128) return cudaErrorInvalidValue;
-        else return max_smem_one<PRF, 4, MODE_FUSED_TMA>(bytes);
-    }
-    if (nv == 4) return max_smem_one<PRF, 4, MODE_FUSED>(bytes);
-    if (nv == 8) return max_smem_one<PRF, 8, MODE_FUSED>(bytes);
-    if (nv == 16) return max_smem_one<PRF, 16, MODE_FUSED>(bytes);
-    return cudaErrorInvalidValue;
 }
 
 }  // namespace
-
-int eval_threads(int prf, int nv, int mode)
-{
-    if (prf == PRF_AES128 && mode == MODE_FUSED_COLSPLIT) return 512;
-    if (prf == PRF_AES128) return nv <= 8 ? DPF_AES_THREADS : 256;
-    return nv <= 8 ? 256 : 384;
-}
-
-int eval_min_blocks(int prf, int nv)
-{
-    if (prf == PRF_AES128) return 1;
-    return nv <= 8 ? 2 : 1;
-}
 
 cudaError_t probe_dynamic_smem_base(uint32_t *base, cudaStream_t stream)
 {
@@ -1099,24 +988,38 @@ cudaError_t upload_aes_table(const uint32_t *te0_256)
 
 cudaError_t launch_eval(int prf, int nv, int mode, const EvalParams &p, int grid, size_t smem, cudaStream_t stream)
 {
-    switch (prf) {
-    case PRF_DUMMY: return launch_prf<PRF_DUMMY>(nv, mode, p, grid, smem, stream);
-    case PRF_SALSA20: return launch_prf<PRF_SALSA20>(nv, mode, p, grid, smem, stream);
-    case PRF_CHACHA20: return launch_prf<PRF_CHACHA20>(nv, mode, p, grid, smem, stream);
-    case PRF_AES128: return launch_prf<PRF_AES128>(nv, mode, p, grid, smem, stream);
-    default: return cudaErrorInvalidValue;
+    const EvalKernel k = find_eval_kernel(prf, nv, mode);
+    if (k.fn == nullptr) return cudaErrorInvalidValue;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 0 || dev >= 64 || k.configured[dev].load(std::memory_order_acquire) != (int)smem + 1) {
+        e = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        /* the kernels live in shared memory; L1 only sees broadcast table rows */
+        e = cudaFuncSetAttribute(k.fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < 64) k.configured[dev].store((int)smem + 1, std::memory_order_release);
     }
+    const dim3 block((unsigned)eval_block_shape(prf, nv, mode).threads);
+    void *args[] = {const_cast<EvalParams *>(&p)};
+    if (p.fuse_top) return cudaLaunchCooperativeKernel(k.fn, dim3((unsigned)grid), block, args, smem, stream);
+    cudaLaunchKernel(k.fn, dim3((unsigned)grid), block, args, smem, stream);   /* as <<<>>>: read back below */
+    return cudaGetLastError();
 }
 
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes)
 {
-    switch (prf) {
-    case PRF_DUMMY: return max_smem_prf<PRF_DUMMY>(nv, mode, bytes);
-    case PRF_SALSA20: return max_smem_prf<PRF_SALSA20>(nv, mode, bytes);
-    case PRF_CHACHA20: return max_smem_prf<PRF_CHACHA20>(nv, mode, bytes);
-    case PRF_AES128: return max_smem_prf<PRF_AES128>(nv, mode, bytes);
-    default: return cudaErrorInvalidValue;
-    }
+    const EvalKernel k = find_eval_kernel(prf, nv, mode);
+    if (k.fn == nullptr) return cudaErrorInvalidValue;
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, k.fn);
+    if (e != cudaSuccess) return e;
+    int dev = 0, optin = 0;
+    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+    if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
+    *bytes = optin - (int)a.sharedSizeBytes;
+    return cudaSuccess;
 }
 
 cudaError_t launch_mac_tma(const MacParams &p, int grid, cudaStream_t stream)
@@ -1153,25 +1056,14 @@ cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t wo
     return cudaGetLastError();
 }
 
-cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
+cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits, int lane_bits,
                                  int cols, int stride, int sm_count, cudaStream_t stream)
 {
     const uint64_t total = rows * (uint64_t)cols;
     const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
     int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
     if (grid < 1) grid = 1;
-    permute_table_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, cols, stride);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_permute_table_et(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
-                                    int cols, int stride, int sm_count, cudaStream_t stream)
-{
-    const uint64_t total = rows * (uint64_t)cols;
-    const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
-    int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
-    if (grid < 1) grid = 1;
-    permute_table_et_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, cols, stride);
+    permute_table_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, lane_bits, cols, stride);
     return cudaGetLastError();
 }
 
@@ -1187,9 +1079,7 @@ cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int e
     if (u.count <= 0) return cudaSuccess;
     const int64_t cap = (int64_t)std::max(sm_count, 1) * 16;
     const int grid_map = (int)std::max<int64_t>(1, std::min<int64_t>((u.count + 255) / 256, cap));
-    if (u.lane_bits && u.bins) update_map_group_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
-    else if (u.lane_bits) update_map_et_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
-    else update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
+    update_map_kernel<<<grid_map, 256, 0, stream>>>(u, w.pos_in, w.ord_in);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     size_t temp_bytes = w.temp_bytes;

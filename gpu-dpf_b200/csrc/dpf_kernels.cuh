@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dpf_core.cuh"
+
 namespace b200dpf {
 
 /* One traversal phase of a launch: which subtrees the work items are, where an item starts and
@@ -108,29 +110,69 @@ struct EvalParams {
     uint32_t off_tile_bar;
 };
 
-/* Kernel modes. */
-enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3,
-       MODE_FUSED_TMA = 4, /* MODE_FUSED with each work item's table rows staged into shared memory by
-                             cp.async.bulk (16-column tables, non-AES PRFs, whole-warp key groups) */
-       /* early-terminated keys (four table rows per leaf): the tree is over leaves, the table, the
-        * leaf cache (EvalParams::n_local), the result and the shares (EvalParams::n) over rows; leaf
-        * position p owns rows 4p..4p+3 of the device table */
-       MODE_FUSED_ET = 5,  /* MODE_FUSED, nv = 4 or 8 */
-       MODE_EXPAND_ET = 6, /* MODE_EXPAND: shares[key][4 * leaf + lane] */
-       /* MODE_FUSED for AES at 16 columns with >= 4 keys per warp: the four lanes of a key quad split
-        * each table row, lane L loading columns 4 (L & 3) .. +3, and the quad's leaf values travel by
-        * SHFL instead, so a row costs the shared-memory data pipe one 16-byte load per lane, not four */
-       MODE_FUSED_COLSPLIT = 7,
-       /* MODE_GROUPED for early-terminated keys, nv = 4: GroupDesc::depth is the bin's leaf depth and
-        * the bin's leaf position p owns its rows 4p..4p+3 */
-       MODE_GROUPED_ET = 8,
-       MODE_COUNT = 9 };
+/* Kernel modes: the MODE of dpf_eval_kernel<PRF, NV, MODE>.  Each is a combination of the properties
+ * of ModeTraits, and mode_traits below is the one place that says which. */
+enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3, MODE_FUSED_TMA = 4,
+       MODE_FUSED_ET = 5, MODE_EXPAND_ET = 6, MODE_FUSED_COLSPLIT = 7, MODE_GROUPED_ET = 8, MODE_COUNT = 9 };
 
-/* Threads per block (for a kernel mode: the column-split AES kernel runs 16 warps) / minimum blocks per SM of the kernel instantiated for
- * (prf, nv) where nv = uint4 (4 int32 columns) of a table row handled per pass:
- * 4, 8 or 16. */
-int eval_threads(int prf, int nv, int mode);
-int eval_min_blocks(int prf, int nv);
+/* What a mode's leaves feed (ModeTraits::feeds). */
+enum { FEEDS_MAC,         /* the inner product against the table: out[key][col] */
+       FEEDS_SHARES,      /* the share vector, shares[key][index] in natural order */
+       FEEDS_FRONTIER };  /* whole seeds of the frontier nodes (frontier_out) */
+/* How a table row reaches the registers of a FEEDS_MAC mode (ModeTraits::row_load). */
+enum { ROWS_BROADCAST,    /* every lane loads the whole row: one broadcast load serves the warp's keys */
+       /* the four lanes of a key quad split each row, lane L loading columns 4 (L & 3) .. +3, and the
+        * quad's leaf values travel by SHFL instead, so a row costs the shared-memory data pipe one
+        * 16-byte load per lane, not four (AES binds that pipe) */
+       ROWS_COLSPLIT,
+       /* each work item's rows are staged into shared memory by one cp.async.bulk (TMA) when the item
+        * is drawn (16-column tables, whole-warp key groups; AES has no shared memory left for them) */
+       ROWS_STAGED };
+
+struct ModeTraits {
+    int feeds;                /* FEEDS_*                                                          */
+    int row_load;             /* ROWS_*                                                           */
+    /* log2 table rows per leaf: 2 for early-terminated keys, whose tree is over leaves while the
+     * table, the leaf cache (EvalParams::n_local), the result and the shares (EvalParams::n) are over
+     * rows: leaf position p owns rows 4p..4p+3 of the device table, shares[key][4 * leaf + l] */
+    int row_shift;
+    /* batch PIR: each key group evaluates its own bin, described by EvalParams::groups */
+    bool grouped;
+};
+
+__host__ __device__ constexpr ModeTraits mode_traits(int mode)
+{
+    switch (mode) {                            /* feeds           row_load        row_shift grouped */
+    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false};
+    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false};
+    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false};
+    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true};
+    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false};
+    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false};
+    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false};
+    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false};
+    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true};
+    default:                  return ModeTraits{-1, -1, 0, false};
+    }
+}
+
+/* Block shape of the evaluation kernel instantiated for (prf, nv, mode), nv = uint4 (4 int32 columns)
+ * of a table row handled per pass: 4, 8 or 16.  The kernel's __launch_bounds__ and the host's grid
+ * and shared-memory plan both read it.  AES needs 128 KiB of the SM's shared memory for its tables,
+ * so one block per SM; accumulators (4*nv registers) decide how many threads fit the register file.
+ * The column-split AES kernel holds 4 row words per leaf instead of 16 and fits 128 registers. */
+#ifndef DPF_AES_THREADS
+#define DPF_AES_THREADS 384      /* 12 warps: on an H100 1.5 % (n=2^20) and 3 % (n=2^16) faster than 8 (256) */
+#endif
+struct BlockShape {
+    int threads, min_blocks;     /* threads per block, minimum resident blocks per SM */
+};
+__host__ __device__ constexpr BlockShape eval_block_shape(int prf, int nv, int mode)
+{
+    if (prf == PRF_AES128)
+        return BlockShape{mode_traits(mode).row_load == ROWS_COLSPLIT ? 512 : nv <= 8 ? DPF_AES_THREADS : 256, 1};
+    return BlockShape{nv <= 8 ? 256 : 384, nv <= 8 ? 2 : 1};
+}
 
 /* Shared-window address of the first dynamic shared memory byte (probed). */
 cudaError_t probe_dynamic_smem_base(uint32_t *base, cudaStream_t stream);
@@ -138,8 +180,8 @@ cudaError_t probe_dynamic_smem_base(uint32_t *base, cudaStream_t stream);
 /* Upload the AES T-table to this device's constant memory. */
 cudaError_t upload_aes_table(const uint32_t *te0_256);
 
-/* One pass of the fused evaluation (mode 0), the share expansion (mode 1) or the
- * frontier build (mode 2; nv must be 4 for modes 1 and 2).
+/* One pass of the evaluation kernel of (prf, nv, mode); cudaErrorInvalidValue when that kernel is not
+ * instantiated (the table is in dpf_kernels.cu).
  * grid = number of persistent blocks; smem_bytes = dynamic shared memory.  With p.fuse_top the
  * launch is cooperative (every block resident), which the in-kernel grid barrier relies on. */
 cudaError_t launch_eval(int prf, int nv, int mode, const EvalParams &p, int grid, size_t smem_bytes,
@@ -180,24 +222,23 @@ cudaError_t launch_keygen(int prf, const int64_t *alphas, const uint8_t *seeds44
 /* Maximum dynamic shared memory the evaluation kernel may be given. */
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
-/* table[q][c] = stage[bitrev_bits(q)][c] for q < rows, c < cols; padded columns
- * [cols, stride) are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM
- * count to cap their grids at a few waves.  With lane_bits = 2 (early-terminated contexts) rows
- * move in runs of four: table[4q + l] = stage[4 bitrev_bits(q) + l], rows = 4 * 2^bits. */
-cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
+/* table[q][c] = stage[(bitrev_bits(q >> lane_bits) << lane_bits) | (q & (2^lane_bits - 1))][c] for
+ * q < rows, c < cols: rows move in runs of 2^lane_bits (one leaf; 4 on early-terminated contexts),
+ * rows = 2^(bits + lane_bits).  Padded columns [cols, stride) are left untouched (pre-zeroed).  The
+ * grid-stride helpers take the device's SM count to cap their grids at a few waves. */
+cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits, int lane_bits,
                                  int cols, int stride, int sm_count, cudaStream_t stream);
-cudaError_t launch_permute_table_et(const int32_t *stage, int32_t *table, uint64_t rows, int bits,
-                                    int cols, int stride, int sm_count, cudaStream_t stream);
 
 /* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
- * j < count, the last occurrence of a position winning.  Position of natural index i:
- *   bins == null   skip unless 0 <= i < n and (i & own_mask) == own_val;
- *                  else bitrev_depth(i >> shift)                      (whole table or one shard)
- *   bins != null   bin g = bins[j] (skip unless 0 <= g < nbins); skip unless 0 <= i < 2^bin_info[g].y;
- *                  else bin_info[g].x + bitrev_{bin_info[g].y}(i)     (grouped context)
- *   bins != null and lane_bits = 2 (early-terminated grouped context, .y = the bin's leaf depth):
- *                  skip unless 0 <= i < 4 << bin_info[g].y;
- *                  else bin_info[g].x + (bitrev_{bin_info[g].y}(i >> 2) << 2 | (i & 3))
+ * j < count, the last occurrence of a position winning.  Natural index i is row i & (2^lane_bits - 1)
+ * of leaf v = i >> lane_bits, and its position is
+ *   bins == null   skip unless 0 <= i < n and (v & own_mask) == own_val;
+ *                  else bitrev_depth(v >> shift) << lane_bits | (i & (2^lane_bits - 1))
+ *                                                                     (whole table or one shard)
+ *   bins != null   bin g = bins[j] (skip unless 0 <= g < nbins; .y = the bin's leaf depth);
+ *                  skip unless 0 <= i < 2^(bin_info[g].y + lane_bits);
+ *                  else bin_info[g].x + (bitrev_{bin_info[g].y}(v) << lane_bits | (i & (2^lane_bits - 1)))
+ *                                                                     (grouped context)
  * Skipped entries are never written. */
 struct UpdateParams {
     const int64_t *idx;       /* [count] natural indices                                      */
@@ -210,11 +251,8 @@ struct UpdateParams {
     uint32_t own_mask, own_val;
     int shift, depth;
     uint32_t table_rows;      /* rows of the device table: the skip marker, larger than every position */
-    int lane_bits;            /* log2 rows per leaf: 0, or 2 on an early-terminated context, where
-                                 row i < n belongs to leaf v = i >> 2, is owned when (v & own_mask)
-                                 == own_val and goes to row 4 bitrev_depth(v >> shift) + (i & 3).
-                                 (It fills the alignment gap before `table`: the struct's layout is
-                                 that of the update kernels without it.)                          */
+    int lane_bits;            /* log2 rows per leaf: 0, or 2 on an early-terminated context
+                                 (it fills the alignment gap before `table`)                      */
     int32_t *table;           /* [table_rows][stride], 64-byte rows; pad columns are not touched */
     int cols, stride;
 };
