@@ -27,6 +27,8 @@ SYMBOLS = [
     "b200dpf_ctx_device", "b200dpf_ctx_last_launches", "b200dpf_ctx_set_subtree_log2",
     "b200dpf_gen_et", "b200dpf_gen_batch_et", "b200dpf_eval_cpu_et", "b200dpf_key_pack_et", "b200dpf_key_unpack_et",
     "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf", "b200dpf_group_create_et",
+    "b200dpf_gen_xor", "b200dpf_gen_batch_xor", "b200dpf_eval_cpu_xor", "b200dpf_key_pack_xor", "b200dpf_key_unpack_xor",
+    "b200dpf_create_xor",
 ]
 
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
@@ -94,6 +96,12 @@ def load():
     L.b200dpf_create_et.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
     L.b200dpf_group_create_et.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
+    L.b200dpf_gen_xor.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
+    L.b200dpf_gen_batch_xor.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
+    L.b200dpf_eval_cpu_xor.argtypes = [_i32p, C.c_int, _u32p]
+    L.b200dpf_key_pack_xor.argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.b200dpf_key_unpack_xor.argtypes = [C.c_char_p, C.c_size_t, _i32p]
+    L.b200dpf_create_xor.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     return L
 
 
@@ -238,18 +246,75 @@ def key_unpack_et(packed):
     return key
 
 
+def _xor_key_n(key):
+    """rows of an XOR-shared key (slot 0 = (d, 7, 0, 0), slot 130 = 128 * 2^d), or -1"""
+    d, w = int(key[0]), int(key[1])
+    if w != 7 or key[2] or key[3] or not 1 <= d <= 24:
+        return -1
+    n = int(np.uint32(key[130 * 4]))
+    return n if n == 128 << d and not key[130 * 4 + 1:130 * 4 + 4].any() else -1
+
+
+def gen_xor(alpha, n, seed_bytes, prf):
+    """XOR-shared key pair for row alpha of an n-row table (DESIGN.md section 10); >= 44 seed bytes"""
+    a = np.zeros(KEY_WORDS, np.int32)
+    b = np.zeros(KEY_WORDS, np.int32)
+    _check(lib().b200dpf_gen_xor(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), "b200dpf_gen_xor")
+    return a, b
+
+
+def gen_batch_xor(alphas, n, seed_bytes, prf, nthreads=0):
+    """seed_bytes: 44 bytes of entropy per key, concatenated"""
+    alphas = np.ascontiguousarray(alphas, np.int64)
+    if len(seed_bytes) != 44 * len(alphas):
+        raise ValueError("gen_batch_xor needs 44 seed bytes per key (%d keys, %d bytes)" % (len(alphas), len(seed_bytes)))
+    a = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    b = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    _check(lib().b200dpf_gen_batch_xor(alphas, bytes(seed_bytes), len(alphas), n, prf, nthreads, a, b), "b200dpf_gen_batch_xor")
+    return a, b
+
+
+def eval_cpu_xor(key, prf):
+    """share bits packed, uint32 [n / 32]: row i is bit (i & 31) of word i >> 5"""
+    key = np.ascontiguousarray(key, np.int32)
+    n = _xor_key_n(key)
+    if n < 0:
+        raise B200DPFError("not an XOR-shared key")
+    out = np.zeros(n // 32, np.uint32)
+    _check(lib().b200dpf_eval_cpu_xor(key, prf, out), "b200dpf_eval_cpu_xor")
+    return out
+
+
+def key_pack_xor(key):
+    key = np.ascontiguousarray(key, np.int32)
+    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
+    n = C.c_size_t()
+    _check(lib().b200dpf_key_pack_xor(key, buf, len(buf), C.byref(n)), "b200dpf_key_pack_xor")
+    return buf.raw[:n.value]
+
+
+def key_unpack_xor(packed):
+    key = np.zeros(KEY_WORDS, np.int32)
+    _check(lib().b200dpf_key_unpack_xor(bytes(packed), len(packed), key), "b200dpf_key_unpack_xor")
+    return key
+
+
 class Context:
     """One table (or one entry-range shard of it) resident on one GPU.  early_termination=True makes a
-    context for early-terminated keys (b200dpf_create_et): four table rows per tree leaf."""
+    context for early-terminated keys (b200dpf_create_et): four table rows per tree leaf.  xor=True makes
+    one for XOR-shared keys (b200dpf_create_xor): 128 rows per leaf, and results that XOR (not add) to
+    the selected row."""
 
-    def __init__(self, table, device=0, shard_rank=0, shard_count=1, early_termination=False):
+    def __init__(self, table, device=0, shard_rank=0, shard_count=1, early_termination=False, xor=False):
+        if xor and early_termination:
+            raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
         table = np.ascontiguousarray(table, np.int32)
         assert table.ndim == 2
         self.n, self.entry_size = table.shape
         self.handle = C.c_void_p()
-        create = lib().b200dpf_create_et if early_termination else lib().b200dpf_create
-        _check(create(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
-                      device, shard_rank, shard_count), "b200dpf_create_et" if early_termination else "b200dpf_create")
+        name = "b200dpf_create_xor" if xor else "b200dpf_create_et" if early_termination else "b200dpf_create"
+        _check(getattr(lib(), name)(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
+                                    device, shard_rank, shard_count), name)
 
     @classmethod
     def multi(cls, table, devices, axis=0):

@@ -141,10 +141,11 @@ struct b200dpf_ctx {
     int shard_rank = 0, shard_count = 1, shard_bits = 0;
     int64_t n_local = 0;
     int depth_local = 0;
-    /* log2 table rows per tree leaf: 0, or 2 on an early-terminated context (b200dpf_create_et).  n,
-     * n_local, the table, the leaf cache and the results count rows; depth, depth_local, the shards,
-     * the work items and the frontier count leaves. */
+    /* log2 table rows per tree leaf: 0, 2 on an early-terminated context (b200dpf_create_et) or 7 on an
+     * XOR-shared one (b200dpf_create_xor).  n, n_local, the table, the leaf cache and the results count
+     * rows; depth, depth_local, the shards, the work items and the frontier count leaves. */
     int lane_bits = 0;
+    bool is_xor() const { return lane_bits == host::XOR_LOG2_ROWS_PER_LEAF; }
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
     DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
@@ -370,8 +371,14 @@ KeyLayout reference_layout() { return KeyLayout{131u, 129u, 0}; }               
 KeyLayout compact_layout(int depth) { return KeyLayout{2u + 4u * (uint32_t)depth, 1u, 1}; }   /* b200dpf_key_pack */
 
 /* compact form of one key straight into `dst` (b200dpf_key_pack without the checks); the magic is
- * "DPF2", or "DPE4" for an early-terminated key */
-constexpr char kMagic[] = "DPF2", kMagicEt[] = "DPE4";
+ * "DPF2", "DPE4" for an early-terminated key or "DPX7" for an XOR-shared one */
+constexpr char kMagic[] = "DPF2", kMagicEt[] = "DPE4", kMagicXor[] = "DPX7";
+
+/* the compact-form magic of the keys a context takes */
+inline const char *ctx_magic(const b200dpf_ctx *c)
+{
+    return c->is_xor() ? kMagicXor : c->lane_bits ? kMagicEt : kMagic;
+}
 
 inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char *magic = kMagic)
 {
@@ -407,9 +414,27 @@ inline int check_key_et_n(const int32_t *key, int64_t b, int64_t n)
                 (long long)kn);
 }
 
-/* key number `b` of a batch must be of the context's kind (standard or early-terminated) and n */
+/* key number `b` of a batch must be an XOR-shared key for n rows */
+inline int check_key_xor_n(const int32_t *key, int64_t b, int64_t n)
+{
+    const int64_t kn = key ? host::key_xor_n(key) : -1;
+    if (kn == n) return B200DPF_OK;
+    if (key && host::key_n(key) >= 0)
+        return fail(B200DPF_EINVAL, "key %lld is a standard key; this XOR-shared context takes keys of b200dpf_gen_xor", (long long)b);
+    if (key && host::key_et_n(key) >= 0)
+        return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this XOR-shared context takes keys of b200dpf_gen_xor",
+                    (long long)b);
+    return fail(B200DPF_EINVAL, "key %lld is not an XOR-shared key for n=%lld (its n: %lld)", (long long)b, (long long)n,
+                (long long)kn);
+}
+
+/* key number `b` of a batch must be of the context's kind (standard, early-terminated or XOR-shared) and n */
 inline int check_key(const b200dpf_ctx *c, const int32_t *key, int64_t b)
 {
+    if (c->is_xor()) return check_key_xor_n(key, b, c->n);
+    if (key && host::key_xor_n(key) >= 0)
+        return fail(B200DPF_EINVAL, "key %lld is an XOR-shared key; this context takes %s keys", (long long)b,
+                    c->lane_bits ? "early-terminated" : "standard");
     if (!c->lane_bits) {
         if (key && host::key_et_n(key) >= 0)
             return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this context takes standard keys", (long long)b);
@@ -443,10 +468,12 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
      * MAC-only passes over that cache.  Without the cache (disabled or lane-split batches) wide
      * entries use one tree expansion per 64 columns. */
     const bool et = c->lane_bits != 0;   /* early-terminated: 32 columns per pass at most */
-    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache) ? 4 : (c->entry_pad <= 32 || et ? 8 : 16);
+    const bool xk = c->is_xor();         /* XOR-shared: 16 columns per pass, no leaf cache */
+    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache || xk) ? 4 : (c->entry_pad <= 32 || et ? 8 : 16);
     const int passes = mode_main == MODE_FUSED ? (want_cache ? 1 : c->entry_pad / (4 * nv)) : 1;
     /* the kernel modes of this context's kind */
-    const int mode_fused = et ? MODE_FUSED_ET : MODE_FUSED, mode_expand = et ? MODE_EXPAND_ET : MODE_EXPAND;
+    const int mode_fused = xk ? MODE_FUSED_XOR : et ? MODE_FUSED_ET : MODE_FUSED;
+    const int mode_expand = xk ? MODE_EXPAND_XOR : et ? MODE_EXPAND_ET : MODE_EXPAND;
     /* optional variant: the rows of each work item staged into shared memory by cp.async.bulk */
     bool tma_rows = K.tma_rows != 0 && K.one_launch != 0 && c->coop_ok != 0 && mode_main == MODE_FUSED && c->entry_pad == 16 &&
                     prf != B200DPF_PRF_AES128 && nkeys >= 17 && !et;
@@ -457,6 +484,9 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     int kpw_log2 = 5;
     if (K.lane_split != 0)
         while (kpw_log2 > 0 && ((int64_t)1 << (kpw_log2 - 1)) >= nkeys) kpw_log2--;
+    /* the XOR kernel splits rows across the four lanes of a key quad, which must hold four keys (the
+     * missing ones of a smaller batch are duplicates whose results are dropped) */
+    if (xk && mode_main == MODE_FUSED) kpw_log2 = std::max(kpw_log2, 2);
     int64_t key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
     /* AES binds the shared-memory data pipe, and a broadcast row load is charged for every lane's copy
      * of the row: with at least 4 keys per warp, each lane of a key quad loads a quarter of the row and
@@ -484,8 +514,13 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
          *   AES n=2^16: auto 319.3k; s=4 317.5k, 5 318.1k, 6 318.1k, 7 300.5k
          *   ChaCha n=2^20: auto 19.18k; s=5 18.94k, 6 19.13k, 7 19.19k */
         const int s_cap = want_frontier ? 7 : ((prf == B200DPF_PRF_AES128) ? 8 : 10);
-        const int s_floor = want_frontier ? 3 : 5;
-        const int64_t items_per_warp = want_frontier ? 24 : 6;
+        /* XOR-shared keys: a leaf is 128 rows of work, so a few items per warp balance the tail and the
+         * smallest items keep every warp busy at small n.  AES, E=16, B=512, H100 80GB HBM3 at a 700 W
+         * power limit, SM clock 1980 MHz, ms per batch (DESIGN.md section 10):
+         *   n=2^16: auto 0.107; s=1 0.103, 2 0.148, 3 0.196, 4 0.262, 5 0.490
+         *   n=2^20: auto 0.971; s=1 0.989, 2 0.980, 3 0.971, 4 0.975, 5 0.975, 6 0.973 */
+        const int s_floor = xk ? 1 : want_frontier ? 3 : 5;
+        const int64_t items_per_warp = xk ? 4 : want_frontier ? 24 : 6;
         s = std::min(c->depth_local, std::min(L.s_max, s_cap));
         while (s > s_floor &&
                ((((int64_t)1 << (c->depth_local - s)) * key_groups) >> (5 - kpw_log2)) < items_per_warp * warps)
@@ -757,7 +792,8 @@ int run_pipeline(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int6
     const b200dpf_ctx::Knobs &K = c->knobs;
     int rc = B200DPF_OK;
     int launches = 0;
-    const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0;
+    /* XOR-shared keys have no leaf cache: a further 16 columns re-walk the tree, 1/128 of the rows */
+    const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0 && !c->is_xor();
     const size_t per_group = 32u * (size_t)c->n_local * sizeof(uint32_t);
     const size_t cap = (size_t)std::max(K.leaf_cache_mb, 1) << 20;
     if (!wide || per_group > cap) {
@@ -1091,33 +1127,93 @@ int b200dpf_key_pack_et(const int32_t *key, uint8_t *out, size_t out_cap, size_t
     return B200DPF_OK;
 }
 
-int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key)
+}  // extern "C"
+
+/* b200dpf_key_unpack_et / _xor: a key of 2^lane_bits rows per leaf and at most max_depth levels */
+static int key_unpack_leaves(const uint8_t *in, size_t in_len, int32_t *key, const char *magic, int lane_bits, int max_depth,
+                             const char *name)
 {
     if (!in || !key) return fail(B200DPF_EINVAL, "null buffer");
-    if (in_len < 32 || std::memcmp(in, kMagicEt, 4) != 0) return fail(B200DPF_EINVAL, "key_unpack_et: bad header");
+    if (in_len < 32 || std::memcmp(in, magic, 4) != 0) return fail(B200DPF_EINVAL, "%s: bad header", name);
     const int depth = in[4];
     bool pad_zero = true;
     for (int i = 5; i < 16; i++) pad_zero = pad_zero && in[i] == 0;
-    if (depth < 1 || depth > host::ET_MAX_DEPTH || !pad_zero || in_len != b200dpf_key_packed_size(depth))
-        return fail(B200DPF_EINVAL, "key_unpack_et: depth %d does not match %zu bytes", depth, in_len);
+    if (depth < 1 || depth > max_depth || !pad_zero || in_len != b200dpf_key_packed_size(depth))
+        return fail(B200DPF_EINVAL, "%s: depth %d does not match %zu bytes", name, depth, in_len);
     std::memset(key, 0, sizeof(int32_t) * host::KEY_WORDS);
     uint8_t *k = reinterpret_cast<uint8_t *>(key);
     k[16 * host::SLOT_DEPTH] = (uint8_t)depth;
-    k[16 * host::SLOT_DEPTH + 4] = (uint8_t)host::ET_LOG2_ROWS_PER_LEAF;
+    k[16 * host::SLOT_DEPTH + 4] = (uint8_t)lane_bits;
     std::memcpy(k + 16 * host::SLOT_ROOT, in + 16, 16);
     for (int L = 0; L < depth; L++) {
         const uint8_t *o = in + 32 + 64 * L;
         std::memcpy(k + 16 * (host::SLOT_CW1 + 2 * L), o, 32);
         std::memcpy(k + 16 * (host::SLOT_CW2 + 2 * L), o + 32, 32);
     }
-    const uint64_t n = (uint64_t)1 << (depth + host::ET_LOG2_ROWS_PER_LEAF);
+    const uint64_t n = (uint64_t)1 << (depth + lane_bits);
     std::memcpy(k + 16 * host::SLOT_N, &n, 8);
     return B200DPF_OK;
 }
 
+extern "C" {
+
+int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key)
+{
+    return key_unpack_leaves(in, in_len, key, kMagicEt, host::ET_LOG2_ROWS_PER_LEAF, host::ET_MAX_DEPTH, "key_unpack_et");
+}
+
+/* ---- XOR-shared keys ---- */
+
+int b200dpf_gen_xor(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf, int32_t *key_a, int32_t *key_b)
+{
+    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
+    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "gen_xor needs at least 44 bytes of seed (got %zu)", seed_len);
+    if (host::gen_xor(alpha, n, seed, prf, key_a, key_b) != 0)
+        return fail(B200DPF_EINVAL, "gen_xor: need power-of-two n in [256, 2^31], 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
+                    (long long)alpha, (long long)n, prf);
+    return B200DPF_OK;
+}
+
+int b200dpf_gen_batch_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int nthreads,
+                          int32_t *keys_a, int32_t *keys_b)
+{
+    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_xor argument");
+    if (!gen_parallel(count, nthreads, [&](int64_t i) {
+            return host::gen_xor(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
+        }))
+        return fail(B200DPF_EINVAL, "gen_batch_xor: invalid alpha/n/prf in batch");
+    return B200DPF_OK;
+}
+
+int b200dpf_eval_cpu_xor(const int32_t *key, int prf, uint32_t *bits)
+{
+    if (!key || !bits) return fail(B200DPF_EINVAL, "null buffer");
+    if (host::key_xor_n(key) < 0) return fail(B200DPF_EINVAL, "eval_cpu_xor: not an XOR-shared key");
+    if (host::eval_cpu_xor(key, prf, bits) != 0) return fail(B200DPF_EINVAL, "eval_cpu_xor: unknown prf id %d", prf);
+    return B200DPF_OK;
+}
+
+int b200dpf_key_pack_xor(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
+{
+    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
+    const int depth = host::key_xor_depth(key);
+    if (depth < 1 || host::key_xor_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack_xor: not an XOR-shared key");
+    const size_t need = b200dpf_key_packed_size(depth);
+    if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack_xor: need %zu bytes, have %zu", need, out_cap);
+    pack_compact(key, out, depth, kMagicXor);
+    if (written) *written = need;
+    return B200DPF_OK;
+}
+
+int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key)
+{
+    return key_unpack_leaves(in, in_len, key, kMagicXor, host::XOR_LOG2_ROWS_PER_LEAF, host::XOR_MAX_DEPTH, "key_unpack_xor");
+}
+
 }  // extern "C"
 
-/* b200dpf_create (lane_bits = 0) and b200dpf_create_et (lane_bits = 2: 2^lane_bits rows per leaf) */
+/* b200dpf_create (lane_bits = 0), b200dpf_create_et (lane_bits = 2: 2^lane_bits rows per leaf) and
+ * b200dpf_create_xor (lane_bits = 7) */
 static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int shard_rank,
                        int shard_count, int lane_bits)
 {
@@ -1215,7 +1311,8 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     const int nv0 = c->entry_pad <= 16 ? 4 : (c->entry_pad <= 32 ? 8 : 4);
     SmemLayout tmp;
     for (int prf = 0; prf < 4; prf++) {
-        smem_layout(c.get(), prf, nv0, lane_bits ? MODE_FUSED_ET : MODE_FUSED, &tmp);
+        if (c->is_xor()) smem_layout(c.get(), prf, 4, MODE_FUSED_XOR, &tmp);
+        else smem_layout(c.get(), prf, nv0, lane_bits ? MODE_FUSED_ET : MODE_FUSED, &tmp);
         smem_layout(c.get(), prf, 4, MODE_FRONTIER, &tmp);
     }
     *out = c.release();
@@ -1234,6 +1331,12 @@ int b200dpf_create_et(b200dpf_ctx **out, const int32_t *table, int64_t n, int en
                       int shard_rank, int shard_count)
 {
     return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::ET_LOG2_ROWS_PER_LEAF);
+}
+
+int b200dpf_create_xor(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
+                       int shard_rank, int shard_count)
+{
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::XOR_LOG2_ROWS_PER_LEAF);
 }
 
 int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *c) { return c ? 1 << c->lane_bits : -1; }
@@ -1320,7 +1423,7 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
             if (validate && (rc = check_key(c, keys[b], b))) return rc;
-            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, c->lane_bits ? kMagicEt : kMagic);
+            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, ctx_magic(c));
         }
         if (!c->multi)
             CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys.ptr) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
@@ -1344,7 +1447,7 @@ int b200dpf_eval_packed(b200dpf_ctx *c, const uint8_t *packed, int64_t nkeys, in
     const size_t stride = b200dpf_key_packed_size(c->depth);
     for (int64_t b = 0; b < nkeys; b++) {
         const uint8_t *k = packed + (size_t)b * stride;
-        if (std::memcmp(k, c->lane_bits ? kMagicEt : kMagic, 4) != 0 || k[4] != (uint8_t)c->depth)
+        if (std::memcmp(k, ctx_magic(c), 4) != 0 || k[4] != (uint8_t)c->depth)
             return fail(B200DPF_EINVAL, "packed key %lld: bad header or depth %d, table has depth %d (n=%lld)", (long long)b,
                         (int)k[4], c->depth, (long long)c->n);
     }

@@ -464,7 +464,8 @@ DPF_HD Seed expand_one(const TA &ta, const Seed &parent, uint32_t pos)
  *     void     leaf_prefetch(local_pos)      called before the leaf pair is expanded
  *     void     leaf_pair(local_pos, v0, v1)  consume leaves local_pos, local_pos+1
  *     void     node_pair(local_pos, c0, c1)  (FULL mode) consume whole seeds
- *     void     leaf_quads(local_pos, w0, w1) (ET) consume all four words of both leaves
+ *     void     leaf_quads(local_pos, w0, w1) (GROUP_LANES32 / GROUP_XOR128) consume all four
+ *                                        words of both leaves
  *     ta                                 AES table policy
  */
 
@@ -502,17 +503,35 @@ DPF_HD Seed add_lanes(const Seed &a, const Seed &b)
     return make_seed(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
 }
 
+/* Add in (Z/2)^128: the level-0 step of an XOR-shared key, whose leaf carries 128 one-bit
+ * table-row shares. */
+DPF_HD Seed xor128(const Seed &a, const Seed &b)
+{
+    return make_seed(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w);
+}
+
+/* The group the level-0 (leaf) step of a key works in, i.e. the kind of key:
+ *   GROUP_ADD128   Z/2^128, of which the leaf keeps the low 32 bits (standard keys);
+ *   GROUP_LANES32  (Z/2^32)^4, four row shares per leaf (early-terminated keys, DESIGN.md section 9);
+ *   GROUP_XOR128   (Z/2)^128, 128 one-bit row shares per leaf (XOR-shared keys, section 10).
+ * Every level above the leaves adds in Z/2^128 for all three. */
+enum { GROUP_ADD128 = 0, GROUP_LANES32 = 1, GROUP_XOR128 = 2 };
+
 /* The two leaves (FULL: frontier nodes) below a node of height 1, at local
- * positions pos and pos+1.  ET (early-terminated keys, DESIGN.md section 9): each leaf
- * keeps all four words of PRF + level-0 correction word, added lane-wise, and hands
- * them to env.leaf_quads(local_pos, w0, w1) -- leaf p's word l is the share of table
- * row 4p + l. */
-template <int PRF, bool FULL, class Env, bool ET = false>
+ * positions pos and pos+1.  GROUP_LANES32 and GROUP_XOR128: each leaf keeps all four
+ * words of PRF + level-0 correction word, combined in the level-0 group, and hands them
+ * to env.leaf_quads(local_pos, w0, w1) -- leaf p's word l is the share of table row
+ * 4p + l (GROUP_LANES32), or its bit b of row 128p + 32l + b (GROUP_XOR128). */
+template <int PRF, bool FULL, class Env, int GROUP = GROUP_ADD128>
 DPF_HD void eval_leaf_pair(Env &env, const Seed &seed, uint32_t pos, int level_base)
 {
     Seed l0, l1;
     const uint32_t bank = seed.x & 1u;
-    if constexpr (ET) {
+    if constexpr (GROUP == GROUP_XOR128) {
+        env.leaf_prefetch(pos);
+        expand_pair<PRF, false>(env.ta, seed, l0, l1);
+        env.leaf_quads(pos, xor128(l0, env.cw(0, bank, 0)), xor128(l1, env.cw(0, bank, 1)));
+    } else if constexpr (GROUP == GROUP_LANES32) {
         env.leaf_prefetch(pos);
         expand_pair<PRF, false>(env.ta, seed, l0, l1);
         env.leaf_quads(pos, add_lanes(l0, env.cw(0, bank, 0)), add_lanes(l1, env.cw(0, bank, 1)));
@@ -545,7 +564,7 @@ DPF_HD void eval_leaf_pair(Env &env, const Seed &seed, uint32_t pos, int level_b
  * binds) holds pending nodes of height 2 and up only.  Every interior pair,
  * whatever its height, goes through the same code, and so do both leaf pairs: the
  * loop body stays small enough for the instruction cache.  Requires s >= 2. */
-template <int PRF, bool FULL, class Env, bool ET = false>
+template <int PRF, bool FULL, class Env, int GROUP = GROUP_ADD128>
 DPF_HD void eval_subtree_by_quads(Env &env, Seed seed, int s, int level_base)
 {
     int h = s;
@@ -565,7 +584,7 @@ DPF_HD void eval_subtree_by_quads(Env &env, Seed seed, int s, int level_base)
         }
 DPF_NO_UNROLL
         for (uint32_t k = 0; k < 2; k++) {
-            eval_leaf_pair<PRF, FULL, Env, ET>(env, c0, 4 * i + 2 * k, level_base);
+            eval_leaf_pair<PRF, FULL, Env, GROUP>(env, c0, 4 * i + 2 * k, level_base);
             c0 = c1;
         }
         if (++i == nquads) break;
@@ -577,11 +596,11 @@ DPF_NO_UNROLL
 /* Salsa20 and ChaCha bind the integer ALU pipe, where the stack's shared-memory
  * traffic costs nothing, and they keep the walk one node pair at a time (the
  * height-2 unit measured about 3 % slower for ChaCha20 at n = 2^16 and 2^18). */
-template <int PRF, bool FULL, class Env, bool ET = false>
+template <int PRF, bool FULL, class Env, int GROUP = GROUP_ADD128>
 DPF_HD void eval_subtree(Env &env, Seed seed, int s, int level_base)
 {
     if (PRF == PRF_AES128 && s >= 2) {
-        eval_subtree_by_quads<PRF, FULL, Env, ET>(env, seed, s, level_base);
+        eval_subtree_by_quads<PRF, FULL, Env, GROUP>(env, seed, s, level_base);
         return;
     }
     int h = s;
@@ -597,7 +616,7 @@ DPF_HD void eval_subtree(Env &env, Seed seed, int s, int level_base)
             seed = add128(c0, env.cw(level, bank, 0));
             h--;
         }
-        eval_leaf_pair<PRF, FULL, Env, ET>(env, seed, 2 * i, level_base);
+        eval_leaf_pair<PRF, FULL, Env, GROUP>(env, seed, 2 * i, level_base);
         h = ctz32(i + 1) + 1;
         if (h < s) seed = env.pop(h);
     }

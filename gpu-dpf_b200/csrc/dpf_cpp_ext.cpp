@@ -216,6 +216,73 @@ std::vector<void *> eval_init_et(const at::Tensor &table, int device, int shard_
     return {static_cast<void *>(ctx)};
 }
 
+/* ---- XOR-shared keys: 128 table rows per tree leaf, results XOR (include/b200dpf.h, b200dpf_gen_xor) ---- */
+
+std::vector<at::Tensor> gen_xor(int64_t k, int64_t n, const std::string &seed, int prf)
+{
+    at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
+    at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
+    check(b200dpf_gen_xor(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf, a.data_ptr<int32_t>(),
+                          b.data_ptr<int32_t>()),
+          "gen_xor");
+    return {a, b};
+}
+
+std::vector<at::Tensor> gen_batch_xor(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
+{
+    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
+    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), "gen_batch_xor: need 44 seed bytes per key");
+    const int64_t count = al.numel();
+    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
+    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
+    {
+        py::gil_scoped_release nogil;
+        check(b200dpf_gen_batch_xor(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf,
+                                    nthreads, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
+              "gen_batch_xor");
+    }
+    return {a, b};
+}
+
+/* the share bits packed: int32 [n / 32], row i = bit (i & 31) of word i >> 5 */
+at::Tensor eval_cpu_xor(const at::Tensor &key, int prf)
+{
+    const int32_t *k = key_ptr(key);
+    /* slot 0 = (d, 7, 0, 0), slot 130 = n = 128 * 2^d; b200dpf_eval_cpu_xor checks the rest */
+    const uint32_t d = (uint32_t)k[0];
+    TORCH_CHECK(k[1] == 7 && d >= 1 && d <= 24, "eval_cpu_xor: not an XOR-shared key");
+    at::Tensor result = torch::empty({(int64_t)4 << d}, at::kInt);
+    check(b200dpf_eval_cpu_xor(k, prf, reinterpret_cast<uint32_t *>(result.data_ptr<int32_t>())), "eval_cpu_xor");
+    return result;
+}
+
+py::bytes key_pack_xor(const at::Tensor &key)
+{
+    const int32_t *k = key_ptr(key);
+    std::string buf(b200dpf_key_packed_size(32), '\0');
+    size_t written = 0;
+    check(b200dpf_key_pack_xor(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), "key_pack_xor");
+    return py::bytes(buf.data(), written);
+}
+
+at::Tensor key_unpack_xor(const std::string &packed)
+{
+    at::Tensor key = torch::zeros({kKeyWords}, at::kInt);
+    check(b200dpf_key_unpack_xor(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()),
+          "key_unpack_xor");
+    return key;
+}
+
+std::vector<void *> eval_init_xor(const at::Tensor &table, int device, int shard_rank, int shard_count)
+{
+    TORCH_CHECK(table.dim() == 2, "eval_init_xor: table must be [num_entries, entry_size]");
+    at::Tensor t = table.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    check(b200dpf_create_xor(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count),
+          "eval_init_xor");
+    return {static_cast<void *>(ctx)};
+}
+
 /* one table on several GPUs of this process (b200dpf_create_multi); axis: 0 auto, 1 entries, 2 keys */
 std::vector<void *> eval_init_multi(const at::Tensor &table, const std::vector<int> &devices, int axis)
 {
@@ -551,4 +618,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("eval_init_et", &eval_init_et, "eval_init for early-terminated keys (four rows per leaf)", py::arg("table"),
           py::arg("device") = 0, py::arg("shard_rank") = 0, py::arg("shard_count") = 1);
     m.def("rows_per_leaf", [](const std::vector<void *> &b) { return b200dpf_ctx_rows_per_leaf(ctx_of(b)); });
+    m.def("gen_xor", &gen_xor, "XOR-shared key pair for row k of an n-row table (seed: >= 44 bytes)");
+    m.def("gen_batch_xor", &gen_batch_xor, "batched XOR-shared keygen (44 seed bytes per key)", py::arg("alphas"),
+          py::arg("n"), py::arg("seeds"), py::arg("prf"), py::arg("nthreads") = 0);
+    m.def("eval_cpu_xor", &eval_cpu_xor, "share bits of every row of an XOR-shared key on the CPU, packed 32 per int32");
+    m.def("key_pack_xor", &key_pack_xor, "compact wire form (\"DPX7\") of an XOR-shared key");
+    m.def("key_unpack_xor", &key_unpack_xor, "restore an XOR-shared int32[524] key from its compact form");
+    m.def("eval_init_xor", &eval_init_xor, "eval_init for XOR-shared keys (128 rows per leaf, XOR results)", py::arg("table"),
+          py::arg("device") = 0, py::arg("shard_rank") = 0, py::arg("shard_count") = 1);
 }

@@ -153,7 +153,10 @@ u128 lanes_neg(u128 a)
     return r;
 }
 
-template <class Rng>
+/* GROUP (dpf_core.cuh) is the group of flat level 0, where the payload lives: Z/2^128 for standard
+ * keys, lane-wise (Z/2^32)^4 for early-terminated keys, (Z/2)^128 for XOR-shared keys, whose add and
+ * subtract are both XOR.  Every other level adds in Z/2^128. */
+template <class Rng, int GROUP = GROUP_ADD128>
 struct KeyBuilder {
     int depth;
     int64_t alpha;
@@ -161,10 +164,19 @@ struct KeyBuilder {
     Rng &g;
     u128 cw1[64], cw2[64];
     u128 root_a, root_b;
-    bool lanes = false;   /* early-terminated key: level 0 adds and subtracts lane-wise */
 
-    u128 add(int L, u128 a, u128 b) const { return (lanes && L == 0) ? lanes_add(a, b) : a + b; }
-    u128 sub(int L, u128 a, u128 b) const { return (lanes && L == 0) ? lanes_add(a, lanes_neg(b)) : a - b; }
+    static u128 add0(u128 a, u128 b)
+    {
+        if (GROUP == GROUP_XOR128) return a ^ b;
+        return GROUP == GROUP_LANES32 ? lanes_add(a, b) : a + b;
+    }
+    static u128 sub0(u128 a, u128 b)
+    {
+        if (GROUP == GROUP_XOR128) return a ^ b;
+        return GROUP == GROUP_LANES32 ? lanes_add(a, lanes_neg(b)) : a - b;
+    }
+    u128 add(int L, u128 a, u128 b) const { return L == 0 ? add0(a, b) : a + b; }
+    u128 sub(int L, u128 a, u128 b) const { return L == 0 ? sub0(a, b) : a - b; }
 
     /* Builds flat level L (domain 2^(depth-L)) for payload `beta` and returns
      * the two servers' seeds on the alpha path just below this level. */
@@ -270,6 +282,22 @@ int64_t key_et_n(const int32_t *key)
     return (int64_t)v.x;
 }
 
+int key_xor_depth(const int32_t *key)
+{
+    const Seed d = key_slot(key, SLOT_DEPTH);
+    if (d.y != (uint32_t)XOR_LOG2_ROWS_PER_LEAF || d.z || d.w || d.x < 1 || d.x > XOR_MAX_DEPTH) return -1;
+    return (int)d.x;
+}
+
+int64_t key_xor_n(const int32_t *key)
+{
+    const Seed v = key_slot(key, SLOT_N);
+    const int depth = key_xor_depth(key);
+    if (depth < 0 || v.y || v.z || v.w) return -1;
+    if ((int64_t)v.x != ((int64_t)1 << (depth + XOR_LOG2_ROWS_PER_LEAF))) return -1;
+    return (int64_t)v.x;
+}
+
 namespace {
 
 template <class Rng>
@@ -314,24 +342,28 @@ int gen_secure(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int
     return gen_with(rng, alpha, n, prf_id, key_a, key_b);
 }
 
-int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
+namespace {
+
+/* A key whose leaves carry 2^LANE_BITS table rows each (early-terminated: 4, XOR-shared: 128): the log
+ * construction over the 2^depth leaves for alpha >> LANE_BITS, level 0 in GROUP, payload beta(alpha). */
+template <int GROUP, int LANE_BITS, class Beta>
+int gen_leaves(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b, Beta beta)
 {
-    if (n < 8 || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0 || alpha < 0 || alpha >= n) return -1;
+    if (n < ((int64_t)2 << LANE_BITS) || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0 || alpha < 0 || alpha >= n) return -1;
     if (prf_id < PRF_DUMMY || prf_id > PRF_AES128) return -1;
     int depth = 0;
-    while (((int64_t)1 << (depth + ET_LOG2_ROWS_PER_LEAF)) < n) depth++;
+    while (((int64_t)1 << (depth + LANE_BITS)) < n) depth++;
 
     ChaCha20Rng rng(seed, seed + 32);
-    KeyBuilder<ChaCha20Rng> kb{depth, alpha >> ET_LOG2_ROWS_PER_LEAF, prf_id, rng, {}, {}, 0, 0};
-    kb.lanes = true;
+    KeyBuilder<ChaCha20Rng, GROUP> kb{depth, alpha >> LANE_BITS, prf_id, rng, {}, {}, 0, 0};
     std::memset(kb.cw1, 0, sizeof kb.cw1);
     std::memset(kb.cw2, 0, sizeof kb.cw2);
-    kb.build(0, (u128)1 << (32 * (alpha & 3)));   /* beta = unit vector of lane alpha & 3 */
+    kb.build(0, beta(alpha));
 
     for (int srv = 0; srv < 2; srv++) {
         int32_t *key = srv ? key_b : key_a;
         std::memset(key, 0, sizeof(int32_t) * KEY_WORDS);
-        set_slot(key, SLOT_DEPTH, (u128)depth | ((u128)ET_LOG2_ROWS_PER_LEAF << 32));
+        set_slot(key, SLOT_DEPTH, (u128)depth | ((u128)LANE_BITS << 32));
         for (int i = 0; i < 64; i++) {
             set_slot(key, SLOT_CW1 + i, kb.cw1[i]);
             set_slot(key, SLOT_CW2 + i, kb.cw2[i]);
@@ -340,6 +372,22 @@ int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t
         set_slot(key, SLOT_N, (u128)n);
     }
     return 0;
+}
+
+}  // namespace
+
+int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
+{
+    /* beta = unit vector of lane alpha & 3 */
+    return gen_leaves<GROUP_LANES32, ET_LOG2_ROWS_PER_LEAF>(alpha, n, seed, prf_id, key_a, key_b,
+                                                            [](int64_t a) { return (u128)1 << (32 * (a & 3)); });
+}
+
+int gen_xor(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
+{
+    /* beta = unit vector of bit alpha & 127 */
+    return gen_leaves<GROUP_XOR128, XOR_LOG2_ROWS_PER_LEAF>(alpha, n, seed, prf_id, key_a, key_b,
+                                                            [](int64_t a) { return (u128)1 << (a & 127); });
 }
 
 namespace {
@@ -376,7 +424,8 @@ struct CpuEnv {
     }
     void leaf_quads(uint32_t local_pos, const Seed &w0, const Seed &w1)
     {
-        /* early-terminated: leaf position p holds leaf bitrev_depth(p), whose word l is row 4 * leaf + l */
+        /* leaf position p holds leaf bitrev_depth(p), whose word l is out[4 * leaf + l]: the share of row
+         * 4 * leaf + l (early-terminated), or the packed share bits of rows 128 * leaf + 32 l .. +31 (XOR) */
         int32_t *o0 = out + 4 * (size_t)bitrev(base_pos + local_pos, depth);
         int32_t *o1 = out + 4 * (size_t)bitrev(base_pos + local_pos + 1, depth);
         o0[0] = (int32_t)w0.x; o0[1] = (int32_t)w0.y; o0[2] = (int32_t)w0.z; o0[3] = (int32_t)w0.w;
@@ -384,7 +433,7 @@ struct CpuEnv {
     }
 };
 
-template <int PRF, bool ET = false>
+template <int PRF, int GROUP = GROUP_ADD128>
 void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
 {
     CpuEnv env;
@@ -398,7 +447,7 @@ void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
     for (uint32_t q = 0; q < nsub; q++) {
         env.base_pos = q << s;
         const Seed r = walk_down<PRF>(env, key_slot(key, SLOT_ROOT), depth - 1, depth - s, q);
-        eval_subtree<PRF, false, CpuEnv, ET>(env, r, s, 0);
+        eval_subtree<PRF, false, CpuEnv, GROUP>(env, r, s, 0);
     }
 }
 
@@ -423,10 +472,25 @@ int eval_cpu_et(const int32_t *key, int prf_id, int32_t *out_n)
     const int depth = key_et_depth(key);
     if (depth < 1 || key_et_n(key) < 0) return -1;
     switch (prf_id) {
-    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, true>(key, depth, out_n); break;
-    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, true>(key, depth, out_n); break;
-    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, true>(key, depth, out_n); break;
-    case PRF_AES128: eval_cpu_impl<PRF_AES128, true>(key, depth, out_n); break;
+    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, GROUP_LANES32>(key, depth, out_n); break;
+    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, GROUP_LANES32>(key, depth, out_n); break;
+    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, GROUP_LANES32>(key, depth, out_n); break;
+    case PRF_AES128: eval_cpu_impl<PRF_AES128, GROUP_LANES32>(key, depth, out_n); break;
+    default: return -1;
+    }
+    return 0;
+}
+
+int eval_cpu_xor(const int32_t *key, int prf_id, uint32_t *bits)
+{
+    const int depth = key_xor_depth(key);
+    if (depth < 1 || key_xor_n(key) < 0) return -1;
+    int32_t *out = reinterpret_cast<int32_t *>(bits);
+    switch (prf_id) {
+    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, GROUP_XOR128>(key, depth, out); break;
+    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, GROUP_XOR128>(key, depth, out); break;
+    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, GROUP_XOR128>(key, depth, out); break;
+    case PRF_AES128: eval_cpu_impl<PRF_AES128, GROUP_XOR128>(key, depth, out); break;
     default: return -1;
     }
     return 0;

@@ -50,5 +50,17 @@ int eval_cpu(const int32_t *key, int prf_id, int32_t *out_n);
 int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b);
 int eval_cpu_et(const int32_t *key, int prf_id, int32_t *out_n);
 
+/* XOR-shared keys (DESIGN.md section 10): a tree of 2^depth leaves over n = 128 * 2^depth table rows,
+ * slot 0 = (depth, 7, 0, 0), slot 130 = n; row i is bit (i & 127) of leaf i >> 7.  The checks return
+ * the tree depth (1..24) or n, or -1 for anything else -- a standard or early-terminated key included. */
+enum : int { XOR_LOG2_ROWS_PER_LEAF = 7, XOR_MAX_DEPTH = 24 };
+int key_xor_depth(const int32_t *key);
+int64_t key_xor_n(const int32_t *key);
+/* Key for row alpha of an n-row table (256 <= n <= 2^31, a power of two), drawn from the ChaCha20 DRBG;
+ * eval_cpu_xor writes its share bits packed, bits[n / 32] in natural order (row i = bit i & 31 of
+ * word i >> 5). */
+int gen_xor(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b);
+int eval_cpu_xor(const int32_t *key, int prf_id, uint32_t *bits);
+
 }  // namespace host
 }  // namespace b200dpf

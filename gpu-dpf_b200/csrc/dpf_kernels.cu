@@ -174,7 +174,7 @@ struct DevEnv {
     /* early-terminated keys (four rows per leaf) prefetch the first row pair before the leaf expansion
      * at 16 columns only: at 32, rows held across the full-width expansion (or two rows in flight
      * beside the next two) spill */
-    static constexpr bool ET_PREFETCH = M.row_shift != 0 && NV == 4;
+    static constexpr bool ET_PREFETCH = M.result == RESULT_ADD && M.row_shift != 0 && NV == 4;
     /* ROWS_STAGED: the work item's 2^s rows were requested with one cp.async.bulk when the item was
      * drawn; they are first needed s-1 node expansions later, which hides the copy */
     const uint4 *tile;          /* this warp's staged rows (shared memory) */
@@ -184,7 +184,9 @@ struct DevEnv {
 
     __device__ __forceinline__ void leaf_prefetch(uint32_t local_pos)
     {
-        if (M.row_load == ROWS_STAGED) {
+        if (M.result == RESULT_XOR) {
+            /* 256 rows per leaf pair: leaf_bits streams them */
+        } else if (M.row_load == ROWS_STAGED) {
             if (tile_pending) {
                 tma::mbar_wait(tile_bar, tile_phase);
                 tile_phase ^= 1u;
@@ -215,8 +217,53 @@ struct DevEnv {
     }
     /* early-terminated keys: leaves local_pos and local_pos + 1 with their four row shares each, against
      * rows 4 local_pos .. 4 local_pos + 7 */
+    /* XOR-shared keys: leaves local_pos and local_pos + 1 with 128 share bits each, against rows 128 local_pos
+     * .. 128 local_pos + 255.  Column split: rows points at this lane's 16 bytes of the row (columns 4 (lane & 3)
+     * .. +3), and acc[4 j + c] is column 4 (lane & 3) + c of key kslot ^ j, whose leaf words come from lane ^ j
+     * by SHFL, one word (32 rows) at a time.  A row costs each lane one 16-byte load and, per key, a mask
+     * from its share bit and 4 LOP3 (acc ^= row & mask).  Correct only when the four lanes of a quad hold
+     * four different keys at the same leaf position (kpw >= 4): launch_eval refuses a column-split launch
+     * with kpw_log2 < 2. */
+    __device__ __forceinline__ void leaf_bits(uint32_t local_pos, const Seed &w0, const Seed &w1)
+    {
+        uint32_t w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};   /* word k: rows 32 k .. 32 k + 31 */
+        const uint4 *r = rows + (size_t)local_pos * 128 * row_stride_v;
+#pragma unroll 1
+        for (int k = 0; k < 8; k++) {
+            uint32_t u[4];
+            u[0] = w[0];
+#pragma unroll
+            for (int j = 1; j < 4; j++) u[j] = __shfl_xor_sync(0xffffffffu, w[0], j);
+#pragma unroll
+            for (int i = 0; i < 7; i++) w[i] = w[i + 1];
+#pragma unroll 1
+            for (int b0 = 0; b0 < 32; b0 += 8) {
+                uint4 t[8];   /* eight rows in flight */
+#pragma unroll
+                for (int i = 0; i < 8; i++) t[i] = __ldg(r + (size_t)i * row_stride_v);
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        const uint32_t m = (uint32_t)((int32_t)(u[j] << (31 - i)) >> 31);   /* bit b0 + i */
+                        acc[4 * j + 0] ^= t[i].x & m;
+                        acc[4 * j + 1] ^= t[i].y & m;
+                        acc[4 * j + 2] ^= t[i].z & m;
+                        acc[4 * j + 3] ^= t[i].w & m;
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < 4; j++) u[j] >>= 8;
+                r += (size_t)8 * row_stride_v;
+            }
+        }
+    }
     __device__ __forceinline__ void leaf_quads(uint32_t local_pos, const Seed &w0, const Seed &w1)
     {
+        if constexpr (M.feeds == FEEDS_MAC && M.result == RESULT_XOR) {
+            leaf_bits(local_pos, w0, w1);
+            return;
+        }
         const uint32_t a[4] = {w0.x, w0.y, w0.z, w0.w}, b[4] = {w1.x, w1.y, w1.z, w1.w};
         if (M.feeds == FEEDS_MAC) {
             if (leaf_out != nullptr) {   /* coalesced: 32 keys x 4 bytes per row */
@@ -482,7 +529,8 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 #pragma unroll
             for (int e = 0; e < 4 * NV; e++) env.acc[e] = 0;
         } else if (M.feeds == FEEDS_SHARES) {
-            env.share_row = p.shares + (size_t)(env.key_valid ? key : 0) * p.n;
+            /* XOR-shared keys: one bit per row, n / 32 words per key */
+            env.share_row = p.shares + (size_t)(env.key_valid ? key : 0) * (M.result == RESULT_XOR ? p.n >> 5 : p.n);
         }
         const uint4 rv = root_s[kslot];
         const Seed root = make_seed(rv.x, rv.y, rv.z, rv.w);
@@ -544,7 +592,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
                 env.leaf_out = (!M.grouped && p.leaf_cache)
                                    ? p.leaf_cache + ((size_t)kg * p.n_local + ((size_t)q << (g_s + M.row_shift))) * 32 + lane
                                    : nullptr;
-                eval_subtree<PRF, false, decltype(env), M.row_shift != 0>(env, r, g_s, 0);
+                eval_subtree<PRF, false, decltype(env), mode_leaf_group(MODE)>(env, r, g_s, 0);
             }
           }
             if (!ahead && draw && lane == 0) t_raw = atomicAdd(ph.counters + kg, chunk);
@@ -555,7 +603,10 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
              * first, so every key receives one red.add per warp and column, not 32/kpw */
             for (int off = kpw; off < 32; off <<= 1) {
 #pragma unroll
-                for (int e = 0; e < 4 * NV; e++) env.acc[e] += __shfl_xor_sync(0xffffffffu, env.acc[e], off);
+                for (int e = 0; e < 4 * NV; e++) {
+                    if constexpr (M.result == RESULT_XOR) env.acc[e] ^= __shfl_xor_sync(0xffffffffu, env.acc[e], off);
+                    else env.acc[e] += __shfl_xor_sync(0xffffffffu, env.acc[e], off);
+                }
             }
             if (M.row_load == ROWS_COLSPLIT) {
                 if (sslot == 0) {
@@ -567,7 +618,11 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
 #pragma unroll
                         for (int c = 0; c < 4; c++) {
                             const uint32_t e = 4u * (uint32_t)(lane & 3) + (uint32_t)c;
-                            if (e < p.ncols) atomicAdd(o + e, env.acc[4 * j + c]);
+                            if constexpr (M.result == RESULT_XOR) {
+                                if (e < p.ncols) atomicXor(o + e, env.acc[4 * j + c]);
+                            } else {
+                                if (e < p.ncols) atomicAdd(o + e, env.acc[4 * j + c]);
+                            }
                         }
                     }
                 }
@@ -924,8 +979,9 @@ EvalKernel eval_kernel()
 }
 
 /* The instantiated kernels of one PRF.  Every mode runs at 16 columns per pass (nv = 4); the fused
- * modes also at 32, the standard one at 64 as well.  Grouped evaluation (both kinds of key) takes 16
- * columns per pass, and the modes that never touch the table need no other width. */
+ * modes of standard and early-terminated keys also at 32, the standard one at 64 as well.  Grouped
+ * evaluation (both kinds of key) and XOR-shared keys take 16 columns per pass, and the modes that never
+ * touch the table need no other width. */
 template <int PRF>
 EvalKernel eval_kernel_of(int nv, int mode)
 {
@@ -938,7 +994,9 @@ EvalKernel eval_kernel_of(int nv, int mode)
         case MODE_FUSED_ET: return eval_kernel<PRF, 4, MODE_FUSED_ET>();
         case MODE_EXPAND_ET: return eval_kernel<PRF, 4, MODE_EXPAND_ET>();
         case MODE_GROUPED_ET: return eval_kernel<PRF, 4, MODE_GROUPED_ET>();
-        case MODE_FUSED_TMA:        /* AES: no shared memory left beside the tables */
+        case MODE_FUSED_XOR: return eval_kernel<PRF, 4, MODE_FUSED_XOR>();
+        case MODE_EXPAND_XOR: return eval_kernel<PRF, 4, MODE_EXPAND_XOR>();
+        case MODE_FUSED_TMA:       /* AES: no shared memory left beside the tables */
             if constexpr (PRF != PRF_AES128) return eval_kernel<PRF, 4, MODE_FUSED_TMA>();
             break;
         case MODE_FUSED_COLSPLIT:   /* Salsa/ChaCha bind the ALU pipe, not the data pipe */
@@ -990,6 +1048,8 @@ cudaError_t launch_eval(int prf, int nv, int mode, const EvalParams &p, int grid
 {
     const EvalKernel k = find_eval_kernel(prf, nv, mode);
     if (k.fn == nullptr) return cudaErrorInvalidValue;
+    /* the column split trades leaf values across the four lanes of a key quad, which must be four keys */
+    if (mode_traits(mode).row_load == ROWS_COLSPLIT && p.kpw_log2 < 2) return cudaErrorInvalidValue;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;

@@ -113,7 +113,13 @@ struct EvalParams {
 /* Kernel modes: the MODE of dpf_eval_kernel<PRF, NV, MODE>.  Each is a combination of the properties
  * of ModeTraits, and mode_traits below is the one place that says which. */
 enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3, MODE_FUSED_TMA = 4,
-       MODE_FUSED_ET = 5, MODE_EXPAND_ET = 6, MODE_FUSED_COLSPLIT = 7, MODE_GROUPED_ET = 8, MODE_COUNT = 9 };
+       MODE_FUSED_ET = 5, MODE_EXPAND_ET = 6, MODE_FUSED_COLSPLIT = 7, MODE_GROUPED_ET = 8,
+       MODE_FUSED_XOR = 9, MODE_EXPAND_XOR = 10, MODE_COUNT = 11 };
+
+/* The group a mode's result lives in (ModeTraits::result). */
+enum { RESULT_ADD,        /* Z/2^32: out[key][col] = sum of share * row, red.global.add */
+       RESULT_XOR };      /* (Z/2)^32: out[key][col] = XOR of the rows whose share bit is set, red.global.xor;
+                           * the shares are bits, packed 32 to a word (XOR-shared keys, DESIGN.md section 10) */
 
 /* What a mode's leaves feed (ModeTraits::feeds). */
 enum { FEEDS_MAC,         /* the inner product against the table: out[key][col] */
@@ -132,28 +138,39 @@ enum { ROWS_BROADCAST,    /* every lane loads the whole row: one broadcast load 
 struct ModeTraits {
     int feeds;                /* FEEDS_*                                                          */
     int row_load;             /* ROWS_*                                                           */
-    /* log2 table rows per leaf: 2 for early-terminated keys, whose tree is over leaves while the
-     * table, the leaf cache (EvalParams::n_local), the result and the shares (EvalParams::n) are over
-     * rows: leaf position p owns rows 4p..4p+3 of the device table, shares[key][4 * leaf + l] */
+    /* log2 table rows per leaf: 2 for early-terminated keys and 7 for XOR-shared ones, whose tree is
+     * over leaves while the table, the leaf cache (EvalParams::n_local), the result and the shares
+     * (EvalParams::n) are over rows: leaf position p owns rows 4p..4p+3 (128p..128p+127) of the device
+     * table, shares[key][4 * leaf + l] */
     int row_shift;
     /* batch PIR: each key group evaluates its own bin, described by EvalParams::groups */
     bool grouped;
+    int result;               /* RESULT_*: also the level-0 group, XOR for RESULT_XOR */
 };
 
 __host__ __device__ constexpr ModeTraits mode_traits(int mode)
 {
-    switch (mode) {                            /* feeds           row_load        row_shift grouped */
-    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false};
-    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false};
-    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false};
-    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true};
-    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false};
-    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false};
-    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false};
-    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false};
-    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true};
-    default:                  return ModeTraits{-1, -1, 0, false};
+    switch (mode) {                            /* feeds           row_load        row_shift grouped result */
+    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false, RESULT_ADD};
+    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false, RESULT_ADD};
+    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false, RESULT_ADD};
+    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD};
+    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false, RESULT_ADD};
+    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false, RESULT_ADD};
+    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false, RESULT_ADD};
+    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false, RESULT_ADD};
+    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD};
+    case MODE_FUSED_XOR:      return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, false, RESULT_XOR};
+    case MODE_EXPAND_XOR:     return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 7, false, RESULT_XOR};
+    default:                  return ModeTraits{-1, -1, 0, false, RESULT_ADD};
     }
+}
+
+/* The level-0 group of a mode's keys (dpf_core.cuh GROUP_*) */
+__host__ __device__ constexpr int mode_leaf_group(int mode)
+{
+    return mode_traits(mode).result == RESULT_XOR ? GROUP_XOR128
+         : mode_traits(mode).row_shift != 0       ? GROUP_LANES32 : GROUP_ADD128;
 }
 
 /* Block shape of the evaluation kernel instantiated for (prf, nv, mode), nv = uint4 (4 int32 columns)

@@ -57,7 +57,7 @@ class DPF(object):
     }
 
     def __init__(self, prf=None, device=0, shard=(0, 1), allow_non_pow2=False, devices=None, axis="auto",
-                 early_termination=False):
+                 early_termination=False, xor=False):
         # devices: None (one GPU: `device`), "all", or a list of device ids -- one process drives them all
         # (b200dpf_create_multi); axis "auto" | "entries" | "keys".  B200DPF_DEVICES / B200DPF_AXIS in the
         # environment set the defaults, so an unchanged `dpf.DPF()` caller (benchmark.py) can scale too.
@@ -89,6 +89,14 @@ class DPF(object):
         if self.early_termination and self.devices:
             raise Exception("early_termination=True has no multi-device variant: use one device per DPF "
                             "(DPF(device=d, shard=(rank, count), early_termination=True))")
+        # xor: two-server XOR PIR (include/b200dpf.h, b200dpf_gen_xor): each leaf carries 128 one-bit row shares,
+        # and the two servers' results XOR (not add) to the selected row: eval_a ^ eval_b == table[k]
+        self.xor = bool(xor)
+        if self.xor and self.early_termination:
+            raise Exception("xor=True and early_termination=True are different kinds of key: pass one of them")
+        if self.xor and self.devices:
+            raise Exception("xor=True has no multi-device variant: use one device per DPF "
+                            "(DPF(device=d, shard=(rank, count), xor=True))")
 
     # ---- client -----------------------------------------------------------
     def gen(self, k, n, seed=None, secure=None):
@@ -100,7 +108,7 @@ class DPF(object):
         generator states of a key it holds and recover the index: that generator is kept only
         for callers that pass an explicit `seed` (deterministic keys, bit-identical to the
         reference's for the same seed: golden and parity tests) and do not ask for secure=True."""
-        if self.early_termination:
+        if self.early_termination or self.xor:
             return self._gen_et(k, n, seed, secure)
         if secure is None:
             secure = seed is None
@@ -117,34 +125,37 @@ class DPF(object):
         return dpf_cpp.gen(k, n, seed, self.prf_method)
 
     def _gen_et(self, k, n, seed, secure):
-        # early-terminated keys draw from the ChaCha20 DRBG only: explicit seeds are >= 44 bytes
+        # early-terminated and XOR-shared keys draw from the ChaCha20 DRBG only: explicit seeds are >= 44 bytes
+        kind = "XOR-shared" if self.xor else "early-terminated"
         if secure is False:
-            raise Exception("early-terminated keys have no secure=False generator: pass >= 44 seed bytes or none")
+            raise Exception("%s keys have no secure=False generator: pass >= 44 seed bytes or none" % kind)
         if seed is None:
             seed = os.urandom(44)
         if not isinstance(seed, (bytes, bytearray)) or len(seed) < 44:
-            raise Exception("early-terminated keys take a seed of at least 44 bytes")
+            raise Exception("%s keys take a seed of at least 44 bytes" % kind)
         if n & (n - 1) != 0 and not self.allow_non_pow2:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
         if k >= n:
             raise Exception("k (%d), the selected element, must be less than n (%d), the number of entries in the table"
                             % (k, n))
-        return dpf_cpp.gen_et(k, _next_pow2(n), bytes(seed), self.prf_method)
+        gen = dpf_cpp.gen_xor if self.xor else dpf_cpp.gen_et
+        return gen(k, _next_pow2(n), bytes(seed), self.prf_method)
 
     def gen_batch(self, indices, n, seeds=None, nthreads=0):
         """Keys for many indices at once: two int32 [B, 524] tensors (multi-threaded keygen).
         seeds=None: ChaCha20-DRBG keys from os.urandom entropy (44 bytes per key); explicit integer
         seeds select the reference's 32-bit mt19937 generator (deterministic, for tests).  With
-        early_termination, explicit seeds are bytes: 44 per key, concatenated."""
-        if self.early_termination:
+        early_termination or xor, explicit seeds are bytes: 44 per key, concatenated."""
+        if self.early_termination or self.xor:
             if n & (n - 1) != 0:
                 raise Exception("Table num entries (%d) must be a power of two" % (n))
             idx = torch.as_tensor(list(indices), dtype=torch.int64)
             if seeds is None:
                 seeds = os.urandom(44 * idx.numel())
             if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * idx.numel():
-                raise Exception("early-terminated gen_batch takes seeds as bytes, 44 per key")
-            return dpf_cpp.gen_batch_et(idx, n, bytes(seeds), self.prf_method, nthreads)
+                raise Exception("%s gen_batch takes seeds as bytes, 44 per key" % ("XOR-shared" if self.xor else "early-terminated"))
+            gen_batch = dpf_cpp.gen_batch_xor if self.xor else dpf_cpp.gen_batch_et
+            return gen_batch(idx, n, bytes(seeds), self.prf_method, nthreads)
         if n & (n - 1) != 0:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
         idx = torch.as_tensor(list(indices), dtype=torch.int64)
@@ -157,7 +168,10 @@ class DPF(object):
 
     # ---- server -----------------------------------------------------------
     def eval_cpu(self, keys, one_hot_only=False):
-        """CPU evaluation (dpf.py:76-86): share vectors, or shares @ table."""
+        """CPU evaluation (dpf.py:76-86): share vectors, or shares @ table.  With xor: share bits (int32 0/1),
+        or the XOR of the rows whose share bit is set."""
+        if self.xor:
+            return self._eval_cpu_xor(keys, one_hot_only)
         eval_one = dpf_cpp.eval_cpu_et if self.early_termination else dpf_cpp.eval_cpu
         if one_hot_only:
             return torch.stack([eval_one(k, self.prf_method) for k in keys])
@@ -165,6 +179,24 @@ class DPF(object):
             raise Exception("Must call `eval_init` before `eval_cpu` with one_hot_only=False")
         one_hots = torch.stack([eval_one(k, self.prf_method) for k in keys])
         return torch.matmul(one_hots, self.table)
+
+    def _eval_cpu_xor(self, keys, one_hot_only):
+        shifts = torch.arange(32, dtype=torch.int32)
+        # packed words [B, n/32] -> bits [B, n]: row i is bit (i & 31) of word i >> 5
+        bits = torch.stack([(dpf_cpp.eval_cpu_xor(k, self.prf_method).view(-1, 1) >> shifts) & 1 for k in keys])
+        bits = bits.reshape(len(keys), -1)
+        if one_hot_only:
+            return bits
+        if self.table is None:
+            raise Exception("Must call `eval_init` before `eval_cpu` with one_hot_only=False")
+        # XOR of the selected rows, bit plane by bit plane: the parity of each plane's selected-row count
+        table = self.table.to(torch.int32)
+        sel = bits.to(torch.int64)
+        out = torch.zeros((len(keys), table.shape[1]), dtype=torch.int32)
+        for b in range(32):
+            plane = ((table >> b) & 1).to(torch.int64)
+            out |= ((torch.matmul(sel, plane) & 1).to(torch.int32) << b)
+        return out
 
     def eval_init(self, table):
         """Upload the table (dpf.py:88-113).  Any entry size; no column padding."""
@@ -185,7 +217,9 @@ class DPF(object):
         self.table = table
         self.table_num_entries = table.shape[0]
         self.table_effective_entry_size = table.shape[1]
-        if self.early_termination:
+        if self.xor:
+            self.buffers = dpf_cpp.eval_init_xor(table, self.device, self.shard[0], self.shard[1])
+        elif self.early_termination:
             self.buffers = dpf_cpp.eval_init_et(table, self.device, self.shard[0], self.shard[1])
         elif self.devices:
             self.buffers = dpf_cpp.eval_init_multi(table, self.devices, {"auto": 0, "entries": 1, "keys": 2}[self.axis])
@@ -248,7 +282,7 @@ class DPF(object):
     def pack_keys(self, keys):
         """Compact wire form of a batch (24% to 56% smaller than int32[524] keys, depending on n): one
         contiguous uint8 tensor [B, 32 + 64*depth], pinned when CUDA is available, for eval_gpu_compact."""
-        pack = dpf_cpp.key_pack_et if self.early_termination else dpf_cpp.key_pack
+        pack = dpf_cpp.key_pack_xor if self.xor else dpf_cpp.key_pack_et if self.early_termination else dpf_cpp.key_pack
         blobs = [pack(k) for k in keys]
         t = torch.frombuffer(bytearray(b"".join(blobs)), dtype=torch.uint8).reshape(len(blobs), -1)
         return t.pin_memory() if torch.cuda.is_available() else t
@@ -262,8 +296,8 @@ class DPF(object):
     def eval_gpu_device(self, keys_dev, out_dev=None, out_ptr=None, accumulate=False):
         """Device-resident, asynchronous variant: keys_dev int32 [B,524] CUDA tensor ->
         int32 [B, entry_size] CUDA tensor, enqueued on the current torch stream.
-        accumulate=True adds into the destination instead of overwriting it; out_ptr may
-        then be a raw (e.g. peer-mapped) device address."""
+        accumulate=True adds into the destination instead of overwriting it (with xor: XORs into
+        it); out_ptr may then be a raw (e.g. peer-mapped) device address."""
         if self.buffers is None:
             raise Exception("Must call `eval_init` before `eval_gpu`")
         if self.devices:
@@ -329,12 +363,13 @@ class DPF(object):
         yield from drain(0)
 
     def expand_gpu_device(self, keys_dev, out_dev=None):
-        """Share vectors on the GPU (the eval_cpu(one_hot_only=True) quantity): int32 [B, n] CUDA tensor."""
+        """Share vectors on the GPU (the eval_cpu(one_hot_only=True) quantity): int32 [B, n] CUDA tensor.
+        With xor the share bits come packed: int32 [B, n / 32], row i = bit (i & 31) of word i >> 5."""
         if self.buffers is None:
             raise Exception("Must call `eval_init` before `expand_gpu_device`")
         assert keys_dev.is_cuda and keys_dev.dtype == torch.int32 and keys_dev.is_contiguous()
         if out_dev is None:
-            out_dev = torch.empty((keys_dev.shape[0], self.table_num_entries), dtype=torch.int32,
+            out_dev = torch.empty((keys_dev.shape[0], self.table_num_entries // (32 if self.xor else 1)), dtype=torch.int32,
                                   device=keys_dev.device)
         stream = torch.cuda.current_stream(keys_dev.device).cuda_stream
         dpf_cpp.expand_gpu_device(keys_dev.data_ptr(), keys_dev.shape[0], self.buffers, self.prf_method,
@@ -376,6 +411,8 @@ class BinnedDPF(DPF):
         if kwargs.get("early_termination"):
             raise Exception("BinnedDPF has no early-terminated variant (early_termination=True): use "
                             "dpf_cpp.group_init_et or b200dpf.GroupContext(early_termination=True)")
+        if kwargs.get("xor"):
+            raise Exception("BinnedDPF has no XOR-shared variant (xor=True): use one dpf.DPF(xor=True) per bin")
         super().__init__(*args, **kwargs)
 
     def eval_init(self, tables):

@@ -61,10 +61,14 @@ class ShardedDPF(object):
     # reduce + the upload of every key to every rank dominate; the batch is split by keys instead
     AUTO_KEYS_MAX_N = 1 << 18
 
-    def __init__(self, prf=None, group=None, device=None, axis="entries", reduce="nccl", early_termination=False):
+    def __init__(self, prf=None, group=None, device=None, axis="entries", reduce="nccl", early_termination=False,
+                 xor=False):
         if early_termination:
             raise Exception("ShardedDPF has no early-terminated variant; a single-process shard is "
                             "dpf.DPF(shard=(rank, count), early_termination=True)")
+        if xor:
+            raise Exception("ShardedDPF has no XOR-shared variant; a single-process shard is "
+                            "dpf.DPF(shard=(rank, count), xor=True), whose results XOR together")
         assert axis in ("entries", "keys", "auto") and reduce in ("nccl", "fused")
         self.group = group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0

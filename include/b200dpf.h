@@ -318,7 +318,9 @@ int b200dpf_eval_device(b200dpf_ctx *ctx, const void *keys_dev, int64_t nkeys, i
  * red.global.add.u32 epilogue performs the cross-shard reduction itself, so
  * sharded evaluation needs no separate collective (SURVEY.md section 8(e),
  * "fused alternative").  The caller orders the clearing of the destination
- * before, and its consumption after, all contributing launches.
+ * before, and its consumption after, all contributing launches.  On an XOR-shared
+ * context (b200dpf_create_xor) it XORs the results into out_dev instead
+ * (red.global.xor.b32), the group those results live in.
  */
 int b200dpf_eval_device_acc(b200dpf_ctx *ctx, const void *keys_dev, int64_t nkeys, int prf,
                             void *out_dev, void *cuda_stream);
@@ -424,9 +426,65 @@ int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key);
 int b200dpf_create_et(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
                       int device, int shard_rank, int shard_count);
 
-/* Table rows per tree leaf: 4 on a context of b200dpf_create_et or b200dpf_group_create_et, 1 otherwise;
- * -1 for null. */
+/* Table rows per tree leaf: 4 on a context of b200dpf_create_et or b200dpf_group_create_et, 128 on one of
+ * b200dpf_create_xor, 1 otherwise; -1 for null. */
 int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *ctx);
+
+/* ------------------------------------------------------------------------------------------- */
+/* XOR-shared keys: 128 table rows per GGM leaf (DESIGN.md section 10).                         */
+/* ------------------------------------------------------------------------------------------- */
+/*
+ * Two-server XOR PIR (a BGI DPF with Chor et al.'s XOR reconstruction).  A leaf's 128-bit output is
+ * 128 one-bit shares, one per table row, so a DPF over n rows walks a tree of n/128 leaves.  Row i is
+ * bit (i & 127) of leaf i >> 7; bit b of a 128-bit value is bit (b & 31) of its little-endian word
+ * b >> 5.
+ *
+ * THE RESULT IS AN XOR, NOT A SUM: out[b][e] = XOR over i of (share_b[i] ? table[i][e] : 0), as uint32,
+ * so the two servers' results XOR to table[alpha] (out_a ^ out_b == table[alpha]).  The shares of the
+ * two servers differ in exactly bit alpha.
+ *
+ * The key is the int32[524] wire format with slot 0 = (d, 7, 0, 0) (d = log2(n) - 7 tree levels) and
+ * slot 130 = n.  Level-0 correction words are XORed in (the group (Z/2)^128).  Every standard and
+ * early-terminated entry point refuses such a key, and the functions below refuse the other two kinds.
+ */
+
+/* Keys for row alpha of an n-row table, 256 <= n <= 2^31 a power of two.  Every draw comes from the
+ * ChaCha20 DRBG of b200dpf_gen_secure; seed_len must be >= 44. */
+int b200dpf_gen_xor(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf,
+                    int32_t *key_a, int32_t *key_b);
+
+/* Batched b200dpf_gen_xor on `nthreads` host threads (0 = one per hardware thread): seeds44 = count x
+ * 44 bytes; keys_a/keys_b: int32[count][524].  Identical keys for any nthreads. */
+int b200dpf_gen_batch_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
+                          int nthreads, int32_t *keys_a, int32_t *keys_b);
+
+/* One server's share bits of every row on the CPU, packed: bits[n / 32] in natural order, row i = bit
+ * (i & 31) of bits[i >> 5] (leaf j gives words 4j .. 4j+3; n read from the key). */
+int b200dpf_eval_cpu_xor(const int32_t *key, int prf, uint32_t *bits);
+
+/* Compact form: the layout and size (b200dpf_key_packed_size(d) = 32 + 64*d) of b200dpf_key_pack,
+ * magic "DPX7".  The standard and early-terminated unpack and packed-evaluation paths refuse it. */
+int b200dpf_key_pack_xor(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written);
+int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key);
+
+/*
+ * A context for XOR-shared keys, arguments as b200dpf_create with n >= 256 and shard_count a power of
+ * two <= n/256.  The device table keeps each leaf's 128 rows together: row 128p + l holds natural row
+ * 128*bitrev(p) + l.  Shard (r, G) owns row i iff ((i >> 7) & (G-1)) == bitrev_g(r); the shards' results
+ * XOR to the whole table's.  On it:
+ *   b200dpf_eval, _eval_gather, _eval_packed ("DPX7" keys), _host_staging, _eval_device, _update_rows,
+ *   _update_rows_device, _ctx_set_option and the introspection functions work as on an early-terminated
+ *   context, with the XOR result above; the host paths return EINVAL for a key of another kind before
+ *   copying anything;
+ *   b200dpf_eval_device_acc XORs the results into out_dev (red.global.xor) instead of adding them;
+ *   b200dpf_expand_device writes the packed share bits, shares_dev = uint32[nkeys][n / 32] as
+ *   b200dpf_eval_cpu_xor.
+ * Entries are evaluated 16 columns per pass; wider entries take one pass (one tree walk) per 16 columns,
+ * so the "leaf_cache", "leaf_cache_mb", "mac_tma" and "tma_rows" options have no effect here.  There is
+ * no multi-device, grouped or GPU-keygen variant.
+ */
+int b200dpf_create_xor(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
+                       int device, int shard_rank, int shard_count);
 
 #ifdef __cplusplus
 }
