@@ -31,6 +31,14 @@ SYMBOLS = [
     "b200dpf_create_xor",
 ]
 
+# The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
+# is slot 0 = (d, lane_bits, 0, 0), 1 <= d <= max depth, slot 130 = 2^(d + lane_bits) as a u64.
+KINDS = {
+    "": (0, 32, "standard"),
+    "_et": (2, 29, "early-terminated"),
+    "_xor": (7, 24, "XOR-shared"),
+}
+
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
 _i64p = np.ctypeslib.ndpointer(dtype=np.int64, flags="C_CONTIGUOUS")
 _u32p = np.ctypeslib.ndpointer(dtype=np.uint32, flags="C_CONTIGUOUS")
@@ -46,20 +54,22 @@ def load():
     L = C.CDLL(LIB_PATH)
     L.b200dpf_version.restype = C.c_char_p
     L.b200dpf_last_error.restype = C.c_char_p
-    L.b200dpf_gen.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
-    L.b200dpf_gen_secure.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
+    for kind in KINDS:
+        getattr(L, "b200dpf_eval_cpu" + kind).argtypes = [_i32p, C.c_int, _u32p if kind == "_xor" else _i32p]
+        getattr(L, "b200dpf_key_pack" + kind).argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        getattr(L, "b200dpf_key_unpack" + kind).argtypes = [C.c_char_p, C.c_size_t, _i32p]
+        getattr(L, "b200dpf_create" + kind).argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
+    for gen in ("", "_secure", "_et", "_xor"):
+        getattr(L, "b200dpf_gen" + gen).argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
+    for drbg in ("_secure", "_et", "_xor"):   # the ChaCha20-DRBG generators: 44 seed bytes per key
+        getattr(L, "b200dpf_gen_batch" + drbg).argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
     L.b200dpf_gen_batch.argtypes = [_i64p, _u32p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
-    L.b200dpf_gen_batch_secure.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
     L.b200dpf_gen_batch_gpu.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    L.b200dpf_eval_cpu.argtypes = [_i32p, C.c_int, _i32p]
     L.b200dpf_key_packed_size.argtypes = [C.c_int]
     L.b200dpf_key_packed_size.restype = C.c_size_t
-    L.b200dpf_key_pack.argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    L.b200dpf_key_unpack.argtypes = [C.c_char_p, C.c_size_t, _i32p]
     L.b200dpf_key_n.argtypes = [_i32p]
     L.b200dpf_key_n.restype = C.c_int64
     L.b200dpf_key_depth.argtypes = [_i32p]
-    L.b200dpf_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     L.b200dpf_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int]
     L.b200dpf_ctx_device_count.argtypes = [C.c_void_p]
     L.b200dpf_ctx_axis.argtypes = [C.c_void_p]
@@ -88,20 +98,8 @@ def load():
     L.b200dpf_ctx_device.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_launches.argtypes = [C.c_void_p]
     L.b200dpf_ctx_set_subtree_log2.argtypes = [C.c_void_p, C.c_int]
-    L.b200dpf_gen_et.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
-    L.b200dpf_gen_batch_et.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
-    L.b200dpf_eval_cpu_et.argtypes = [_i32p, C.c_int, _i32p]
-    L.b200dpf_key_pack_et.argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    L.b200dpf_key_unpack_et.argtypes = [C.c_char_p, C.c_size_t, _i32p]
-    L.b200dpf_create_et.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
     L.b200dpf_group_create_et.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
-    L.b200dpf_gen_xor.argtypes = [C.c_int64, C.c_int64, C.c_char_p, C.c_size_t, C.c_int, _i32p, _i32p]
-    L.b200dpf_gen_batch_xor.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
-    L.b200dpf_eval_cpu_xor.argtypes = [_i32p, C.c_int, _u32p]
-    L.b200dpf_key_pack_xor.argtypes = [_i32p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    L.b200dpf_key_unpack_xor.argtypes = [C.c_char_p, C.c_size_t, _i32p]
-    L.b200dpf_create_xor.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]
     return L
 
 
@@ -129,10 +127,7 @@ def gen(alpha, n, seed32, prf):
 
 
 def gen_secure(alpha, n, seed_bytes, prf):
-    a = np.zeros(KEY_WORDS, np.int32)
-    b = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_gen_secure(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), "b200dpf_gen_secure")
-    return a, b
+    return _gen_drbg("_secure", alpha, n, seed_bytes, prf)
 
 
 def gen_batch(alphas, n, seeds32, prf, nthreads=0):
@@ -170,133 +165,122 @@ def gen_batch_gpu(alphas, n, seed_bytes, prf, device=0, out_ptrs=None):
     return a, b
 
 
-def key_pack(key):
+def _key_n(key, kind):
+    """rows of a key of `kind` (a KINDS suffix), or -1"""
+    lane_bits, max_depth, _ = KINDS[kind]
+    d = int(key[0])
+    if key[1] != lane_bits or key[2] or key[3] or not 1 <= d <= max_depth:
+        return -1
+    n = int(np.uint32(key[130 * 4])) | int(np.uint32(key[130 * 4 + 1])) << 32
+    return n if n == 1 << (d + lane_bits) and not key[130 * 4 + 2:130 * 4 + 4].any() else -1
+
+
+def _xor_key_n(key):
+    """rows of an XOR-shared key, or -1 (_key_n(key, "_xor") under the name existing callers use)"""
+    return _key_n(key, "_xor")
+
+
+def _gen_drbg(suffix, alpha, n, seed_bytes, prf):
+    a = np.zeros(KEY_WORDS, np.int32)
+    b = np.zeros(KEY_WORDS, np.int32)
+    name = "b200dpf_gen" + suffix
+    _check(getattr(lib(), name)(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), name)
+    return a, b
+
+
+def _gen_batch_drbg(kind, alphas, n, seed_bytes, prf, nthreads):
+    alphas = np.ascontiguousarray(alphas, np.int64)
+    name = "b200dpf_gen_batch" + kind
+    if len(seed_bytes) != 44 * len(alphas):
+        raise ValueError("gen_batch%s needs 44 seed bytes per key (%d keys, %d bytes)" % (kind, len(alphas), len(seed_bytes)))
+    a = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    b = np.zeros((len(alphas), KEY_WORDS), np.int32)
+    _check(getattr(lib(), name)(alphas, bytes(seed_bytes), len(alphas), n, prf, nthreads, a, b), name)
+    return a, b
+
+
+def _eval_cpu(kind, key, prf):
     key = np.ascontiguousarray(key, np.int32)
-    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
-    n = C.c_size_t()
-    _check(lib().b200dpf_key_pack(key, buf, len(buf), C.byref(n)), "b200dpf_key_pack")
-    return buf.raw[:n.value]
-
-
-def key_unpack(packed):
-    key = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_key_unpack(bytes(packed), len(packed), key), "b200dpf_key_unpack")
-    return key
-
-
-def eval_cpu(key, prf):
-    key = np.ascontiguousarray(key, np.int32)
-    n = lib().b200dpf_key_n(key)
+    n = _key_n(key, kind)
     if n < 0:
-        raise B200DPFError("malformed key")
-    out = np.zeros(n, np.int32)
-    _check(lib().b200dpf_eval_cpu(key, prf, out), "b200dpf_eval_cpu")
+        raise B200DPFError("not an %s key" % KINDS[kind][2] if kind else "malformed key")
+    out = np.zeros(n // 32, np.uint32) if kind == "_xor" else np.zeros(n, np.int32)
+    name = "b200dpf_eval_cpu" + kind
+    _check(getattr(lib(), name)(key, prf, out), name)
     return out
 
 
-def _et_key_n(key):
-    """rows of an early-terminated key (slot 0 = (d, 2, 0, 0), slot 130 = 4 * 2^d), or -1"""
-    d, w = int(key[0]), int(key[1])
-    if w != 2 or key[2] or key[3] or not 1 <= d <= 29:
-        return -1
-    n = int(np.uint32(key[130 * 4]))
-    return n if n == 4 << d and not key[130 * 4 + 1:130 * 4 + 4].any() else -1
+def _key_pack(kind, key):
+    key = np.ascontiguousarray(key, np.int32)
+    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
+    n = C.c_size_t()
+    name = "b200dpf_key_pack" + kind
+    _check(getattr(lib(), name)(key, buf, len(buf), C.byref(n)), name)
+    return buf.raw[:n.value]
+
+
+def _key_unpack(kind, packed):
+    key = np.zeros(KEY_WORDS, np.int32)
+    name = "b200dpf_key_unpack" + kind
+    _check(getattr(lib(), name)(bytes(packed), len(packed), key), name)
+    return key
+
+
+def key_pack(key):
+    return _key_pack("", key)
+
+
+def key_unpack(packed):
+    return _key_unpack("", packed)
+
+
+def eval_cpu(key, prf):
+    return _eval_cpu("", key, prf)
 
 
 def gen_et(alpha, n, seed_bytes, prf):
     """early-terminated key pair for row alpha of an n-row table (DESIGN.md section 9); >= 44 seed bytes"""
-    a = np.zeros(KEY_WORDS, np.int32)
-    b = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_gen_et(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), "b200dpf_gen_et")
-    return a, b
+    return _gen_drbg("_et", alpha, n, seed_bytes, prf)
 
 
 def gen_batch_et(alphas, n, seed_bytes, prf, nthreads=0):
     """seed_bytes: 44 bytes of entropy per key, concatenated"""
-    alphas = np.ascontiguousarray(alphas, np.int64)
-    if len(seed_bytes) != 44 * len(alphas):
-        raise ValueError("gen_batch_et needs 44 seed bytes per key (%d keys, %d bytes)" % (len(alphas), len(seed_bytes)))
-    a = np.zeros((len(alphas), KEY_WORDS), np.int32)
-    b = np.zeros((len(alphas), KEY_WORDS), np.int32)
-    _check(lib().b200dpf_gen_batch_et(alphas, bytes(seed_bytes), len(alphas), n, prf, nthreads, a, b), "b200dpf_gen_batch_et")
-    return a, b
+    return _gen_batch_drbg("_et", alphas, n, seed_bytes, prf, nthreads)
 
 
 def eval_cpu_et(key, prf):
-    key = np.ascontiguousarray(key, np.int32)
-    n = _et_key_n(key)
-    if n < 0:
-        raise B200DPFError("not an early-terminated key")
-    out = np.zeros(n, np.int32)
-    _check(lib().b200dpf_eval_cpu_et(key, prf, out), "b200dpf_eval_cpu_et")
-    return out
+    return _eval_cpu("_et", key, prf)
 
 
 def key_pack_et(key):
-    key = np.ascontiguousarray(key, np.int32)
-    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
-    n = C.c_size_t()
-    _check(lib().b200dpf_key_pack_et(key, buf, len(buf), C.byref(n)), "b200dpf_key_pack_et")
-    return buf.raw[:n.value]
+    return _key_pack("_et", key)
 
 
 def key_unpack_et(packed):
-    key = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_key_unpack_et(bytes(packed), len(packed), key), "b200dpf_key_unpack_et")
-    return key
-
-
-def _xor_key_n(key):
-    """rows of an XOR-shared key (slot 0 = (d, 7, 0, 0), slot 130 = 128 * 2^d), or -1"""
-    d, w = int(key[0]), int(key[1])
-    if w != 7 or key[2] or key[3] or not 1 <= d <= 24:
-        return -1
-    n = int(np.uint32(key[130 * 4]))
-    return n if n == 128 << d and not key[130 * 4 + 1:130 * 4 + 4].any() else -1
+    return _key_unpack("_et", packed)
 
 
 def gen_xor(alpha, n, seed_bytes, prf):
     """XOR-shared key pair for row alpha of an n-row table (DESIGN.md section 10); >= 44 seed bytes"""
-    a = np.zeros(KEY_WORDS, np.int32)
-    b = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_gen_xor(alpha, n, bytes(seed_bytes), len(seed_bytes), prf, a, b), "b200dpf_gen_xor")
-    return a, b
+    return _gen_drbg("_xor", alpha, n, seed_bytes, prf)
 
 
 def gen_batch_xor(alphas, n, seed_bytes, prf, nthreads=0):
     """seed_bytes: 44 bytes of entropy per key, concatenated"""
-    alphas = np.ascontiguousarray(alphas, np.int64)
-    if len(seed_bytes) != 44 * len(alphas):
-        raise ValueError("gen_batch_xor needs 44 seed bytes per key (%d keys, %d bytes)" % (len(alphas), len(seed_bytes)))
-    a = np.zeros((len(alphas), KEY_WORDS), np.int32)
-    b = np.zeros((len(alphas), KEY_WORDS), np.int32)
-    _check(lib().b200dpf_gen_batch_xor(alphas, bytes(seed_bytes), len(alphas), n, prf, nthreads, a, b), "b200dpf_gen_batch_xor")
-    return a, b
+    return _gen_batch_drbg("_xor", alphas, n, seed_bytes, prf, nthreads)
 
 
 def eval_cpu_xor(key, prf):
     """share bits packed, uint32 [n / 32]: row i is bit (i & 31) of word i >> 5"""
-    key = np.ascontiguousarray(key, np.int32)
-    n = _xor_key_n(key)
-    if n < 0:
-        raise B200DPFError("not an XOR-shared key")
-    out = np.zeros(n // 32, np.uint32)
-    _check(lib().b200dpf_eval_cpu_xor(key, prf, out), "b200dpf_eval_cpu_xor")
-    return out
+    return _eval_cpu("_xor", key, prf)
 
 
 def key_pack_xor(key):
-    key = np.ascontiguousarray(key, np.int32)
-    buf = C.create_string_buffer(lib().b200dpf_key_packed_size(32))
-    n = C.c_size_t()
-    _check(lib().b200dpf_key_pack_xor(key, buf, len(buf), C.byref(n)), "b200dpf_key_pack_xor")
-    return buf.raw[:n.value]
+    return _key_pack("_xor", key)
 
 
 def key_unpack_xor(packed):
-    key = np.zeros(KEY_WORDS, np.int32)
-    _check(lib().b200dpf_key_unpack_xor(bytes(packed), len(packed), key), "b200dpf_key_unpack_xor")
-    return key
+    return _key_unpack("_xor", packed)
 
 
 class Context:
@@ -312,7 +296,8 @@ class Context:
         assert table.ndim == 2
         self.n, self.entry_size = table.shape
         self.handle = C.c_void_p()
-        name = "b200dpf_create_xor" if xor else "b200dpf_create_et" if early_termination else "b200dpf_create"
+        self.kind = "_xor" if xor else "_et" if early_termination else ""
+        name = "b200dpf_create" + self.kind
         _check(getattr(lib(), name)(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
                                     device, shard_rank, shard_count), name)
 

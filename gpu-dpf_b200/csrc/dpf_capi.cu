@@ -141,11 +141,12 @@ struct b200dpf_ctx {
     int shard_rank = 0, shard_count = 1, shard_bits = 0;
     int64_t n_local = 0;
     int depth_local = 0;
-    /* log2 table rows per tree leaf: 0, 2 on an early-terminated context (b200dpf_create_et) or 7 on an
-     * XOR-shared one (b200dpf_create_xor).  n, n_local, the table, the leaf cache and the results count
-     * rows; depth, depth_local, the shards, the work items and the frontier count leaves. */
-    int lane_bits = 0;
-    bool is_xor() const { return lane_bits == host::XOR_LOG2_ROWS_PER_LEAF; }
+    /* the kind of key the context takes (host::KindInfo): standard, early-terminated (b200dpf_create_et) or
+     * XOR-shared (b200dpf_create_xor).  A leaf carries 2^lane_bits() table rows: n, n_local, the table, the
+     * leaf cache and the results count rows; depth, depth_local, the shards, the work items and the
+     * frontier count leaves. */
+    int kind = host::KIND_STANDARD;
+    int lane_bits() const { return host::kKinds[kind].lane_bits; }
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
     DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
@@ -370,17 +371,8 @@ struct KeyLayout {
 KeyLayout reference_layout() { return KeyLayout{131u, 129u, 0}; }                       /* dpf_wrapper.cu:26-46 */
 KeyLayout compact_layout(int depth) { return KeyLayout{2u + 4u * (uint32_t)depth, 1u, 1}; }   /* b200dpf_key_pack */
 
-/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks); the magic is
- * "DPF2", "DPE4" for an early-terminated key or "DPX7" for an XOR-shared one */
-constexpr char kMagic[] = "DPF2", kMagicEt[] = "DPE4", kMagicXor[] = "DPX7";
-
-/* the compact-form magic of the keys a context takes */
-inline const char *ctx_magic(const b200dpf_ctx *c)
-{
-    return c->is_xor() ? kMagicXor : c->lane_bits ? kMagicEt : kMagic;
-}
-
-inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char *magic = kMagic)
+/* compact form of one key straight into `dst` (b200dpf_key_pack without the checks); `magic` is its kind's */
+inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char *magic)
 {
     const uint8_t *k = reinterpret_cast<const uint8_t *>(key);
     std::memset(dst, 0, 16);
@@ -395,52 +387,55 @@ inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char
     }
 }
 
-/* key number `b` of a batch (null: none) must have been generated for the table's n */
-inline int check_key_n(const int32_t *key, int64_t b, int64_t n)
+/* What the contexts and the launch planner do differently per kind of key (host::kKinds has the key
+ * format): the kernel modes, and the limits of one kind. */
+struct KindOps {
+    int mode_fused, mode_expand;
+    int mode_grouped;       /* -1: no grouped contexts */
+    int max_nv;             /* fused passes: at most 4 * max_nv columns (early-terminated 32, XOR-shared 16) */
+    bool leaf_cache;        /* wide entries may cache leaves (XOR-shared: a further 16 columns re-walk the tree) */
+    bool tma_rows;          /* the B200DPF_TMA_ROWS variant exists */
+    int min_kpw_log2;       /* fused launches: at least 2^this keys per warp (the XOR kernel splits rows across a
+                             * key quad; the missing keys of a smaller batch are duplicates whose results are dropped) */
+    int leaf_items;         /* > 0: automatic s for leaves of many rows -- items down to s = 1, this many per warp */
+    const char *gen;        /* the generator of the kind's keys, in messages */
+};
+constexpr KindOps kKindOps[host::KIND_COUNT] = {
+    {MODE_FUSED, MODE_EXPAND, MODE_GROUPED, 16, true, true, 0, 0, "b200dpf_gen"},
+    {MODE_FUSED_ET, MODE_EXPAND_ET, MODE_GROUPED_ET, 8, true, false, 0, 0, "b200dpf_gen_et"},
+    {MODE_FUSED_XOR, MODE_EXPAND_XOR, -1, 4, false, false, 2, 4, "b200dpf_gen_xor"},
+};
+
+/* "a standard", "an early-terminated", "an XOR-shared": the article of a kind's name */
+inline const char *article(int kind) { return kind == host::KIND_STANDARD ? "a" : "an"; }
+
+/* The refusal of entry point `name` of a key that is not of `kind` */
+int fail_not_kind(int kind, const char *name)
 {
-    const int64_t kn = key ? host::key_n(key) : -1;
-    if (kn == n) return B200DPF_OK;
-    return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, table has n=%lld", (long long)b, (long long)kn, (long long)n);
+    if (kind == host::KIND_STANDARD) return fail(B200DPF_EINVAL, "%s: malformed key", name);
+    return fail(B200DPF_EINVAL, "%s: not an %s key", name, host::kKinds[kind].name);
 }
 
-/* key number `b` of a batch must be an early-terminated key for n rows */
-inline int check_key_et_n(const int32_t *key, int64_t b, int64_t n)
+/* Key number `b` of a batch (null: none) must be a key of `kind` for the n rows of the context's table, or
+ * of its bin `bin` (>= 0).  Only a refused key is decoded twice. */
+int check_key(int kind, int64_t n, const int32_t *key, int64_t b, int bin)
 {
-    const int64_t kn = key ? host::key_et_n(key) : -1;
+    const int64_t kn = key ? host::key_n(key, kind) : -1;
     if (kn == n) return B200DPF_OK;
-    if (key && host::key_n(key) >= 0)
-        return fail(B200DPF_EINVAL, "key %lld is a standard key; this early-terminated context takes keys of b200dpf_gen_et", (long long)b);
-    return fail(B200DPF_EINVAL, "key %lld is not an early-terminated key for n=%lld (its n: %lld)", (long long)b, (long long)n,
-                (long long)kn);
-}
-
-/* key number `b` of a batch must be an XOR-shared key for n rows */
-inline int check_key_xor_n(const int32_t *key, int64_t b, int64_t n)
-{
-    const int64_t kn = key ? host::key_xor_n(key) : -1;
-    if (kn == n) return B200DPF_OK;
-    if (key && host::key_n(key) >= 0)
-        return fail(B200DPF_EINVAL, "key %lld is a standard key; this XOR-shared context takes keys of b200dpf_gen_xor", (long long)b);
-    if (key && host::key_et_n(key) >= 0)
-        return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this XOR-shared context takes keys of b200dpf_gen_xor",
-                    (long long)b);
-    return fail(B200DPF_EINVAL, "key %lld is not an XOR-shared key for n=%lld (its n: %lld)", (long long)b, (long long)n,
-                (long long)kn);
-}
-
-/* key number `b` of a batch must be of the context's kind (standard, early-terminated or XOR-shared) and n */
-inline int check_key(const b200dpf_ctx *c, const int32_t *key, int64_t b)
-{
-    if (c->is_xor()) return check_key_xor_n(key, b, c->n);
-    if (key && host::key_xor_n(key) >= 0)
-        return fail(B200DPF_EINVAL, "key %lld is an XOR-shared key; this context takes %s keys", (long long)b,
-                    c->lane_bits ? "early-terminated" : "standard");
-    if (!c->lane_bits) {
-        if (key && host::key_et_n(key) >= 0)
-            return fail(B200DPF_EINVAL, "key %lld is an early-terminated key; this context takes standard keys", (long long)b);
-        return check_key_n(key, b, c->n);
-    }
-    return check_key_et_n(key, b, c->n);
+    const int other = key ? host::key_kind(key) : -1;
+    const host::KindInfo &k = host::kKinds[kind];
+    char where[32] = "table";
+    if (bin >= 0) snprintf(where, sizeof where, "bin %d", bin);
+    if (kind == host::KIND_STANDARD && other > 0)
+        return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, %s has n=%lld (it is %s %s key; this context takes standard keys)",
+                    (long long)b, (long long)kn, where, (long long)n, article(other), host::kKinds[other].name);
+    if (kind == host::KIND_STANDARD)
+        return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, %s has n=%lld", (long long)b, (long long)kn, where, (long long)n);
+    if (other >= 0 && other != kind)
+        return fail(B200DPF_EINVAL, "key %lld is %s %s key; this %s context takes keys of %s", (long long)b, article(other),
+                    host::kKinds[other].name, k.name, kKindOps[kind].gen);
+    return fail(B200DPF_EINVAL, "key %lld is not %s %s key for n=%lld (its n: %lld)", (long long)b, article(kind), k.name,
+                (long long)n, (long long)kn);
 }
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
@@ -467,26 +462,20 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
      * columns, NV = 4), which also caches each leaf's low word; every other column is produced by
      * MAC-only passes over that cache.  Without the cache (disabled or lane-split batches) wide
      * entries use one tree expansion per 64 columns. */
-    const bool et = c->lane_bits != 0;   /* early-terminated: 32 columns per pass at most */
-    const bool xk = c->is_xor();         /* XOR-shared: 16 columns per pass, no leaf cache */
-    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache || xk) ? 4 : (c->entry_pad <= 32 || et ? 8 : 16);
+    const KindOps &ops = kKindOps[c->kind];
+    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache) ? 4 : std::min(ops.max_nv, c->entry_pad <= 32 ? 8 : 16);
     const int passes = mode_main == MODE_FUSED ? (want_cache ? 1 : c->entry_pad / (4 * nv)) : 1;
-    /* the kernel modes of this context's kind */
-    const int mode_fused = xk ? MODE_FUSED_XOR : et ? MODE_FUSED_ET : MODE_FUSED;
-    const int mode_expand = xk ? MODE_EXPAND_XOR : et ? MODE_EXPAND_ET : MODE_EXPAND;
     /* optional variant: the rows of each work item staged into shared memory by cp.async.bulk */
     bool tma_rows = K.tma_rows != 0 && K.one_launch != 0 && c->coop_ok != 0 && mode_main == MODE_FUSED && c->entry_pad == 16 &&
-                    prf != B200DPF_PRF_AES128 && nkeys >= 17 && !et;
-    const int mode_plain = mode_main == MODE_FUSED ? mode_fused : mode_expand;
+                    prf != B200DPF_PRF_AES128 && nkeys >= 17 && ops.tma_rows;
+    const int mode_plain = mode_main == MODE_FUSED ? ops.mode_fused : ops.mode_expand;
     int mode_kernel = tma_rows ? MODE_FUSED_TMA : mode_plain;
     /* keys per warp: a full warp of keys when the batch allows; for small batches the
      * spare lanes take adjacent subtrees of the same keys (single-query latency mode) */
     int kpw_log2 = 5;
     if (K.lane_split != 0)
         while (kpw_log2 > 0 && ((int64_t)1 << (kpw_log2 - 1)) >= nkeys) kpw_log2--;
-    /* the XOR kernel splits rows across the four lanes of a key quad, which must hold four keys (the
-     * missing ones of a smaller batch are duplicates whose results are dropped) */
-    if (xk && mode_main == MODE_FUSED) kpw_log2 = std::max(kpw_log2, 2);
+    if (mode_main == MODE_FUSED) kpw_log2 = std::max(kpw_log2, ops.min_kpw_log2);
     int64_t key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
     /* AES binds the shared-memory data pipe, and a broadcast row load is charged for every lane's copy
      * of the row: with at least 4 keys per warp, each lane of a key quad loads a quarter of the row and
@@ -519,8 +508,8 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
          * power limit, SM clock 1980 MHz, ms per batch (DESIGN.md section 10):
          *   n=2^16: auto 0.107; s=1 0.103, 2 0.148, 3 0.196, 4 0.262, 5 0.490
          *   n=2^20: auto 0.971; s=1 0.989, 2 0.980, 3 0.971, 4 0.975, 5 0.975, 6 0.973 */
-        const int s_floor = xk ? 1 : want_frontier ? 3 : 5;
-        const int64_t items_per_warp = xk ? 4 : want_frontier ? 24 : 6;
+        const int s_floor = ops.leaf_items ? 1 : want_frontier ? 3 : 5;
+        const int64_t items_per_warp = ops.leaf_items ? ops.leaf_items : want_frontier ? 24 : 6;
         s = std::min(c->depth_local, std::min(L.s_max, s_cap));
         while (s > s_floor &&
                ((((int64_t)1 << (c->depth_local - s)) * key_groups) >> (5 - kpw_log2)) < items_per_warp * warps)
@@ -719,7 +708,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
     };
     if (mode_main == MODE_EXPAND) {
         p.shares = reinterpret_cast<uint32_t *>(out_dev);
-        return launch_main(4, mode_expand);
+        return launch_main(4, ops.mode_expand);
     }
     p.out = reinterpret_cast<uint32_t *>(out_dev);
     if (want_cache) {
@@ -731,7 +720,7 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         p.col_off_v = 0;
         p.col_off = 0;
         p.ncols = (uint32_t)std::min(16, c->entry_size);
-        rc = launch_main(4, mode_fused);
+        rc = launch_main(4, ops.mode_fused);
         if (rc) return rc;
         MacParams m;
         std::memset(&m, 0, sizeof m);
@@ -792,8 +781,7 @@ int run_pipeline(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int6
     const b200dpf_ctx::Knobs &K = c->knobs;
     int rc = B200DPF_OK;
     int launches = 0;
-    /* XOR-shared keys have no leaf cache: a further 16 columns re-walk the tree, 1/128 of the rows */
-    const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0 && !c->is_xor();
+    const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0 && kKindOps[c->kind].leaf_cache;
     const size_t per_group = 32u * (size_t)c->n_local * sizeof(uint32_t);
     const size_t cap = (size_t)std::max(K.leaf_cache_mb, 1) << 20;
     if (!wide || per_group > cap) {
@@ -943,6 +931,84 @@ bool gen_parallel(int64_t count, int nthreads, GenOne gen_one)
     return std::find(rcs.begin(), rcs.end(), -1) == rcs.end();
 }
 
+/* The CPU entry points of every kind of key; `name` is the entry point's, without "b200dpf_", in messages. */
+
+/* one key pair from the ChaCha20 DRBG: b200dpf_gen_secure for standard keys */
+int gen_drbg_one(int kind, int64_t alpha, int64_t n, const uint8_t *seed, int prf, int32_t *key_a, int32_t *key_b)
+{
+    if (kind == host::KIND_STANDARD) return host::gen_secure(alpha, n, seed, prf, key_a, key_b);
+    return host::gen_leaves(kind, alpha, n, seed, prf, key_a, key_b);
+}
+
+int gen_drbg(int kind, const char *name, int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf,
+             int32_t *key_a, int32_t *key_b)
+{
+    const host::KindInfo &k = host::kKinds[kind];
+    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
+    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "%s needs at least 44 bytes of seed (got %zu)", name, seed_len);
+    if (gen_drbg_one(kind, alpha, n, seed, prf, key_a, key_b) != 0)
+        return fail(B200DPF_EINVAL, "%s: need power-of-two n in [%lld, 2^%d], 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
+                    name, (long long)k.n_min, ilog2(k.n_max), (long long)alpha, (long long)n, prf);
+    return B200DPF_OK;
+}
+
+int gen_batch_drbg(int kind, const char *name, const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
+                   int nthreads, int32_t *keys_a, int32_t *keys_b)
+{
+    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad %s argument", name);
+    if (!gen_parallel(count, nthreads, [&](int64_t i) {
+            return gen_drbg_one(kind, alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
+        }))
+        return fail(B200DPF_EINVAL, "%s: invalid alpha/n/prf in batch", name);
+    return B200DPF_OK;
+}
+
+int eval_cpu_kind(int kind, const char *name, const int32_t *key, int prf, int32_t *out)
+{
+    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
+    const int rc = host::eval_cpu(key, kind, prf, out);
+    if (rc == -1) return fail_not_kind(kind, name);
+    if (rc) return fail(B200DPF_EINVAL, "%s: unknown prf id %d", name, prf);
+    return B200DPF_OK;
+}
+
+int key_pack_kind(int kind, const char *name, const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
+{
+    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
+    const int depth = host::key_depth(key, kind);
+    if (depth < 1 || host::key_n(key, kind) < 0) return fail_not_kind(kind, name);
+    const size_t need = b200dpf_key_packed_size(depth);
+    if (out_cap < need) return fail(B200DPF_EINVAL, "%s: need %zu bytes, have %zu", name, need, out_cap);
+    pack_compact(key, out, depth, host::kKinds[kind].magic);
+    if (written) *written = need;
+    return B200DPF_OK;
+}
+
+int key_unpack_kind(int kind, const char *name, const uint8_t *in, size_t in_len, int32_t *key)
+{
+    const host::KindInfo &k = host::kKinds[kind];
+    if (!in || !key) return fail(B200DPF_EINVAL, "null buffer");
+    if (in_len < 32 || std::memcmp(in, k.magic, 4) != 0) return fail(B200DPF_EINVAL, "%s: bad header", name);
+    const int depth = in[4];
+    bool pad_zero = true;
+    for (int i = 5; i < 16; i++) pad_zero = pad_zero && in[i] == 0;
+    if (depth < 1 || depth > k.max_depth || !pad_zero || in_len != b200dpf_key_packed_size(depth))
+        return fail(B200DPF_EINVAL, "%s: depth %d does not match %zu bytes", name, depth, in_len);
+    std::memset(key, 0, sizeof(int32_t) * host::KEY_WORDS);
+    uint8_t *kb = reinterpret_cast<uint8_t *>(key);
+    kb[16 * host::SLOT_DEPTH] = (uint8_t)depth;
+    kb[16 * host::SLOT_DEPTH + 4] = (uint8_t)k.lane_bits;
+    std::memcpy(kb + 16 * host::SLOT_ROOT, in + 16, 16);
+    for (int L = 0; L < depth; L++) {
+        const uint8_t *o = in + 32 + 64 * L;
+        std::memcpy(kb + 16 * (host::SLOT_CW1 + 2 * L), o, 32);
+        std::memcpy(kb + 16 * (host::SLOT_CW2 + 2 * L), o + 32, 32);
+    }
+    const uint64_t n = (uint64_t)1 << (depth + k.lane_bits);
+    std::memcpy(kb + 16 * host::SLOT_N, &n, 8);
+    return B200DPF_OK;
+}
+
 }  // namespace
 
 /* multi-device contexts (defined at the end of this file) */
@@ -973,12 +1039,7 @@ int b200dpf_gen(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, 
 int b200dpf_gen_secure(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf,
                        int32_t *key_a, int32_t *key_b)
 {
-    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
-    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "gen_secure needs at least 44 bytes of seed (got %zu)", seed_len);
-    if (host::gen_secure(alpha, n, seed, prf, key_a, key_b) != 0)
-        return fail(B200DPF_EINVAL, "gen_secure: need power-of-two n >= 2, 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
-                    (long long)alpha, (long long)n, prf);
-    return B200DPF_OK;
+    return gen_drbg(host::KIND_STANDARD, "gen_secure", alpha, n, seed, seed_len, prf, key_a, key_b);
 }
 
 int b200dpf_gen_batch(const int64_t *alphas, const uint32_t *seeds32, int64_t count, int64_t n, int prf,
@@ -995,12 +1056,7 @@ int b200dpf_gen_batch(const int64_t *alphas, const uint32_t *seeds32, int64_t co
 int b200dpf_gen_batch_secure(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
                              int nthreads, int32_t *keys_a, int32_t *keys_b)
 {
-    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_secure argument");
-    if (!gen_parallel(count, nthreads, [&](int64_t i) {
-            return host::gen_secure(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
-        }))
-        return fail(B200DPF_EINVAL, "gen_batch_secure: invalid alpha/n/prf in batch");
-    return B200DPF_OK;
+    return gen_batch_drbg(host::KIND_STANDARD, "gen_batch_secure", alphas, seeds44, count, n, prf, nthreads, keys_a, keys_b);
 }
 
 int b200dpf_gen_batch_gpu(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int device,
@@ -1039,188 +1095,91 @@ int b200dpf_gen_batch_gpu(const int64_t *alphas, const uint8_t *seeds44, int64_t
 
 int b200dpf_eval_cpu(const int32_t *key, int prf, int32_t *out_n)
 {
-    if (!key || !out_n) return fail(B200DPF_EINVAL, "null buffer");
-    if (host::eval_cpu(key, prf, out_n) != 0) return fail(B200DPF_EINVAL, "eval_cpu: malformed key or prf id");
-    return B200DPF_OK;
+    return eval_cpu_kind(host::KIND_STANDARD, "eval_cpu", key, prf, out_n);
 }
 
 size_t b200dpf_key_packed_size(int depth) { return depth >= 1 && depth <= 32 ? (size_t)32 + 64u * (size_t)depth : 0; }
 
 int b200dpf_key_pack(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
 {
-    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
-    const int depth = host::key_depth(key);
-    if (depth < 1 || host::key_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack: malformed key");
-    const size_t need = b200dpf_key_packed_size(depth);
-    if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack: need %zu bytes, have %zu", need, out_cap);
-    pack_compact(key, out, depth);
-    if (written) *written = need;
-    return B200DPF_OK;
+    return key_pack_kind(host::KIND_STANDARD, "key_pack", key, out, out_cap, written);
 }
 
 int b200dpf_key_unpack(const uint8_t *in, size_t in_len, int32_t *key)
 {
-    if (!in || !key) return fail(B200DPF_EINVAL, "null buffer");
-    if (in_len < 32 || std::memcmp(in, "DPF2", 4) != 0) return fail(B200DPF_EINVAL, "key_unpack: bad header");
-    const int depth = in[4];
-    bool pad_zero = true;
-    for (int i = 5; i < 16; i++) pad_zero = pad_zero && in[i] == 0;
-    if (depth < 1 || depth > 32 || !pad_zero || in_len != b200dpf_key_packed_size(depth))
-        return fail(B200DPF_EINVAL, "key_unpack: depth %d does not match %zu bytes", depth, in_len);
-    std::memset(key, 0, sizeof(int32_t) * host::KEY_WORDS);
-    uint8_t *k = reinterpret_cast<uint8_t *>(key);
-    k[16 * host::SLOT_DEPTH] = (uint8_t)depth;
-    std::memcpy(k + 16 * host::SLOT_ROOT, in + 16, 16);
-    for (int L = 0; L < depth; L++) {
-        const uint8_t *o = in + 32 + 64 * L;
-        std::memcpy(k + 16 * (host::SLOT_CW1 + 2 * L), o, 32);
-        std::memcpy(k + 16 * (host::SLOT_CW2 + 2 * L), o + 32, 32);
-    }
-    const uint64_t n = (uint64_t)1 << depth;
-    std::memcpy(k + 16 * host::SLOT_N, &n, 8);
-    return B200DPF_OK;
+    return key_unpack_kind(host::KIND_STANDARD, "key_unpack", in, in_len, key);
 }
 
-int64_t b200dpf_key_n(const int32_t *key) { return key ? host::key_n(key) : -1; }
-int b200dpf_key_depth(const int32_t *key) { return key ? host::key_depth(key) : -1; }
+int64_t b200dpf_key_n(const int32_t *key) { return key ? host::key_n(key, host::KIND_STANDARD) : -1; }
+int b200dpf_key_depth(const int32_t *key) { return key ? host::key_depth(key, host::KIND_STANDARD) : -1; }
 
 /* ---- early-terminated keys ---- */
 
 int b200dpf_gen_et(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf, int32_t *key_a, int32_t *key_b)
 {
-    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
-    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "gen_et needs at least 44 bytes of seed (got %zu)", seed_len);
-    if (host::gen_et(alpha, n, seed, prf, key_a, key_b) != 0)
-        return fail(B200DPF_EINVAL, "gen_et: need power-of-two n in [8, 2^31], 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
-                    (long long)alpha, (long long)n, prf);
-    return B200DPF_OK;
+    return gen_drbg(host::KIND_ET, "gen_et", alpha, n, seed, seed_len, prf, key_a, key_b);
 }
 
 int b200dpf_gen_batch_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int nthreads,
                          int32_t *keys_a, int32_t *keys_b)
 {
-    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_et argument");
-    if (!gen_parallel(count, nthreads, [&](int64_t i) {
-            return host::gen_et(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
-        }))
-        return fail(B200DPF_EINVAL, "gen_batch_et: invalid alpha/n/prf in batch");
-    return B200DPF_OK;
+    return gen_batch_drbg(host::KIND_ET, "gen_batch_et", alphas, seeds44, count, n, prf, nthreads, keys_a, keys_b);
 }
 
 int b200dpf_eval_cpu_et(const int32_t *key, int prf, int32_t *out_n)
 {
-    if (!key || !out_n) return fail(B200DPF_EINVAL, "null buffer");
-    if (host::key_et_n(key) < 0) return fail(B200DPF_EINVAL, "eval_cpu_et: not an early-terminated key");
-    if (host::eval_cpu_et(key, prf, out_n) != 0) return fail(B200DPF_EINVAL, "eval_cpu_et: unknown prf id %d", prf);
-    return B200DPF_OK;
+    return eval_cpu_kind(host::KIND_ET, "eval_cpu_et", key, prf, out_n);
 }
 
 int b200dpf_key_pack_et(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
 {
-    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
-    const int depth = host::key_et_depth(key);
-    if (depth < 1 || host::key_et_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack_et: not an early-terminated key");
-    const size_t need = b200dpf_key_packed_size(depth);
-    if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack_et: need %zu bytes, have %zu", need, out_cap);
-    pack_compact(key, out, depth, kMagicEt);
-    if (written) *written = need;
-    return B200DPF_OK;
+    return key_pack_kind(host::KIND_ET, "key_pack_et", key, out, out_cap, written);
 }
-
-}  // extern "C"
-
-/* b200dpf_key_unpack_et / _xor: a key of 2^lane_bits rows per leaf and at most max_depth levels */
-static int key_unpack_leaves(const uint8_t *in, size_t in_len, int32_t *key, const char *magic, int lane_bits, int max_depth,
-                             const char *name)
-{
-    if (!in || !key) return fail(B200DPF_EINVAL, "null buffer");
-    if (in_len < 32 || std::memcmp(in, magic, 4) != 0) return fail(B200DPF_EINVAL, "%s: bad header", name);
-    const int depth = in[4];
-    bool pad_zero = true;
-    for (int i = 5; i < 16; i++) pad_zero = pad_zero && in[i] == 0;
-    if (depth < 1 || depth > max_depth || !pad_zero || in_len != b200dpf_key_packed_size(depth))
-        return fail(B200DPF_EINVAL, "%s: depth %d does not match %zu bytes", name, depth, in_len);
-    std::memset(key, 0, sizeof(int32_t) * host::KEY_WORDS);
-    uint8_t *k = reinterpret_cast<uint8_t *>(key);
-    k[16 * host::SLOT_DEPTH] = (uint8_t)depth;
-    k[16 * host::SLOT_DEPTH + 4] = (uint8_t)lane_bits;
-    std::memcpy(k + 16 * host::SLOT_ROOT, in + 16, 16);
-    for (int L = 0; L < depth; L++) {
-        const uint8_t *o = in + 32 + 64 * L;
-        std::memcpy(k + 16 * (host::SLOT_CW1 + 2 * L), o, 32);
-        std::memcpy(k + 16 * (host::SLOT_CW2 + 2 * L), o + 32, 32);
-    }
-    const uint64_t n = (uint64_t)1 << (depth + lane_bits);
-    std::memcpy(k + 16 * host::SLOT_N, &n, 8);
-    return B200DPF_OK;
-}
-
-extern "C" {
 
 int b200dpf_key_unpack_et(const uint8_t *in, size_t in_len, int32_t *key)
 {
-    return key_unpack_leaves(in, in_len, key, kMagicEt, host::ET_LOG2_ROWS_PER_LEAF, host::ET_MAX_DEPTH, "key_unpack_et");
+    return key_unpack_kind(host::KIND_ET, "key_unpack_et", in, in_len, key);
 }
 
 /* ---- XOR-shared keys ---- */
 
 int b200dpf_gen_xor(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_len, int prf, int32_t *key_a, int32_t *key_b)
 {
-    if (!key_a || !key_b) return fail(B200DPF_EINVAL, "null key buffer");
-    if (!seed || seed_len < 44) return fail(B200DPF_EINVAL, "gen_xor needs at least 44 bytes of seed (got %zu)", seed_len);
-    if (host::gen_xor(alpha, n, seed, prf, key_a, key_b) != 0)
-        return fail(B200DPF_EINVAL, "gen_xor: need power-of-two n in [256, 2^31], 0 <= alpha < n, valid prf (alpha=%lld n=%lld prf=%d)",
-                    (long long)alpha, (long long)n, prf);
-    return B200DPF_OK;
+    return gen_drbg(host::KIND_XOR, "gen_xor", alpha, n, seed, seed_len, prf, key_a, key_b);
 }
 
 int b200dpf_gen_batch_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int nthreads,
                           int32_t *keys_a, int32_t *keys_b)
 {
-    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_xor argument");
-    if (!gen_parallel(count, nthreads, [&](int64_t i) {
-            return host::gen_xor(alphas[i], n, seeds44 + 44 * i, prf, keys_a + i * host::KEY_WORDS, keys_b + i * host::KEY_WORDS);
-        }))
-        return fail(B200DPF_EINVAL, "gen_batch_xor: invalid alpha/n/prf in batch");
-    return B200DPF_OK;
+    return gen_batch_drbg(host::KIND_XOR, "gen_batch_xor", alphas, seeds44, count, n, prf, nthreads, keys_a, keys_b);
 }
 
 int b200dpf_eval_cpu_xor(const int32_t *key, int prf, uint32_t *bits)
 {
-    if (!key || !bits) return fail(B200DPF_EINVAL, "null buffer");
-    if (host::key_xor_n(key) < 0) return fail(B200DPF_EINVAL, "eval_cpu_xor: not an XOR-shared key");
-    if (host::eval_cpu_xor(key, prf, bits) != 0) return fail(B200DPF_EINVAL, "eval_cpu_xor: unknown prf id %d", prf);
-    return B200DPF_OK;
+    return eval_cpu_kind(host::KIND_XOR, "eval_cpu_xor", key, prf, reinterpret_cast<int32_t *>(bits));
 }
 
 int b200dpf_key_pack_xor(const int32_t *key, uint8_t *out, size_t out_cap, size_t *written)
 {
-    if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
-    const int depth = host::key_xor_depth(key);
-    if (depth < 1 || host::key_xor_n(key) < 0) return fail(B200DPF_EINVAL, "key_pack_xor: not an XOR-shared key");
-    const size_t need = b200dpf_key_packed_size(depth);
-    if (out_cap < need) return fail(B200DPF_EINVAL, "key_pack_xor: need %zu bytes, have %zu", need, out_cap);
-    pack_compact(key, out, depth, kMagicXor);
-    if (written) *written = need;
-    return B200DPF_OK;
+    return key_pack_kind(host::KIND_XOR, "key_pack_xor", key, out, out_cap, written);
 }
 
 int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key)
 {
-    return key_unpack_leaves(in, in_len, key, kMagicXor, host::XOR_LOG2_ROWS_PER_LEAF, host::XOR_MAX_DEPTH, "key_unpack_xor");
+    return key_unpack_kind(host::KIND_XOR, "key_unpack_xor", in, in_len, key);
 }
 
 }  // extern "C"
 
-/* b200dpf_create (lane_bits = 0), b200dpf_create_et (lane_bits = 2: 2^lane_bits rows per leaf) and
- * b200dpf_create_xor (lane_bits = 7) */
+/* b200dpf_create, b200dpf_create_et and b200dpf_create_xor: a context for keys of `kind` */
 static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int shard_rank,
-                       int shard_count, int lane_bits)
+                       int shard_count, int kind)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!table) return fail(B200DPF_EINVAL, "null table");
-    const int64_t n_min = (int64_t)2 << lane_bits;
+    const int lane_bits = host::kKinds[kind].lane_bits;
+    const int64_t n_min = host::kKinds[kind].n_min;
     if (n < n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0)
         return fail(B200DPF_EINVAL, "table size n=%lld must be a power of two in [%lld, 2^31]", (long long)n, (long long)n_min);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
@@ -1233,7 +1192,7 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     int rc = ctx_open(device, true, &guard, &c);
     if (rc) return rc;
     c->n = n;
-    c->lane_bits = lane_bits;
+    c->kind = kind;
     c->depth = ilog2(n) - lane_bits;   /* the tree is over leaves */
     c->entry_size = entry_size;
     /* rows padded to what one pass reads: 16, 32 or a multiple of 64 int32 */
@@ -1311,8 +1270,7 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     const int nv0 = c->entry_pad <= 16 ? 4 : (c->entry_pad <= 32 ? 8 : 4);
     SmemLayout tmp;
     for (int prf = 0; prf < 4; prf++) {
-        if (c->is_xor()) smem_layout(c.get(), prf, 4, MODE_FUSED_XOR, &tmp);
-        else smem_layout(c.get(), prf, nv0, lane_bits ? MODE_FUSED_ET : MODE_FUSED, &tmp);
+        smem_layout(c.get(), prf, std::min(nv0, kKindOps[kind].max_nv), kKindOps[kind].mode_fused, &tmp);
         smem_layout(c.get(), prf, 4, MODE_FRONTIER, &tmp);
     }
     *out = c.release();
@@ -1324,22 +1282,22 @@ extern "C" {
 int b200dpf_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
                    int shard_rank, int shard_count)
 {
-    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, 0);
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::KIND_STANDARD);
 }
 
 int b200dpf_create_et(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
                       int shard_rank, int shard_count)
 {
-    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::ET_LOG2_ROWS_PER_LEAF);
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::KIND_ET);
 }
 
 int b200dpf_create_xor(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device,
                        int shard_rank, int shard_count)
 {
-    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::XOR_LOG2_ROWS_PER_LEAF);
+    return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::KIND_XOR);
 }
 
-int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *c) { return c ? 1 << c->lane_bits : -1; }
+int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *c) { return c ? 1 << c->lane_bits() : -1; }
 
 int b200dpf_destroy(b200dpf_ctx *c)
 {
@@ -1383,7 +1341,7 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     int rc = check_eval_args(c, keys, nkeys, prf, out);
     if (rc) return rc;
     for (int64_t b = 0; b < nkeys; b++)
-        if ((rc = check_key(c, keys + b * host::KEY_WORDS, b))) return rc;
+        if ((rc = check_key(c->kind, c->n, keys + b * host::KEY_WORDS, b, -1))) return rc;
     if (!is_pinned_host(keys)) {
         /* pageable keys have to be staged by the CPU anyway: stage only their live 32 + 64*depth bytes
          * (44 % of a key at n = 2^14, 63 % at 2^20) and let the DMA of a chunk overlap the next one */
@@ -1422,8 +1380,8 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
         for (int64_t b = b0; b < b1; b++) {
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
-            if (validate && (rc = check_key(c, keys[b], b))) return rc;
-            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, ctx_magic(c));
+            if (validate && (rc = check_key(c->kind, c->n, keys[b], b, -1))) return rc;
+            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, host::kKinds[c->kind].magic);
         }
         if (!c->multi)
             CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys.ptr) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
@@ -1447,7 +1405,7 @@ int b200dpf_eval_packed(b200dpf_ctx *c, const uint8_t *packed, int64_t nkeys, in
     const size_t stride = b200dpf_key_packed_size(c->depth);
     for (int64_t b = 0; b < nkeys; b++) {
         const uint8_t *k = packed + (size_t)b * stride;
-        if (std::memcmp(k, ctx_magic(c), 4) != 0 || k[4] != (uint8_t)c->depth)
+        if (std::memcmp(k, host::kKinds[c->kind].magic, 4) != 0 || k[4] != (uint8_t)c->depth)
             return fail(B200DPF_EINVAL, "packed key %lld: bad header or depth %d, table has depth %d (n=%lld)", (long long)b,
                         (int)k[4], c->depth, (long long)c->n);
     }
@@ -1808,16 +1766,17 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
 /* ------------------------------------------------------------------------------------------- */
 /* Grouped evaluation: the batch-PIR front end (SURVEY.md section 8(f) rank 4).                  */
 /* ------------------------------------------------------------------------------------------- */
-/* b200dpf_group_create (lane_bits = 0) and b200dpf_group_create_et (lane_bits = 2: 2^lane_bits rows per
- * leaf).  n and the row offsets count rows, the depths (per bin and the context's deepest) leaves. */
+/* b200dpf_group_create and b200dpf_group_create_et: a grouped context for keys of `kind`.  n and the row
+ * offsets count rows, the depths (per bin and the context's deepest) leaves. */
 static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
-                             int device, int lane_bits)
+                             int device, int kind)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!tables || !n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
-    const int64_t n_min = (int64_t)2 << lane_bits;
+    const int lane_bits = host::kKinds[kind].lane_bits;
+    const int64_t n_min = host::kKinds[kind].n_min;
     int64_t n_max = 0, rows = 0;
     for (int g = 0; g < nbins; g++) {
         if (!tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
@@ -1835,7 +1794,7 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
     GroupBins *B = c->bins.get();
     c->n = n_max;                      /* the launch plan (shared memory for correction words) is sized by the deepest bin */
-    c->lane_bits = lane_bits;
+    c->kind = kind;
     c->depth = ilog2(n_max) - lane_bits;
     c->entry_size = entry_size;
     c->entry_pad = (entry_size + 15) & ~15;       /* 16 columns per pass */
@@ -1872,13 +1831,13 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
 int b200dpf_group_create(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
                          int device)
 {
-    return group_create_impl(out, tables, n, nbins, entry_size, device, 0);
+    return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_STANDARD);
 }
 
 int b200dpf_group_create_et(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
                             int device)
 {
-    return group_create_impl(out, tables, n, nbins, entry_size, device, host::ET_LOG2_ROWS_PER_LEAF);
+    return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_ET);
 }
 
 int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
@@ -1894,12 +1853,8 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     for (int64_t b = 0; b < nkeys; b++) {
         const int g = bins[b];
         if (g < 0 || g >= nbins) return fail(B200DPF_EINVAL, "key %lld: bin %d out of range [0,%d)", (long long)b, g, nbins);
-        if (c->lane_bits) {
-            const int rc = check_key_et_n(keys + b * host::KEY_WORDS, b, B->n[(size_t)g]);
-            if (rc) return rc;
-        } else if (host::key_n(keys + b * host::KEY_WORDS) != B->n[(size_t)g])
-            return fail(B200DPF_EINVAL, "key %lld was generated for n=%lld, bin %d has n=%lld", (long long)b,
-                        (long long)host::key_n(keys + b * host::KEY_WORDS), g, (long long)B->n[(size_t)g]);
+        const int rc = check_key(c->kind, B->n[(size_t)g], keys + b * host::KEY_WORDS, b, g);
+        if (rc) return rc;
         count[(size_t)g + 1]++;
     }
     for (int g = 0; g < nbins; g++) count[(size_t)g + 1] += count[(size_t)g];
@@ -1908,8 +1863,8 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
      * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
     const KeyLayout kl = compact_layout(c->depth);
-    const int mode = c->lane_bits ? MODE_GROUPED_ET : MODE_GROUPED;
-    const char *magic = c->lane_bits ? kMagicEt : kMagic;
+    const int mode = kKindOps[c->kind].mode_grouped;
+    const char *magic = host::kKinds[c->kind].magic;
     const size_t stride = (size_t)kl.stride_v * 16u;
     const size_t key_bytes = (size_t)nkeys * stride;
     int rc = reserve_host_keys(c, key_bytes);
@@ -2112,7 +2067,7 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     u.shift = c->shard_bits;
     u.depth = c->depth_local;
     u.table_rows = (uint32_t)update_table_rows(c);
-    u.lane_bits = c->lane_bits;
+    u.lane_bits = c->lane_bits();
     u.table = c->d_table.ptr;
     u.cols = c->entry_size;
     u.stride = c->entry_pad;
@@ -2136,7 +2091,7 @@ int update_host_enqueue(b200dpf_ctx *c, const int64_t *idx, const int32_t *bins,
     if (c->shard_count > 1) {             /* a shard copies only its own rows */
         const uint32_t mask = (uint32_t)c->shard_count - 1u, val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
         for (int64_t j = 0; j < count; j++)
-            if (((uint32_t)(idx[j] >> c->lane_bits) & mask) == val) {
+            if (((uint32_t)(idx[j] >> c->lane_bits()) & mask) == val) {
                 own_idx.push_back(idx[j]);
                 own_rows.insert(own_rows.end(), rows + j * c->entry_size, rows + (j + 1) * c->entry_size);
             }

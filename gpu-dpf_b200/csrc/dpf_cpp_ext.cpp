@@ -51,44 +51,92 @@ const int32_t *key_ptr(const at::Tensor &key)
     return key.data_ptr<int32_t>();
 }
 
-/* dpf_wrapper.cu:49-68 */
-std::vector<at::Tensor> gen(int64_t k, int64_t n, const std::string &seed, int prf)
+/* The kinds of key (include/b200dpf.h): log2 table rows per leaf and maximum depth.  A key is slot 0 =
+ * (d, lane_bits, 0, 0), 1 <= d <= max_depth, slot 130 = 2^(d + lane_bits) as a u64. */
+struct KeyKind {
+    int lane_bits, max_depth;
+};
+constexpr KeyKind kStandard{0, 32}, kEarlyTerminated{2, 29}, kXorShared{7, 24};
+
+/* rows of a key of `kind`, or -1 */
+int64_t key_rows(const int32_t *k, const KeyKind &kind)
+{
+    const uint32_t *w = reinterpret_cast<const uint32_t *>(k);
+    if (w[1] != (uint32_t)kind.lane_bits || w[2] || w[3] || w[0] < 1 || w[0] > (uint32_t)kind.max_depth) return -1;
+    const uint64_t n = (uint64_t)w[4 * 130] | (uint64_t)w[4 * 130 + 1] << 32;
+    return n == (uint64_t)1 << (w[0] + kind.lane_bits) && !w[4 * 130 + 2] && !w[4 * 130 + 3] ? (int64_t)n : -1;
+}
+
+/* One helper per operation; `what` names the Python function in errors.  dpf_wrapper.cu:49-68 is gen. */
+std::vector<at::Tensor> gen_with(int (*fn)(int64_t, int64_t, const uint8_t *, size_t, int, int32_t *, int32_t *),
+                                 const char *what, int64_t k, int64_t n, const std::string &seed, int prf)
 {
     at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
     at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_gen(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf,
-                      a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
-          "gen");
+    check(fn(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
+          what);
     return {a, b};
 }
 
-/* same construction from a ChaCha20 DRBG keyed by >= 44 bytes of caller entropy */
-std::vector<at::Tensor> gen_secure(int64_t k, int64_t n, const std::string &seed, int prf)
+/* batched keygen from the ChaCha20 DRBG: seeds = 44 bytes of entropy per key, concatenated */
+std::vector<at::Tensor> gen_batch_with(int (*fn)(const int64_t *, const uint8_t *, int64_t, int64_t, int, int, int32_t *, int32_t *),
+                                       const char *what, const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf,
+                                       int nthreads)
 {
-    at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_gen_secure(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf,
-                             a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
-          "gen_secure");
+    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
+    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), what, ": need 44 seed bytes per key");
+    const int64_t count = al.numel();
+    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
+    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
+    {
+        py::gil_scoped_release nogil;
+        check(fn(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf, nthreads,
+                 a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
+              what);
+    }
     return {a, b};
 }
 
-/* compact wire form: int32[524] key tensor <-> bytes (24 + 64*depth) */
-py::bytes key_pack(const at::Tensor &key)
+/* the key's share of every row: int32 [n], or (XOR-shared keys, out_shift = 5) its share bits packed 32 per
+ * int32, row i = bit (i & 31) of word i >> 5.  dpf_wrapper.cu:70-84 is eval_cpu. */
+template <class Out>
+at::Tensor eval_cpu_with(int (*fn)(const int32_t *, int, Out *), const char *what, const KeyKind &kind, int out_shift,
+                         const char *not_kind, const at::Tensor &key, int prf)
+{
+    const int32_t *k = key_ptr(key);
+    const int64_t n = key_rows(k, kind);
+    TORCH_CHECK(n > 0, what, ": ", not_kind);
+    at::Tensor result = torch::empty({n >> out_shift}, at::kInt);
+    check(fn(k, prf, reinterpret_cast<Out *>(result.data_ptr<int32_t>())), what);
+    return result;
+}
+
+/* compact wire form: int32[524] key tensor <-> bytes (32 + 64*depth) */
+py::bytes key_pack_with(int (*fn)(const int32_t *, uint8_t *, size_t, size_t *), const char *what, const at::Tensor &key)
 {
     const int32_t *k = key_ptr(key);
     std::string buf(b200dpf_key_packed_size(32), '\0');
     size_t written = 0;
-    check(b200dpf_key_pack(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), "key_pack");
+    check(fn(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), what);
     return py::bytes(buf.data(), written);
 }
 
-at::Tensor key_unpack(const std::string &packed)
+at::Tensor key_unpack_with(int (*fn)(const uint8_t *, size_t, int32_t *), const char *what, const std::string &packed)
 {
     at::Tensor key = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_key_unpack(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()),
-          "key_unpack");
+    check(fn(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()), what);
     return key;
+}
+
+std::vector<void *> eval_init_with(int (*fn)(b200dpf_ctx **, const int32_t *, int64_t, int, int, int, int), const char *what,
+                                   const at::Tensor &table, int device, int shard_rank, int shard_count)
+{
+    TORCH_CHECK(table.dim() == 2, what, ": table must be [num_entries, entry_size]");
+    /* dpf_wrapper.cu:107 converts each element with item<int>(); one vectorised cast here */
+    at::Tensor t = table.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    check(fn(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count), what);
+    return {static_cast<void *>(ctx)};
 }
 
 /* batched keygen: alphas int64[B], seeds int64[B] (low 32 bits used) -> two int32[B,524] tensors */
@@ -111,176 +159,58 @@ std::vector<at::Tensor> gen_batch(const at::Tensor &alphas, int64_t n, const at:
     return {a, b};
 }
 
-/* batched keygen from the ChaCha20 DRBG: seeds = 44 bytes of entropy per key, concatenated */
-std::vector<at::Tensor> gen_batch_secure(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
-{
-    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
-    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), "gen_batch_secure: need 44 seed bytes per key");
-    const int64_t count = al.numel();
-    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
-    {
-        py::gil_scoped_release nogil;
-        check(b200dpf_gen_batch_secure(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf,
-                                       nthreads, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
-              "gen_batch_secure");
-    }
-    return {a, b};
-}
+using Keys = std::vector<at::Tensor>;
+using Ctx = std::vector<void *>;
 
-/* dpf_wrapper.cu:70-84 */
+Keys gen(int64_t k, int64_t n, const std::string &seed, int prf) { return gen_with(b200dpf_gen, "gen", k, n, seed, prf); }
 at::Tensor eval_cpu(const at::Tensor &key, int prf)
 {
-    const int32_t *k = key_ptr(key);
-    const int64_t n = b200dpf_key_n(k);
-    TORCH_CHECK(n > 0, "eval_cpu: malformed key");
-    at::Tensor result = torch::empty({n}, at::kInt);
-    check(b200dpf_eval_cpu(k, prf, result.data_ptr<int32_t>()), "eval_cpu");
-    return result;
+    return eval_cpu_with(b200dpf_eval_cpu, "eval_cpu", kStandard, 0, "malformed key", key, prf);
 }
-
-std::vector<void *> eval_init_sharded(const at::Tensor &table, int device, int shard_rank, int shard_count)
+py::bytes key_pack(const at::Tensor &key) { return key_pack_with(b200dpf_key_pack, "key_pack", key); }
+at::Tensor key_unpack(const std::string &packed) { return key_unpack_with(b200dpf_key_unpack, "key_unpack", packed); }
+Keys gen_secure(int64_t k, int64_t n, const std::string &seed, int prf) { return gen_with(b200dpf_gen_secure, "gen_secure", k, n, seed, prf); }
+Keys gen_batch_secure(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
 {
-    TORCH_CHECK(table.dim() == 2, "eval_init: table must be [num_entries, entry_size]");
-    /* dpf_wrapper.cu:107 converts each element with item<int>(); one vectorised cast here */
-    at::Tensor t = table.to(at::kInt).contiguous();
-    b200dpf_ctx *ctx = nullptr;
-    check(b200dpf_create(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count),
-          "eval_init");
-    return {static_cast<void *>(ctx)};
+    return gen_batch_with(b200dpf_gen_batch_secure, "gen_batch_secure", alphas, n, seeds, prf, nthreads);
 }
-
-/* ---- early-terminated keys: four table rows per tree leaf (include/b200dpf.h, b200dpf_gen_et) ---- */
-
-std::vector<at::Tensor> gen_et(int64_t k, int64_t n, const std::string &seed, int prf)
+Ctx eval_init_sharded(const at::Tensor &table, int device, int shard_rank, int shard_count)
 {
-    at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_gen_et(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf, a.data_ptr<int32_t>(),
-                         b.data_ptr<int32_t>()),
-          "gen_et");
-    return {a, b};
+    return eval_init_with(b200dpf_create, "eval_init", table, device, shard_rank, shard_count);
 }
 
-std::vector<at::Tensor> gen_batch_et(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
+/* early-terminated keys: four table rows per tree leaf (include/b200dpf.h, b200dpf_gen_et) */
+Keys gen_et(int64_t k, int64_t n, const std::string &seed, int prf) { return gen_with(b200dpf_gen_et, "gen_et", k, n, seed, prf); }
+Keys gen_batch_et(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
 {
-    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
-    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), "gen_batch_et: need 44 seed bytes per key");
-    const int64_t count = al.numel();
-    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
-    {
-        py::gil_scoped_release nogil;
-        check(b200dpf_gen_batch_et(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf,
-                                   nthreads, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
-              "gen_batch_et");
-    }
-    return {a, b};
+    return gen_batch_with(b200dpf_gen_batch_et, "gen_batch_et", alphas, n, seeds, prf, nthreads);
 }
-
 at::Tensor eval_cpu_et(const at::Tensor &key, int prf)
 {
-    const int32_t *k = key_ptr(key);
-    /* slot 0 = (d, 2, 0, 0), slot 130 = n = 4 * 2^d; b200dpf_eval_cpu_et checks the rest */
-    const uint32_t d = (uint32_t)k[0];
-    TORCH_CHECK(k[1] == 2 && d >= 1 && d <= 29, "eval_cpu_et: not an early-terminated key");
-    at::Tensor result = torch::empty({(int64_t)4 << d}, at::kInt);
-    check(b200dpf_eval_cpu_et(k, prf, result.data_ptr<int32_t>()), "eval_cpu_et");
-    return result;
+    return eval_cpu_with(b200dpf_eval_cpu_et, "eval_cpu_et", kEarlyTerminated, 0, "not an early-terminated key", key, prf);
 }
-
-py::bytes key_pack_et(const at::Tensor &key)
+py::bytes key_pack_et(const at::Tensor &key) { return key_pack_with(b200dpf_key_pack_et, "key_pack_et", key); }
+at::Tensor key_unpack_et(const std::string &packed) { return key_unpack_with(b200dpf_key_unpack_et, "key_unpack_et", packed); }
+Ctx eval_init_et(const at::Tensor &table, int device, int shard_rank, int shard_count)
 {
-    const int32_t *k = key_ptr(key);
-    std::string buf(b200dpf_key_packed_size(32), '\0');
-    size_t written = 0;
-    check(b200dpf_key_pack_et(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), "key_pack_et");
-    return py::bytes(buf.data(), written);
+    return eval_init_with(b200dpf_create_et, "eval_init_et", table, device, shard_rank, shard_count);
 }
 
-at::Tensor key_unpack_et(const std::string &packed)
+/* XOR-shared keys: 128 table rows per tree leaf, results XOR (include/b200dpf.h, b200dpf_gen_xor) */
+Keys gen_xor(int64_t k, int64_t n, const std::string &seed, int prf) { return gen_with(b200dpf_gen_xor, "gen_xor", k, n, seed, prf); }
+Keys gen_batch_xor(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
 {
-    at::Tensor key = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_key_unpack_et(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()),
-          "key_unpack_et");
-    return key;
+    return gen_batch_with(b200dpf_gen_batch_xor, "gen_batch_xor", alphas, n, seeds, prf, nthreads);
 }
-
-std::vector<void *> eval_init_et(const at::Tensor &table, int device, int shard_rank, int shard_count)
-{
-    TORCH_CHECK(table.dim() == 2, "eval_init_et: table must be [num_entries, entry_size]");
-    at::Tensor t = table.to(at::kInt).contiguous();
-    b200dpf_ctx *ctx = nullptr;
-    check(b200dpf_create_et(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count),
-          "eval_init_et");
-    return {static_cast<void *>(ctx)};
-}
-
-/* ---- XOR-shared keys: 128 table rows per tree leaf, results XOR (include/b200dpf.h, b200dpf_gen_xor) ---- */
-
-std::vector<at::Tensor> gen_xor(int64_t k, int64_t n, const std::string &seed, int prf)
-{
-    at::Tensor a = torch::zeros({kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_gen_xor(k, n, reinterpret_cast<const uint8_t *>(seed.data()), seed.size(), prf, a.data_ptr<int32_t>(),
-                          b.data_ptr<int32_t>()),
-          "gen_xor");
-    return {a, b};
-}
-
-std::vector<at::Tensor> gen_batch_xor(const at::Tensor &alphas, int64_t n, const std::string &seeds, int prf, int nthreads)
-{
-    at::Tensor al = alphas.to(at::kLong).contiguous().cpu();
-    TORCH_CHECK(al.dim() == 1 && (int64_t)seeds.size() == 44 * al.numel(), "gen_batch_xor: need 44 seed bytes per key");
-    const int64_t count = al.numel();
-    at::Tensor a = torch::zeros({count, kKeyWords}, at::kInt);
-    at::Tensor b = torch::zeros({count, kKeyWords}, at::kInt);
-    {
-        py::gil_scoped_release nogil;
-        check(b200dpf_gen_batch_xor(al.data_ptr<int64_t>(), reinterpret_cast<const uint8_t *>(seeds.data()), count, n, prf,
-                                    nthreads, a.data_ptr<int32_t>(), b.data_ptr<int32_t>()),
-              "gen_batch_xor");
-    }
-    return {a, b};
-}
-
-/* the share bits packed: int32 [n / 32], row i = bit (i & 31) of word i >> 5 */
 at::Tensor eval_cpu_xor(const at::Tensor &key, int prf)
 {
-    const int32_t *k = key_ptr(key);
-    /* slot 0 = (d, 7, 0, 0), slot 130 = n = 128 * 2^d; b200dpf_eval_cpu_xor checks the rest */
-    const uint32_t d = (uint32_t)k[0];
-    TORCH_CHECK(k[1] == 7 && d >= 1 && d <= 24, "eval_cpu_xor: not an XOR-shared key");
-    at::Tensor result = torch::empty({(int64_t)4 << d}, at::kInt);
-    check(b200dpf_eval_cpu_xor(k, prf, reinterpret_cast<uint32_t *>(result.data_ptr<int32_t>())), "eval_cpu_xor");
-    return result;
+    return eval_cpu_with(b200dpf_eval_cpu_xor, "eval_cpu_xor", kXorShared, 5, "not an XOR-shared key", key, prf);
 }
-
-py::bytes key_pack_xor(const at::Tensor &key)
+py::bytes key_pack_xor(const at::Tensor &key) { return key_pack_with(b200dpf_key_pack_xor, "key_pack_xor", key); }
+at::Tensor key_unpack_xor(const std::string &packed) { return key_unpack_with(b200dpf_key_unpack_xor, "key_unpack_xor", packed); }
+Ctx eval_init_xor(const at::Tensor &table, int device, int shard_rank, int shard_count)
 {
-    const int32_t *k = key_ptr(key);
-    std::string buf(b200dpf_key_packed_size(32), '\0');
-    size_t written = 0;
-    check(b200dpf_key_pack_xor(k, reinterpret_cast<uint8_t *>(&buf[0]), buf.size(), &written), "key_pack_xor");
-    return py::bytes(buf.data(), written);
-}
-
-at::Tensor key_unpack_xor(const std::string &packed)
-{
-    at::Tensor key = torch::zeros({kKeyWords}, at::kInt);
-    check(b200dpf_key_unpack_xor(reinterpret_cast<const uint8_t *>(packed.data()), packed.size(), key.data_ptr<int32_t>()),
-          "key_unpack_xor");
-    return key;
-}
-
-std::vector<void *> eval_init_xor(const at::Tensor &table, int device, int shard_rank, int shard_count)
-{
-    TORCH_CHECK(table.dim() == 2, "eval_init_xor: table must be [num_entries, entry_size]");
-    at::Tensor t = table.to(at::kInt).contiguous();
-    b200dpf_ctx *ctx = nullptr;
-    check(b200dpf_create_xor(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, shard_rank, shard_count),
-          "eval_init_xor");
-    return {static_cast<void *>(ctx)};
+    return eval_init_with(b200dpf_create_xor, "eval_init_xor", table, device, shard_rank, shard_count);
 }
 
 /* one table on several GPUs of this process (b200dpf_create_multi); axis: 0 auto, 1 entries, 2 keys */

@@ -249,53 +249,32 @@ Seed prf(int prf_id, const Seed &s, uint32_t pos)
     }
 }
 
-int key_depth(const int32_t *key)
+int key_depth(const int32_t *key, int kind)
 {
+    const KindInfo &k = kKinds[kind];
     const Seed d = key_slot(key, SLOT_DEPTH);
-    if (d.y || d.z || d.w || d.x < 1 || d.x > 32) return -1;
+    if (d.y != (uint32_t)k.lane_bits || d.z || d.w || d.x < 1 || d.x > (uint32_t)k.max_depth) return -1;
     return (int)d.x;
 }
 
-int64_t key_n(const int32_t *key)
+/* slot 130 = 2^(depth + lane_bits) as a u64: a standard key of depth 32 has n = 2^32, and the other kinds
+ * (n <= 2^31) a zero high word */
+int64_t key_n(const int32_t *key, int kind)
 {
     const Seed v = key_slot(key, SLOT_N);
-    const int depth = key_depth(key);
+    const int depth = key_depth(key, kind);
     if (depth < 0 || v.z || v.w) return -1;
     const int64_t n = ((int64_t)v.y << 32) | v.x;
-    if (n != ((int64_t)1 << depth)) return -1;
+    if (n != ((int64_t)1 << (depth + kKinds[kind].lane_bits))) return -1;
     return n;
 }
 
-int key_et_depth(const int32_t *key)
+int key_kind(const int32_t *key)
 {
-    const Seed d = key_slot(key, SLOT_DEPTH);
-    if (d.y != (uint32_t)ET_LOG2_ROWS_PER_LEAF || d.z || d.w || d.x < 1 || d.x > ET_MAX_DEPTH) return -1;
-    return (int)d.x;
-}
-
-int64_t key_et_n(const int32_t *key)
-{
-    const Seed v = key_slot(key, SLOT_N);
-    const int depth = key_et_depth(key);
-    if (depth < 0 || v.y || v.z || v.w) return -1;
-    if ((int64_t)v.x != ((int64_t)1 << (depth + ET_LOG2_ROWS_PER_LEAF))) return -1;
-    return (int64_t)v.x;
-}
-
-int key_xor_depth(const int32_t *key)
-{
-    const Seed d = key_slot(key, SLOT_DEPTH);
-    if (d.y != (uint32_t)XOR_LOG2_ROWS_PER_LEAF || d.z || d.w || d.x < 1 || d.x > XOR_MAX_DEPTH) return -1;
-    return (int)d.x;
-}
-
-int64_t key_xor_n(const int32_t *key)
-{
-    const Seed v = key_slot(key, SLOT_N);
-    const int depth = key_xor_depth(key);
-    if (depth < 0 || v.y || v.z || v.w) return -1;
-    if ((int64_t)v.x != ((int64_t)1 << (depth + XOR_LOG2_ROWS_PER_LEAF))) return -1;
-    return (int64_t)v.x;
+    const uint32_t lane_bits = key_slot(key, SLOT_DEPTH).y;
+    for (int kind = 0; kind < KIND_COUNT; kind++)
+        if (lane_bits == (uint32_t)kKinds[kind].lane_bits) return key_n(key, kind) >= 0 ? kind : -1;
+    return -1;
 }
 
 namespace {
@@ -344,26 +323,27 @@ int gen_secure(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int
 
 namespace {
 
-/* A key whose leaves carry 2^LANE_BITS table rows each (early-terminated: 4, XOR-shared: 128): the log
- * construction over the 2^depth leaves for alpha >> LANE_BITS, level 0 in GROUP, payload beta(alpha). */
-template <int GROUP, int LANE_BITS, class Beta>
-int gen_leaves(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b, Beta beta)
+/* A key whose leaves carry 2^lane_bits table rows each (early-terminated: 4, XOR-shared: 128): the log
+ * construction over the 2^depth leaves for alpha >> lane_bits, level 0 in GROUP, payload beta. */
+template <int GROUP>
+int gen_leaves_in(const KindInfo &k, int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a,
+                  int32_t *key_b, u128 beta)
 {
-    if (n < ((int64_t)2 << LANE_BITS) || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0 || alpha < 0 || alpha >= n) return -1;
+    if (n < k.n_min || n > k.n_max || (n & (n - 1)) != 0 || alpha < 0 || alpha >= n) return -1;
     if (prf_id < PRF_DUMMY || prf_id > PRF_AES128) return -1;
     int depth = 0;
-    while (((int64_t)1 << (depth + LANE_BITS)) < n) depth++;
+    while (((int64_t)1 << (depth + k.lane_bits)) < n) depth++;
 
     ChaCha20Rng rng(seed, seed + 32);
-    KeyBuilder<ChaCha20Rng, GROUP> kb{depth, alpha >> LANE_BITS, prf_id, rng, {}, {}, 0, 0};
+    KeyBuilder<ChaCha20Rng, GROUP> kb{depth, alpha >> k.lane_bits, prf_id, rng, {}, {}, 0, 0};
     std::memset(kb.cw1, 0, sizeof kb.cw1);
     std::memset(kb.cw2, 0, sizeof kb.cw2);
-    kb.build(0, beta(alpha));
+    kb.build(0, beta);
 
     for (int srv = 0; srv < 2; srv++) {
         int32_t *key = srv ? key_b : key_a;
         std::memset(key, 0, sizeof(int32_t) * KEY_WORDS);
-        set_slot(key, SLOT_DEPTH, (u128)depth | ((u128)LANE_BITS << 32));
+        set_slot(key, SLOT_DEPTH, (u128)depth | ((u128)k.lane_bits << 32));
         for (int i = 0; i < 64; i++) {
             set_slot(key, SLOT_CW1 + i, kb.cw1[i]);
             set_slot(key, SLOT_CW2 + i, kb.cw2[i]);
@@ -376,18 +356,15 @@ int gen_leaves(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int
 
 }  // namespace
 
-int gen_et(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
+int gen_leaves(int kind, int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
 {
-    /* beta = unit vector of lane alpha & 3 */
-    return gen_leaves<GROUP_LANES32, ET_LOG2_ROWS_PER_LEAF>(alpha, n, seed, prf_id, key_a, key_b,
-                                                            [](int64_t a) { return (u128)1 << (32 * (a & 3)); });
-}
-
-int gen_xor(int64_t alpha, int64_t n, const uint8_t seed[44], int prf_id, int32_t *key_a, int32_t *key_b)
-{
-    /* beta = unit vector of bit alpha & 127 */
-    return gen_leaves<GROUP_XOR128, XOR_LOG2_ROWS_PER_LEAF>(alpha, n, seed, prf_id, key_a, key_b,
-                                                            [](int64_t a) { return (u128)1 << (a & 127); });
+    const KindInfo &k = kKinds[kind];
+    /* beta = unit vector of 32-bit lane alpha & 3, or of bit alpha & 127 */
+    if (kind == KIND_ET)
+        return gen_leaves_in<kKinds[KIND_ET].group>(k, alpha, n, seed, prf_id, key_a, key_b, (u128)1 << (32 * (alpha & 3)));
+    if (kind == KIND_XOR)
+        return gen_leaves_in<kKinds[KIND_XOR].group>(k, alpha, n, seed, prf_id, key_a, key_b, (u128)1 << (alpha & 127));
+    return -1;
 }
 
 namespace {
@@ -433,8 +410,8 @@ struct CpuEnv {
     }
 };
 
-template <int PRF, int GROUP = GROUP_ADD128>
-void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
+template <int PRF>
+void eval_cpu_impl(const int32_t *key, int group, int depth, int32_t *out)
 {
     CpuEnv env;
     env.ta.te0 = aes_te0();
@@ -447,51 +424,26 @@ void eval_cpu_impl(const int32_t *key, int depth, int32_t *out)
     for (uint32_t q = 0; q < nsub; q++) {
         env.base_pos = q << s;
         const Seed r = walk_down<PRF>(env, key_slot(key, SLOT_ROOT), depth - 1, depth - s, q);
-        eval_subtree<PRF, false, CpuEnv, GROUP>(env, r, s, 0);
+        if (group == GROUP_XOR128) eval_subtree<PRF, false, CpuEnv, GROUP_XOR128>(env, r, s, 0);
+        else if (group == GROUP_LANES32) eval_subtree<PRF, false, CpuEnv, GROUP_LANES32>(env, r, s, 0);
+        else eval_subtree<PRF, false, CpuEnv, GROUP_ADD128>(env, r, s, 0);
     }
 }
 
 }  // namespace
 
-int eval_cpu(const int32_t *key, int prf_id, int32_t *out_n)
+int eval_cpu(const int32_t *key, int kind, int prf_id, int32_t *out)
 {
-    const int depth = key_depth(key);
-    if (depth < 1 || depth > 31 || key_n(key) < 0) return -1;
+    const int depth = key_depth(key, kind);
+    /* a standard key of depth 32 has 2^32 rows, more than the output can hold */
+    if (depth < 1 || (kind == KIND_STANDARD && depth > 31) || key_n(key, kind) < 0) return -1;
+    const int group = kKinds[kind].group;
     switch (prf_id) {
-    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY>(key, depth, out_n); break;
-    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20>(key, depth, out_n); break;
-    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20>(key, depth, out_n); break;
-    case PRF_AES128: eval_cpu_impl<PRF_AES128>(key, depth, out_n); break;
-    default: return -1;
-    }
-    return 0;
-}
-
-int eval_cpu_et(const int32_t *key, int prf_id, int32_t *out_n)
-{
-    const int depth = key_et_depth(key);
-    if (depth < 1 || key_et_n(key) < 0) return -1;
-    switch (prf_id) {
-    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, GROUP_LANES32>(key, depth, out_n); break;
-    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, GROUP_LANES32>(key, depth, out_n); break;
-    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, GROUP_LANES32>(key, depth, out_n); break;
-    case PRF_AES128: eval_cpu_impl<PRF_AES128, GROUP_LANES32>(key, depth, out_n); break;
-    default: return -1;
-    }
-    return 0;
-}
-
-int eval_cpu_xor(const int32_t *key, int prf_id, uint32_t *bits)
-{
-    const int depth = key_xor_depth(key);
-    if (depth < 1 || key_xor_n(key) < 0) return -1;
-    int32_t *out = reinterpret_cast<int32_t *>(bits);
-    switch (prf_id) {
-    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY, GROUP_XOR128>(key, depth, out); break;
-    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20, GROUP_XOR128>(key, depth, out); break;
-    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20, GROUP_XOR128>(key, depth, out); break;
-    case PRF_AES128: eval_cpu_impl<PRF_AES128, GROUP_XOR128>(key, depth, out); break;
-    default: return -1;
+    case PRF_DUMMY: eval_cpu_impl<PRF_DUMMY>(key, group, depth, out); break;
+    case PRF_SALSA20: eval_cpu_impl<PRF_SALSA20>(key, group, depth, out); break;
+    case PRF_CHACHA20: eval_cpu_impl<PRF_CHACHA20>(key, group, depth, out); break;
+    case PRF_AES128: eval_cpu_impl<PRF_AES128>(key, group, depth, out); break;
+    default: return -2;
     }
     return 0;
 }

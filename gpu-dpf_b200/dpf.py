@@ -17,6 +17,7 @@ columns), and one process can own an entry-range shard of the table
 The module-level test_* / *_perf helpers mirror the reference's self-tests
 (dpf.py:139-356): same names and defaults, same pass criteria.
 """
+import collections
 import os
 import random
 import sys
@@ -35,6 +36,18 @@ except ImportError as exc:  # fail loudly: there is no Python/CPU stand-in for t
     raise ImportError(
         "dpf_cpp extension not built (run `python gpu-dpf_b200/build.py`); "
         "the DPF engine has no fallback implementation: %s" % exc)
+
+
+# What DPF does differently per kind of key (include/b200dpf.h): the dpf_cpp functions, whether explicit seeds
+# are ChaCha20-DRBG bytes only (at least 44 per key) or may also select the reference's 32-bit mt19937
+# generator, and the name in messages.  `gen` / `gen_batch` are the ChaCha20-DRBG generators.
+_Kind = collections.namedtuple("_Kind", "name drbg_only gen gen_batch eval_cpu eval_init pack")
+_STANDARD = _Kind("standard", False, dpf_cpp.gen_secure, dpf_cpp.gen_batch_secure, dpf_cpp.eval_cpu,
+                  dpf_cpp.eval_init_sharded, dpf_cpp.key_pack)
+_EARLY_TERMINATED = _Kind("early-terminated", True, dpf_cpp.gen_et, dpf_cpp.gen_batch_et, dpf_cpp.eval_cpu_et,
+                          dpf_cpp.eval_init_et, dpf_cpp.key_pack_et)
+_XOR_SHARED = _Kind("XOR-shared", True, dpf_cpp.gen_xor, dpf_cpp.gen_batch_xor, dpf_cpp.eval_cpu_xor,
+                    dpf_cpp.eval_init_xor, dpf_cpp.key_pack_xor)
 
 
 class DPF(object):
@@ -97,6 +110,7 @@ class DPF(object):
         if self.xor and self.devices:
             raise Exception("xor=True has no multi-device variant: use one device per DPF "
                             "(DPF(device=d, shard=(rank, count), xor=True))")
+        self.kind = _XOR_SHARED if self.xor else _EARLY_TERMINATED if self.early_termination else _STANDARD
 
     # ---- client -----------------------------------------------------------
     def gen(self, k, n, seed=None, secure=None):
@@ -108,8 +122,15 @@ class DPF(object):
         generator states of a key it holds and recover the index: that generator is kept only
         for callers that pass an explicit `seed` (deterministic keys, bit-identical to the
         reference's for the same seed: golden and parity tests) and do not ask for secure=True."""
-        if self.early_termination or self.xor:
-            return self._gen_et(k, n, seed, secure)
+        if self.kind.drbg_only:
+            # early-terminated and XOR-shared keys draw from the ChaCha20 DRBG only: explicit seeds are >= 44 bytes
+            if secure is False:
+                raise Exception("%s keys have no secure=False generator: pass >= 44 seed bytes or none" % self.kind.name)
+            if seed is None:
+                seed = os.urandom(44)
+            if not isinstance(seed, (bytes, bytearray)) or len(seed) < 44:
+                raise Exception("%s keys take a seed of at least 44 bytes" % self.kind.name)
+            seed, secure = bytes(seed), True
         if secure is None:
             secure = seed is None
         if seed is None:
@@ -119,51 +140,27 @@ class DPF(object):
         if k >= n:
             raise Exception("k (%d), the selected element, must be less than n (%d), the number of entries in the table"
                             % (k, n))
-        n = _next_pow2(n)
-        if secure:
-            return dpf_cpp.gen_secure(k, n, seed, self.prf_method)
-        return dpf_cpp.gen(k, n, seed, self.prf_method)
-
-    def _gen_et(self, k, n, seed, secure):
-        # early-terminated and XOR-shared keys draw from the ChaCha20 DRBG only: explicit seeds are >= 44 bytes
-        kind = "XOR-shared" if self.xor else "early-terminated"
-        if secure is False:
-            raise Exception("%s keys have no secure=False generator: pass >= 44 seed bytes or none" % kind)
-        if seed is None:
-            seed = os.urandom(44)
-        if not isinstance(seed, (bytes, bytearray)) or len(seed) < 44:
-            raise Exception("%s keys take a seed of at least 44 bytes" % kind)
-        if n & (n - 1) != 0 and not self.allow_non_pow2:
-            raise Exception("Table num entries (%d) must be a power of two" % (n))
-        if k >= n:
-            raise Exception("k (%d), the selected element, must be less than n (%d), the number of entries in the table"
-                            % (k, n))
-        gen = dpf_cpp.gen_xor if self.xor else dpf_cpp.gen_et
-        return gen(k, _next_pow2(n), bytes(seed), self.prf_method)
+        return (self.kind.gen if secure else dpf_cpp.gen)(k, _next_pow2(n), seed, self.prf_method)
 
     def gen_batch(self, indices, n, seeds=None, nthreads=0):
         """Keys for many indices at once: two int32 [B, 524] tensors (multi-threaded keygen).
         seeds=None: ChaCha20-DRBG keys from os.urandom entropy (44 bytes per key); explicit integer
         seeds select the reference's 32-bit mt19937 generator (deterministic, for tests).  With
         early_termination or xor, explicit seeds are bytes: 44 per key, concatenated."""
-        if self.early_termination or self.xor:
-            if n & (n - 1) != 0:
-                raise Exception("Table num entries (%d) must be a power of two" % (n))
-            idx = torch.as_tensor(list(indices), dtype=torch.int64)
-            if seeds is None:
-                seeds = os.urandom(44 * idx.numel())
-            if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * idx.numel():
-                raise Exception("%s gen_batch takes seeds as bytes, 44 per key" % ("XOR-shared" if self.xor else "early-terminated"))
-            gen_batch = dpf_cpp.gen_batch_xor if self.xor else dpf_cpp.gen_batch_et
-            return gen_batch(idx, n, bytes(seeds), self.prf_method, nthreads)
         if n & (n - 1) != 0:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
         idx = torch.as_tensor(list(indices), dtype=torch.int64)
+        if self.kind.drbg_only:
+            if seeds is None:
+                seeds = os.urandom(44 * idx.numel())
+            if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * idx.numel():
+                raise Exception("%s gen_batch takes seeds as bytes, 44 per key" % self.kind.name)
+            return self.kind.gen_batch(idx, n, bytes(seeds), self.prf_method, nthreads)
         if idx.numel() and int(idx.max()) >= n:
             raise Exception("k (%d), the selected element, must be less than n (%d), the number of entries in the table"
                             % (int(idx.max()), n))
         if seeds is None:
-            return dpf_cpp.gen_batch_secure(idx, n, os.urandom(44 * idx.numel()), self.prf_method, nthreads)
+            return self.kind.gen_batch(idx, n, os.urandom(44 * idx.numel()), self.prf_method, nthreads)
         return dpf_cpp.gen_batch(idx, n, torch.as_tensor(seeds, dtype=torch.int64), self.prf_method, nthreads)
 
     # ---- server -----------------------------------------------------------
@@ -172,7 +169,7 @@ class DPF(object):
         or the XOR of the rows whose share bit is set."""
         if self.xor:
             return self._eval_cpu_xor(keys, one_hot_only)
-        eval_one = dpf_cpp.eval_cpu_et if self.early_termination else dpf_cpp.eval_cpu
+        eval_one = self.kind.eval_cpu
         if one_hot_only:
             return torch.stack([eval_one(k, self.prf_method) for k in keys])
         if self.table is None:
@@ -183,7 +180,7 @@ class DPF(object):
     def _eval_cpu_xor(self, keys, one_hot_only):
         shifts = torch.arange(32, dtype=torch.int32)
         # packed words [B, n/32] -> bits [B, n]: row i is bit (i & 31) of word i >> 5
-        bits = torch.stack([(dpf_cpp.eval_cpu_xor(k, self.prf_method).view(-1, 1) >> shifts) & 1 for k in keys])
+        bits = torch.stack([(self.kind.eval_cpu(k, self.prf_method).view(-1, 1) >> shifts) & 1 for k in keys])
         bits = bits.reshape(len(keys), -1)
         if one_hot_only:
             return bits
@@ -217,14 +214,10 @@ class DPF(object):
         self.table = table
         self.table_num_entries = table.shape[0]
         self.table_effective_entry_size = table.shape[1]
-        if self.xor:
-            self.buffers = dpf_cpp.eval_init_xor(table, self.device, self.shard[0], self.shard[1])
-        elif self.early_termination:
-            self.buffers = dpf_cpp.eval_init_et(table, self.device, self.shard[0], self.shard[1])
-        elif self.devices:
+        if self.devices:      # standard keys only: __init__ refuses the other kinds with devices
             self.buffers = dpf_cpp.eval_init_multi(table, self.devices, {"auto": 0, "entries": 1, "keys": 2}[self.axis])
         else:
-            self.buffers = dpf_cpp.eval_init_sharded(table, self.device, self.shard[0], self.shard[1])
+            self.buffers = self.kind.eval_init(table, self.device, self.shard[0], self.shard[1])
 
     def update_rows(self, indices, rows):
         """Replace rows of the uploaded table in place: table[indices[j]] := rows[j] for natural indices (the
@@ -282,8 +275,7 @@ class DPF(object):
     def pack_keys(self, keys):
         """Compact wire form of a batch (24% to 56% smaller than int32[524] keys, depending on n): one
         contiguous uint8 tensor [B, 32 + 64*depth], pinned when CUDA is available, for eval_gpu_compact."""
-        pack = dpf_cpp.key_pack_xor if self.xor else dpf_cpp.key_pack_et if self.early_termination else dpf_cpp.key_pack
-        blobs = [pack(k) for k in keys]
+        blobs = [self.kind.pack(k) for k in keys]
         t = torch.frombuffer(bytearray(b"".join(blobs)), dtype=torch.uint8).reshape(len(blobs), -1)
         return t.pin_memory() if torch.cuda.is_available() else t
 

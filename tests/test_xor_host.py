@@ -89,7 +89,7 @@ def test_keygen_every_depth(logn, orc):
         assert list(k[:4]) == [d, 7, 0, 0]
         assert int(np.uint32(k[520])) == n and not k[521:524].any()
         assert not k[4 + 4 * 2 * d:4 * 65].any()              # cw_1 beyond level d-1 is zero
-        assert B._xor_key_n(k) == n
+        assert B._key_n(k, "_xor") == n
     leaf = alpha >> 7
     va, vb = xor_oracle.leaf_value(orc, a, leaf, prf), xor_oracle.leaf_value(orc, b, leaf, prf)
     assert va ^ vb == 1 << (alpha & 127)
@@ -163,6 +163,29 @@ def test_refusals_between_key_kinds():
         B.eval_cpu_xor(std, B.PRF_AES128)
     with pytest.raises(B.B200DPFError):
         B.eval_cpu_et(xk, B.PRF_AES128)
+
+
+@pytest.mark.parametrize("key_kind", ["", "_et", "_xor"])
+@pytest.mark.parametrize("entry_kind", ["", "_et", "_xor"])
+def test_each_entry_point_takes_exactly_its_kind(key_kind, entry_kind):
+    """eval_cpu*, key_pack* and key_unpack* accept keys of their own kind and refuse every other kind with
+    EINVAL; b200dpf_key_n / _key_depth see only standard keys."""
+    L = B.lib()
+    n = 1 << 10
+    key = dict(zip(("", "_et", "_xor"), _keys_of_every_kind(n)))[key_kind]
+    packed = getattr(B, "key_pack" + key_kind)(key)
+    want = 0 if key_kind == entry_kind else EINVAL
+    out = np.zeros(n // 32, np.uint32) if entry_kind == "_xor" else np.zeros(n, np.int32)
+    assert getattr(L, "b200dpf_eval_cpu" + entry_kind)(key, B.PRF_AES128, out) == want
+    buf = C.create_string_buffer(L.b200dpf_key_packed_size(32))
+    assert getattr(L, "b200dpf_key_pack" + entry_kind)(key, buf, len(buf), None) == want
+    unpacked = np.zeros(524, np.int32)
+    assert getattr(L, "b200dpf_key_unpack" + entry_kind)(packed, len(packed), unpacked) == want
+    if want == 0:
+        assert np.array_equal(unpacked, key)
+    depth = 10 - B.KINDS[key_kind][0]
+    assert L.b200dpf_key_n(key) == (n if key_kind == "" else -1)
+    assert L.b200dpf_key_depth(key) == (depth if key_kind == "" else -1)
 
 
 def test_argument_checks():
