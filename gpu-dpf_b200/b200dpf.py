@@ -28,7 +28,7 @@ SYMBOLS = [
     "b200dpf_gen_et", "b200dpf_gen_batch_et", "b200dpf_eval_cpu_et", "b200dpf_key_pack_et", "b200dpf_key_unpack_et",
     "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf", "b200dpf_group_create_et",
     "b200dpf_gen_xor", "b200dpf_gen_batch_xor", "b200dpf_eval_cpu_xor", "b200dpf_key_pack_xor", "b200dpf_key_unpack_xor",
-    "b200dpf_create_xor",
+    "b200dpf_create_xor", "b200dpf_group_create_xor",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -99,7 +99,8 @@ def load():
     L.b200dpf_ctx_last_launches.argtypes = [C.c_void_p]
     L.b200dpf_ctx_set_subtree_log2.argtypes = [C.c_void_p, C.c_int]
     L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
-    L.b200dpf_group_create_et.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
+    for kind in ("_et", "_xor"):
+        getattr(L, "b200dpf_group_create" + kind).argtypes = L.b200dpf_group_create.argtypes
     return L
 
 
@@ -410,9 +411,13 @@ class Context:
 class GroupContext(Context):
     """Many tables ("bins") of one entry size behind one context: the batch-PIR front end
     (b200dpf_group_create / b200dpf_group_eval).  early_termination=True makes the context for
-    early-terminated keys (b200dpf_group_create_et): bins of >= 8 rows, four rows per tree leaf."""
+    early-terminated keys (b200dpf_group_create_et): bins of >= 8 rows, four rows per tree leaf.  xor=True
+    makes it for XOR-shared keys (b200dpf_group_create_xor): bins of >= 256 rows, 128 rows per tree leaf,
+    and results that XOR (not add) to the selected row."""
 
-    def __init__(self, tables, device=0, early_termination=False):
+    def __init__(self, tables, device=0, early_termination=False, xor=False):
+        if xor and early_termination:
+            raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
         self.tables = [np.ascontiguousarray(t, np.int32) for t in tables]
         assert all(t.ndim == 2 and t.shape[1] == self.tables[0].shape[1] for t in self.tables)
         self.entry_size = self.tables[0].shape[1]
@@ -420,7 +425,7 @@ class GroupContext(Context):
         sizes = np.array([t.shape[0] for t in self.tables], np.int64)
         ptrs = (C.c_void_p * len(self.tables))(*[t.ctypes.data for t in self.tables])
         self.handle = C.c_void_p()
-        name = "b200dpf_group_create_et" if early_termination else "b200dpf_group_create"
+        name = "b200dpf_group_create" + ("_xor" if xor else "_et" if early_termination else "")
         _check(getattr(lib(), name)(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size, device), name)
 
     @property

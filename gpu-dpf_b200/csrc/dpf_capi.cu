@@ -125,6 +125,8 @@ struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behi
     std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
     DeviceBuffer<GroupDesc> d_descs;   /* both hold at least 1,024 descriptors */
     PinnedBuffer<GroupDesc> h_descs;
+    DeviceBuffer<WorkUnit> d_units;    /* modes that draw work units: the list; both hold at least 1,024 */
+    PinnedBuffer<WorkUnit> h_units;
     std::vector<int64_t> perm;         /* sorted position -> caller's index, of the last evaluation */
     DeviceBuffer<uint2> d_bin_info;    /* [nbins] (row_off, depth) for row updates, uploaded on first use */
 };
@@ -391,7 +393,7 @@ inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char
  * format): the kernel modes, and the limits of one kind. */
 struct KindOps {
     int mode_fused, mode_expand;
-    int mode_grouped;       /* -1: no grouped contexts */
+    int mode_grouped;
     int max_nv;             /* fused passes: at most 4 * max_nv columns (early-terminated 32, XOR-shared 16) */
     bool leaf_cache;        /* wide entries may cache leaves (XOR-shared: a further 16 columns re-walk the tree) */
     bool tma_rows;          /* the B200DPF_TMA_ROWS variant exists */
@@ -403,7 +405,7 @@ struct KindOps {
 constexpr KindOps kKindOps[host::KIND_COUNT] = {
     {MODE_FUSED, MODE_EXPAND, MODE_GROUPED, 16, true, true, 0, 0, "b200dpf_gen"},
     {MODE_FUSED_ET, MODE_EXPAND_ET, MODE_GROUPED_ET, 8, true, false, 0, 0, "b200dpf_gen_et"},
-    {MODE_FUSED_XOR, MODE_EXPAND_XOR, -1, 4, false, false, 2, 4, "b200dpf_gen_xor"},
+    {MODE_FUSED_XOR, MODE_EXPAND_XOR, MODE_GROUPED_XOR, 4, false, false, 2, 4, "b200dpf_gen_xor"},
 };
 
 /* "a standard", "an early-terminated", "an XOR-shared": the article of a kind's name */
@@ -1766,7 +1768,7 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
 /* ------------------------------------------------------------------------------------------- */
 /* Grouped evaluation: the batch-PIR front end (SURVEY.md section 8(f) rank 4).                  */
 /* ------------------------------------------------------------------------------------------- */
-/* b200dpf_group_create and b200dpf_group_create_et: a grouped context for keys of `kind`.  n and the row
+/* b200dpf_group_create, _et and _xor: a grouped context for keys of `kind`.  n and the row
  * offsets count rows, the depths (per bin and the context's deepest) leaves. */
 static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
                              int device, int kind)
@@ -1840,6 +1842,12 @@ int b200dpf_group_create_et(b200dpf_ctx **out, const int32_t *const *tables, con
     return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_ET);
 }
 
+int b200dpf_group_create_xor(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                             int device)
+{
+    return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_XOR);
+}
+
 int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
 {
     if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
@@ -1887,23 +1895,27 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         for (auto &th : pool) th.join();
     }
     /* key groups and their work-item size: big items amortise the root-to-subtree walk every item
-     * pays (there is no frontier: bins are small), small items keep every warp busy */
+     * pays (there is no frontier: bins are small), small items keep every warp busy.  Leaves of many
+     * rows (KindOps::leaf_items) take items down to s = 1, as on a plain context. */
     SmemLayout L;
     rc = smem_layout(c, prf, 4, mode, &L);
     if (rc) return rc;
     const int64_t warps = (int64_t)L.grid * (L.threads / 32);
     int64_t ngroups = 0;
     for (int g = 0; g < nbins; g++) ngroups += (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32;
+    const KindOps &ops = kKindOps[c->kind];
     int s_target = c->knobs.subtree_log2 > 0 ? c->knobs.subtree_log2 : 6;
     s_target = std::min(s_target, L.s_max);
     if (c->knobs.subtree_log2 <= 0) {
-        for (; s_target > 3; s_target--) {
+        const int s_floor = ops.leaf_items ? 1 : 3;
+        const int64_t items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
+        for (; s_target > s_floor; s_target--) {
             int64_t items = 0;
             for (int g = 0; g < nbins; g++) {
                 const int64_t kg = (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32;
                 items += kg << std::max(0, B->depth[(size_t)g] - s_target);
             }
-            if (items >= 2 * warps) break;
+            if (items >= items_wanted) break;
         }
     }
     const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
@@ -1929,17 +1941,47 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             }
         }
     }
+    /* modes that draw work units: every key group's items, in group-major order, cut evenly into units of
+     * at most one item per warp of a block.  A unit's items run side by side, so a launch takes about
+     * (units per block) unit times: whole-block units unless the launch holds fewer items than the grid
+     * has warps, and then about items / blocks per unit, so that every block has work.  A key group with
+     * fewer items than its unit size leaves the rest of its unit's warps idle. */
+    const bool units = mode_traits(mode).units;
+    int64_t nunits = 0;
+    if (units) {
+        int64_t items = 0;
+        for (int64_t gi = 0; gi < ngroups; gi++) items += B->h_descs.ptr[gi].nsub;
+        const int64_t per_unit = std::clamp<int64_t>((items + L.grid - 1) / L.grid, 1, L.threads / 32);
+        for (int64_t gi = 0; gi < ngroups; gi++) nunits += (B->h_descs.ptr[gi].nsub + per_unit - 1) / per_unit;
+        const size_t units_bytes = std::max<size_t>((size_t)nunits, 1024) * sizeof(WorkUnit);
+        rc = B->h_units.reserve(units_bytes);
+        if (!rc) rc = B->d_units.reserve(units_bytes);
+        if (rc) return rc;
+        WorkUnit *w = B->h_units.ptr;
+        for (int64_t gi = 0; gi < ngroups; gi++) {
+            const uint64_t nsub = B->h_descs.ptr[gi].nsub;
+            const uint64_t parts = (nsub + (uint64_t)per_unit - 1) / (uint64_t)per_unit;
+            for (uint64_t j = 0; j < parts; j++) {
+                const uint64_t first = nsub * j / parts, end = nsub * (j + 1) / parts;
+                *w++ = WorkUnit{(uint32_t)gi, (uint32_t)first, (uint32_t)(end - first), 0u};
+            }
+        }
+    }
     const int passes = c->entry_pad / 16;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
     rc = reserve_device_io(c, key_bytes, out_elems);
     if (!rc) rc = reserve_host_out(c, out_elems);
     if (rc) return rc;
-    const size_t n_counters = (size_t)passes * (size_t)ngroups;
+    /* per pass: one ticket counter per key group, or the one unit counter */
+    const size_t pass_counters = units ? 1u : (size_t)ngroups;
+    const size_t n_counters = (size_t)passes * pass_counters;
     rc = c->d_counters.reserve(n_counters * sizeof(uint32_t));
     if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, B->h_descs.ptr, (size_t)ngroups * sizeof(GroupDesc), cudaMemcpyHostToDevice, c->stream));
+    if (units)
+        CUDA_TRY(cudaMemcpyAsync(B->d_units.ptr, B->h_units.ptr, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, c->stream));
     if (c->coop_state_dirty) {
         CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), c->stream));
         c->bar_epoch = 0;
@@ -1952,6 +1994,8 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     p.keys = reinterpret_cast<const uint4 *>(c->d_keys.ptr);
     p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
     p.groups = B->d_descs.ptr;
+    p.units = B->d_units.ptr;
+    p.nunits = (uint32_t)nunits;
     fill_phase(L, s_max, &p.main);
     p.main.counters = c->d_counters.ptr;
     p.out = reinterpret_cast<uint32_t *>(c->d_out.ptr);
@@ -1968,7 +2012,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         p.col_off = (uint32_t)(pass * 16);
         p.ncols = (uint32_t)std::max(0, std::min(16, c->entry_size - pass * 16));
         if (p.ncols == 0) break;
-        p.main.counters = c->d_counters.ptr + (size_t)pass * (size_t)ngroups;
+        p.main.counters = c->d_counters.ptr + (size_t)pass * pass_counters;
         if (p.fuse_top) {
             p.grid_bar = c->d_gridbar.ptr;
             c->bar_epoch += (uint32_t)L.grid;

@@ -229,11 +229,12 @@ std::vector<void *> eval_init_multi(const at::Tensor &table, const std::vector<i
     return {static_cast<void *>(ctx)};
 }
 
-/* batch PIR: many tables ("bins") of one entry size behind one context (b200dpf_group_create, or
- * b200dpf_group_create_et for early-terminated keys) */
-std::vector<void *> group_init_kind(const std::vector<at::Tensor> &tables, int device, bool et)
+/* batch PIR: many tables ("bins") of one entry size behind one context, for keys of one kind
+ * (b200dpf_group_create, _et or _xor, named `what` in messages) */
+std::vector<void *> group_init_with(const std::vector<at::Tensor> &tables, int device,
+                                    int (*create)(b200dpf_ctx **, const int32_t *const *, const int64_t *, int, int, int),
+                                    const char *what)
 {
-    const char *what = et ? "group_init_et" : "group_init";
     TORCH_CHECK(!tables.empty(), what, ": no tables");
     std::vector<at::Tensor> keep;
     std::vector<const int32_t *> ptrs;
@@ -245,14 +246,24 @@ std::vector<void *> group_init_kind(const std::vector<at::Tensor> &tables, int d
         sizes.push_back(keep.back().size(0));
     }
     b200dpf_ctx *ctx = nullptr;
-    auto create = et ? b200dpf_group_create_et : b200dpf_group_create;
     check(create(&ctx, ptrs.data(), sizes.data(), (int)ptrs.size(), (int)tables[0].size(1), device), what);
     return {static_cast<void *>(ctx)};
 }
 
-std::vector<void *> group_init(const std::vector<at::Tensor> &tables, int device) { return group_init_kind(tables, device, false); }
+std::vector<void *> group_init(const std::vector<at::Tensor> &tables, int device)
+{
+    return group_init_with(tables, device, b200dpf_group_create, "group_init");
+}
 
-std::vector<void *> group_init_et(const std::vector<at::Tensor> &tables, int device) { return group_init_kind(tables, device, true); }
+std::vector<void *> group_init_et(const std::vector<at::Tensor> &tables, int device)
+{
+    return group_init_with(tables, device, b200dpf_group_create_et, "group_init_et");
+}
+
+std::vector<void *> group_init_xor(const std::vector<at::Tensor> &tables, int device)
+{
+    return group_init_with(tables, device, b200dpf_group_create_xor, "group_init_xor");
+}
 
 /* keys int32 [B,524], bins int32/int64 [B] -> int32 [B, E]: key b evaluated on table bins[b] */
 at::Tensor group_eval(const at::Tensor &keys, const at::Tensor &bins, const std::vector<void *> &buffers, int prf)
@@ -518,6 +529,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("group_init", &group_init, "batch PIR: one context over many tables (bins)", py::arg("tables"), py::arg("device") = 0);
     m.def("group_init_et", &group_init_et, "batch PIR for early-terminated keys (four rows per leaf)", py::arg("tables"),
           py::arg("device") = 0);
+    m.def("group_init_xor", &group_init_xor, "batch PIR for XOR-shared keys (128 rows per leaf, XOR results)",
+          py::arg("tables"), py::arg("device") = 0);
     m.def("group_eval", &group_eval, "batch PIR: evaluate (bin, key) pairs in one launch");
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),
           py::arg("devices"), py::arg("axis") = 0);

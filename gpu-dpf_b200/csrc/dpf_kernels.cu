@@ -428,6 +428,35 @@ __device__ __forceinline__ unsigned long long global_ns()
     return t;
 }
 
+/* The correction words of the kpw keys of a key group -> shared, [level][bank][bit][key], and their root
+ * seeds; keys past `key_last` load key_last's words */
+template <int THREADS>
+__device__ __forceinline__ void load_key_group(const EvalParams &p, int depth, int key_first, int key_last, int kpw,
+                                               uint4 *cw_s, uint32_t *cwlo_s, uint4 *root_s)
+{
+    const int tid = threadIdx.x;
+    const int per_key = depth * 4;
+    for (int i = tid; i < per_key * kpw; i += THREADS) {
+        const int k = i / per_key;            /* key within the group   */
+        const int e = i - k * per_key;        /* (bank, level, bit)     */
+        const int bank = e / (depth * 2);
+        const int lb = e - bank * (depth * 2);     /* 2*level + bit       */
+        int key = key_first + k;
+        if (key > key_last) key = key_last;
+        const int level = lb >> 1, bit = lb & 1;
+        const uint32_t slot = p.key_compact ? 2u + 4u * (uint32_t)level + 2u * (uint32_t)bank + (uint32_t)bit
+                                            : (bank ? 65u : 1u) + (uint32_t)lb;
+        const uint4 v = __ldg(p.keys + (size_t)key * p.key_stride_v + slot);
+        cw_s[((level * 2 + bank) * 2 + bit) * 32 + k] = v;
+        if (level == 0) cwlo_s[(bank * 2 + bit) * 32 + k] = v.x;
+    }
+    if (tid < kpw) {
+        int key = key_first + tid;
+        if (key > key_last) key = key_last;
+        root_s[tid] = __ldg(p.keys + (size_t)key * p.key_stride_v + p.key_root_v);
+    }
+}
+
 /* `quota`: tickets this WARP may draw in this call over all key groups (0xffffffff = no limit). */
 template <int PRF, int NV, int THREADS, int MODE>
 __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams &ph,
@@ -497,29 +526,7 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
         if (tid == 0) *flag_s = (*reinterpret_cast<volatile uint32_t *>(ph.counters + kg) < g_tickets) ? 1 : 0;
         __syncthreads();
         const bool has_work = (*flag_s != 0);
-        if (has_work) {
-            /* correction words of this key group -> shared, [level][bank][bit][key] */
-            const int per_key = g_depth * 4;
-            for (int i = tid; i < per_key * kpw; i += THREADS) {
-                const int k = i / per_key;            /* key within the group   */
-                const int e = i - k * per_key;        /* (bank, level, bit)     */
-                const int bank = e / (g_depth * 2);
-                const int lb = e - bank * (g_depth * 2);   /* 2*level + bit       */
-                int key = g_key_first + k;
-                if (key > g_key_last) key = g_key_last;
-                const int level = lb >> 1, bit = lb & 1;
-                const uint32_t slot = p.key_compact ? 2u + 4u * (uint32_t)level + 2u * (uint32_t)bank + (uint32_t)bit
-                                                    : (bank ? 65u : 1u) + (uint32_t)lb;
-                const uint4 v = __ldg(p.keys + (size_t)key * p.key_stride_v + slot);
-                cw_s[((level * 2 + bank) * 2 + bit) * 32 + k] = v;
-                if (level == 0) cwlo_s[(bank * 2 + bit) * 32 + k] = v.x;
-            }
-            if (tid < kpw) {
-                int key = g_key_first + tid;
-                if (key > g_key_last) key = g_key_last;
-                root_s[tid] = __ldg(p.keys + (size_t)key * p.key_stride_v + p.key_root_v);
-            }
-        }
+        if (has_work) load_key_group<THREADS>(p, g_depth, g_key_first, g_key_last, kpw, cw_s, cwlo_s, root_s);
         __syncthreads();
         if (!has_work) continue;
 
@@ -637,6 +644,86 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
     }
 }
 
+/* The main phase of a mode that draws work units (ModeTraits::units: grouped, one key group = 32 keys of one
+ * bin, column split).  run_phase makes every block visit every key group -- a counter read and two barriers
+ * each, about 3.7 us per group (DESIGN.md section 9) -- which would be most of the time of XOR-shared keys.
+ * Here thread 0 draws the block's next unit of the host's list; the block loads correction words and roots
+ * only when the unit's key group is not the one already in shared memory, and its warps split the unit's
+ * items.  Each unit ends with the flush of the accumulators: XOR is associative, so a flush per unit is
+ * exact.  A block reads nothing of a key group it draws no unit of. */
+template <int PRF, int NV, int THREADS, int MODE>
+__device__ __forceinline__ void run_units(const EvalParams &p, const PhaseParams &ph, const typename TablePolicy<PRF>::type &ta)
+{
+    constexpr ModeTraits M = mode_traits(MODE);
+    static_assert(M.grouped && M.feeds == FEEDS_MAC && M.row_load == ROWS_COLSPLIT && M.result == RESULT_XOR,
+                  "work units: grouped column-split XOR evaluation only");
+    constexpr uint32_t NW = THREADS / 32;
+    const int tid = threadIdx.x;
+    const int lane = tid & 31;
+    const uint32_t warp = (uint32_t)tid >> 5;
+
+    uint4 *cw_s = reinterpret_cast<uint4 *>(g_dyn_smem + p.off_cw);
+    uint32_t *cwlo_s = reinterpret_cast<uint32_t *>(g_dyn_smem + p.off_cwlo);
+    uint4 *root_s = reinterpret_cast<uint4 *>(g_dyn_smem + p.off_root);
+    volatile uint32_t *draw_s = reinterpret_cast<volatile uint32_t *>(g_dyn_smem + p.off_flag);   /* 2 slots */
+
+    DevEnv<PRF, NV, THREADS, MODE> env;   /* lane = key: 32 keys per warp, one subtree slot */
+    env.ta = ta;
+    env.cw_lane = cw_s + lane;
+    env.cwlo_lane = cwlo_s + lane;
+    env.kpw = 32;
+    env.stack_lo = reinterpret_cast<uint4 *>(g_dyn_smem + p.off_stack_lo) + tid;
+    env.stack_hi = reinterpret_cast<uint4 *>(g_dyn_smem + p.off_stack_hi) + tid - ph.stack_split * THREADS;
+    env.stack_split = ph.stack_split;
+    env.row_stride_v = p.row_stride_v;
+    env.depth = p.depth;
+    env.leaf_out = nullptr;
+    env.key_valid = true;
+
+    uint32_t loaded = 0xffffffffu;        /* the key group in shared memory (block-uniform) */
+    for (uint32_t i = 0;; i++) {
+        /* the two slots take turns: slot i & 1 is written again at draw i + 2, and every thread has read it
+         * before it passes the barrier of draw i + 1 */
+        if (tid == 0) draw_s[i & 1] = atomicAdd(ph.counters, 1u);
+        __syncthreads();                  /* also: every warp is done with the previous unit */
+        const uint32_t u = draw_s[i & 1];
+        if (u >= p.nunits) break;
+        const WorkUnit unit = p.units[u];
+        const GroupDesc g = p.groups[unit.group];
+        const int key_first = (int)g.key_first, key_last = (int)(g.key_first + g.nkeys) - 1;
+        if (unit.group != loaded) {
+            load_key_group<THREADS>(p, g.depth, key_first, key_last, 32, cw_s, cwlo_s, root_s);
+            __syncthreads();
+            loaded = unit.group;
+        }
+        if (warp >= unit.count) continue;
+
+        const uint4 rv = root_s[lane];
+        const Seed root = make_seed(rv.x, rv.y, rv.z, rv.w);
+#pragma unroll
+        for (int e = 0; e < 4 * NV; e++) env.acc[e] = 0;
+        const uint4 *table = p.table + g.table_off_v + p.col_off_v + (lane & 3);
+        for (uint32_t q = unit.first + warp; q < unit.first + unit.count; q += NW) {
+            const Seed r = walk_down<PRF>(env, root, g.depth - 1, g.depth - g.s, q);
+            env.rows = table + ((size_t)q << (g.s + M.row_shift)) * p.row_stride_v;
+            env.pos_base = q << g.s;
+            eval_subtree<PRF, false, decltype(env), mode_leaf_group(MODE)>(env, r, g.s, 0);
+        }
+        /* acc[4 j + c] is column 4 (lane & 3) + c of key lane ^ j (DevEnv::leaf_bits) */
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int kj = key_first + (lane ^ j);
+            if (kj > key_last) continue;
+            uint32_t *o = p.out + (size_t)kj * p.out_stride + p.col_off;
+#pragma unroll
+            for (int c = 0; c < 4; c++) {
+                const uint32_t e = 4u * (uint32_t)(lane & 3) + (uint32_t)c;
+                if (e < p.ncols) atomicXor(o + e, env.acc[4 * j + c]);
+            }
+        }
+    }
+}
+
 template <int PRF, int NV, int MODE>
 __global__ void __launch_bounds__(eval_block_shape(PRF, NV, MODE).threads, eval_block_shape(PRF, NV, MODE).min_blocks)
 dpf_eval_kernel(const __grid_constant__ EvalParams p)
@@ -694,7 +781,8 @@ dpf_eval_kernel(const __grid_constant__ EvalParams p)
                 for (uint32_t i = tid; i < p.rearm_words; i += THREADS) p.rearm[i] = 0u;
         }
     }
-    run_phase<PRF, NV, THREADS, MODE>(p, p.main, ta);
+    if constexpr (mode_traits(MODE).units) run_units<PRF, NV, THREADS, MODE>(p, p.main, ta);
+    else run_phase<PRF, NV, THREADS, MODE>(p, p.main, ta);
     if (stamp) stamp[4] = global_ns();
 }
 
@@ -980,7 +1068,7 @@ EvalKernel eval_kernel()
 
 /* The instantiated kernels of one PRF.  Every mode runs at 16 columns per pass (nv = 4); the fused
  * modes of standard and early-terminated keys also at 32, the standard one at 64 as well.  Grouped
- * evaluation (both kinds of key) and XOR-shared keys take 16 columns per pass, and the modes that never
+ * evaluation (every kind of key) and XOR-shared keys take 16 columns per pass, and the modes that never
  * touch the table need no other width. */
 template <int PRF>
 EvalKernel eval_kernel_of(int nv, int mode)
@@ -996,6 +1084,7 @@ EvalKernel eval_kernel_of(int nv, int mode)
         case MODE_GROUPED_ET: return eval_kernel<PRF, 4, MODE_GROUPED_ET>();
         case MODE_FUSED_XOR: return eval_kernel<PRF, 4, MODE_FUSED_XOR>();
         case MODE_EXPAND_XOR: return eval_kernel<PRF, 4, MODE_EXPAND_XOR>();
+        case MODE_GROUPED_XOR: return eval_kernel<PRF, 4, MODE_GROUPED_XOR>();
         case MODE_FUSED_TMA:       /* AES: no shared memory left beside the tables */
             if constexpr (PRF != PRF_AES128) return eval_kernel<PRF, 4, MODE_FUSED_TMA>();
             break;

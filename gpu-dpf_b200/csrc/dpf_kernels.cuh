@@ -36,11 +36,17 @@ struct PhaseParams {
 struct GroupDesc {
     uint32_t key_first;       /* first key of the group in the (bin-sorted) key array       */
     uint32_t nkeys;           /* 1..32                                                      */
-    int32_t depth;            /* log2 of the bin's table size (MODE_GROUPED_ET: of its leaves) */
+    int32_t depth;            /* log2 of the bin's table size (MODE_GROUPED_ET, _XOR: of its leaves) */
     int32_t s;                /* log2 leaves per work item for this group                   */
     uint32_t nsub;            /* work items (2^s-leaf subtrees) = 2^(depth - s)             */
     uint32_t pad;
     uint64_t table_off_v;     /* bin's first row, in uint4 units from EvalParams::table     */
+};
+
+/* What a block of a mode that draws work units (ModeTraits::units) takes in one draw: work items
+ * [first, first + count) of key group `group`.  The host lists them in group-major order. */
+struct WorkUnit {
+    uint32_t group, first, count, pad;
 };
 
 /* Parameters of one evaluation launch (one pass over <= 16*NVMAX columns). */
@@ -64,7 +70,7 @@ struct EvalParams {
     uint32_t col_off;         /* first int32 column of this pass                        */
     uint32_t ncols;           /* valid int32 columns in this pass (<= 4*NV)             */
     int depth;                /* log2 n                                                 */
-    const GroupDesc *groups;  /* MODE_GROUPED(_ET): [key_groups] descriptors (else null)  */
+    const GroupDesc *groups;  /* grouped modes: [key_groups] descriptors (else null)    */
     PhaseParams main;         /* the phase that produces the result (or, in the stand-alone
                                  frontier kernel, the frontier)                          */
     /* single-launch pipeline: the launch first clears its own accumulators and ticket
@@ -108,13 +114,16 @@ struct EvalParams {
     uint32_t off_tile;        /* MODE_FUSED_TMA: per warp, one work item's rows (64 << s bytes),
                                  then one 8-byte mbarrier per warp at off_tile_bar        */
     uint32_t off_tile_bar;
+    /* modes that draw work units: the list, drawn through main.counters[0] (one counter per pass) */
+    const WorkUnit *units;
+    uint32_t nunits;
 };
 
 /* Kernel modes: the MODE of dpf_eval_kernel<PRF, NV, MODE>.  Each is a combination of the properties
  * of ModeTraits, and mode_traits below is the one place that says which. */
 enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3, MODE_FUSED_TMA = 4,
        MODE_FUSED_ET = 5, MODE_EXPAND_ET = 6, MODE_FUSED_COLSPLIT = 7, MODE_GROUPED_ET = 8,
-       MODE_FUSED_XOR = 9, MODE_EXPAND_XOR = 10, MODE_COUNT = 11 };
+       MODE_FUSED_XOR = 9, MODE_EXPAND_XOR = 10, MODE_GROUPED_XOR = 11, MODE_COUNT = 12 };
 
 /* The group a mode's result lives in (ModeTraits::result). */
 enum { RESULT_ADD,        /* Z/2^32: out[key][col] = sum of share * row, red.global.add */
@@ -146,23 +155,27 @@ struct ModeTraits {
     /* batch PIR: each key group evaluates its own bin, described by EvalParams::groups */
     bool grouped;
     int result;               /* RESULT_*: also the level-0 group, XOR for RESULT_XOR */
+    /* the main phase draws work units (EvalParams::units, one per block and draw) instead of walking
+     * every key group's tickets: a block touches only the key groups it draws units of */
+    bool units;
 };
 
 __host__ __device__ constexpr ModeTraits mode_traits(int mode)
 {
-    switch (mode) {                            /* feeds           row_load        row_shift grouped result */
-    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false, RESULT_ADD};
-    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false, RESULT_ADD};
-    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false, RESULT_ADD};
-    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD};
-    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false, RESULT_ADD};
-    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false, RESULT_ADD};
-    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false, RESULT_ADD};
-    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false, RESULT_ADD};
-    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD};
-    case MODE_FUSED_XOR:      return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, false, RESULT_XOR};
-    case MODE_EXPAND_XOR:     return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 7, false, RESULT_XOR};
-    default:                  return ModeTraits{-1, -1, 0, false, RESULT_ADD};
+    switch (mode) {                            /* feeds           row_load        row_shift grouped result   units */
+    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false, RESULT_ADD, false};
+    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false, RESULT_ADD, false};
+    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false, RESULT_ADD, false};
+    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD, false};
+    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false, RESULT_ADD, false};
+    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false, RESULT_ADD, false};
+    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false, RESULT_ADD, false};
+    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false, RESULT_ADD, false};
+    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD, false};
+    case MODE_FUSED_XOR:      return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, false, RESULT_XOR, false};
+    case MODE_EXPAND_XOR:     return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 7, false, RESULT_XOR, false};
+    case MODE_GROUPED_XOR:    return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, true,  RESULT_XOR, true};
+    default:                  return ModeTraits{-1, -1, 0, false, RESULT_ADD, false};
     }
 }
 

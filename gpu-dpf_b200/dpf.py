@@ -404,7 +404,8 @@ class BinnedDPF(DPF):
             raise Exception("BinnedDPF has no early-terminated variant (early_termination=True): use "
                             "dpf_cpp.group_init_et or b200dpf.GroupContext(early_termination=True)")
         if kwargs.get("xor"):
-            raise Exception("BinnedDPF has no XOR-shared variant (xor=True): use one dpf.DPF(xor=True) per bin")
+            raise Exception("BinnedDPF has no XOR-shared variant (xor=True): use "
+                            "dpf_cpp.group_init_xor or b200dpf.GroupContext(xor=True)")
         super().__init__(*args, **kwargs)
 
     def eval_init(self, tables):

@@ -209,12 +209,20 @@ int b200dpf_ctx_axis(const b200dpf_ctx *ctx);
  * b200dpf_group_eval takes only keys of b200dpf_gen_et for n[bins[b]] rows (a standard key is EINVAL
  * before anything is copied), out[b][e] is what b200dpf_eval on b200dpf_create_et(table bins[b]) gives,
  * b200dpf_group_update_rows works as on a standard grouped context and b200dpf_ctx_rows_per_leaf is 4.
- * A standard grouped context refuses early-terminated keys (EINVAL).
+ * b200dpf_group_create_xor makes it for XOR-shared keys (b200dpf_gen_xor, see below): every n[g] a
+ * power of two in [256, 2^31], each bin laid out as by b200dpf_create_xor.  There b200dpf_group_eval
+ * takes only keys of b200dpf_gen_xor for n[bins[b]] rows (any other key is EINVAL before anything is
+ * copied), out[b][e] is what b200dpf_eval on b200dpf_create_xor(table bins[b]) gives -- an XOR, so
+ * out_a[b] ^ out_b[b] == table bins[b][alpha] --, b200dpf_group_update_rows works as on the other grouped
+ * contexts and b200dpf_ctx_rows_per_leaf is 128.  Each grouped context refuses keys of the other two
+ * kinds (EINVAL).
  */
 int b200dpf_group_create(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
                          int entry_size, int device);
 int b200dpf_group_create_et(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
                             int entry_size, int device);
+int b200dpf_group_create_xor(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
+                             int entry_size, int device);
 int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf,
                        int32_t *out);
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
@@ -427,7 +435,7 @@ int b200dpf_create_et(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int en
                       int device, int shard_rank, int shard_count);
 
 /* Table rows per tree leaf: 4 on a context of b200dpf_create_et or b200dpf_group_create_et, 128 on one of
- * b200dpf_create_xor, 1 otherwise; -1 for null. */
+ * b200dpf_create_xor or b200dpf_group_create_xor, 1 otherwise; -1 for null. */
 int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *ctx);
 
 /* ------------------------------------------------------------------------------------------- */
@@ -480,8 +488,9 @@ int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key);
  *   b200dpf_expand_device writes the packed share bits, shares_dev = uint32[nkeys][n / 32] as
  *   b200dpf_eval_cpu_xor.
  * Entries are evaluated 16 columns per pass; wider entries take one pass (one tree walk) per 16 columns,
- * so the "leaf_cache", "leaf_cache_mb", "mac_tma" and "tma_rows" options have no effect here.  There is
- * no multi-device, grouped or GPU-keygen variant.
+ * so the "leaf_cache", "leaf_cache_mb", "mac_tma" and "tma_rows" options have no effect here.  The
+ * grouped (batch-PIR) variant is b200dpf_group_create_xor; there is no multi-device or GPU-keygen
+ * variant.
  */
 int b200dpf_create_xor(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
                        int device, int shard_rank, int shard_count);

@@ -36,4 +36,15 @@ ga = grp.eval(np.stack([k[0] for k in ks]), bins, 2)
 gb = grp.eval(np.stack([k[1] for k in ks]), bins, 2)
 assert np.array_equal((ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32), np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
 grp.close()
+# grouped XOR-shared launch: blocks draw work units and reload a key group's words between units
+tables = [rng.randint(-2**31, 2**31, size=(m, 20), dtype=np.int64).astype(np.int32) for m in (256, 4096, 1024)]
+grp = b200dpf.GroupContext(tables, xor=True)
+bins = np.array([0, 1, 2, 1, 1, 2, 1] * 7, np.int32)
+alphas = np.array([rng.randint(0, tables[g].shape[0]) for g in bins], np.int64)
+for prf in range(4):
+    ka, kb = zip(*[b200dpf.gen_xor(int(al), tables[g].shape[0], bytes(range(i, i + 44)), prf)
+                   for i, (al, g) in enumerate(zip(alphas, bins))])
+    ga, gb = grp.eval(np.stack(ka), bins, prf), grp.eval(np.stack(kb), bins, prf)
+    assert np.array_equal(ga ^ gb, np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
+grp.close()
 print("sanitize run ok")
