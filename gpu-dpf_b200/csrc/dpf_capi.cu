@@ -161,24 +161,12 @@ struct b200dpf_ctx {
     int sm_count = 0;
     uint32_t smem_base = 0;
     int last_launches = 0;
-    /* tuning knobs: defaults from the environment, read ONCE at b200dpf_create; changed per
-     * context with b200dpf_ctx_set_option */
+    /* tuning knobs, described by kKnobs: defaults from the environment, read ONCE at b200dpf_create;
+     * changed per context with b200dpf_ctx_set_option */
     struct Knobs {
-        int leaf_cache = 1;        /* B200DPF_LEAF_CACHE     wide entries: cache leaves, MAC-only passes  */
-        int leaf_cache_mb = 16384; /* B200DPF_LEAF_CACHE_MB  cap; larger batches are evaluated in chunks   */
-        int lane_split = 1;        /* B200DPF_LANE_SPLIT     batches < 32 keys: lane = (key, subtree)      */
-        int frontier = 1;          /* B200DPF_FRONTIER       expand the tree top once per evaluation       */
-        int frontier_mb = 256;     /* B200DPF_FRONTIER_MB                                                  */
-        int subtree_log2 = 0;      /* B200DPF_S              0 = automatic                                  */
-        int mac_tma = 1;           /* B200DPF_MAC_TMA        cp.async.bulk-staged MAC passes               */
-        int one_launch = 1;        /* B200DPF_ONE_LAUNCH     whole evaluation as one cooperative launch    */
-        int balance_top = 1;       /* B200DPF_BALANCE_TOP    even per-block shares of the tree-top phase    */
-        int timing = 0;            /* B200DPF_TIMING         per-block phase time stamps (diagnostics)      */
-        int top_log2 = 0;          /* B200DPF_TOP_LOG2       log2 leaves-of-the-frontier per tree-top item (0 = estimate) */
-        int tma_rows = 0;          /* B200DPF_TMA_ROWS       fused kernel: stage each item's rows with cp.async.bulk
-                                                             (16-column tables, Salsa/ChaCha/dummy); on an H100 at n=2^20
-                                                             +4 % for Salsa20, -2 % for ChaCha20 against broadcast
-                                                             loads, other sizes unmeasured -- so off */
+        int leaf_cache, leaf_cache_mb, lane_split, frontier, frontier_mb, subtree_log2, mac_tma, one_launch,
+            balance_top, timing, top_log2, tma_rows;
+        Knobs();   /* the defaults of kKnobs */
     } knobs;
     DeviceBuffer<unsigned long long> d_timing;   /* [blocks][8] */
     int coop_ok = 0;               /* device supports cooperative launches                                 */
@@ -219,6 +207,34 @@ struct SmemLayoutCache {
     SmemLayout entry[4][3][MODE_COUNT];
     bool valid[4][3][MODE_COUNT] = {};
 };
+
+namespace {
+
+/* One tuning option: its field, default, environment variable (read by b200dpf_create and the other
+ * plain-context constructors; unchecked, as atoi reads it) and b200dpf_ctx_set_option name and range. */
+using Kn = b200dpf_ctx::Knobs;
+using KnobField = int Kn::*;
+struct KnobInfo { KnobField field; int dflt; const char *env, *name; int lo, hi; };
+constexpr KnobInfo kKnobs[] = {
+    {&Kn::leaf_cache, 1, "B200DPF_LEAF_CACHE", "leaf_cache", 0, 1},                /* wide entries: cache leaves, MAC-only passes */
+    {&Kn::leaf_cache_mb, 16384, "B200DPF_LEAF_CACHE_MB", "leaf_cache_mb", 1, 1 << 20},  /* cap; larger batches go in chunks */
+    {&Kn::lane_split, 1, "B200DPF_LANE_SPLIT", "lane_split", 0, 1},                /* batches < 32 keys: lane = (key, subtree) */
+    {&Kn::frontier, 1, "B200DPF_FRONTIER", "frontier", 0, 1},                      /* expand the tree top once per evaluation */
+    {&Kn::frontier_mb, 256, "B200DPF_FRONTIER_MB", "frontier_mb", 1, 1 << 16},
+    {&Kn::subtree_log2, 0, "B200DPF_S", "subtree_log2", 0, 16},                    /* 0 = automatic */
+    {&Kn::mac_tma, 1, "B200DPF_MAC_TMA", "mac_tma", 0, 1},                         /* cp.async.bulk-staged MAC passes */
+    {&Kn::one_launch, 1, "B200DPF_ONE_LAUNCH", "one_launch", 0, 1},                /* whole evaluation as one cooperative launch */
+    {&Kn::balance_top, 1, "B200DPF_BALANCE_TOP", "balance_top", 0, 1},             /* even per-block shares of the tree-top phase */
+    {&Kn::timing, 0, "B200DPF_TIMING", "timing", 0, 1},                            /* per-block phase time stamps (diagnostics) */
+    {&Kn::top_log2, 0, "B200DPF_TOP_LOG2", "top_log2", 0, 7},   /* log2 leaves-of-the-frontier per tree-top item (0 = estimate) */
+    /* fused kernel: stage each item's rows with cp.async.bulk (16-column tables, Salsa/ChaCha/dummy); on an H100 at
+     * n=2^20 +4 % for Salsa20, -2 % for ChaCha20 against broadcast loads, other sizes unmeasured -- so off */
+    {&Kn::tma_rows, 0, "B200DPF_TMA_ROWS", "tma_rows", 0, 1},
+};
+
+}  // namespace
+
+b200dpf_ctx::Knobs::Knobs() { for (const KnobInfo &k : kKnobs) this->*k.field = k.dflt; }
 
 namespace {
 
@@ -301,27 +317,10 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
     return B200DPF_OK;
 }
 
-/* s = the deepest pending-sibling stack any phase of the launch needs */
-void fill_common(const b200dpf_ctx *c, const SmemLayout &L, int s, int64_t nkeys, int kpw_log2, EvalParams *p,
-                 size_t *smem)
+/* Dynamic shared memory of a launch on layout L whose deepest pending-sibling stack is s levels */
+size_t smem_bytes(const SmemLayout &L, int s)
 {
-    std::memset(p, 0, sizeof *p);
-    p->depth = c->depth;
-    p->nkeys = (int)nkeys;
-    p->kpw_log2 = kpw_log2;
-    p->key_groups = (int)((nkeys + (1 << kpw_log2) - 1) >> kpw_log2);
-    p->table = reinterpret_cast<const uint4 *>(c->d_table.ptr);
-    p->row_stride_v = (uint32_t)c->entry_pad / 4u;
-    p->out_stride = (uint32_t)c->entry_size;
-    p->n = (uint64_t)c->n;
-    p->off_cw = L.off_meta;
-    p->off_cwlo = L.off_small;
-    p->off_root = p->off_cwlo + 512u;
-    p->off_flag = p->off_root + 512u;
-    p->off_stack_lo = L.off_lo;
-    p->off_stack_hi = L.off_hi;
-    p->off_tab = L.off_tab;
-    *smem = L.smem_fixed ? L.smem_fixed : (size_t)L.off_lo + (size_t)(s > 1 ? s - 1 : 0) * L.level_bytes;
+    return L.smem_fixed ? L.smem_fixed : (size_t)L.off_lo + (size_t)(s > 1 ? s - 1 : 0) * L.level_bytes;
 }
 
 int env_int(const char *name, int dflt)
@@ -447,46 +446,121 @@ void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
     ph->stack_split = std::min(L.cap_lo, std::max(s - 1, 0));
 }
 
-/*
- * One evaluation of <= one leaf-cache-full of keys:
- *   one launch  : [clear result + tickets, build frontier | grid barrier | main]  (+ MAC passes)
- *   legacy      : memset tickets, memset result, frontier kernel, main kernel x passes
- * mode_main is MODE_FUSED (out = [nkeys][entry_size] int32) or MODE_EXPAND
- * (out = [nkeys][n] int32 share vectors).
- */
-constexpr int kRetryWithoutCooperativeLaunch = -1000;   /* internal to run_pipeline */
+/* What one run of the launcher evaluates, and where; its EvalPlan says how. */
+struct EvalJob {
+    const void *keys;
+    KeyLayout kl;
+    int64_t nkeys;
+    int prf, mode_main;       /* mode_main: MODE_FUSED (out = [nkeys][entry_size] int32) or MODE_EXPAND (out = [nkeys][n] shares) */
+    void *out;
+    cudaStream_t stream;
+    bool clear_out;           /* false: accumulate into out (b200dpf_eval_device_acc) */
+    bool leaf_cache;          /* plain contexts, wide entries: cache the leaves, MAC-only passes for the other columns */
+    /* grouped contexts: the key groups' descriptors and work units; `timed`: ev_t0 / ev_t1 bracket the launches */
+    const GroupDesc *groups; const WorkUnit *units; uint32_t nunits;
+    bool timed;
+};
 
-int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int64_t nkeys, int prf, int mode_main,
-                       void *out_dev, cudaStream_t stream, bool clear_out, bool want_cache)
+/*
+ * How one evaluation (or one leaf-cache chunk of it) runs.  plan_eval (plain contexts) and plan_group_eval
+ * (grouped ones) decide all of it from the context's shape, its knobs and the kernels' shared-memory
+ * layouts, before anything is allocated or enqueued; launch_plan carries it out:
+ *   one launch : [clear result + tickets, build frontier | grid barrier | main]  (+ passes, MAC passes)
+ *   otherwise  : memset tickets, memset result, frontier kernel, main kernel x passes (+ MAC passes)
+ */
+struct EvalPlan {
+    int mode, nv, passes;     /* main-phase kernel (MODE_*, uint4 columns per pass) and its passes over the columns */
+    int kpw_log2;             /* log2 keys per warp */
+    int64_t key_groups;
+    int s;                    /* log2 leaves per main-phase work item (grouped: the largest of any key group) */
+    int s_group;              /* grouped: a key group's s is this, within [1, its bin's depth] (group_s) */
+    int f_rel, s_top;         /* frontier depth below the shard root, log2 leaves per tree-top item (0 = no frontier) */
+    bool one_launch;          /* cooperative launches that clear their own accumulators before a grid barrier */
+    bool grouped;             /* key groups of GroupDesc; no tree-top phase */
+    bool leaf_cache, timing;  /* timing: per-block phase time stamps */
+    bool tma_rows;            /* MODE_FUSED_TMA: each warp stages its item's rows in a tile after the stack */
+    size_t tile_bytes;        /* all warps' tiles, then their mbarriers at off_tile_bar */
+    uint32_t off_tile, off_tile_bar;
+    SmemLayout L, LF;         /* main phase; tree-top phase (the stand-alone frontier kernel's unless one_launch) */
+    size_t smem, smem_top;    /* dynamic shared memory of the main launches and of the frontier kernel */
+    size_t pass_counters, top_counters;        /* main-phase tickets per pass; tree-top tickets (0: none) */
+    size_t frontier_bytes, leaf_cache_bytes;
+    PhaseParams main, top;    /* without their counters and frontier */
+    uint32_t nfront, top_block_quota;          /* nfront: frontier nodes per key (this shard) */
+    /* MAC-only passes: the cp.async.bulk variant or the register-staged one, its grid, position ranges per key group */
+    bool mac_tma; int mac_grid; uint32_t mac_ranges;
+};
+
+/* Work-item size: from s down to s_floor, the first s at which the launch has at least `wanted` items */
+template <class Items> int shrink_s(int s, int s_floor, int64_t wanted, Items items)
+{
+    while (s > s_floor && items(s) < wanted) s--;
+    return s;
+}
+
+/* The work-item size of a key group of a bin of `depth` levels on a grouped context */
+int group_s(const EvalPlan &P, int depth) { return std::max(1, std::min(depth, P.s_group)); }
+
+/* The fields of EvalParams that every launch of job J on layout L shares; the others are zero. */
+void fill_common(const b200dpf_ctx *c, const SmemLayout &L, const EvalJob &J, const EvalPlan &P, EvalParams *p)
+{
+    std::memset(p, 0, sizeof *p);
+    p->keys = reinterpret_cast<const uint4 *>(J.keys);
+    p->key_stride_v = J.kl.stride_v; p->key_root_v = J.kl.root_v; p->key_compact = J.kl.compact;
+    p->depth = c->depth;
+    p->nkeys = (int)J.nkeys; p->kpw_log2 = P.kpw_log2; p->key_groups = (int)P.key_groups;
+    p->groups = J.groups; p->units = J.units; p->nunits = J.nunits;
+    p->table = reinterpret_cast<const uint4 *>(c->d_table.ptr);
+    p->row_stride_v = (uint32_t)c->entry_pad / 4u;
+    p->out_stride = (uint32_t)c->entry_size;
+    p->n = (uint64_t)c->n;
+    p->off_cw = L.off_meta;
+    p->off_cwlo = L.off_small;
+    p->off_root = p->off_cwlo + 512u;
+    p->off_flag = p->off_root + 512u;
+    p->off_stack_lo = L.off_lo;
+    p->off_stack_hi = L.off_hi;
+    p->off_tab = L.off_tab;
+}
+
+/* The plan of job J on a plain context. */
+int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
 {
     const b200dpf_ctx::Knobs &K = c->knobs;
+    const KindOps &ops = kKindOps[c->kind];
+    const int prf = J.prf;
+    const int64_t nkeys = J.nkeys;
+    const bool fused = J.mode_main == MODE_FUSED;
+    EvalPlan &P = *out = EvalPlan{};
+    int &kpw_log2 = P.kpw_log2, &s = P.s, &f_rel = P.f_rel, &s_top = P.s_top;   /* the names the arithmetic below uses */
+    int64_t &key_groups = P.key_groups;
+    SmemLayout &L = P.L;
+    P.leaf_cache = J.leaf_cache;
     /* Entries wider than 32 columns: the tree is expanded ONCE by the best-shaped kernel (16
      * columns, NV = 4), which also caches each leaf's low word; every other column is produced by
      * MAC-only passes over that cache.  Without the cache (disabled or lane-split batches) wide
      * entries use one tree expansion per 64 columns. */
-    const KindOps &ops = kKindOps[c->kind];
-    const int nv = (mode_main != MODE_FUSED || c->entry_pad <= 16 || want_cache) ? 4 : std::min(ops.max_nv, c->entry_pad <= 32 ? 8 : 16);
-    const int passes = mode_main == MODE_FUSED ? (want_cache ? 1 : c->entry_pad / (4 * nv)) : 1;
+    P.nv = (!fused || c->entry_pad <= 16 || P.leaf_cache) ? 4 : std::min(ops.max_nv, c->entry_pad <= 32 ? 8 : 16);
+    P.passes = fused ? (P.leaf_cache ? 1 : c->entry_pad / (4 * P.nv)) : 1;
     /* optional variant: the rows of each work item staged into shared memory by cp.async.bulk */
-    bool tma_rows = K.tma_rows != 0 && K.one_launch != 0 && c->coop_ok != 0 && mode_main == MODE_FUSED && c->entry_pad == 16 &&
-                    prf != B200DPF_PRF_AES128 && nkeys >= 17 && ops.tma_rows;
-    const int mode_plain = mode_main == MODE_FUSED ? ops.mode_fused : ops.mode_expand;
-    int mode_kernel = tma_rows ? MODE_FUSED_TMA : mode_plain;
+    P.tma_rows = K.tma_rows != 0 && K.one_launch != 0 && c->coop_ok != 0 && fused && c->entry_pad == 16 &&
+                 prf != B200DPF_PRF_AES128 && nkeys >= 17 && ops.tma_rows;
+    const int mode_plain = fused ? ops.mode_fused : ops.mode_expand;
+    P.mode = P.tma_rows ? MODE_FUSED_TMA : mode_plain;
     /* keys per warp: a full warp of keys when the batch allows; for small batches the
      * spare lanes take adjacent subtrees of the same keys (single-query latency mode) */
-    int kpw_log2 = 5;
+    kpw_log2 = 5;
     if (K.lane_split != 0)
         while (kpw_log2 > 0 && ((int64_t)1 << (kpw_log2 - 1)) >= nkeys) kpw_log2--;
-    if (mode_main == MODE_FUSED) kpw_log2 = std::max(kpw_log2, ops.min_kpw_log2);
-    int64_t key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
+    if (fused) kpw_log2 = std::max(kpw_log2, ops.min_kpw_log2);
+    key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
     /* AES binds the shared-memory data pipe, and a broadcast row load is charged for every lane's copy
      * of the row: with at least 4 keys per warp, each lane of a key quad loads a quarter of the row and
      * the quad trades leaf values by SHFL instead (DESIGN.md section 3).  Decided before the layout: the
      * kernel runs more threads, so its stack holds fewer levels (s_max).  kpw_log2 only grows below. */
-    if (mode_kernel == MODE_FUSED && prf == B200DPF_PRF_AES128 && nv == 4 && kpw_log2 >= 2)
-        mode_kernel = MODE_FUSED_COLSPLIT;
-    SmemLayout L;
-    int rc = smem_layout(c, prf, nv, mode_kernel, &L);
+    if (P.mode == MODE_FUSED && prf == B200DPF_PRF_AES128 && P.nv == 4 && kpw_log2 >= 2)
+        P.mode = MODE_FUSED_COLSPLIT;
+    int rc = smem_layout(c, prf, P.nv, P.mode, &L);
     if (rc) return rc;
     const int64_t warps = (int64_t)L.grid * (L.threads / 32);
 
@@ -495,7 +569,6 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
      * must be big; with one the walk is (almost) free and small items balance the
      * tail. */
     const bool want_frontier = K.frontier != 0;
-    int s;
     if (K.subtree_log2 > 0) {
         s = std::min(K.subtree_log2, std::min(c->depth_local, L.s_max));
     } else {
@@ -512,23 +585,21 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
          *   n=2^20: auto 0.971; s=1 0.989, 2 0.980, 3 0.971, 4 0.975, 5 0.975, 6 0.973 */
         const int s_floor = ops.leaf_items ? 1 : want_frontier ? 3 : 5;
         const int64_t items_per_warp = ops.leaf_items ? ops.leaf_items : want_frontier ? 24 : 6;
-        s = std::min(c->depth_local, std::min(L.s_max, s_cap));
-        while (s > s_floor &&
-               ((((int64_t)1 << (c->depth_local - s)) * key_groups) >> (5 - kpw_log2)) < items_per_warp * warps)
-            s--;
+        s = shrink_s(std::min(c->depth_local, std::min(L.s_max, s_cap)), s_floor, items_per_warp * warps, [&](int t) {
+            return (((int64_t)1 << (c->depth_local - t)) * key_groups) >> (5 - kpw_log2);
+        });
     }
     if (s < 1) s = 1;
-    size_t tile_bytes = 0;
-    if (tma_rows) {
+    if (P.tma_rows) {
         /* one tile of 2^s 64-byte rows per warp, after the sibling stack */
         const int warps_blk = L.threads / 32;
         if (K.subtree_log2 <= 0) s = std::min(s, 6);
-        tile_bytes = (size_t)warps_blk * ((size_t)64 << s) + 8u * (size_t)warps_blk + 16u;
-        if ((size_t)L.off_lo + (size_t)(std::max(s, 7) - 1) * L.level_bytes + tile_bytes > (size_t)L.budget) {
-            tma_rows = false;               /* does not fit beside correction words and stack: broadcast loads */
-            mode_kernel = mode_plain;
-            tile_bytes = 0;
-            rc = smem_layout(c, prf, nv, mode_kernel, &L);
+        P.tile_bytes = (size_t)warps_blk * ((size_t)64 << s) + 8u * (size_t)warps_blk + 16u;
+        if ((size_t)L.off_lo + (size_t)(std::max(s, 7) - 1) * L.level_bytes + P.tile_bytes > (size_t)L.budget) {
+            P.tma_rows = false;             /* does not fit beside correction words and stack: broadcast loads */
+            P.mode = mode_plain;
+            P.tile_bytes = 0;
+            rc = smem_layout(c, prf, P.nv, P.mode, &L);
             if (rc) return rc;
         }
     }
@@ -538,9 +609,8 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
     }
     const int spw_log2 = 5 - kpw_log2;
-    if (want_cache && kpw_log2 != 5) return fail(B200DPF_ESTATE, "internal: leaf cache planned for a lane-split batch");
+    if (P.leaf_cache && kpw_log2 != 5) return fail(B200DPF_ESTATE, "internal: leaf cache planned for a lane-split batch");
 
-    int f_rel = 0;                                /* frontier depth below the shard root (0 = none) */
     if (want_frontier && rel >= 2) {
         const int64_t cap_bytes = (int64_t)K.frontier_mb << 20;
         f_rel = rel;
@@ -548,54 +618,20 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
         if (f_rel < 2 || f_rel < spw_log2 + 1) f_rel = 0;
     }
 
-    const bool one_launch = K.one_launch != 0 && c->coop_ok != 0;
-    const size_t n_main_counters = (size_t)passes * (size_t)key_groups;
-    rc = c->d_counters.reserve(n_main_counters * sizeof(uint32_t));
-    if (rc) return rc;
-    {
-        bool grown = false;
-        rc = c->d_top_counters.reserve(std::max<size_t>((size_t)key_groups, 64) * sizeof(uint32_t), &grown);
-        if (rc) return rc;
-        if (grown) c->coop_state_dirty = true;
-    }
-    if (f_rel > 0) {
-        rc = c->d_frontier.reserve(((size_t)key_groups * (16 << kpw_log2)) << f_rel);
-        if (rc) return rc;
-    }
-
-    rc = wait_last(c, stream);
-    if (rc) return rc;
-
-    if (!one_launch || c->coop_state_dirty) {
-        CUDA_TRY(cudaMemsetAsync(c->d_top_counters.ptr, 0, c->d_top_counters.cap, stream));
-        CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), stream));
-        c->bar_epoch = 0;
-        c->coop_state_dirty = false;
-    }
-    if (!one_launch) {
-        CUDA_TRY(cudaMemsetAsync(c->d_counters.ptr, 0, n_main_counters * sizeof(uint32_t), stream));
-        if (mode_main == MODE_FUSED && clear_out)
-            CUDA_TRY(cudaMemsetAsync(out_dev, 0, (size_t)nkeys * c->entry_size * sizeof(int32_t), stream));
-        c->coop_state_dirty = true;     /* the stand-alone frontier kernel leaves its tickets used */
-    }
-    c->last_launches = 0;
+    P.one_launch = K.one_launch != 0 && c->coop_ok != 0;
+    P.pass_counters = (size_t)key_groups;
+    P.top_counters = std::max<size_t>((size_t)key_groups, 64);
+    if (f_rel > 0) P.frontier_bytes = ((size_t)key_groups * (16 << kpw_log2)) << f_rel;
 
     /* ---- the tree-top phase (frontier build) ---- */
-    EvalParams p;
-    size_t smem;
-    PhaseParams top;
-    std::memset(&top, 0, sizeof top);
-    int s_top = 0;
+    P.LF = L;
     if (f_rel > 0) {
-        SmemLayout LF = L;
-        if (!one_launch) {
-            rc = smem_layout(c, prf, 4, MODE_FRONTIER, &LF);
-            if (rc) return rc;
-        }
+        if (!P.one_launch && (rc = smem_layout(c, prf, 4, MODE_FRONTIER, &P.LF))) return rc;
+        const SmemLayout &LF = P.LF;
         s_top = std::max(1, std::min(f_rel - spw_log2, std::min(5, LF.s_max)));
         if (K.top_log2 > 0) {
             s_top = std::max(1, std::min(K.top_log2, std::min(f_rel - spw_log2, LF.s_max)));
-        } else if (one_launch && K.balance_top) {
+        } else if (P.one_launch && K.balance_top) {
             /* Size of a tree-top item.  The blocks that start at a key group share its 2^(f_rel - s_top)
              * items; an item is (walk to its subtree root) + 2^s_top - 1 node pairs, all sequential.
              * Estimate the phase as rounds x steps x step time, where a step costs the larger of the
@@ -621,198 +657,255 @@ int run_pipeline_chunk(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl
                 }
             }
         }
-        fill_phase(LF, s_top, &top);
-        top.nsub = (uint32_t)1 << (f_rel - s_top);
-        top.sub_first = (uint32_t)c->shard_rank << (f_rel - s_top);
-        top.walk_first_level = c->depth - 1;
-        top.walk_steps = c->shard_bits + f_rel - s_top;
-        top.level_base = c->depth_local - f_rel;
-        top.counters = c->d_top_counters.ptr;
-        if (!one_launch) {
-            fill_common(c, LF, s_top, nkeys, kpw_log2, &p, &smem);
-            p.keys = reinterpret_cast<const uint4 *>(keys_dev);
-            p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
-            p.main = top;
-            p.nfront = (uint32_t)1 << f_rel;
-            p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier.ptr);
-            CUDA_TRY(launch_eval(prf, 4, MODE_FRONTIER, p, LF.grid, smem, stream));
-            c->last_launches++;
-        }
+        fill_phase(LF, s_top, &P.top);
+        P.top.nsub = (uint32_t)1 << (f_rel - s_top);
+        P.top.sub_first = (uint32_t)c->shard_rank << (f_rel - s_top);
+        P.top.walk_first_level = c->depth - 1;
+        P.top.walk_steps = c->shard_bits + f_rel - s_top;
+        P.top.level_base = c->depth_local - f_rel;
+        P.smem_top = smem_bytes(LF, s_top);
+        P.nfront = (uint32_t)1 << f_rel;
     }
 
     /* ---- the main phase ---- */
-    fill_common(c, L, std::max(s, s_top), nkeys, kpw_log2, &p, &smem);
-    p.keys = reinterpret_cast<const uint4 *>(keys_dev);
-    p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
-    if (tma_rows) {
-        p.off_tile = (uint32_t)((smem + 15) & ~(size_t)15);
-        p.off_tile_bar = p.off_tile + (uint32_t)((size_t)(L.threads / 32) * ((size_t)64 << s));
-        smem = (size_t)p.off_tile + tile_bytes;
+    P.smem = smem_bytes(L, std::max(s, s_top));
+    if (P.tma_rows) {
+        P.off_tile = (uint32_t)((P.smem + 15) & ~(size_t)15);
+        P.off_tile_bar = P.off_tile + (uint32_t)((size_t)(L.threads / 32) * ((size_t)64 << s));
+        P.smem = (size_t)P.off_tile + P.tile_bytes;
     }
-    fill_phase(L, s, &p.main);
-    p.main.nsub = (uint32_t)1 << rel;
-    p.main.sub_first = (uint32_t)c->shard_rank << rel;
+    fill_phase(L, s, &P.main);
+    P.main.nsub = (uint32_t)1 << rel;
+    P.main.sub_first = (uint32_t)c->shard_rank << rel;
     if (f_rel > 0) {
-        p.main.frontier_in = reinterpret_cast<const uint4 *>(c->d_frontier.ptr);
-        p.nfront = (uint32_t)1 << f_rel;
-        p.main.front_shift = rel - f_rel;
-        p.main.walk_first_level = c->depth_local - f_rel - 1;
-        p.main.walk_steps = rel - f_rel;
+        P.main.front_shift = rel - f_rel;
+        P.main.walk_first_level = c->depth_local - f_rel - 1;
+        P.main.walk_steps = rel - f_rel;
     } else {
-        p.main.walk_first_level = c->depth - 1;
-        p.main.walk_steps = c->depth - s;
+        P.main.walk_first_level = c->depth - 1;
+        P.main.walk_steps = c->depth - s;
     }
+    if (P.one_launch) {
+        const uint64_t items = (uint64_t)key_groups * (uint64_t)(P.top.nsub >> spw_log2);
+        P.top_block_quota = K.balance_top ? (uint32_t)std::max<uint64_t>(1, (items + (uint64_t)L.grid - 1) / (uint64_t)L.grid)
+                                          : 0x7fffffffu;
+        P.timing = K.timing != 0;
+    }
+
+    /* ---- wide entries: the leaf-caching pass, then the MAC-only passes ---- */
+    if (P.leaf_cache) {
+        P.mode = ops.mode_fused;                   /* the kind's fused kernel, on the layout planned above */
+        P.leaf_cache_bytes = (size_t)key_groups * 32u * (size_t)c->n_local * sizeof(uint32_t);
+        P.mac_tma = K.mac_tma != 0;
+        /* register-staged variant: 8 warps per block */
+        const int64_t mac_warps = (int64_t)c->sm_count * 2 * 8;
+        const int64_t ranges = std::max<int64_t>(1, (2 * mac_warps + key_groups - 1) / key_groups);
+        /* TMA variant: one block per SM; a block takes 8 key groups x one position range */
+        const int64_t kg_blocks = (key_groups + 7) / 8;
+        const int64_t tr = std::max<int64_t>(1, (2 * (int64_t)c->sm_count + kg_blocks - 1) / kg_blocks);
+        P.mac_grid = P.mac_tma ? c->sm_count : c->sm_count * 2;
+        P.mac_ranges = (uint32_t)(P.mac_tma ? std::min<int64_t>(tr, std::max<int64_t>(1, c->n_local / 256))
+                                            : std::min<int64_t>(ranges, std::max<int64_t>(1, c->n_local / 64)));
+    }
+    return B200DPF_OK;
+}
+
+/* The plan of one evaluation on a grouped context, whose bin-sorted keys of bin g are at positions
+ * count[g] .. count[g + 1].  Key groups and their work-item size: big items amortise the root-to-subtree
+ * walk every item pays (there is no frontier: bins are small), small items keep every warp busy.  Leaves
+ * of many rows (KindOps::leaf_items) take items down to s = 1, as on a plain context.  One cooperative
+ * launch per 16 columns; the first one clears the result and every pass's tickets. */
+int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, EvalPlan *out)
+{
+    const GroupBins *B = c->bins.get();
+    const KindOps &ops = kKindOps[c->kind];
+    const int nbins = (int)B->n.size();
+    EvalPlan &P = *out = EvalPlan{};
+    const SmemLayout &L = P.L;
+    P.grouped = P.one_launch = true;
+    P.mode = ops.mode_grouped;
+    P.nv = 4; P.passes = c->entry_pad / 16;     /* 16 columns per pass */
+    P.kpw_log2 = 5;
+    int rc = smem_layout(c, prf, P.nv, P.mode, &P.L);
+    if (rc) return rc;
+    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
+    auto groups_of = [&](int g) { return (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32; };
+    for (int g = 0; g < nbins; g++) P.key_groups += groups_of(g);
+    P.s_group = std::min(c->knobs.subtree_log2 > 0 ? c->knobs.subtree_log2 : 6, L.s_max);
+    if (c->knobs.subtree_log2 <= 0) {
+        const int s_floor = ops.leaf_items ? 1 : 3;
+        const int64_t items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
+        P.s_group = shrink_s(P.s_group, s_floor, items_wanted, [&](int t) {
+            int64_t items = 0;
+            for (int g = 0; g < nbins; g++) items += groups_of(g) << std::max(0, B->depth[(size_t)g] - t);
+            return items;
+        });
+    }
+    P.s = 1;
+    for (int g = 0; g < nbins; g++)
+        if (count[(size_t)g + 1] > count[(size_t)g]) P.s = std::max(P.s, group_s(P, B->depth[(size_t)g]));
+    /* per pass: one ticket counter per key group, or the one unit counter */
+    P.pass_counters = mode_traits(P.mode).units ? 1u : (size_t)P.key_groups;
+    P.smem = smem_bytes(L, P.s);
+    fill_phase(L, P.s, &P.main);
+    return B200DPF_OK;
+}
+
+/* Carry out plan P of job J: reserve what it asks for, order it after the context's last operation, clear,
+ * launch and make that the context's last operation.  A device that cannot keep the whole persistent grid
+ * resident (a partitioned GPU, say) refuses the first cooperative launch before anything of the evaluation
+ * ran: a plain context then falls back, for its life, to separate launches, planned again. */
+int launch_plan(b200dpf_ctx *c, const EvalJob &J, const EvalPlan &P)
+{
+    const bool fused = J.mode_main == MODE_FUSED;
+    const size_t n_counters = (size_t)P.passes * P.pass_counters;
+    bool grown = false;
+    int rc = c->d_counters.reserve(n_counters * sizeof(uint32_t));
+    if (!rc && P.top_counters) rc = c->d_top_counters.reserve(P.top_counters * sizeof(uint32_t), &grown);
+    if (grown) c->coop_state_dirty = true;
+    if (!rc && P.frontier_bytes) rc = c->d_frontier.reserve(P.frontier_bytes);
+    if (!rc) rc = wait_last(c, J.stream);
+    if (rc) return rc;
+
+    if (!P.one_launch || c->coop_state_dirty) {
+        if (P.top_counters) CUDA_TRY(cudaMemsetAsync(c->d_top_counters.ptr, 0, c->d_top_counters.cap, J.stream));
+        CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), J.stream));
+        c->bar_epoch = 0;
+        c->coop_state_dirty = false;
+    }
+    if (!P.one_launch) {
+        CUDA_TRY(cudaMemsetAsync(c->d_counters.ptr, 0, n_counters * sizeof(uint32_t), J.stream));
+        if (fused && J.clear_out)
+            CUDA_TRY(cudaMemsetAsync(J.out, 0, (size_t)J.nkeys * c->entry_size * sizeof(int32_t), J.stream));
+        c->coop_state_dirty = true;     /* the stand-alone frontier kernel leaves its tickets used */
+    }
+    if (P.timing) rc = c->d_timing.reserve((size_t)P.L.grid * 8 * sizeof(unsigned long long));
+    if (!rc && P.leaf_cache_bytes) rc = c->d_leaf_cache.reserve(P.leaf_cache_bytes);
+    if (rc) return rc;
+    if (P.timing) CUDA_TRY(cudaMemsetAsync(c->d_timing.ptr, 0, c->d_timing.cap, J.stream));
+    c->last_launches = 0;
+    if (J.timed) CUDA_TRY(cudaEventRecord(c->ev_t0, J.stream));
+
+    EvalParams p;
+    PhaseParams top = P.top;
+    if (P.f_rel > 0) top.counters = c->d_top_counters.ptr;
+    uint4 *const frontier = reinterpret_cast<uint4 *>(c->d_frontier.ptr);
+    if (P.f_rel > 0 && !P.one_launch) {           /* the stand-alone frontier kernel */
+        fill_common(c, P.LF, J, P, &p);
+        p.main = top; p.nfront = P.nfront; p.frontier_out = frontier;
+        CUDA_TRY(launch_eval(J.prf, 4, MODE_FRONTIER, p, P.LF.grid, P.smem_top, J.stream));
+        c->last_launches++;
+    }
+
+    fill_common(c, P.L, J, P, &p);
+    p.main = P.main;
     p.main.counters = c->d_counters.ptr;
-    if (one_launch) {
+    if (P.f_rel > 0) p.main.frontier_in = frontier;
+    p.nfront = P.nfront;
+    p.off_tile = P.off_tile; p.off_tile_bar = P.off_tile_bar;
+    if (P.one_launch) {
         p.fuse_top = 1;
-        p.top = top;                      /* nsub == 0: no frontier, the top phase only clears */
-        p.frontier_out = reinterpret_cast<uint4 *>(c->d_frontier.ptr);
-        if (mode_main == MODE_FUSED && clear_out) {
-            p.zero_a = reinterpret_cast<uint32_t *>(out_dev);
-            p.zero_a_words = (uint64_t)nkeys * (uint64_t)c->entry_size;
+        if (fused && J.clear_out) { p.zero_a = reinterpret_cast<uint32_t *>(J.out); p.zero_a_words = (uint64_t)J.nkeys * c->entry_size; }
+        p.zero_b = c->d_counters.ptr; p.zero_b_words = n_counters;
+        if (!P.grouped) {
+            p.top = top;                  /* nsub == 0: no frontier, the top phase only clears */
+            p.frontier_out = frontier;
+            p.rearm = c->d_top_counters.ptr; p.rearm_words = (uint32_t)P.key_groups;
+            p.top_block_quota = P.top_block_quota;
         }
-        p.zero_b = c->d_counters.ptr;
-        p.zero_b_words = n_main_counters;
-        p.rearm = c->d_top_counters.ptr;
-        p.rearm_words = (uint32_t)key_groups;
-        {
-            const uint64_t items = (uint64_t)key_groups * (uint64_t)(top.nsub >> spw_log2);
-            p.top_block_quota = K.balance_top ? (uint32_t)std::max<uint64_t>(1, (items + (uint64_t)L.grid - 1) / (uint64_t)L.grid)
-                                              : 0x7fffffffu;
-        }
-        if (K.timing) {
-            rc = c->d_timing.reserve((size_t)L.grid * 8 * sizeof(unsigned long long));
-            if (rc) return rc;
-            CUDA_TRY(cudaMemsetAsync(c->d_timing.ptr, 0, c->d_timing.cap, stream));
-            p.timing = c->d_timing.ptr;
-        }
+        if (P.timing) p.timing = c->d_timing.ptr;
         p.grid_bar = c->d_gridbar.ptr;
-        c->bar_epoch += (uint32_t)L.grid;
+        c->bar_epoch += (uint32_t)P.L.grid;
         p.grid_bar_target = c->bar_epoch;
     }
-    auto launch_main = [&](int nv_l, int mode_l) -> int {
-        const cudaError_t e = launch_eval(prf, nv_l, mode_l, p, L.grid, smem, stream);
+
+    bool coop_refused = false;
+    auto launch_main = [&]() -> int {
+        const cudaError_t e = launch_eval(J.prf, P.nv, P.mode, p, P.L.grid, P.smem, J.stream);
         if (e != cudaSuccess) {
             c->coop_state_dirty = true;
-            if (e == cudaErrorCooperativeLaunchTooLarge && p.fuse_top) {
-                /* this device cannot keep the whole persistent grid resident (a partitioned GPU, say):
-                 * nothing of this evaluation has been enqueued yet, so fall back -- for the life of the
-                 * context -- to the pipeline of separate launches */
-                cudaGetLastError();
-                c->coop_ok = 0;
-                return kRetryWithoutCooperativeLaunch;
-            }
-            return fail(B200DPF_ECUDA, "evaluation kernel launch: %s", cudaGetErrorString(e));
+            coop_refused = e == cudaErrorCooperativeLaunchTooLarge && p.fuse_top && !P.grouped;
+            return fail(B200DPF_ECUDA, "%s: %s", P.grouped ? "grouped evaluation launch" : "evaluation kernel launch",
+                        cudaGetErrorString(e));
         }
         c->last_launches++;
         p.fuse_top = 0;                   /* later passes of this evaluation reuse the frontier */
         return B200DPF_OK;
     };
-    if (mode_main == MODE_EXPAND) {
-        p.shares = reinterpret_cast<uint32_t *>(out_dev);
-        return launch_main(4, ops.mode_expand);
+    if (J.mode_main == MODE_EXPAND) {
+        p.shares = reinterpret_cast<uint32_t *>(J.out);
+        rc = launch_main();
+    } else {
+        p.out = reinterpret_cast<uint32_t *>(J.out);
+        if (P.leaf_cache) { p.leaf_cache = c->d_leaf_cache.ptr; p.n_local = (uint64_t)c->n_local; }
+        for (int pass = 0; pass < P.passes && rc == B200DPF_OK; pass++) {
+            p.col_off_v = (uint32_t)(pass * P.nv);
+            p.col_off = (uint32_t)(pass * 4 * P.nv);
+            p.ncols = (uint32_t)std::max(0, std::min(4 * P.nv, c->entry_size - pass * 4 * P.nv));
+            if (p.ncols == 0) break;
+            p.main.counters = c->d_counters.ptr + (size_t)pass * P.pass_counters;
+            rc = launch_main();
+        }
     }
-    p.out = reinterpret_cast<uint32_t *>(out_dev);
-    if (want_cache) {
-        const size_t cache_bytes = (size_t)key_groups * 32u * (size_t)c->n_local * sizeof(uint32_t);
-        rc = c->d_leaf_cache.reserve(cache_bytes);
-        if (rc) return rc;
-        p.leaf_cache = c->d_leaf_cache.ptr;
-        p.n_local = (uint64_t)c->n_local;
-        p.col_off_v = 0;
-        p.col_off = 0;
-        p.ncols = (uint32_t)std::min(16, c->entry_size);
-        rc = launch_main(4, ops.mode_fused);
-        if (rc) return rc;
+    if (coop_refused) {
+        cudaGetLastError();
+        c->coop_ok = 0;
+        EvalPlan Q;
+        return (rc = plan_eval(c, J, &Q)) ? rc : launch_plan(c, J, Q);
+    }
+    if (rc) return rc;
+
+    if (P.leaf_cache) {
         MacParams m;
         std::memset(&m, 0, sizeof m);
-        m.leaf_cache = p.leaf_cache;
-        m.table = p.table;
-        m.row_stride_v = p.row_stride_v;
-        m.out = p.out;
-        m.out_stride = p.out_stride;
-        m.nkeys = (int)nkeys;
-        m.key_groups = (int)key_groups;
-        m.n_local = (uint64_t)c->n_local;
-        const bool use_tma = K.mac_tma != 0;
-        const int mac_grid = c->sm_count * 2;                      /* register-staged variant */
-        const int64_t mac_warps = (int64_t)mac_grid * 8;
-        int64_t ranges = std::max<int64_t>(1, (2 * mac_warps + key_groups - 1) / key_groups);
-        ranges = std::min<int64_t>(ranges, std::max<int64_t>(1, c->n_local / 64));
-        /* TMA variant: one block per SM; a block takes 8 key groups x one position range */
-        const int64_t kg_blocks = (key_groups + 7) / 8;
-        int64_t tr = std::max<int64_t>(1, (2 * (int64_t)c->sm_count + kg_blocks - 1) / kg_blocks);
-        tr = std::min<int64_t>(tr, std::max<int64_t>(1, c->n_local / 256));
+        m.leaf_cache = p.leaf_cache; m.table = p.table; m.row_stride_v = p.row_stride_v;
+        m.out = p.out; m.out_stride = p.out_stride;
+        m.nkeys = (int)J.nkeys; m.key_groups = (int)P.key_groups; m.n_local = (uint64_t)c->n_local;
+        m.ranges_per_group = P.mac_ranges;
         for (int blk = 0; blk * 64 < c->entry_size; blk++) {       /* 64-column slices of the rows */
-            m.col_off_v = (uint32_t)(blk * 16);
-            m.col_off = (uint32_t)(blk * 64);
+            m.col_off_v = (uint32_t)(blk * 16); m.col_off = (uint32_t)(blk * 64);
             m.ncols = (uint32_t)std::min(64, c->entry_size - blk * 64);
             m.col_skip = blk == 0 ? 16u : 0u;                      /* columns 0..15 came from the fused pass */
             if (m.ncols <= m.col_skip) continue;
-            if (use_tma) {
-                m.ranges_per_group = (uint32_t)tr;
-                CUDA_TRY(launch_mac_tma(m, c->sm_count, stream));
-            } else {
-                m.ranges_per_group = (uint32_t)ranges;
-                CUDA_TRY(launch_mac(16, m, mac_grid, stream));
-            }
+            if (P.mac_tma) CUDA_TRY(launch_mac_tma(m, P.mac_grid, J.stream));
+            else CUDA_TRY(launch_mac(16, m, P.mac_grid, J.stream));
             c->last_launches++;
         }
-        return B200DPF_OK;
     }
-    for (int pass = 0; pass < passes; pass++) {
-        p.col_off_v = (uint32_t)(pass * nv);
-        p.col_off = (uint32_t)(pass * 4 * nv);
-        p.ncols = (uint32_t)std::max(0, std::min(4 * nv, c->entry_size - pass * 4 * nv));
-        if (p.ncols == 0) break;
-        p.main.counters = c->d_counters.ptr + (size_t)pass * key_groups;
-        rc = launch_main(nv, mode_kernel);
-        if (rc) return rc;
-    }
-    return B200DPF_OK;
+    if (J.timed) { CUDA_TRY(cudaEventRecord(c->ev_t1, J.stream)); c->timed = true; }
+    return mark_last(c, J.stream);
 }
 
 /*
- * One evaluation.  Wide entries whose leaf cache (nkeys x n_local x 4 bytes) would exceed the cap
- * are evaluated in batch chunks that fit -- the cache is what makes columns beyond the first 16
- * cost a MAC pass instead of a tree expansion, so shrinking the chunk beats dropping the cache.
+ * One evaluation on a plain context.  Wide entries whose leaf cache (nkeys x n_local x 4 bytes) would
+ * exceed the cap are evaluated in batch chunks that fit -- the cache is what makes columns beyond the
+ * first 16 cost a MAC pass instead of a tree expansion, so shrinking the chunk beats dropping the cache.
  */
 int run_pipeline(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int64_t nkeys, int prf, int mode_main,
                  void *out_dev, cudaStream_t stream, bool clear_out = true)
 {
     const b200dpf_ctx::Knobs &K = c->knobs;
-    int rc = B200DPF_OK;
-    int launches = 0;
     const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0 && kKindOps[c->kind].leaf_cache;
     const size_t per_group = 32u * (size_t)c->n_local * sizeof(uint32_t);
     const size_t cap = (size_t)std::max(K.leaf_cache_mb, 1) << 20;
-    if (!wide || per_group > cap) {
-        /* not a cached evaluation (or one key group alone overflows the cap: re-expand per 64 columns) */
-        rc = run_pipeline_chunk(c, keys_dev, kl, nkeys, prf, mode_main, out_dev, stream, clear_out, false);
-        if (rc == kRetryWithoutCooperativeLaunch)
-            rc = run_pipeline_chunk(c, keys_dev, kl, nkeys, prf, mode_main, out_dev, stream, clear_out, false);
-        launches = c->last_launches;
-    } else {
-        const int64_t groups_per_chunk = (int64_t)std::max<size_t>(1, cap / per_group);
-        const int64_t chunk = groups_per_chunk * 32;
-        for (int64_t k0 = 0; k0 < nkeys && rc == B200DPF_OK; k0 += chunk) {
-            const int64_t kn = std::min(chunk, nkeys - k0);
-            const char *kp = reinterpret_cast<const char *>(keys_dev) + (size_t)k0 * kl.stride_v * 16u;
-            char *op = reinterpret_cast<char *>(out_dev) + (size_t)k0 * c->entry_size * sizeof(int32_t);
-            /* a ragged tail below 17 keys would be lane-split, which the cache layout excludes */
-            rc = run_pipeline_chunk(c, kp, kl, kn, prf, mode_main, op, stream, clear_out, kn >= 17);
-            if (rc == kRetryWithoutCooperativeLaunch)
-                rc = run_pipeline_chunk(c, kp, kl, kn, prf, mode_main, op, stream, clear_out, kn >= 17);
-            launches += c->last_launches;
-        }
+    /* not a cached evaluation, or one key group alone overflows the cap (re-expand per 64 columns): one chunk */
+    const bool cached = wide && per_group <= cap;
+    const int64_t chunk = cached ? (int64_t)std::max<size_t>(1, cap / per_group) * 32 : nkeys;
+    EvalJob J{keys_dev, kl, nkeys, prf, mode_main, out_dev, stream, clear_out};
+    int rc = B200DPF_OK, launches = 0;
+    for (int64_t k0 = 0; k0 < nkeys && rc == B200DPF_OK; k0 += chunk) {
+        J.nkeys = std::min(chunk, nkeys - k0);
+        J.keys = reinterpret_cast<const char *>(keys_dev) + (size_t)k0 * kl.stride_v * 16u;
+        J.out = reinterpret_cast<char *>(out_dev) + (size_t)k0 * c->entry_size * sizeof(int32_t);
+        /* a ragged tail below 17 keys would be lane-split, which the cache layout excludes */
+        J.leaf_cache = cached && J.nkeys >= 17;
+        EvalPlan P;
+        rc = plan_eval(c, J, &P);
+        if (!rc) rc = launch_plan(c, J, P);
+        launches += c->last_launches;
     }
     c->last_launches = launches;
-    return rc ? rc : mark_last(c, stream);
-}
-
-int run_eval(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, int prf, void *out_dev, cudaStream_t stream)
-{
-    return run_pipeline(c, keys_dev, reference_layout(), nkeys, prf, MODE_FUSED, out_dev, stream);
+    return rc;
 }
 
 bool is_pinned_host(const void *ptr)
@@ -891,23 +984,9 @@ int ctx_open(int device, bool read_env, std::optional<DeviceGuard> *guard, std::
     CUDA_TRY(cudaEventCreate(&c->ev_t1));
     rc = c->d_gridbar.reserve(sizeof(uint32_t));
     if (rc) return rc;
-    if (read_env) {
-        /* the environment is consulted here and nowhere else (b200dpf_ctx_set_option changes a
-         * live context) */
-        b200dpf_ctx::Knobs &K = c->knobs;
-        K.leaf_cache = env_int("B200DPF_LEAF_CACHE", K.leaf_cache);
-        K.leaf_cache_mb = env_int("B200DPF_LEAF_CACHE_MB", K.leaf_cache_mb);
-        K.lane_split = env_int("B200DPF_LANE_SPLIT", K.lane_split);
-        K.frontier = env_int("B200DPF_FRONTIER", K.frontier);
-        K.frontier_mb = env_int("B200DPF_FRONTIER_MB", K.frontier_mb);
-        K.subtree_log2 = env_int("B200DPF_S", K.subtree_log2);
-        K.mac_tma = env_int("B200DPF_MAC_TMA", K.mac_tma);
-        K.one_launch = env_int("B200DPF_ONE_LAUNCH", K.one_launch);
-        K.balance_top = env_int("B200DPF_BALANCE_TOP", K.balance_top);
-        K.timing = env_int("B200DPF_TIMING", K.timing);
-        K.top_log2 = env_int("B200DPF_TOP_LOG2", K.top_log2);
-        K.tma_rows = env_int("B200DPF_TMA_ROWS", K.tma_rows);
-    }
+    /* the environment is consulted here and nowhere else (b200dpf_ctx_set_option changes a live context) */
+    if (read_env)
+        for (const KnobInfo &k : kKnobs) c->knobs.*k.field = env_int(k.env, k.dflt);
     CUDA_TRY(probe_dynamic_smem_base(&c->smem_base, c->stream));
     CUDA_TRY(upload_aes_table(host::aes_te0()));
     *out = std::move(c);
@@ -1434,7 +1513,8 @@ int b200dpf_eval_device(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, int
     if (c->multi) return fail(B200DPF_ESTATE, "multi-device contexts take host buffers (b200dpf_eval / b200dpf_eval_packed)");
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    return run_eval(c, keys_dev, nkeys, prf, out_dev, reinterpret_cast<cudaStream_t>(cuda_stream));
+    return run_pipeline(c, keys_dev, reference_layout(), nkeys, prf, MODE_FUSED, out_dev,
+                        reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 int b200dpf_eval_device_acc(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, int prf, void *out_dev, void *cuda_stream)
@@ -1480,18 +1560,10 @@ int b200dpf_ctx_set_option(b200dpf_ctx *c, const char *name, int value)
 {
     if (!c || !name) return fail(B200DPF_EINVAL, "null argument");
     if (c->multi) return multi_set_option(c, name, value);
-    struct { const char *name; int *slot; int lo, hi; } opts[] = {
-        {"leaf_cache", &c->knobs.leaf_cache, 0, 1},       {"leaf_cache_mb", &c->knobs.leaf_cache_mb, 1, 1 << 20},
-        {"lane_split", &c->knobs.lane_split, 0, 1},       {"frontier", &c->knobs.frontier, 0, 1},
-        {"frontier_mb", &c->knobs.frontier_mb, 1, 1 << 16}, {"subtree_log2", &c->knobs.subtree_log2, 0, 16},
-        {"mac_tma", &c->knobs.mac_tma, 0, 1},             {"one_launch", &c->knobs.one_launch, 0, 1},
-        {"balance_top", &c->knobs.balance_top, 0, 1},     {"timing", &c->knobs.timing, 0, 1},
-        {"tma_rows", &c->knobs.tma_rows, 0, 1},           {"top_log2", &c->knobs.top_log2, 0, 7},
-    };
-    for (auto &o : opts)
-        if (std::strcmp(o.name, name) == 0) {
-            if (value < o.lo || value > o.hi) return fail(B200DPF_EINVAL, "option %s=%d out of range [%d,%d]", name, value, o.lo, o.hi);
-            *o.slot = value;
+    for (const KnobInfo &k : kKnobs)
+        if (std::strcmp(k.name, name) == 0) {
+            if (value < k.lo || value > k.hi) return fail(B200DPF_EINVAL, "option %s=%d out of range [%d,%d]", name, value, k.lo, k.hi);
+            c->knobs.*k.field = value;
             return B200DPF_OK;
         }
     return fail(B200DPF_EINVAL, "unknown option '%s'", name);
@@ -1871,7 +1943,6 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
      * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
     const KeyLayout kl = compact_layout(c->depth);
-    const int mode = kKindOps[c->kind].mode_grouped;
     const char *magic = host::kKinds[c->kind].magic;
     const size_t stride = (size_t)kl.stride_v * 16u;
     const size_t key_bytes = (size_t)nkeys * stride;
@@ -1894,40 +1965,19 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         pack_range(0, nkeys / nthr);
         for (auto &th : pool) th.join();
     }
-    /* key groups and their work-item size: big items amortise the root-to-subtree walk every item
-     * pays (there is no frontier: bins are small), small items keep every warp busy.  Leaves of many
-     * rows (KindOps::leaf_items) take items down to s = 1, as on a plain context. */
-    SmemLayout L;
-    rc = smem_layout(c, prf, 4, mode, &L);
+    EvalPlan P;
+    rc = plan_group_eval(c, prf, count, &P);
     if (rc) return rc;
-    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
-    int64_t ngroups = 0;
-    for (int g = 0; g < nbins; g++) ngroups += (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32;
-    const KindOps &ops = kKindOps[c->kind];
-    int s_target = c->knobs.subtree_log2 > 0 ? c->knobs.subtree_log2 : 6;
-    s_target = std::min(s_target, L.s_max);
-    if (c->knobs.subtree_log2 <= 0) {
-        const int s_floor = ops.leaf_items ? 1 : 3;
-        const int64_t items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
-        for (; s_target > s_floor; s_target--) {
-            int64_t items = 0;
-            for (int g = 0; g < nbins; g++) {
-                const int64_t kg = (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32;
-                items += kg << std::max(0, B->depth[(size_t)g] - s_target);
-            }
-            if (items >= items_wanted) break;
-        }
-    }
+    const int64_t ngroups = P.key_groups;
     const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
     rc = B->h_descs.reserve(descs_bytes);
     if (!rc) rc = B->d_descs.reserve(descs_bytes);
     if (rc) return rc;
-    int s_max = 1;
     {
         int64_t gi = 0;
         for (int g = 0; g < nbins; g++) {
             const int depth = B->depth[(size_t)g];
-            const int s = std::max(1, std::min(depth, s_target));
+            const int s = group_s(P, depth);
             for (int64_t k = count[(size_t)g]; k < count[(size_t)g + 1]; k += 32, gi++) {
                 GroupDesc &d = B->h_descs.ptr[gi];
                 d.key_first = (uint32_t)k;
@@ -1937,7 +1987,6 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
                 d.nsub = (uint32_t)1 << (depth - s);
                 d.pad = 0;
                 d.table_off_v = B->row_off[(size_t)g] * (uint64_t)(c->entry_pad / 4);
-                s_max = std::max(s_max, s);
             }
         }
     }
@@ -1946,12 +1995,12 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
      * (units per block) unit times: whole-block units unless the launch holds fewer items than the grid
      * has warps, and then about items / blocks per unit, so that every block has work.  A key group with
      * fewer items than its unit size leaves the rest of its unit's warps idle. */
-    const bool units = mode_traits(mode).units;
+    const bool units = mode_traits(P.mode).units;
     int64_t nunits = 0;
     if (units) {
         int64_t items = 0;
         for (int64_t gi = 0; gi < ngroups; gi++) items += B->h_descs.ptr[gi].nsub;
-        const int64_t per_unit = std::clamp<int64_t>((items + L.grid - 1) / L.grid, 1, L.threads / 32);
+        const int64_t per_unit = std::clamp<int64_t>((items + P.L.grid - 1) / P.L.grid, 1, P.L.threads / 32);
         for (int64_t gi = 0; gi < ngroups; gi++) nunits += (B->h_descs.ptr[gi].nsub + per_unit - 1) / per_unit;
         const size_t units_bytes = std::max<size_t>((size_t)nunits, 1024) * sizeof(WorkUnit);
         rc = B->h_units.reserve(units_bytes);
@@ -1967,71 +2016,20 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             }
         }
     }
-    const int passes = c->entry_pad / 16;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
     rc = reserve_device_io(c, key_bytes, out_elems);
     if (!rc) rc = reserve_host_out(c, out_elems);
-    if (rc) return rc;
-    /* per pass: one ticket counter per key group, or the one unit counter */
-    const size_t pass_counters = units ? 1u : (size_t)ngroups;
-    const size_t n_counters = (size_t)passes * pass_counters;
-    rc = c->d_counters.reserve(n_counters * sizeof(uint32_t));
     if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, B->h_descs.ptr, (size_t)ngroups * sizeof(GroupDesc), cudaMemcpyHostToDevice, c->stream));
     if (units)
         CUDA_TRY(cudaMemcpyAsync(B->d_units.ptr, B->h_units.ptr, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, c->stream));
-    if (c->coop_state_dirty) {
-        CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), c->stream));
-        c->bar_epoch = 0;
-        c->coop_state_dirty = false;
-    }
-    EvalParams p;
-    size_t smem;
-    fill_common(c, L, s_max, nkeys, 5, &p, &smem);
-    p.key_groups = (int)ngroups;
-    p.keys = reinterpret_cast<const uint4 *>(c->d_keys.ptr);
-    p.key_stride_v = kl.stride_v; p.key_root_v = kl.root_v; p.key_compact = kl.compact;
-    p.groups = B->d_descs.ptr;
-    p.units = B->d_units.ptr;
-    p.nunits = (uint32_t)nunits;
-    fill_phase(L, s_max, &p.main);
-    p.main.counters = c->d_counters.ptr;
-    p.out = reinterpret_cast<uint32_t *>(c->d_out.ptr);
-    /* one cooperative launch per 16 columns; the first one clears the result and every pass's tickets */
-    p.fuse_top = 1;
-    p.zero_a = p.out;
-    p.zero_a_words = out_elems;
-    p.zero_b = c->d_counters.ptr;
-    p.zero_b_words = n_counters;
-    c->last_launches = 0;
-    CUDA_TRY(cudaEventRecord(c->ev_t0, c->stream));
-    for (int pass = 0; pass < passes; pass++) {
-        p.col_off_v = (uint32_t)(pass * 4);
-        p.col_off = (uint32_t)(pass * 16);
-        p.ncols = (uint32_t)std::max(0, std::min(16, c->entry_size - pass * 16));
-        if (p.ncols == 0) break;
-        p.main.counters = c->d_counters.ptr + (size_t)pass * pass_counters;
-        if (p.fuse_top) {
-            p.grid_bar = c->d_gridbar.ptr;
-            c->bar_epoch += (uint32_t)L.grid;
-            p.grid_bar_target = c->bar_epoch;
-        }
-        const cudaError_t e = launch_eval(prf, 4, mode, p, L.grid, smem, c->stream);
-        if (e != cudaSuccess) {
-            c->coop_state_dirty = true;
-            return fail(B200DPF_ECUDA, "grouped evaluation launch: %s", cudaGetErrorString(e));
-        }
-        c->last_launches++;
-        p.fuse_top = 0;
-    }
-    CUDA_TRY(cudaEventRecord(c->ev_t1, c->stream));
-    c->timed = true;
-    CUDA_TRY(cudaMemcpyAsync(c->h_out.ptr, c->d_out.ptr, out_elems * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-    rc = mark_last(c, c->stream);
+    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, c->stream, true, false,
+                    B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
+    rc = launch_plan(c, J, P);
+    if (!rc) rc = download_out(c, c->h_out.ptr, true, out_elems);
     if (rc) return rc;
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
     for (int64_t pos = 0; pos < nkeys; pos++)       /* back to the caller's order */
         std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out.ptr + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
     return B200DPF_OK;
