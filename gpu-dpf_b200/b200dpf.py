@@ -21,7 +21,7 @@ SYMBOLS = [
     "b200dpf_version", "b200dpf_last_error", "b200dpf_gen", "b200dpf_gen_secure", "b200dpf_gen_batch", "b200dpf_gen_batch_secure", "b200dpf_gen_batch_gpu", "b200dpf_eval_cpu",
     "b200dpf_key_packed_size", "b200dpf_key_pack", "b200dpf_key_unpack", "b200dpf_key_n", "b200dpf_key_depth", "b200dpf_create", "b200dpf_destroy", "b200dpf_eval",
     "b200dpf_eval_packed", "b200dpf_eval_gather", "b200dpf_ctx_set_option", "b200dpf_create_multi", "b200dpf_ctx_device_count", "b200dpf_ctx_axis", "b200dpf_ctx_read_timing",
-    "b200dpf_group_create", "b200dpf_group_eval", "b200dpf_group_bins", "b200dpf_ctx_last_device_ms",
+    "b200dpf_group_create", "b200dpf_group_eval", "b200dpf_group_eval_device", "b200dpf_group_bins", "b200dpf_ctx_last_device_ms",
     "b200dpf_update_rows", "b200dpf_update_rows_device", "b200dpf_group_update_rows",
     "b200dpf_host_staging", "b200dpf_eval_device", "b200dpf_eval_device_acc", "b200dpf_expand_device", "b200dpf_ctx_n", "b200dpf_ctx_entry_size",
     "b200dpf_ctx_device", "b200dpf_ctx_last_launches", "b200dpf_ctx_set_subtree_log2",
@@ -75,6 +75,7 @@ def load():
     L.b200dpf_ctx_axis.argtypes = [C.c_void_p]
     L.b200dpf_group_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
     L.b200dpf_group_eval.argtypes = [C.c_void_p, _i32p, _i32p, C.c_int64, C.c_int, _i32p]
+    L.b200dpf_group_eval_device.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
     L.b200dpf_group_bins.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_device_ms.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_device_ms.restype = C.c_double
@@ -439,6 +440,14 @@ class GroupContext(Context):
         out = np.zeros((keys.shape[0], self.entry_size), np.int32)
         _check(lib().b200dpf_group_eval(self.handle, keys, bins, keys.shape[0], prf, out), "b200dpf_group_eval")
         return out
+
+    def eval_device(self, keys_ptr, bins, prf, out_ptr, stream=0):
+        """eval from device keys (int32 [len(bins), 524] at keys_ptr) into device results (int32
+        [len(bins), entry_size] at out_ptr), enqueued on `stream` with no host synchronisation.  `bins` stays
+        on the host: the launch is planned from it."""
+        bins = np.ascontiguousarray(bins, np.int32).reshape(-1)
+        _check(lib().b200dpf_group_eval_device(self.handle, C.c_void_p(keys_ptr), bins, len(bins), prf,
+                                               C.c_void_p(out_ptr), C.c_void_p(stream)), "b200dpf_group_eval_device")
 
     def update_rows(self, bins, indices, rows):
         """row indices[j] of bin bins[j] := rows[j] (last occurrence wins); synchronous"""

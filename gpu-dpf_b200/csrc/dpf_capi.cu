@@ -129,6 +129,19 @@ struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behi
     PinnedBuffer<WorkUnit> h_units;
     std::vector<int64_t> perm;         /* sorted position -> caller's index, of the last evaluation */
     DeviceBuffer<uint2> d_bin_info;    /* [nbins] (row_off, depth) for row updates, uploaded on first use */
+    /* b200dpf_group_eval_device: its own pinned staging, whose uploads (on the caller's stream) may still be
+     * pending when the call returns; ev_staged follows them, and the next call waits for it before it
+     * rewrites or regrows any of the three.  d_order: [nkeys] (caller's index, bin depth) by sorted position */
+    PinnedBuffer<GroupDesc> h_descs_dev;
+    PinnedBuffer<WorkUnit> h_units_dev;
+    PinnedBuffer<uint2> h_order;
+    DeviceBuffer<uint2> d_order;
+    cudaEvent_t ev_staged = nullptr;
+    bool staged_pending = false;
+    ~GroupBins()
+    {
+        if (ev_staged) cudaEventDestroy(ev_staged);
+    }
 };
 
 struct b200dpf_ctx {
@@ -1920,57 +1933,54 @@ int b200dpf_group_create_xor(b200dpf_ctx **out, const int32_t *const *tables, co
     return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_XOR);
 }
 
-int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
+/* The argument checks of both grouped evaluations, before anything else */
+static int check_group_args(const b200dpf_ctx *c, const void *keys, const int32_t *bins, int64_t nkeys, int prf, const void *out)
 {
     if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
     if (!keys || !bins || !out) return fail(B200DPF_EINVAL, "null buffer");
     if (nkeys < 1 || nkeys > (int64_t)1 << 24) return fail(B200DPF_EINVAL, "nkeys=%lld out of range", (long long)nkeys);
     if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
+    return B200DPF_OK;
+}
+
+/* Counting sort of the keys by bin (a key group must not mix bins): the keys of bin g go to sorted positions
+ * count[g] .. count[g + 1], in the caller's order, and B->perm maps a sorted position to the caller's index.
+ * Every bin id is checked and, given host `keys`, every key, key by key. */
+static int group_sort(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, std::vector<int64_t> *count_out)
+{
     GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
-    /* counting sort by bin: a key group must not mix bins */
-    std::vector<int64_t> count((size_t)nbins + 1, 0);
+    std::vector<int64_t> &count = *count_out;
+    count.assign((size_t)nbins + 1, 0);
     for (int64_t b = 0; b < nkeys; b++) {
         const int g = bins[b];
         if (g < 0 || g >= nbins) return fail(B200DPF_EINVAL, "key %lld: bin %d out of range [0,%d)", (long long)b, g, nbins);
-        const int rc = check_key(c->kind, B->n[(size_t)g], keys + b * host::KEY_WORDS, b, g);
-        if (rc) return rc;
+        if (keys) {
+            const int rc = check_key(c->kind, B->n[(size_t)g], keys + b * host::KEY_WORDS, b, g);
+            if (rc) return rc;
+        }
         count[(size_t)g + 1]++;
     }
     for (int g = 0; g < nbins; g++) count[(size_t)g + 1] += count[(size_t)g];
-    DeviceGuard guard(c->device);
-    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
-     * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
-    const KeyLayout kl = compact_layout(c->depth);
-    const char *magic = host::kKinds[c->kind].magic;
-    const size_t stride = (size_t)kl.stride_v * 16u;
-    const size_t key_bytes = (size_t)nkeys * stride;
-    int rc = reserve_host_keys(c, key_bytes);
-    if (rc) return rc;
     B->perm.assign((size_t)nkeys, 0);
-    {
-        std::vector<int64_t> next(count.begin(), count.end() - 1);
-        for (int64_t b = 0; b < nkeys; b++) B->perm[(size_t)(next[(size_t)bins[b]]++)] = b;
-        uint8_t *stage = reinterpret_cast<uint8_t *>(c->h_keys.ptr);
-        auto pack_range = [&](int64_t p0, int64_t p1) {
-            for (int64_t pos = p0; pos < p1; pos++) {
-                const int64_t b = B->perm[(size_t)pos];
-                pack_compact(keys + b * host::KEY_WORDS, stage + (size_t)pos * stride, B->depth[(size_t)bins[b]], magic);
-            }
-        };
-        const int nthr = (int)std::min<int64_t>(std::min<int64_t>(8, std::max(1u, std::thread::hardware_concurrency())), nkeys / 2048 + 1);
-        std::vector<std::thread> pool;
-        for (int t = 1; t < nthr; t++) pool.emplace_back(pack_range, nkeys * t / nthr, nkeys * (t + 1) / nthr);
-        pack_range(0, nkeys / nthr);
-        for (auto &th : pool) th.join();
-    }
-    EvalPlan P;
-    rc = plan_group_eval(c, prf, count, &P);
+    std::vector<int64_t> next(count.begin(), count.end() - 1);
+    for (int64_t b = 0; b < nkeys; b++) B->perm[(size_t)(next[(size_t)bins[b]]++)] = b;
+    return B200DPF_OK;
+}
+
+/* The plan of an evaluation of keys sorted by group_sort, with its key groups' descriptors in h_descs and, for
+ * modes that draw work units, its units in h_units (*nunits of them); the device lists grow to match. */
+static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, PinnedBuffer<GroupDesc> &h_descs,
+                      PinnedBuffer<WorkUnit> &h_units, EvalPlan *out, int64_t *nunits_out)
+{
+    GroupBins *B = c->bins.get();
+    const int nbins = (int)B->n.size();
+    EvalPlan &P = *out;
+    int rc = plan_group_eval(c, prf, count, &P);
     if (rc) return rc;
     const int64_t ngroups = P.key_groups;
     const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
-    rc = B->h_descs.reserve(descs_bytes);
+    rc = h_descs.reserve(descs_bytes);
     if (!rc) rc = B->d_descs.reserve(descs_bytes);
     if (rc) return rc;
     {
@@ -1979,7 +1989,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             const int depth = B->depth[(size_t)g];
             const int s = group_s(P, depth);
             for (int64_t k = count[(size_t)g]; k < count[(size_t)g + 1]; k += 32, gi++) {
-                GroupDesc &d = B->h_descs.ptr[gi];
+                GroupDesc &d = h_descs.ptr[gi];
                 d.key_first = (uint32_t)k;
                 d.nkeys = (uint32_t)std::min<int64_t>(32, count[(size_t)g + 1] - k);
                 d.depth = depth;
@@ -1995,20 +2005,19 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
      * (units per block) unit times: whole-block units unless the launch holds fewer items than the grid
      * has warps, and then about items / blocks per unit, so that every block has work.  A key group with
      * fewer items than its unit size leaves the rest of its unit's warps idle. */
-    const bool units = mode_traits(P.mode).units;
-    int64_t nunits = 0;
-    if (units) {
+    int64_t &nunits = *nunits_out = 0;
+    if (mode_traits(P.mode).units) {
         int64_t items = 0;
-        for (int64_t gi = 0; gi < ngroups; gi++) items += B->h_descs.ptr[gi].nsub;
+        for (int64_t gi = 0; gi < ngroups; gi++) items += h_descs.ptr[gi].nsub;
         const int64_t per_unit = std::clamp<int64_t>((items + P.L.grid - 1) / P.L.grid, 1, P.L.threads / 32);
-        for (int64_t gi = 0; gi < ngroups; gi++) nunits += (B->h_descs.ptr[gi].nsub + per_unit - 1) / per_unit;
+        for (int64_t gi = 0; gi < ngroups; gi++) nunits += (h_descs.ptr[gi].nsub + per_unit - 1) / per_unit;
         const size_t units_bytes = std::max<size_t>((size_t)nunits, 1024) * sizeof(WorkUnit);
-        rc = B->h_units.reserve(units_bytes);
+        rc = h_units.reserve(units_bytes);
         if (!rc) rc = B->d_units.reserve(units_bytes);
         if (rc) return rc;
-        WorkUnit *w = B->h_units.ptr;
+        WorkUnit *w = h_units.ptr;
         for (int64_t gi = 0; gi < ngroups; gi++) {
-            const uint64_t nsub = B->h_descs.ptr[gi].nsub;
+            const uint64_t nsub = h_descs.ptr[gi].nsub;
             const uint64_t parts = (nsub + (uint64_t)per_unit - 1) / (uint64_t)per_unit;
             for (uint64_t j = 0; j < parts; j++) {
                 const uint64_t first = nsub * j / parts, end = nsub * (j + 1) / parts;
@@ -2016,15 +2025,64 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
             }
         }
     }
+    return B200DPF_OK;
+}
+
+/* Upload the descriptors and units of plan P (group_plan) into the device lists, on `stream`. */
+static int group_upload_lists(b200dpf_ctx *c, const EvalPlan &P, const GroupDesc *h_descs, const WorkUnit *h_units,
+                              int64_t nunits, cudaStream_t stream)
+{
+    GroupBins *B = c->bins.get();
+    CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, h_descs, (size_t)P.key_groups * sizeof(GroupDesc), cudaMemcpyHostToDevice, stream));
+    if (mode_traits(P.mode).units)
+        CUDA_TRY(cudaMemcpyAsync(B->d_units.ptr, h_units, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, stream));
+    return B200DPF_OK;
+}
+
+int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
+{
+    int rc = check_group_args(c, keys, bins, nkeys, prf, out);
+    if (rc) return rc;
+    GroupBins *B = c->bins.get();
+    std::vector<int64_t> count;
+    rc = group_sort(c, keys, bins, nkeys, &count);
+    if (rc) return rc;
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
+     * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
+    const KeyLayout kl = compact_layout(c->depth);
+    const char *magic = host::kKinds[c->kind].magic;
+    const size_t stride = (size_t)kl.stride_v * 16u;
+    const size_t key_bytes = (size_t)nkeys * stride;
+    rc = reserve_host_keys(c, key_bytes);
+    if (rc) return rc;
+    {
+        uint8_t *stage = reinterpret_cast<uint8_t *>(c->h_keys.ptr);
+        auto pack_range = [&](int64_t p0, int64_t p1) {
+            for (int64_t pos = p0; pos < p1; pos++) {
+                const int64_t b = B->perm[(size_t)pos];
+                pack_compact(keys + b * host::KEY_WORDS, stage + (size_t)pos * stride, B->depth[(size_t)bins[b]], magic);
+            }
+        };
+        const int nthr = (int)std::min<int64_t>(std::min<int64_t>(8, std::max(1u, std::thread::hardware_concurrency())), nkeys / 2048 + 1);
+        std::vector<std::thread> pool;
+        for (int t = 1; t < nthr; t++) pool.emplace_back(pack_range, nkeys * t / nthr, nkeys * (t + 1) / nthr);
+        pack_range(0, nkeys / nthr);
+        for (auto &th : pool) th.join();
+    }
+    EvalPlan P;
+    int64_t nunits = 0;
+    rc = group_plan(c, prf, count, B->h_descs, B->h_units, &P, &nunits);
+    if (rc) return rc;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
     rc = reserve_device_io(c, key_bytes, out_elems);
     if (!rc) rc = reserve_host_out(c, out_elems);
     if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
-    CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, B->h_descs.ptr, (size_t)ngroups * sizeof(GroupDesc), cudaMemcpyHostToDevice, c->stream));
-    if (units)
-        CUDA_TRY(cudaMemcpyAsync(B->d_units.ptr, B->h_units.ptr, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, c->stream));
+    rc = group_upload_lists(c, P, B->h_descs.ptr, B->h_units.ptr, nunits, c->stream);
+    if (rc) return rc;
     const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, c->stream, true, false,
                     B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
     rc = launch_plan(c, J, P);
@@ -2033,6 +2091,60 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     for (int64_t pos = 0; pos < nkeys; pos++)       /* back to the caller's order */
         std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out.ptr + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
     return B200DPF_OK;
+}
+
+/* The same evaluation from device keys into device results, enqueued on the caller's stream: the host sorts
+ * and plans from the bins alone, a gather kernel packs the keys into bin order (what pack_compact does on the
+ * host path), the evaluation is that of b200dpf_group_eval, and a scatter kernel puts the results back into
+ * the caller's order.  The only host wait is for the previous call's uploads from the pinned staging. */
+int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_t *bins, int64_t nkeys, int prf,
+                              void *out_dev, void *cuda_stream)
+{
+    int rc = check_group_args(c, keys_dev, bins, nkeys, prf, out_dev);
+    if (rc) return rc;
+    if ((reinterpret_cast<uintptr_t>(keys_dev) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_dev) & 3u) != 0)
+        return fail(B200DPF_EINVAL, "keys_dev must be 16-byte aligned and out_dev 4-byte aligned");
+    GroupBins *B = c->bins.get();
+    std::vector<int64_t> count;
+    rc = group_sort(c, nullptr, bins, nkeys, &count);
+    if (rc) return rc;
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!B->ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&B->ev_staged, cudaEventDisableTiming));
+    if (B->staged_pending) {             /* the previous call's uploads read the staging rewritten below */
+        CUDA_TRY(cudaEventSynchronize(B->ev_staged));
+        B->staged_pending = false;
+    }
+    EvalPlan P;
+    int64_t nunits = 0;
+    rc = group_plan(c, prf, count, B->h_descs_dev, B->h_units_dev, &P, &nunits);
+    const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
+    if (!rc) rc = B->h_order.reserve(order_bytes);
+    if (!rc) rc = B->d_order.reserve(order_bytes);
+    if (rc) return rc;
+    for (int64_t pos = 0; pos < nkeys; pos++) {
+        const int64_t b = B->perm[(size_t)pos];
+        B->h_order.ptr[pos] = make_uint2((uint32_t)b, (uint32_t)B->depth[(size_t)bins[b]]);
+    }
+    const KeyLayout kl = compact_layout(c->depth);
+    rc = reserve_device_io(c, (size_t)nkeys * kl.stride_v * 16u, (size_t)nkeys * c->entry_size);
+    if (!rc) rc = wait_last(c, stream);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(B->d_order.ptr, B->h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+    rc = group_upload_lists(c, P, B->h_descs_dev.ptr, B->h_units_dev.ptr, nunits, stream);
+    if (rc) return rc;
+    CUDA_TRY(cudaEventRecord(B->ev_staged, stream));
+    B->staged_pending = true;
+    uint32_t magic = 0;
+    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
+    CUDA_TRY(launch_group_gather(keys_dev, B->d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
+    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
+                    B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
+    rc = launch_plan(c, J, P);
+    if (rc) return rc;
+    CUDA_TRY(launch_group_scatter(c->d_out.ptr, B->d_order.ptr, nkeys, c->entry_size, out_dev, stream));
+    return mark_last(c, stream);
 }
 
 /* ------------------------------------------------------------------------------------------- */

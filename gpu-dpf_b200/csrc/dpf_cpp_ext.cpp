@@ -284,6 +284,21 @@ at::Tensor group_eval(const at::Tensor &keys, const at::Tensor &bins, const std:
     return result;
 }
 
+/* the same from device keys (int32 [nkeys, 524] at keys_ptr) into device results (int32 [nkeys, E] at out_ptr),
+ * enqueued on the stream handle passed as an integer; bins is a CPU int32 tensor [nkeys] (the launch is planned
+ * from it on the host) */
+void group_eval_device(int64_t keys_ptr, const at::Tensor &bins, int64_t nkeys, const std::vector<void *> &buffers, int prf,
+                       int64_t out_ptr, int64_t stream)
+{
+    TORCH_CHECK(bins.device().is_cpu(), "group_eval_device: bins must be a CPU tensor (the host plans the launch from "
+                "them, and reading them from the device would need a synchronisation)");
+    TORCH_CHECK(bins.scalar_type() == at::kInt && bins.dim() == 1 && bins.is_contiguous() && bins.size(0) == nkeys,
+                "group_eval_device: bins must be a contiguous CPU int32 tensor [nkeys]");
+    check(b200dpf_group_eval_device(ctx_of(buffers), reinterpret_cast<const void *>(keys_ptr), bins.data_ptr<int32_t>(), nkeys,
+                                    prf, reinterpret_cast<void *>(out_ptr), reinterpret_cast<void *>(stream)),
+          "group_eval_device");
+}
+
 /* row updates of a live table (b200dpf_update_rows): indices int64 [count] natural, rows int32 [count, E],
  * both CPU tensors; synchronous */
 void update_rows(const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
@@ -532,6 +547,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("group_init_xor", &group_init_xor, "batch PIR for XOR-shared keys (128 rows per leaf, XOR results)",
           py::arg("tables"), py::arg("device") = 0);
     m.def("group_eval", &group_eval, "batch PIR: evaluate (bin, key) pairs in one launch");
+    m.def("group_eval_device", &group_eval_device, "batch PIR from device keys into device results, enqueued on a stream",
+          py::arg("keys_ptr"), py::arg("bins"), py::arg("nkeys"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"),
+          py::arg("stream"));
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),
           py::arg("devices"), py::arg("axis") = 0);
     m.def("update_rows", &update_rows, "table[indices[j]] := rows[j] on a live context (CPU tensors)");

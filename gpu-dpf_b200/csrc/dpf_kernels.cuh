@@ -259,6 +259,17 @@ cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits, int lane_bits,
                                  int cols, int stride, int sm_count, cudaStream_t stream);
 
+/* Device-resident grouped evaluation (dpf_group_io.cu), one warp per key, no host synchronisation.
+ * order[pos] = (the caller's index of the key at bin-sorted position pos, the depth of its bin).
+ *   gather : compact[pos] = the compact form of keys[order[pos].x] (wire format, 131 uint4 each) for a tree
+ *            of depth order[pos].y, with `magic` (the kind's, little-endian) in its header, stride_v uint4
+ *            apart: the bytes pack_compact writes on the host.
+ *   scatter: out[order[pos].x][c] = sorted[pos][c] for c < entry_size (int32 rows). */
+cudaError_t launch_group_gather(const void *keys, const uint2 *order, int64_t nkeys, uint32_t magic, uint32_t stride_v,
+                                void *compact, cudaStream_t stream);
+cudaError_t launch_group_scatter(const int32_t *sorted, const uint2 *order, int64_t nkeys, int entry_size, void *out,
+                                 cudaStream_t stream);
+
 /* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
  * j < count, the last occurrence of a position winning.  Natural index i is row i & (2^lane_bits - 1)
  * of leaf v = i >> lane_bits, and its position is

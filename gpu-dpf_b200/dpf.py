@@ -434,6 +434,33 @@ class BinnedDPF(DPF):
             keys = torch.stack(list(keys))
         return dpf_cpp.group_eval(keys.contiguous(), torch.as_tensor(bins), self.buffers, self.prf_method)
 
+    def eval_gpu_device(self, keys_dev, bins, out_dev=None):
+        """Device-resident, asynchronous variant of eval_gpu: keys_dev int32 [B, 524] CUDA tensor ->
+        int32 [B, entry_size] CUDA tensor (out_dev, if given, is filled), enqueued on the current torch
+        stream.  `bins` (one bin per key) stays on the host: the launch is planned from it without a sync."""
+        if getattr(bins, "is_cuda", False):
+            raise Exception("BinnedDPF.eval_gpu_device: bins must be on the host (a list, array or CPU tensor): the launch is planned from them, "
+                            "and reading them from the device would need a synchronisation")
+        if not (isinstance(keys_dev, torch.Tensor) and keys_dev.is_cuda and keys_dev.dtype == torch.int32
+                and keys_dev.is_contiguous() and keys_dev.dim() == 2 and keys_dev.shape[1] == 524
+                and keys_dev.device.index == self.device):
+            raise Exception("BinnedDPF.eval_gpu_device: keys_dev must be a contiguous int32 [B, 524] tensor on cuda:%d" % self.device)
+        bins = torch.as_tensor(bins)
+        if bins.dim() != 1 or bins.numel() != keys_dev.shape[0] or bins.is_floating_point() or bins.dtype == torch.bool:
+            raise Exception("BinnedDPF.eval_gpu_device: bins must be a 1-D integer tensor with one bin per key")
+        if self.buffers is None:
+            raise Exception("BinnedDPF.eval_gpu_device: must call `eval_init` first")
+        shape = (keys_dev.shape[0], self.table_effective_entry_size)
+        if out_dev is None:
+            out_dev = torch.empty(shape, dtype=torch.int32, device=keys_dev.device)
+        elif not (isinstance(out_dev, torch.Tensor) and out_dev.is_cuda and out_dev.dtype == torch.int32
+                  and out_dev.is_contiguous() and out_dev.device == keys_dev.device and tuple(out_dev.shape) == shape):
+            raise Exception("BinnedDPF.eval_gpu_device: out_dev must be a contiguous int32 [%d, %d] tensor on %s" % (shape + (keys_dev.device,)))
+        stream = torch.cuda.current_stream(keys_dev.device).cuda_stream
+        dpf_cpp.group_eval_device(keys_dev.data_ptr(), bins.to(torch.int32).contiguous(), keys_dev.shape[0], self.buffers,
+                                  self.prf_method, out_dev.data_ptr(), stream)
+        return out_dev
+
     def update_rows(self, bins, indices, rows):
         """Replace rows of live bins: row indices[j] of bin bins[j] := rows[j] (the last occurrence of a
         (bin, index) pair wins); synchronous.  A bin or index out of range raises, and nothing is applied."""

@@ -225,6 +225,37 @@ int b200dpf_group_create_xor(b200dpf_ctx **ctx, const int32_t *const *tables, co
                              int entry_size, int device);
 int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf,
                        int32_t *out);
+
+/*
+ * Device-resident grouped evaluation: the computation of b200dpf_group_eval with keys and results in
+ * device memory on the context's GPU, enqueued on `cuda_stream` (a cudaStream_t; NULL is the default
+ * stream) with no host synchronisation, on every kind of grouped context.
+ *   keys_dev: int32 [nkeys][524] (16-byte aligned), the wire format b200dpf_eval_device takes.
+ *   bins:     int32 [nkeys] in HOST memory.  How many keys each bin has shapes the launch (key groups,
+ *             work-item size, descriptors), so the host plans from the bins; reading them from the device
+ *             would need a synchronisation.  In batch PIR the bin of each key is the layout of the query
+ *             batch, which the server knows without reading the keys.
+ *   out_dev:  int32 [nkeys][entry_size] (4-byte aligned).  out_dev[b] is bit for bit what
+ *             b200dpf_group_eval returns for key b: sums mod 2^32 on standard and early-terminated
+ *             contexts, XORs on XOR-shared ones.
+ * The arguments are checked as by b200dpf_group_eval, before anything is enqueued: a context that is
+ * not grouped is ESTATE; a null buffer, nkeys outside [1, 2^24], an unknown prf, a misaligned buffer or a
+ * bin id outside [0, nbins) is EINVAL.  The keys themselves are NOT validated (as on b200dpf_eval_device):
+ * a key's own header is never used to size or index anything -- its depth comes from its bin -- so a
+ * malformed or wrong-kind key gives a meaningless result for that key, and nothing is read beyond its
+ * 2096 bytes and its bin's table.  Both buffers must stay valid until the stream reaches the end of the
+ * evaluation.
+ * Ordering: the call joins the context's one-operation-in-flight chain (see "Threading" above), so it is
+ * ordered against earlier and later b200dpf_group_eval, b200dpf_group_eval_device and
+ * b200dpf_group_update_rows calls on any stream.
+ * Host staging: the sort order, descriptors and work units go up from pinned buffers the context reuses.
+ * A call never waits for its own work, but before it rewrites that staging it waits on the host until
+ * the PREVIOUS b200dpf_group_eval_device call's uploads (not its kernels) have run.
+ * b200dpf_ctx_last_device_ms times the evaluation launches only (as for b200dpf_group_eval: the key gather
+ * and result scatter are outside), and b200dpf_ctx_last_launches counts them.
+ */
+int b200dpf_group_eval_device(b200dpf_ctx *ctx, const void *keys_dev, const int32_t *bins, int64_t nkeys, int prf,
+                              void *out_dev, void *cuda_stream);
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
 
 /*
@@ -349,7 +380,7 @@ int b200dpf_ctx_entry_size(const b200dpf_ctx *ctx);
 int b200dpf_ctx_device(const b200dpf_ctx *ctx);
 
 /* Device time in milliseconds of the kernels of the most recent b200dpf_eval / _eval_packed /
- * _eval_gather / _group_eval on this context (CUDA events around the launches, copies excluded);
+ * _eval_gather / _group_eval / _group_eval_device on this context (CUDA events around the launches, copies excluded);
  * negative if none. */
 double b200dpf_ctx_last_device_ms(b200dpf_ctx *ctx);
 

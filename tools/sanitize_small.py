@@ -47,4 +47,29 @@ for prf in range(4):
     ga, gb = grp.eval(np.stack(ka), bins, prf), grp.eval(np.stack(kb), bins, prf)
     assert np.array_equal(ga ^ gb, np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
 grp.close()
+# device-resident grouped evaluation, one context per kind: key gather, evaluation and result scatter on a
+# caller's stream, two calls in flight (the second waits for the first's staging uploads only)
+import torch  # noqa: E402
+tables = [rng.randint(-2**31, 2**31, size=(m, 20), dtype=np.int64).astype(np.int32) for m in (256, 4096, 1024)]
+bins = np.array([0, 1, 2, 1, 1, 2, 1] * 7, np.int32)
+alphas = np.array([rng.randint(0, tables[g].shape[0]) for g in bins], np.int64)
+for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b200dpf.gen_batch_et),
+                ({"xor": True}, b200dpf.gen_batch_xor)):
+    grp = b200dpf.GroupContext(tables, **kw)
+    ka, kb = np.zeros((len(bins), 524), np.int32), np.zeros((len(bins), 524), np.int32)
+    for g in range(3):
+        sel = np.nonzero(bins == g)[0]
+        ka[sel], kb[sel] = gen(alphas[sel], tables[g].shape[0], bytes(range(44)) * len(sel), 2)
+    stream = torch.cuda.Stream()
+    keys = [torch.from_numpy(k).cuda() for k in (ka, kb)]
+    outs = [torch.empty((len(bins), 20), dtype=torch.int32, device="cuda") for _ in range(2)]
+    torch.cuda.synchronize()
+    for k, o in zip(keys, outs):
+        grp.eval_device(k.data_ptr(), bins, 2, o.data_ptr(), stream.cuda_stream)
+    stream.synchronize()
+    ga, gb = outs[0].cpu().numpy(), outs[1].cpu().numpy()
+    assert np.array_equal(ga, grp.eval(ka, bins, 2)) and np.array_equal(gb, grp.eval(kb, bins, 2))
+    rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
+    assert np.array_equal(rec, np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
+    grp.close()
 print("sanitize run ok")
