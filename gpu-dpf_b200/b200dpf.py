@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(HERE, "libb200dpf.so")
 KEY_WORDS = 524
 PRF_DUMMY, PRF_SALSA20, PRF_CHACHA20, PRF_AES128 = 0, 1, 2, 3
 PRF_NAMES = {0: "DUMMY", 1: "SALSA20", 2: "CHACHA20", 3: "AES128"}
+KEYS_WIRE, KEYS_COMPACT = 0, 1
 
 # every symbol include/b200dpf.h declares
 SYMBOLS = [
@@ -29,6 +30,7 @@ SYMBOLS = [
     "b200dpf_create_et", "b200dpf_ctx_rows_per_leaf", "b200dpf_group_create_et",
     "b200dpf_gen_xor", "b200dpf_gen_batch_xor", "b200dpf_eval_cpu_xor", "b200dpf_key_pack_xor", "b200dpf_key_unpack_xor",
     "b200dpf_create_xor", "b200dpf_group_create_xor",
+    "b200dpf_group_query_bytes", "b200dpf_group_eval_queries_device",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -77,6 +79,9 @@ def load():
     L.b200dpf_group_eval.argtypes = [C.c_void_p, _i32p, _i32p, C.c_int64, C.c_int, _i32p]
     L.b200dpf_group_eval_device.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
     L.b200dpf_group_bins.argtypes = [C.c_void_p]
+    L.b200dpf_group_query_bytes.argtypes = [C.c_void_p]
+    L.b200dpf_group_query_bytes.restype = C.c_int64
+    L.b200dpf_group_eval_queries_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
     L.b200dpf_ctx_last_device_ms.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_device_ms.restype = C.c_double
     L.b200dpf_ctx_read_timing.argtypes = [C.c_void_p, np.ctypeslib.ndpointer(dtype=np.uint64, flags="C_CONTIGUOUS"), C.c_int,
@@ -426,7 +431,8 @@ class GroupContext(Context):
         sizes = np.array([t.shape[0] for t in self.tables], np.int64)
         ptrs = (C.c_void_p * len(self.tables))(*[t.ctypes.data for t in self.tables])
         self.handle = C.c_void_p()
-        name = "b200dpf_group_create" + ("_xor" if xor else "_et" if early_termination else "")
+        self.kind = "_xor" if xor else "_et" if early_termination else ""
+        name = "b200dpf_group_create" + self.kind
         _check(getattr(lib(), name)(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size, device), name)
 
     @property
@@ -448,6 +454,44 @@ class GroupContext(Context):
         bins = np.ascontiguousarray(bins, np.int32).reshape(-1)
         _check(lib().b200dpf_group_eval_device(self.handle, C.c_void_p(keys_ptr), bins, len(bins), prf,
                                                C.c_void_p(out_ptr), C.c_void_p(stream)), "b200dpf_group_eval_device")
+
+    @property
+    def query_bytes(self):
+        """bytes of one compact query (pack_queries): one compact key per bin, at the bin's depth"""
+        return lib().b200dpf_group_query_bytes(self.handle)
+
+    def eval_queries_device(self, keys_ptr, nqueries, prf, out_ptr, stream=0, compact=False):
+        """batch-PIR queries of one key per bin from device memory into device results (int32 [nqueries, nbins,
+        entry_size] at out_ptr), enqueued on `stream` with no host synchronisation.  keys_ptr holds int32
+        [nqueries, nbins, 524] wire-format keys, or with compact=True uint8 [nqueries, query_bytes] compact
+        queries (pack_queries).  The launch plan depends on nqueries alone and is reused while nqueries, prf
+        and the options stay those of the previous call."""
+        fmt = KEYS_COMPACT if compact else KEYS_WIRE
+        _check(lib().b200dpf_group_eval_queries_device(self.handle, C.c_void_p(keys_ptr), fmt, nqueries, prf,
+                                                       C.c_void_p(out_ptr), C.c_void_p(stream)),
+               "b200dpf_group_eval_queries_device")
+
+    def pack_queries(self, keys):
+        """int32 [Q, nbins, 524] wire-format keys (key g of query q for bin g) -> uint8 [Q, query_bytes] compact
+        queries: each query its keys' compact forms (key_pack of the context's kind) back to back.  A key that
+        is not of the context's kind, or not for its bin's size, raises."""
+        keys = np.ascontiguousarray(keys, np.int32)
+        nbins = len(self.tables)
+        if keys.ndim != 3 or keys.shape[1:] != (nbins, KEY_WORDS):
+            raise ValueError("pack_queries: keys must be int32 [Q, %d, %d], got shape %s" % (nbins, KEY_WORDS, keys.shape))
+        lane_bits = KINDS[self.kind][0]
+        sizes = [lib().b200dpf_key_packed_size(t.shape[0].bit_length() - 1 - lane_bits) for t in self.tables]
+        out = np.empty((keys.shape[0], sum(sizes)), np.uint8)
+        for q in range(keys.shape[0]):
+            off = 0
+            for g, size in enumerate(sizes):
+                packed = _key_pack(self.kind, keys[q, g])
+                if len(packed) != size:
+                    raise ValueError("pack_queries: key %d of query %d is for another bin size (%d packed bytes, bin %d "
+                                     "takes %d)" % (g, q, len(packed), g, size))
+                out[q, off:off + size] = np.frombuffer(packed, np.uint8)
+                off += size
+        return out
 
     def update_rows(self, bins, indices, rows):
         """row indices[j] of bin bins[j] := rows[j] (last occurrence wins); synchronous"""

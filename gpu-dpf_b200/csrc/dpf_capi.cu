@@ -118,6 +118,7 @@ constexpr size_t kKeyBytes = host::KEY_WORDS * sizeof(int32_t);   /* one key in 
 
 struct SmemLayoutCache;   /* per (prf, nv, mode) launch layouts, filled on first use */
 struct MultiState;        /* b200dpf_create_multi: per-device sub-contexts + worker threads */
+struct GroupQueries;      /* b200dpf_group_eval_queries_device: its cached plan and device lists */
 
 struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behind one context */
     std::vector<int64_t> n;
@@ -138,10 +139,8 @@ struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behi
     DeviceBuffer<uint2> d_order;
     cudaEvent_t ev_staged = nullptr;
     bool staged_pending = false;
-    ~GroupBins()
-    {
-        if (ev_staged) cudaEventDestroy(ev_staged);
-    }
+    std::unique_ptr<GroupQueries> queries;   /* made on first use */
+    ~GroupBins();
 };
 
 struct b200dpf_ctx {
@@ -503,6 +502,45 @@ struct EvalPlan {
     /* MAC-only passes: the cp.async.bulk variant or the register-staged one, its grid, position ranges per key group */
     bool mac_tma; int mac_grid; uint32_t mac_ranges;
 };
+
+}  // namespace
+
+/* b200dpf_group_eval_queries_device: Q queries of one key per bin are sorted by bin by a fixed transpose
+ * (sorted position g * Q + q holds key g of query q), so the plan, its device lists and the reordering depend
+ * on Q alone.  They are kept from one call to the next, in lists no other entry point writes, and made again
+ * when Q or the prf changes or an option is set (b200dpf_ctx_set_option and _set_subtree_log2 clear `valid`).
+ * The pinned staging of the lists may still be read by their uploads when a call returns; ev_staged follows
+ * those, and the next new shape waits for it before it rewrites or regrows the staging. */
+struct GroupQueries {
+    bool valid = false;
+    int64_t nq = 0;
+    int prf = -1;
+    EvalPlan P;
+    int64_t nunits = 0;
+    PinnedBuffer<GroupDesc> h_descs;
+    DeviceBuffer<GroupDesc> d_descs;
+    PinnedBuffer<WorkUnit> h_units;
+    DeviceBuffer<WorkUnit> d_units;
+    PinnedBuffer<uint2> h_order;     /* [nq * nbins] (caller's index q * nbins + g, depth of bin g) by sorted position */
+    DeviceBuffer<uint2> d_order;
+    PinnedBuffer<uint2> h_bins;      /* [nbins] (uint4 offset of bin g's key in a compact query, depth of g) */
+    DeviceBuffer<uint2> d_bins;      /* the same on the device, uploaded once with the first plan */
+    bool bins_uploaded = false;
+    uint64_t query_v = 0;            /* uint4 per compact query */
+    cudaEvent_t ev_staged = nullptr;
+    bool staged_pending = false;
+    ~GroupQueries()
+    {
+        if (ev_staged) cudaEventDestroy(ev_staged);
+    }
+};
+
+GroupBins::~GroupBins()
+{
+    if (ev_staged) cudaEventDestroy(ev_staged);
+}
+
+namespace {
 
 /* Work-item size: from s down to s_floor, the first s at which the launch has at least `wanted` items */
 template <class Items> int shrink_s(int s, int s_floor, int64_t wanted, Items items)
@@ -1562,10 +1600,17 @@ int b200dpf_ctx_last_launches(const b200dpf_ctx *c)
     return c->multi ? multi_last_launches(c) : c->last_launches;
 }
 
+/* The plans a grouped context keeps were made under its old options */
+static void options_changed(b200dpf_ctx *c)
+{
+    if (c->bins && c->bins->queries) c->bins->queries->valid = false;
+}
+
 int b200dpf_ctx_set_subtree_log2(b200dpf_ctx *c, int s)
 {
     if (!c || s < 0 || s > 16) return fail(B200DPF_EINVAL, "subtree log2 out of range");
     c->knobs.subtree_log2 = s;
+    options_changed(c);
     return B200DPF_OK;
 }
 
@@ -1577,6 +1622,7 @@ int b200dpf_ctx_set_option(b200dpf_ctx *c, const char *name, int value)
         if (std::strcmp(k.name, name) == 0) {
             if (value < k.lo || value > k.hi) return fail(B200DPF_EINVAL, "option %s=%d out of range [%d,%d]", name, value, k.lo, k.hi);
             c->knobs.*k.field = value;
+            options_changed(c);
             return B200DPF_OK;
         }
     return fail(B200DPF_EINVAL, "unknown option '%s'", name);
@@ -1968,10 +2014,12 @@ static int group_sort(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, 
     return B200DPF_OK;
 }
 
-/* The plan of an evaluation of keys sorted by group_sort, with its key groups' descriptors in h_descs and, for
- * modes that draw work units, its units in h_units (*nunits of them); the device lists grow to match. */
+/* The plan of an evaluation of keys sorted by bin (bin g at positions count[g] .. count[g + 1]), with its key
+ * groups' descriptors in h_descs and, for modes that draw work units, its units in h_units (*nunits of them);
+ * the device lists d_descs and d_units grow to match. */
 static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, PinnedBuffer<GroupDesc> &h_descs,
-                      PinnedBuffer<WorkUnit> &h_units, EvalPlan *out, int64_t *nunits_out)
+                      PinnedBuffer<WorkUnit> &h_units, DeviceBuffer<GroupDesc> &d_descs, DeviceBuffer<WorkUnit> &d_units,
+                      EvalPlan *out, int64_t *nunits_out)
 {
     GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
@@ -1981,7 +2029,7 @@ static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
     const int64_t ngroups = P.key_groups;
     const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
     rc = h_descs.reserve(descs_bytes);
-    if (!rc) rc = B->d_descs.reserve(descs_bytes);
+    if (!rc) rc = d_descs.reserve(descs_bytes);
     if (rc) return rc;
     {
         int64_t gi = 0;
@@ -2013,7 +2061,7 @@ static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
         for (int64_t gi = 0; gi < ngroups; gi++) nunits += (h_descs.ptr[gi].nsub + per_unit - 1) / per_unit;
         const size_t units_bytes = std::max<size_t>((size_t)nunits, 1024) * sizeof(WorkUnit);
         rc = h_units.reserve(units_bytes);
-        if (!rc) rc = B->d_units.reserve(units_bytes);
+        if (!rc) rc = d_units.reserve(units_bytes);
         if (rc) return rc;
         WorkUnit *w = h_units.ptr;
         for (int64_t gi = 0; gi < ngroups; gi++) {
@@ -2029,13 +2077,12 @@ static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
 }
 
 /* Upload the descriptors and units of plan P (group_plan) into the device lists, on `stream`. */
-static int group_upload_lists(b200dpf_ctx *c, const EvalPlan &P, const GroupDesc *h_descs, const WorkUnit *h_units,
-                              int64_t nunits, cudaStream_t stream)
+static int group_upload_lists(const EvalPlan &P, const GroupDesc *h_descs, const WorkUnit *h_units, int64_t nunits,
+                              GroupDesc *d_descs, WorkUnit *d_units, cudaStream_t stream)
 {
-    GroupBins *B = c->bins.get();
-    CUDA_TRY(cudaMemcpyAsync(B->d_descs.ptr, h_descs, (size_t)P.key_groups * sizeof(GroupDesc), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(d_descs, h_descs, (size_t)P.key_groups * sizeof(GroupDesc), cudaMemcpyHostToDevice, stream));
     if (mode_traits(P.mode).units)
-        CUDA_TRY(cudaMemcpyAsync(B->d_units.ptr, h_units, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(d_units, h_units, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, stream));
     return B200DPF_OK;
 }
 
@@ -2073,7 +2120,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     }
     EvalPlan P;
     int64_t nunits = 0;
-    rc = group_plan(c, prf, count, B->h_descs, B->h_units, &P, &nunits);
+    rc = group_plan(c, prf, count, B->h_descs, B->h_units, B->d_descs, B->d_units, &P, &nunits);
     if (rc) return rc;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
     rc = reserve_device_io(c, key_bytes, out_elems);
@@ -2081,7 +2128,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = group_upload_lists(c, P, B->h_descs.ptr, B->h_units.ptr, nunits, c->stream);
+    rc = group_upload_lists(P, B->h_descs.ptr, B->h_units.ptr, nunits, B->d_descs.ptr, B->d_units.ptr, c->stream);
     if (rc) return rc;
     const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, c->stream, true, false,
                     B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
@@ -2118,7 +2165,7 @@ int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_
     }
     EvalPlan P;
     int64_t nunits = 0;
-    rc = group_plan(c, prf, count, B->h_descs_dev, B->h_units_dev, &P, &nunits);
+    rc = group_plan(c, prf, count, B->h_descs_dev, B->h_units_dev, B->d_descs, B->d_units, &P, &nunits);
     const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
     if (!rc) rc = B->h_order.reserve(order_bytes);
     if (!rc) rc = B->d_order.reserve(order_bytes);
@@ -2132,7 +2179,7 @@ int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_
     if (!rc) rc = wait_last(c, stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(B->d_order.ptr, B->h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-    rc = group_upload_lists(c, P, B->h_descs_dev.ptr, B->h_units_dev.ptr, nunits, stream);
+    rc = group_upload_lists(P, B->h_descs_dev.ptr, B->h_units_dev.ptr, nunits, B->d_descs.ptr, B->d_units.ptr, stream);
     if (rc) return rc;
     CUDA_TRY(cudaEventRecord(B->ev_staged, stream));
     B->staged_pending = true;
@@ -2144,6 +2191,109 @@ int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_
     rc = launch_plan(c, J, P);
     if (rc) return rc;
     CUDA_TRY(launch_group_scatter(c->d_out.ptr, B->d_order.ptr, nkeys, c->entry_size, out_dev, stream));
+    return mark_last(c, stream);
+}
+
+int64_t b200dpf_group_query_bytes(const b200dpf_ctx *c)
+{
+    if (!c || !c->bins) return -1;
+    int64_t bytes = 0;
+    for (int d : c->bins->depth) bytes += (int64_t)b200dpf_key_packed_size(d);
+    return bytes;
+}
+
+/* Make the plan of nq queries (one key per bin) in Qs, on the host from nq alone: bin g's keys are sorted
+ * positions g * nq .. (g + 1) * nq.  The staging is rewritten only after the previous plan's uploads ran. */
+static int group_queries_plan(b200dpf_ctx *c, GroupQueries &Qs, int64_t nq, int prf)
+{
+    GroupBins *B = c->bins.get();
+    const int nbins = (int)B->n.size();
+    const int64_t nkeys = nq * nbins;
+    Qs.valid = false;
+    if (!Qs.ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&Qs.ev_staged, cudaEventDisableTiming));
+    if (Qs.staged_pending) {
+        CUDA_TRY(cudaEventSynchronize(Qs.ev_staged));
+        Qs.staged_pending = false;
+    }
+    std::vector<int64_t> count((size_t)nbins + 1);
+    for (int g = 0; g <= nbins; g++) count[(size_t)g] = g * nq;
+    int rc = group_plan(c, prf, count, Qs.h_descs, Qs.h_units, Qs.d_descs, Qs.d_units, &Qs.P, &Qs.nunits);
+    const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
+    if (!rc) rc = Qs.h_order.reserve(order_bytes);
+    if (!rc) rc = Qs.d_order.reserve(order_bytes);
+    if (rc) return rc;
+    for (int g = 0; g < nbins; g++)
+        for (int64_t q = 0; q < nq; q++)
+            Qs.h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->depth[(size_t)g]);
+    if (!Qs.h_bins.ptr) {
+        rc = Qs.h_bins.reserve((size_t)nbins * sizeof(uint2));
+        if (!rc) rc = Qs.d_bins.reserve((size_t)nbins * sizeof(uint2));
+        if (rc) return rc;
+        uint32_t off_v = 0;
+        for (int g = 0; g < nbins; g++) {
+            Qs.h_bins.ptr[g] = make_uint2(off_v, (uint32_t)B->depth[(size_t)g]);
+            off_v += (uint32_t)(b200dpf_key_packed_size(B->depth[(size_t)g]) / 16u);
+        }
+        Qs.query_v = off_v;
+    }
+    return B200DPF_OK;
+}
+
+/* b200dpf_group_eval_device for Q queries of one key per bin: the plan, its device lists and the reordering are
+ * those of the previous call when Q, the prf and the options are (GroupQueries), and a call then only enqueues
+ * the stream wait, the gather, the evaluation and the scatter. */
+int b200dpf_group_eval_queries_device(b200dpf_ctx *c, const void *keys_dev, int key_format, int64_t nqueries, int prf,
+                                      void *out_dev, void *cuda_stream)
+{
+    if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
+    if (!keys_dev || !out_dev) return fail(B200DPF_EINVAL, "null buffer");
+    GroupBins *B = c->bins.get();
+    const int nbins = (int)B->n.size();
+    if (nqueries < 1 || nqueries > ((int64_t)1 << 24) / nbins)
+        return fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24", (long long)nqueries, nbins);
+    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
+    if (key_format != B200DPF_KEYS_WIRE && key_format != B200DPF_KEYS_COMPACT)
+        return fail(B200DPF_EINVAL, "unknown key_format %d", key_format);
+    if ((reinterpret_cast<uintptr_t>(keys_dev) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_dev) & 3u) != 0)
+        return fail(B200DPF_EINVAL, "keys_dev must be 16-byte aligned and out_dev 4-byte aligned");
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!B->queries) B->queries.reset(new (std::nothrow) GroupQueries());
+    if (!B->queries) return fail(B200DPF_ENOMEM, "out of host memory");
+    GroupQueries &Qs = *B->queries;
+    const int64_t nkeys = nqueries * nbins;
+    const bool replan = !Qs.valid || Qs.nq != nqueries || Qs.prf != prf;
+    int rc = replan ? group_queries_plan(c, Qs, nqueries, prf) : B200DPF_OK;
+    const KeyLayout kl = compact_layout(c->depth);
+    if (!rc) rc = reserve_device_io(c, (size_t)nkeys * kl.stride_v * 16u, (size_t)nkeys * c->entry_size);
+    if (!rc) rc = wait_last(c, stream);
+    if (rc) return rc;
+    if (replan) {
+        CUDA_TRY(cudaMemcpyAsync(Qs.d_order.ptr, Qs.h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+        if (!Qs.bins_uploaded)
+            CUDA_TRY(cudaMemcpyAsync(Qs.d_bins.ptr, Qs.h_bins.ptr, (size_t)nbins * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+        Qs.bins_uploaded = true;
+        rc = group_upload_lists(Qs.P, Qs.h_descs.ptr, Qs.h_units.ptr, Qs.nunits, Qs.d_descs.ptr, Qs.d_units.ptr, stream);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(Qs.ev_staged, stream));
+        Qs.staged_pending = true;
+        Qs.nq = nqueries;
+        Qs.prf = prf;
+        Qs.valid = true;
+    }
+    uint32_t magic = 0;
+    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
+    if (key_format == B200DPF_KEYS_WIRE)
+        CUDA_TRY(launch_group_gather(keys_dev, Qs.d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
+    else
+        CUDA_TRY(launch_group_gather_queries(keys_dev, Qs.d_bins.ptr, nkeys, (uint32_t)nqueries, Qs.query_v, magic,
+                                             kl.stride_v, c->d_keys.ptr, stream));
+    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
+                    Qs.d_descs.ptr, Qs.d_units.ptr, (uint32_t)Qs.nunits, true};
+    rc = launch_plan(c, J, Qs.P);
+    if (rc) return rc;
+    CUDA_TRY(launch_group_scatter(c->d_out.ptr, Qs.d_order.ptr, nkeys, c->entry_size, out_dev, stream));
     return mark_last(c, stream);
 }
 

@@ -299,6 +299,18 @@ void group_eval_device(int64_t keys_ptr, const at::Tensor &bins, int64_t nkeys, 
           "group_eval_device");
 }
 
+/* batch-PIR queries of one key per bin (b200dpf_group_eval_queries_device): device keys at keys_ptr, int32
+ * [nqueries, nbins, 524], or with `compact` uint8 [nqueries, group_query_bytes] compact queries, into device
+ * results int32 [nqueries, nbins, E] at out_ptr, enqueued on the stream handle passed as an integer */
+void group_eval_queries_device(int64_t keys_ptr, int64_t nqueries, const std::vector<void *> &buffers, int prf, int64_t out_ptr,
+                               int64_t stream, bool compact)
+{
+    check(b200dpf_group_eval_queries_device(ctx_of(buffers), reinterpret_cast<const void *>(keys_ptr),
+                                            compact ? B200DPF_KEYS_COMPACT : B200DPF_KEYS_WIRE, nqueries, prf,
+                                            reinterpret_cast<void *>(out_ptr), reinterpret_cast<void *>(stream)),
+          "group_eval_queries_device");
+}
+
 /* row updates of a live table (b200dpf_update_rows): indices int64 [count] natural, rows int32 [count, E],
  * both CPU tensors; synchronous */
 void update_rows(const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
@@ -550,6 +562,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("group_eval_device", &group_eval_device, "batch PIR from device keys into device results, enqueued on a stream",
           py::arg("keys_ptr"), py::arg("bins"), py::arg("nkeys"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"),
           py::arg("stream"));
+    m.def("group_eval_queries_device", &group_eval_queries_device,
+          "batch PIR: queries of one key per bin from device memory into device results, enqueued on a stream",
+          py::arg("keys_ptr"), py::arg("nqueries"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"), py::arg("stream"),
+          py::arg("compact") = false);
+    m.def("group_query_bytes", [](const std::vector<void *> &b) { return b200dpf_group_query_bytes(ctx_of(b)); },
+          "bytes of one compact query of a grouped context (one compact key per bin); -1 if not grouped");
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),
           py::arg("devices"), py::arg("axis") = 0);
     m.def("update_rows", &update_rows, "table[indices[j]] := rows[j] on a live context (CPU tensors)");

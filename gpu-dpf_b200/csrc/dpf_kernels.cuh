@@ -269,6 +269,11 @@ cudaError_t launch_group_gather(const void *keys, const uint2 *order, int64_t nk
                                 void *compact, cudaStream_t stream);
 cudaError_t launch_group_scatter(const int32_t *sorted, const uint2 *order, int64_t nkeys, int entry_size, void *out,
                                  cudaStream_t stream);
+/* Queries of one compact key per bin (b200dpf_group_eval_queries_device), nq of them, query_v uint4 each;
+ * bins[g] = (uint4 offset of bin g's key in a query, depth of bin g).  compact[g * nq + q] = key g of query q,
+ * its header rewritten to (magic, depth, 0, 0), stride_v uint4 apart: the bytes pack_compact writes. */
+cudaError_t launch_group_gather_queries(const void *queries, const uint2 *bins, int64_t nkeys, uint32_t nq, uint64_t query_v,
+                                        uint32_t magic, uint32_t stride_v, void *compact, cudaStream_t stream);
 
 /* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
  * j < count, the last occurrence of a position winning.  Natural index i is row i & (2^lane_bits - 1)

@@ -461,6 +461,42 @@ class BinnedDPF(DPF):
                                   self.prf_method, out_dev.data_ptr(), stream)
         return out_dev
 
+    def eval_queries_device(self, keys_dev, out_dev=None):
+        """Batch-PIR queries of one key per bin, device-resident and asynchronous: keys_dev is a CUDA tensor of
+        Q queries, either int32 [Q, nbins, 524] wire-format keys (key g of a query for bin g) or uint8
+        [Q, query_bytes] compact queries (the keys' key_pack forms back to back, dpf_cpp.group_query_bytes
+        bytes); returns int32 [Q, nbins, entry_size] (out_dev, if given, is filled), enqueued on the current
+        torch stream.  The launch plan depends on Q alone and is reused from one call of the same Q to the next."""
+        name = "BinnedDPF.eval_queries_device"
+        if self.buffers is None:
+            raise Exception("%s: must call `eval_init` first" % name)
+        nbins = len(self.bin_sizes)
+        if not (isinstance(keys_dev, torch.Tensor) and keys_dev.is_cuda and keys_dev.is_contiguous()
+                and keys_dev.device.index == self.device and keys_dev.dtype in (torch.int32, torch.uint8)):
+            raise Exception("%s: keys_dev must be a contiguous CUDA tensor on cuda:%d, int32 [Q, %d, 524] or uint8 "
+                            "[Q, query_bytes]" % (name, self.device, nbins))
+        if keys_dev.dtype == torch.int32:
+            compact = False
+            if keys_dev.dim() != 3 or tuple(keys_dev.shape[1:]) != (nbins, 524):
+                raise Exception("%s: int32 keys_dev must be [Q, %d, 524] (one wire-format key per bin per query), got %s"
+                                % (name, nbins, tuple(keys_dev.shape)))
+        else:
+            compact = True
+            qb = dpf_cpp.group_query_bytes(self.buffers)
+            if keys_dev.dim() != 2 or keys_dev.shape[1] != qb:
+                raise Exception("%s: uint8 keys_dev must be [Q, %d] (one compact query per row), got %s"
+                                % (name, qb, tuple(keys_dev.shape)))
+        shape = (keys_dev.shape[0], nbins, self.table_effective_entry_size)
+        if out_dev is None:
+            out_dev = torch.empty(shape, dtype=torch.int32, device=keys_dev.device)
+        elif not (isinstance(out_dev, torch.Tensor) and out_dev.is_cuda and out_dev.dtype == torch.int32
+                  and out_dev.is_contiguous() and out_dev.device == keys_dev.device and tuple(out_dev.shape) == shape):
+            raise Exception("%s: out_dev must be a contiguous int32 [%d, %d, %d] tensor on %s" % ((name,) + shape + (keys_dev.device,)))
+        stream = torch.cuda.current_stream(keys_dev.device).cuda_stream
+        dpf_cpp.group_eval_queries_device(keys_dev.data_ptr(), keys_dev.shape[0], self.buffers, self.prf_method,
+                                          out_dev.data_ptr(), stream, compact)
+        return out_dev
+
     def update_rows(self, bins, indices, rows):
         """Replace rows of live bins: row indices[j] of bin bins[j] := rows[j] (the last occurrence of a
         (bin, index) pair wins); synchronous.  A bin or index out of range raises, and nothing is applied."""

@@ -259,6 +259,45 @@ int b200dpf_group_eval_device(b200dpf_ctx *ctx, const void *keys_dev, const int3
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
 
 /*
+ * Batch-PIR query batches: b200dpf_group_eval_device for the one shape batch PIR uses, where every query
+ * carries exactly one key for every bin (dummy keys for the bins it does not need, so the server learns
+ * nothing from which bins a query uses).  Works on every kind of grouped context.
+ *   keys_dev: nqueries queries, query-major; query q has one key for every bin g = 0 .. nbins-1, in bin
+ *             order, in one of two formats (16-byte aligned either way):
+ *     B200DPF_KEYS_WIRE     int32 [nqueries][nbins][524], the format b200dpf_group_eval_device and
+ *                           b200dpf_gen_batch_gpu use.
+ *     B200DPF_KEYS_COMPACT  uint8 [nqueries][b200dpf_group_query_bytes(ctx)]: a query is its nbins keys back to
+ *                           back, each in its kind's compact form (b200dpf_key_pack, _et or _xor) at its bin's
+ *                           depth d, so b200dpf_key_packed_size(d) bytes -- always a multiple of 16.  These are
+ *                           the bytes the evaluation reads: a key for a 2^10-row bin is 672 bytes of its 2096
+ *                           (early-terminated: 544, XOR-shared: 224).
+ *   out_dev:  int32 [nqueries][nbins][entry_size] (4-byte aligned).  out_dev[q][g] is bit for bit what
+ *             b200dpf_group_eval_device (and so b200dpf_group_eval) returns for the same keys with bins =
+ *             0, 1, .., nbins-1 repeated nqueries times: sums mod 2^32, or XORs on XOR-shared contexts.
+ * The arguments are checked before anything is enqueued: a context that is not grouped is ESTATE; a null
+ * buffer, nqueries < 1, nqueries * nbins > 2^24, an unknown prf or key_format, or a misaligned buffer is EINVAL.
+ * The keys are NOT validated, as on b200dpf_group_eval_device: a key's depth comes from its bin, never from its
+ * header (a compact key's magic and depth bytes are ignored too), and nothing is read beyond the key's own bytes.
+ * Both buffers must stay valid until the stream reaches the end of the evaluation.
+ * Ordering: the call joins the context's one-operation-in-flight chain (see "Threading" above), so it is
+ * ordered against every other grouped evaluation and row update of the context, on any stream.
+ * Cached plan: with one key per bin per query, the sort by bin is a fixed transpose and the whole launch plan
+ * depends on nqueries alone.  It is made on the host in O(nbins + key groups + work units), kept on the device
+ * in lists only this entry point uses, and reused while nqueries, prf and the context's options
+ * (b200dpf_ctx_set_option, b200dpf_ctx_set_subtree_log2) stay those of its previous call.  Such a call uploads
+ * nothing and never waits on the host: it only enqueues a stream wait, the key gather, the evaluation and the
+ * result scatter.  A call with a new shape plans again and uploads the plan from pinned staging; before it
+ * rewrites that staging it waits on the host until the previous new shape's uploads (not its kernels) have run.
+ * b200dpf_ctx_last_device_ms times the evaluation launches only (the gather and scatter are outside), and
+ * b200dpf_ctx_last_launches counts them.
+ * b200dpf_group_query_bytes: the size of one compact query; -1 on a null or non-grouped context.
+ */
+enum { B200DPF_KEYS_WIRE = 0, B200DPF_KEYS_COMPACT = 1 };
+int64_t b200dpf_group_query_bytes(const b200dpf_ctx *ctx);
+int b200dpf_group_eval_queries_device(b200dpf_ctx *ctx, const void *keys_dev, int key_format, int64_t nqueries,
+                                      int prf, void *out_dev, void *cuda_stream);
+
+/*
  * Row updates of a live table (no counterpart in the reference, whose only way to change a row is a
  * new eval_init).  table[indices[j]] := rows[j] for j = 0 .. count-1, with NATURAL indices (the
  * numbering keys use); rows: int32 [count][entry_size].  Only the touched rows move: nothing else is

@@ -72,4 +72,28 @@ for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b2
     rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
     assert np.array_equal(rec, np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
     grp.close()
+# batch-PIR query batches, one context per kind, wire keys and compact queries: 5 queries of one key per bin,
+# the second call of each format reusing the cached plan
+nq = 5
+qalphas = np.array([[rng.randint(0, t.shape[0]) for t in tables] for _ in range(nq)], np.int64)
+for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b200dpf.gen_batch_et),
+                ({"xor": True}, b200dpf.gen_batch_xor)):
+    grp = b200dpf.GroupContext(tables, **kw)
+    ka, kb = np.zeros((nq, 3, 524), np.int32), np.zeros((nq, 3, 524), np.int32)
+    for g in range(3):
+        ka[:, g], kb[:, g] = gen(qalphas[:, g], tables[g].shape[0], bytes(range(44)) * nq, 2)
+    tiled = np.tile(np.arange(3, dtype=np.int32), nq)
+    for compact in (False, True):
+        keys = [torch.from_numpy(grp.pack_queries(k) if compact else k).cuda() for k in (ka, kb)]
+        outs = [torch.empty((nq, 3, 20), dtype=torch.int32, device="cuda") for _ in range(2)]
+        torch.cuda.synchronize()
+        for k, o in zip(keys, outs):
+            grp.eval_queries_device(k.data_ptr(), nq, 2, o.data_ptr(), stream.cuda_stream, compact=compact)
+        stream.synchronize()
+        ga, gb = outs[0].cpu().numpy().reshape(-1, 20), outs[1].cpu().numpy().reshape(-1, 20)
+        assert np.array_equal(ga, grp.eval(ka.reshape(-1, 524), tiled, 2))
+        assert np.array_equal(gb, grp.eval(kb.reshape(-1, 524), tiled, 2))
+        rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
+        assert np.array_equal(rec, np.stack([tables[g][al] for g, al in zip(tiled, qalphas.reshape(-1))]))
+    grp.close()
 print("sanitize run ok")
