@@ -26,6 +26,18 @@ for n, entry in ((512, 16), (2048, 40)):
         a2, b2 = ctx.eval(ka2, 1), ctx.eval(kb2, 1)
         assert np.array_equal((a2.astype(np.uint32) - b2.astype(np.uint32)).astype(np.int32), table[alphas])
     ctx.close()
+# one-launch tree-top phase with more key groups (140) than AES blocks (132 on an H100 SXM): blocks take the
+# host's per-block quota of 128-leaf items, then leave the balanced round by __syncthreads_and
+n, nkeys = 256, 140 * 32
+table = rng.randint(-2**31, 2**31, size=(n, 16), dtype=np.int64).astype(np.int32)
+ctx = b200dpf.Context(table)
+for name, value in (("subtree_log2", 1), ("top_log2", 7), ("balance_top", 1), ("one_launch", 1)):
+    ctx.set_option(name, value)
+alphas = rng.randint(0, n, size=nkeys)
+ka, kb = b200dpf.gen_batch(alphas, n, np.arange(nkeys) + 9, 3)
+a, b = ctx.eval(ka, 3), ctx.eval(kb, 3)
+assert np.array_equal((a.astype(np.uint32) - b.astype(np.uint32)).astype(np.int32), table[alphas])
+ctx.close()
 # grouped (batch-PIR) launch
 tables = [rng.randint(-2**31, 2**31, size=(m, 16), dtype=np.int64).astype(np.int32) for m in (256, 1024, 64)]
 grp = b200dpf.GroupContext(tables)
