@@ -31,6 +31,7 @@ SYMBOLS = [
     "b200dpf_gen_xor", "b200dpf_gen_batch_xor", "b200dpf_eval_cpu_xor", "b200dpf_key_pack_xor", "b200dpf_key_unpack_xor",
     "b200dpf_create_xor", "b200dpf_group_create_xor",
     "b200dpf_group_query_bytes", "b200dpf_group_eval_queries_device",
+    "b200dpf_gen_batch_gpu_et", "b200dpf_gen_batch_gpu_xor", "b200dpf_group_gen_queries_device",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -66,7 +67,9 @@ def load():
     for drbg in ("_secure", "_et", "_xor"):   # the ChaCha20-DRBG generators: 44 seed bytes per key
         getattr(L, "b200dpf_gen_batch" + drbg).argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
     L.b200dpf_gen_batch.argtypes = [_i64p, _u32p, C.c_int64, C.c_int64, C.c_int, C.c_int, _i32p, _i32p]
-    L.b200dpf_gen_batch_gpu.argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    for kind in KINDS:
+        getattr(L, "b200dpf_gen_batch_gpu" + kind).argtypes = [_i64p, C.c_char_p, C.c_int64, C.c_int64, C.c_int, C.c_int,
+                                                               C.c_void_p, C.c_void_p]
     L.b200dpf_key_packed_size.argtypes = [C.c_int]
     L.b200dpf_key_packed_size.restype = C.c_size_t
     L.b200dpf_key_n.argtypes = [_i32p]
@@ -82,6 +85,8 @@ def load():
     L.b200dpf_group_query_bytes.argtypes = [C.c_void_p]
     L.b200dpf_group_query_bytes.restype = C.c_int64
     L.b200dpf_group_eval_queries_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
+    L.b200dpf_group_gen_queries_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]
     L.b200dpf_ctx_last_device_ms.argtypes = [C.c_void_p]
     L.b200dpf_ctx_last_device_ms.restype = C.c_double
     L.b200dpf_ctx_read_timing.argtypes = [C.c_void_p, np.ctypeslib.ndpointer(dtype=np.uint64, flags="C_CONTIGUOUS"), C.c_int,
@@ -159,16 +164,21 @@ def gen_batch_secure(alphas, n, seed_bytes, prf, nthreads=0):
 def gen_batch_gpu(alphas, n, seed_bytes, prf, device=0, out_ptrs=None):
     """GPU keygen; same keys as gen_batch_secure for the same seeds.  out_ptrs=(ptr_a, ptr_b): device
     addresses to leave the keys at (int32 [count, 524] each) instead of returning host arrays."""
+    return _gen_batch_gpu("", alphas, n, seed_bytes, prf, device, out_ptrs)
+
+
+def _gen_batch_gpu(kind, alphas, n, seed_bytes, prf, device, out_ptrs):
     alphas = np.ascontiguousarray(alphas, np.int64)
+    name = "b200dpf_gen_batch_gpu" + kind
     assert len(seed_bytes) == 44 * len(alphas)
     if out_ptrs is not None:
-        _check(lib().b200dpf_gen_batch_gpu(alphas, bytes(seed_bytes), len(alphas), n, prf, device,
-                                           C.c_void_p(out_ptrs[0]), C.c_void_p(out_ptrs[1])), "b200dpf_gen_batch_gpu")
+        _check(getattr(lib(), name)(alphas, bytes(seed_bytes), len(alphas), n, prf, device,
+                                    C.c_void_p(out_ptrs[0]), C.c_void_p(out_ptrs[1])), name)
         return None
     a = np.zeros((len(alphas), KEY_WORDS), np.int32)
     b = np.zeros((len(alphas), KEY_WORDS), np.int32)
-    _check(lib().b200dpf_gen_batch_gpu(alphas, bytes(seed_bytes), len(alphas), n, prf, device,
-                                       a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p)), "b200dpf_gen_batch_gpu")
+    _check(getattr(lib(), name)(alphas, bytes(seed_bytes), len(alphas), n, prf, device,
+                                a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p)), name)
     return a, b
 
 
@@ -255,6 +265,11 @@ def gen_batch_et(alphas, n, seed_bytes, prf, nthreads=0):
     return _gen_batch_drbg("_et", alphas, n, seed_bytes, prf, nthreads)
 
 
+def gen_batch_gpu_et(alphas, n, seed_bytes, prf, device=0, out_ptrs=None):
+    """gen_batch_et on a GPU: the same keys for the same seeds; out_ptrs as for gen_batch_gpu"""
+    return _gen_batch_gpu("_et", alphas, n, seed_bytes, prf, device, out_ptrs)
+
+
 def eval_cpu_et(key, prf):
     return _eval_cpu("_et", key, prf)
 
@@ -275,6 +290,11 @@ def gen_xor(alpha, n, seed_bytes, prf):
 def gen_batch_xor(alphas, n, seed_bytes, prf, nthreads=0):
     """seed_bytes: 44 bytes of entropy per key, concatenated"""
     return _gen_batch_drbg("_xor", alphas, n, seed_bytes, prf, nthreads)
+
+
+def gen_batch_gpu_xor(alphas, n, seed_bytes, prf, device=0, out_ptrs=None):
+    """gen_batch_xor on a GPU: the same keys for the same seeds; out_ptrs as for gen_batch_gpu"""
+    return _gen_batch_gpu("_xor", alphas, n, seed_bytes, prf, device, out_ptrs)
 
 
 def eval_cpu_xor(key, prf):
@@ -470,6 +490,19 @@ class GroupContext(Context):
         _check(lib().b200dpf_group_eval_queries_device(self.handle, C.c_void_p(keys_ptr), fmt, nqueries, prf,
                                                        C.c_void_p(out_ptr), C.c_void_p(stream)),
                "b200dpf_group_eval_queries_device")
+
+    def gen_queries_device(self, alphas_ptr, seeds_ptr, nqueries, prf, out_a_ptr, out_b_ptr, stream=0, compact=False):
+        """both servers' batch-PIR queries for eval_queries_device, made on the GPU from device buffers and
+        enqueued on `stream` with no host synchronisation: alphas_ptr int64 [nqueries, nbins] (the row of bin g
+        query q selects, taken mod the bin's size), seeds_ptr uint8 [nqueries, nbins, 44] (entropy from a
+        CSPRNG).  out_a_ptr / out_b_ptr receive int32 [nqueries, nbins, 524] wire-format keys, or with
+        compact=True uint8 [nqueries, query_bytes] compact queries; key (q, g) is gen_batch<kind>'s for the same
+        row, bin size and seed (and pack_queries' bytes of it)."""
+        fmt = KEYS_COMPACT if compact else KEYS_WIRE
+        _check(lib().b200dpf_group_gen_queries_device(self.handle, C.c_void_p(alphas_ptr), C.c_void_p(seeds_ptr), nqueries,
+                                                      prf, fmt, C.c_void_p(out_a_ptr), C.c_void_p(out_b_ptr),
+                                                      C.c_void_p(stream)),
+               "b200dpf_group_gen_queries_device")
 
     def pack_queries(self, keys):
         """int32 [Q, nbins, 524] wire-format keys (key g of query q for bin g) -> uint8 [Q, query_bytes] compact

@@ -523,15 +523,21 @@ struct GroupQueries {
     DeviceBuffer<WorkUnit> d_units;
     PinnedBuffer<uint2> h_order;     /* [nq * nbins] (caller's index q * nbins + g, depth of bin g) by sorted position */
     DeviceBuffer<uint2> d_order;
+    /* The layout of one query, shared with b200dpf_group_gen_queries_device (group_query_bins): made and
+     * uploaded once, by whichever of the two entry points needs it first, and never rewritten.  ev_bins follows
+     * the upload; every stream that reads d_bins or d_te0 waits on it first. */
     PinnedBuffer<uint2> h_bins;      /* [nbins] (uint4 offset of bin g's key in a compact query, depth of g) */
-    DeviceBuffer<uint2> d_bins;      /* the same on the device, uploaded once with the first plan */
-    bool bins_uploaded = false;
+    DeviceBuffer<uint2> d_bins;
+    PinnedBuffer<uint32_t> h_te0;    /* the key generator's AES table (global memory) */
+    DeviceBuffer<uint32_t> d_te0;
+    cudaEvent_t ev_bins = nullptr;   /* non-null once the uploads are enqueued */
     uint64_t query_v = 0;            /* uint4 per compact query */
     cudaEvent_t ev_staged = nullptr;
     bool staged_pending = false;
     ~GroupQueries()
     {
         if (ev_staged) cudaEventDestroy(ev_staged);
+        if (ev_bins) cudaEventDestroy(ev_bins);
     }
 };
 
@@ -1095,6 +1101,54 @@ int gen_batch_drbg(int kind, const char *name, const int64_t *alphas, const uint
     return B200DPF_OK;
 }
 
+/* gen_batch_drbg on a GPU (b200dpf_gen_batch_gpu, _et, _xor): host alphas and seeds, keys to host or device
+ * memory; `cpu_name` is the CPU entry point of the same keys, named when there is no device */
+int gen_batch_gpu_kind(int kind, const char *name, const char *cpu_name, const int64_t *alphas, const uint8_t *seeds44,
+                       int64_t count, int64_t n, int prf, int device, int32_t *keys_a, int32_t *keys_b)
+{
+    const host::KindInfo &k = host::kKinds[kind];
+    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad %s argument", name);
+    if (n < k.n_min || n > k.n_max || (n & (n - 1)) != 0)
+        return fail(B200DPF_EINVAL, "n=%lld must be a power of two in [%lld, 2^%d]", (long long)n, (long long)k.n_min, ilog2(k.n_max));
+    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
+    for (int64_t i = 0; i < count; i++)
+        if (alphas[i] < 0 || alphas[i] >= n) return fail(B200DPF_EINVAL, "%s: alpha[%lld]=%lld out of range", name, (long long)i, (long long)alphas[i]);
+    if (count == 0) return B200DPF_OK;
+    std::optional<DeviceGuard> guard;
+    char hint[64];
+    snprintf(hint, sizeof hint, "use b200dpf_%s on the CPU", cpu_name);
+    int rc = open_device(device, hint, &guard);
+    if (rc) return rc;
+    const size_t key_bytes = (size_t)count * kKeyBytes;
+    DeviceBuffer<int64_t> d_alphas;
+    DeviceBuffer<uint8_t> d_seeds;
+    DeviceBuffer<uint32_t> d_te0;
+    DeviceBuffer<uint4> d_a, d_b;
+    rc = d_alphas.reserve((size_t)count * sizeof(int64_t));
+    if (!rc) rc = d_seeds.reserve((size_t)count * 44);
+    if (!rc) rc = d_te0.reserve(256 * sizeof(uint32_t));
+    if (!rc) rc = d_a.reserve(key_bytes);
+    if (!rc) rc = d_b.reserve(key_bytes);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(d_alphas.ptr, alphas, (size_t)count * sizeof(int64_t), cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(d_seeds.ptr, seeds44, (size_t)count * 44, cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    KeygenParams p{};
+    p.alphas = d_alphas.ptr;
+    p.seeds44 = d_seeds.ptr;
+    p.count = count;
+    p.depth = ilog2(n) - k.lane_bits;
+    p.lane_bits = k.lane_bits;
+    p.te0 = d_te0.ptr;
+    p.out_a = d_a.ptr;
+    p.out_b = d_b.ptr;
+    if (e == cudaSuccess) e = launch_keygen(prf, k.group, p, nullptr);
+    if (e == cudaSuccess) e = cudaMemcpy(keys_a, d_a.ptr, key_bytes, cudaMemcpyDefault);      /* host or device destination */
+    if (e == cudaSuccess) e = cudaMemcpy(keys_b, d_b.ptr, key_bytes, cudaMemcpyDefault);
+    if (e != cudaSuccess) return fail(B200DPF_ECUDA, "%s: %s", name, cudaGetErrorString(e));
+    return B200DPF_OK;
+}
+
 int eval_cpu_kind(int kind, const char *name, const int32_t *key, int prf, int32_t *out)
 {
     if (!key || !out) return fail(B200DPF_EINVAL, "null buffer");
@@ -1194,35 +1248,8 @@ int b200dpf_gen_batch_secure(const int64_t *alphas, const uint8_t *seeds44, int6
 int b200dpf_gen_batch_gpu(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int device,
                           int32_t *keys_a, int32_t *keys_b)
 {
-    if (!alphas || !seeds44 || !keys_a || !keys_b || count < 0) return fail(B200DPF_EINVAL, "bad gen_batch_gpu argument");
-    if (n < 2 || n > ((int64_t)1 << 32) || (n & (n - 1)) != 0) return fail(B200DPF_EINVAL, "n=%lld must be a power of two in [2, 2^32]", (long long)n);
-    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
-    for (int64_t i = 0; i < count; i++)
-        if (alphas[i] < 0 || alphas[i] >= n) return fail(B200DPF_EINVAL, "gen_batch_gpu: alpha[%lld]=%lld out of range", (long long)i, (long long)alphas[i]);
-    if (count == 0) return B200DPF_OK;
-    std::optional<DeviceGuard> guard;
-    int rc = open_device(device, "use b200dpf_gen_batch_secure on the CPU", &guard);
-    if (rc) return rc;
-    const size_t key_bytes = (size_t)count * kKeyBytes;
-    DeviceBuffer<int64_t> d_alphas;
-    DeviceBuffer<uint8_t> d_seeds;
-    DeviceBuffer<uint32_t> d_te0;
-    DeviceBuffer<uint4> d_a, d_b;
-    rc = d_alphas.reserve((size_t)count * sizeof(int64_t));
-    if (!rc) rc = d_seeds.reserve((size_t)count * 44);
-    if (!rc) rc = d_te0.reserve(256 * sizeof(uint32_t));
-    if (!rc) rc = d_a.reserve(key_bytes);
-    if (!rc) rc = d_b.reserve(key_bytes);
-    if (rc) return rc;
-    cudaError_t e = cudaMemcpy(d_alphas.ptr, alphas, (size_t)count * sizeof(int64_t), cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(d_seeds.ptr, seeds44, (size_t)count * 44, cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-        e = launch_keygen(prf, d_alphas.ptr, d_seeds.ptr, count, ilog2(n), (uint64_t)n, d_te0.ptr, d_a.ptr, d_b.ptr, nullptr);
-    if (e == cudaSuccess) e = cudaMemcpy(keys_a, d_a.ptr, key_bytes, cudaMemcpyDefault);      /* host or device destination */
-    if (e == cudaSuccess) e = cudaMemcpy(keys_b, d_b.ptr, key_bytes, cudaMemcpyDefault);
-    if (e != cudaSuccess) return fail(B200DPF_ECUDA, "gen_batch_gpu: %s", cudaGetErrorString(e));
-    return B200DPF_OK;
+    return gen_batch_gpu_kind(host::KIND_STANDARD, "gen_batch_gpu", "gen_batch_secure", alphas, seeds44, count, n, prf, device,
+                              keys_a, keys_b);
 }
 
 int b200dpf_eval_cpu(const int32_t *key, int prf, int32_t *out_n)
@@ -1258,6 +1285,13 @@ int b200dpf_gen_batch_et(const int64_t *alphas, const uint8_t *seeds44, int64_t 
     return gen_batch_drbg(host::KIND_ET, "gen_batch_et", alphas, seeds44, count, n, prf, nthreads, keys_a, keys_b);
 }
 
+int b200dpf_gen_batch_gpu_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int device,
+                             int32_t *keys_a, int32_t *keys_b)
+{
+    return gen_batch_gpu_kind(host::KIND_ET, "gen_batch_gpu_et", "gen_batch_et", alphas, seeds44, count, n, prf, device, keys_a,
+                              keys_b);
+}
+
 int b200dpf_eval_cpu_et(const int32_t *key, int prf, int32_t *out_n)
 {
     return eval_cpu_kind(host::KIND_ET, "eval_cpu_et", key, prf, out_n);
@@ -1284,6 +1318,13 @@ int b200dpf_gen_batch_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t
                           int32_t *keys_a, int32_t *keys_b)
 {
     return gen_batch_drbg(host::KIND_XOR, "gen_batch_xor", alphas, seeds44, count, n, prf, nthreads, keys_a, keys_b);
+}
+
+int b200dpf_gen_batch_gpu_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf, int device,
+                              int32_t *keys_a, int32_t *keys_b)
+{
+    return gen_batch_gpu_kind(host::KIND_XOR, "gen_batch_gpu_xor", "gen_batch_xor", alphas, seeds44, count, n, prf, device, keys_a,
+                              keys_b);
 }
 
 int b200dpf_eval_cpu_xor(const int32_t *key, int prf, uint32_t *bits)
@@ -2225,9 +2266,22 @@ static int group_queries_plan(b200dpf_ctx *c, GroupQueries &Qs, int64_t nq, int 
     for (int g = 0; g < nbins; g++)
         for (int64_t q = 0; q < nq; q++)
             Qs.h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->depth[(size_t)g]);
-    if (!Qs.h_bins.ptr) {
-        rc = Qs.h_bins.reserve((size_t)nbins * sizeof(uint2));
+    return B200DPF_OK;
+}
+
+/* The query layout of GroupQueries (h_bins / d_bins, query_v) and the generator's AES table, for a call about to
+ * read them on `stream`.  The first such call on the context makes them, enqueues their uploads on its stream and
+ * records ev_bins after them; every call, that one included, makes its stream wait on ev_bins, so a stream that is not
+ * the uploader's never reads the tables before they are complete. */
+static int group_query_bins(b200dpf_ctx *c, GroupQueries &Qs, cudaStream_t stream)
+{
+    if (!Qs.ev_bins) {
+        const GroupBins *B = c->bins.get();
+        const int nbins = (int)B->n.size();
+        int rc = Qs.h_bins.reserve((size_t)nbins * sizeof(uint2));
         if (!rc) rc = Qs.d_bins.reserve((size_t)nbins * sizeof(uint2));
+        if (!rc) rc = Qs.h_te0.reserve(256 * sizeof(uint32_t));
+        if (!rc) rc = Qs.d_te0.reserve(256 * sizeof(uint32_t));
         if (rc) return rc;
         uint32_t off_v = 0;
         for (int g = 0; g < nbins; g++) {
@@ -2235,7 +2289,19 @@ static int group_queries_plan(b200dpf_ctx *c, GroupQueries &Qs, int64_t nq, int 
             off_v += (uint32_t)(b200dpf_key_packed_size(B->depth[(size_t)g]) / 16u);
         }
         Qs.query_v = off_v;
+        std::memcpy(Qs.h_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t));
+        cudaEvent_t ev = nullptr;
+        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        cudaError_t e = cudaMemcpyAsync(Qs.d_bins.ptr, Qs.h_bins.ptr, (size_t)nbins * sizeof(uint2), cudaMemcpyHostToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(Qs.d_te0.ptr, Qs.h_te0.ptr, 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, stream);
+        if (e == cudaSuccess) e = cudaEventRecord(ev, stream);
+        if (e != cudaSuccess) {
+            cudaEventDestroy(ev);
+            return fail(B200DPF_ECUDA, "query layout upload: %s", cudaGetErrorString(e));
+        }
+        Qs.ev_bins = ev;
     }
+    CUDA_TRY(cudaStreamWaitEvent(stream, Qs.ev_bins, 0));
     return B200DPF_OK;
 }
 
@@ -2271,9 +2337,6 @@ int b200dpf_group_eval_queries_device(b200dpf_ctx *c, const void *keys_dev, int 
     if (rc) return rc;
     if (replan) {
         CUDA_TRY(cudaMemcpyAsync(Qs.d_order.ptr, Qs.h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-        if (!Qs.bins_uploaded)
-            CUDA_TRY(cudaMemcpyAsync(Qs.d_bins.ptr, Qs.h_bins.ptr, (size_t)nbins * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-        Qs.bins_uploaded = true;
         rc = group_upload_lists(Qs.P, Qs.h_descs.ptr, Qs.h_units.ptr, Qs.nunits, Qs.d_descs.ptr, Qs.d_units.ptr, stream);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(Qs.ev_staged, stream));
@@ -2284,17 +2347,64 @@ int b200dpf_group_eval_queries_device(b200dpf_ctx *c, const void *keys_dev, int 
     }
     uint32_t magic = 0;
     std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
-    if (key_format == B200DPF_KEYS_WIRE)
+    if (key_format == B200DPF_KEYS_WIRE) {
         CUDA_TRY(launch_group_gather(keys_dev, Qs.d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
-    else
+    } else {
+        rc = group_query_bins(c, Qs, stream);
+        if (rc) return rc;
         CUDA_TRY(launch_group_gather_queries(keys_dev, Qs.d_bins.ptr, nkeys, (uint32_t)nqueries, Qs.query_v, magic,
                                              kl.stride_v, c->d_keys.ptr, stream));
+    }
     const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
                     Qs.d_descs.ptr, Qs.d_units.ptr, (uint32_t)Qs.nunits, true};
     rc = launch_plan(c, J, Qs.P);
     if (rc) return rc;
     CUDA_TRY(launch_group_scatter(c->d_out.ptr, Qs.d_order.ptr, nkeys, c->entry_size, out_dev, stream));
     return mark_last(c, stream);
+}
+
+/* The client's side of b200dpf_group_eval_queries_device: one keygen launch (one thread per (query, bin) pair,
+ * dpf_keygen.cu) writes both servers' queries.  It reads only the query layout of the context, not its tables,
+ * so it neither joins the one-operation-in-flight chain nor touches the cached plan. */
+int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, const uint8_t *seeds_dev, int64_t nqueries,
+                                     int prf, int key_format, void *out_a_dev, void *out_b_dev, void *cuda_stream)
+{
+    if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
+    if (!alphas_dev || !seeds_dev || !out_a_dev || !out_b_dev) return fail(B200DPF_EINVAL, "null buffer");
+    GroupBins *B = c->bins.get();
+    const int nbins = (int)B->n.size();
+    if (nqueries < 1 || nqueries > ((int64_t)1 << 24) / nbins)
+        return fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24", (long long)nqueries, nbins);
+    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
+    if (key_format != B200DPF_KEYS_WIRE && key_format != B200DPF_KEYS_COMPACT)
+        return fail(B200DPF_EINVAL, "unknown key_format %d", key_format);
+    if (((reinterpret_cast<uintptr_t>(out_a_dev) | reinterpret_cast<uintptr_t>(out_b_dev)) & 15u) != 0)
+        return fail(B200DPF_EINVAL, "out_a_dev and out_b_dev must be 16-byte aligned");
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!B->queries) B->queries.reset(new (std::nothrow) GroupQueries());
+    if (!B->queries) return fail(B200DPF_ENOMEM, "out of host memory");
+    GroupQueries &Qs = *B->queries;
+    const int rc = group_query_bins(c, Qs, stream);
+    if (rc) return rc;
+    const host::KindInfo &k = host::kKinds[c->kind];
+    KeygenParams p{};
+    p.alphas = alphas_dev;
+    p.seeds44 = seeds_dev;
+    p.count = nqueries * nbins;
+    p.lane_bits = k.lane_bits;
+    p.bins = Qs.d_bins.ptr;
+    p.nq = (uint32_t)nqueries;
+    p.nbins = (uint32_t)nbins;
+    p.query_v = Qs.query_v;
+    p.compact = key_format == B200DPF_KEYS_COMPACT;
+    std::memcpy(&p.magic, k.magic, 4);
+    p.te0 = Qs.d_te0.ptr;
+    p.out_a = static_cast<uint4 *>(out_a_dev);
+    p.out_b = static_cast<uint4 *>(out_b_dev);
+    CUDA_TRY(launch_keygen(prf, k.group, p, stream));
+    return B200DPF_OK;
 }
 
 /* ------------------------------------------------------------------------------------------- */

@@ -517,6 +517,31 @@ DPF_HD Seed xor128(const Seed &a, const Seed &b)
  * Every level above the leaves adds in Z/2^128 for all three. */
 enum { GROUP_ADD128 = 0, GROUP_LANES32 = 1, GROUP_XOR128 = 2 };
 
+typedef unsigned __int128 u128;
+
+/* Add and subtract in the level-0 group of a key, on 128-bit values: the key generators' arithmetic
+ * (host::KeyBuilder and the keygen kernel, dpf_keygen.cu).  In (Z/2^32)^4 the lanes do not carry into
+ * each other; in (Z/2)^128 both are XOR. */
+template <int GROUP>
+DPF_HD u128 level0_add(u128 a, u128 b)
+{
+    if (GROUP == GROUP_XOR128) return a ^ b;
+    if (GROUP == GROUP_ADD128) return a + b;
+    u128 r = 0;
+    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)((uint32_t)(a >> (32 * l)) + (uint32_t)(b >> (32 * l))) << (32 * l);
+    return r;
+}
+
+template <int GROUP>
+DPF_HD u128 level0_sub(u128 a, u128 b)
+{
+    if (GROUP == GROUP_XOR128) return a ^ b;
+    if (GROUP == GROUP_ADD128) return a - b;
+    u128 r = 0;
+    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)((uint32_t)(a >> (32 * l)) - (uint32_t)(b >> (32 * l))) << (32 * l);
+    return r;
+}
+
 /* The two leaves (FULL: frontier nodes) below a node of height 1, at local
  * positions pos and pos+1.  GROUP_LANES32 and GROUP_XOR128: each leaf keeps all four
  * words of PRF + level-0 correction word, combined in the level-0 group, and hands them

@@ -311,6 +311,20 @@ void group_eval_queries_device(int64_t keys_ptr, int64_t nqueries, const std::ve
           "group_eval_queries_device");
 }
 
+/* both servers' batch-PIR queries made on the GPU (b200dpf_group_gen_queries_device): alphas int64 [nqueries, nbins]
+ * at alphas_ptr, seeds uint8 [nqueries, nbins, 44] at seeds_ptr, into int32 [nqueries, nbins, 524] wire-format keys
+ * or with `compact` uint8 [nqueries, group_query_bytes] compact queries at out_a_ptr and out_b_ptr, enqueued on the
+ * stream handle passed as an integer */
+void group_gen_queries_device(int64_t alphas_ptr, int64_t seeds_ptr, int64_t nqueries, const std::vector<void *> &buffers,
+                              int prf, int64_t out_a_ptr, int64_t out_b_ptr, int64_t stream, bool compact)
+{
+    check(b200dpf_group_gen_queries_device(ctx_of(buffers), reinterpret_cast<const int64_t *>(alphas_ptr),
+                                           reinterpret_cast<const uint8_t *>(seeds_ptr), nqueries, prf,
+                                           compact ? B200DPF_KEYS_COMPACT : B200DPF_KEYS_WIRE, reinterpret_cast<void *>(out_a_ptr),
+                                           reinterpret_cast<void *>(out_b_ptr), reinterpret_cast<void *>(stream)),
+          "group_gen_queries_device");
+}
+
 /* row updates of a live table (b200dpf_update_rows): indices int64 [count] natural, rows int32 [count, E],
  * both CPU tensors; synchronous */
 void update_rows(const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
@@ -566,6 +580,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
           "batch PIR: queries of one key per bin from device memory into device results, enqueued on a stream",
           py::arg("keys_ptr"), py::arg("nqueries"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"), py::arg("stream"),
           py::arg("compact") = false);
+    m.def("group_gen_queries_device", &group_gen_queries_device,
+          "batch PIR: both servers' queries of one key per bin made on the GPU from device rows and seeds, enqueued on a stream",
+          py::arg("alphas_ptr"), py::arg("seeds_ptr"), py::arg("nqueries"), py::arg("buffers"), py::arg("prf"),
+          py::arg("out_a_ptr"), py::arg("out_b_ptr"), py::arg("stream"), py::arg("compact") = false);
     m.def("group_query_bytes", [](const std::vector<void *> &b) { return b200dpf_group_query_bytes(ctx_of(b)); },
           "bytes of one compact query of a grouped context (one compact key per bin); -1 if not grouped");
     m.def("eval_init_multi", &eval_init_multi, "eval_init over several GPUs of this process", py::arg("table"),

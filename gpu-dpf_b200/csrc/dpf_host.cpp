@@ -138,24 +138,9 @@ u128 random128_odd(Rng &g)
     return k;
 }
 
-/* Lane-wise arithmetic in (Z/2^32)^4: the payload level of an early-terminated key. */
-u128 lanes_add(u128 a, u128 b)
-{
-    u128 r = 0;
-    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)((uint32_t)(a >> (32 * l)) + (uint32_t)(b >> (32 * l))) << (32 * l);
-    return r;
-}
-
-u128 lanes_neg(u128 a)
-{
-    u128 r = 0;
-    for (int l = 0; l < 4; l++) r |= (u128)(uint32_t)(0u - (uint32_t)(a >> (32 * l))) << (32 * l);
-    return r;
-}
-
 /* GROUP (dpf_core.cuh) is the group of flat level 0, where the payload lives: Z/2^128 for standard
  * keys, lane-wise (Z/2^32)^4 for early-terminated keys, (Z/2)^128 for XOR-shared keys, whose add and
- * subtract are both XOR.  Every other level adds in Z/2^128. */
+ * subtract are both XOR (level0_add / level0_sub).  Every other level adds in Z/2^128. */
 template <class Rng, int GROUP = GROUP_ADD128>
 struct KeyBuilder {
     int depth;
@@ -165,18 +150,8 @@ struct KeyBuilder {
     u128 cw1[64], cw2[64];
     u128 root_a, root_b;
 
-    static u128 add0(u128 a, u128 b)
-    {
-        if (GROUP == GROUP_XOR128) return a ^ b;
-        return GROUP == GROUP_LANES32 ? lanes_add(a, b) : a + b;
-    }
-    static u128 sub0(u128 a, u128 b)
-    {
-        if (GROUP == GROUP_XOR128) return a ^ b;
-        return GROUP == GROUP_LANES32 ? lanes_add(a, lanes_neg(b)) : a - b;
-    }
-    u128 add(int L, u128 a, u128 b) const { return L == 0 ? add0(a, b) : a + b; }
-    u128 sub(int L, u128 a, u128 b) const { return L == 0 ? sub0(a, b) : a - b; }
+    u128 add(int L, u128 a, u128 b) const { return L == 0 ? level0_add<GROUP>(a, b) : a + b; }
+    u128 sub(int L, u128 a, u128 b) const { return L == 0 ? level0_sub<GROUP>(a, b) : a - b; }
 
     /* Builds flat level L (domain 2^(depth-L)) for payload `beta` and returns
      * the two servers' seeds on the alpha path just below this level. */

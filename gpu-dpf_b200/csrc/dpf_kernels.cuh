@@ -245,9 +245,25 @@ struct PeerParts {
 cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t words, int sm_count, cudaStream_t stream);
 
 /* Batched key generation on the device (dpf_keygen.cu): one thread per key pair, ChaCha20-DRBG draws
- * from 44 seed bytes per key; keys in the reference wire format, [count][131] 128-bit slots each. */
-cudaError_t launch_keygen(int prf, const int64_t *alphas, const uint8_t *seeds44, int64_t count, int depth, uint64_t n,
-                          const uint32_t *te0, uint4 *keys_a, uint4 *keys_b, cudaStream_t stream);
+ * from 44 seed bytes per key, level 0 in `group` (GROUP_*, the kind's), trees of depth + lane_bits bits of
+ * alpha.  A flat batch (bins == null) makes `count` keys of one depth, alphas[k] and seeds44[44 k], into
+ * [count][131] wire-format slots.  A query batch makes key g of query q at thread k = g * nq + q, from
+ * alphas [nq][nbins] and seeds44 [nq][nbins][44], depth bins[g].y, into the wire format [nq][nbins][131]
+ * or (compact) the b200dpf_key_pack bytes at uint4 offset q * query_v + bins[g].x, magic in the header. */
+struct KeygenParams {
+    const int64_t *alphas;
+    const uint8_t *seeds44;
+    int64_t count;
+    int depth, lane_bits;      /* depth: flat batches only */
+    const uint2 *bins;         /* query batches: [nbins] (uint4 offset of the key in a compact query, depth) */
+    uint32_t nq, nbins;
+    uint64_t query_v;          /* uint4 per compact query */
+    int compact;
+    uint32_t magic;            /* compact: the kind's, little-endian */
+    const uint32_t *te0;       /* AES Te0, 256 words of global memory */
+    uint4 *out_a, *out_b;
+};
+cudaError_t launch_keygen(int prf, int group, const KeygenParams &p, cudaStream_t stream);
 
 /* Maximum dynamic shared memory the evaluation kernel may be given. */
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);

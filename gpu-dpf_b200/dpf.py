@@ -497,6 +497,41 @@ class BinnedDPF(DPF):
                                           out_dev.data_ptr(), stream, compact)
         return out_dev
 
+    def gen_queries_device(self, indices_dev, seeds_dev=None, compact=True):
+        """Both servers' batch-PIR queries, made on the GPU for the queries eval_queries_device takes (a load
+        generator's or a benchmark's client side): indices_dev is an int64 [Q, nbins] CUDA tensor, the row of bin
+        g that query q selects (taken mod the bin's size); seeds_dev a uint8 [Q, nbins, 44] CUDA tensor of key
+        entropy, or None for os.urandom bytes.  Returns two CUDA tensors, uint8 [Q, query_bytes] compact queries
+        (compact=True) or int32 [Q, nbins, 524] wire-format keys, enqueued on the current torch stream; key
+        (q, g) is the one gen_in_bin(g, index, secure=True) makes from the same 44 seed bytes."""
+        name = "BinnedDPF.gen_queries_device"
+        if self.buffers is None:
+            raise Exception("%s: must call `eval_init` first" % name)
+        nbins = len(self.bin_sizes)
+        if not (isinstance(indices_dev, torch.Tensor) and indices_dev.is_cuda and indices_dev.dtype == torch.int64
+                and indices_dev.is_contiguous() and indices_dev.device.index == self.device
+                and indices_dev.dim() == 2 and indices_dev.shape[1] == nbins):
+            raise Exception("%s: indices_dev must be a contiguous int64 [Q, %d] tensor on cuda:%d" % (name, nbins, self.device))
+        nq = indices_dev.shape[0]
+        if seeds_dev is None:
+            seeds_dev = torch.frombuffer(bytearray(os.urandom(44 * nq * nbins)), dtype=torch.uint8).reshape(nq, nbins, 44)
+            seeds_dev = seeds_dev.to(indices_dev.device)
+        elif not (isinstance(seeds_dev, torch.Tensor) and seeds_dev.is_cuda and seeds_dev.dtype == torch.uint8
+                  and seeds_dev.is_contiguous() and seeds_dev.device == indices_dev.device
+                  and tuple(seeds_dev.shape) == (nq, nbins, 44)):
+            raise Exception("%s: seeds_dev must be a contiguous uint8 [%d, %d, 44] tensor on %s"
+                            % (name, nq, nbins, indices_dev.device))
+        if compact:
+            shape, dtype = (nq, dpf_cpp.group_query_bytes(self.buffers)), torch.uint8
+        else:
+            shape, dtype = (nq, nbins, 524), torch.int32
+        out_a = torch.empty(shape, dtype=dtype, device=indices_dev.device)
+        out_b = torch.empty(shape, dtype=dtype, device=indices_dev.device)
+        stream = torch.cuda.current_stream(indices_dev.device).cuda_stream
+        dpf_cpp.group_gen_queries_device(indices_dev.data_ptr(), seeds_dev.data_ptr(), nq, self.buffers, self.prf_method,
+                                         out_a.data_ptr(), out_b.data_ptr(), stream, compact)
+        return out_a, out_b
+
     def update_rows(self, bins, indices, rows):
         """Replace rows of live bins: row indices[j] of bin bins[j] := rows[j] (the last occurrence of a
         (bin, index) pair wins); synchronous.  A bin or index out of range raises, and nothing is applied."""

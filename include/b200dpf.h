@@ -288,6 +288,9 @@ int b200dpf_group_bins(const b200dpf_ctx *ctx);
  * nothing and never waits on the host: it only enqueues a stream wait, the key gather, the evaluation and the
  * result scatter.  A call with a new shape plans again and uploads the plan from pinned staging; before it
  * rewrites that staging it waits on the host until the previous new shape's uploads (not its kernels) have run.
+ * The per-bin layout of a compact query is uploaded once, by the first call of this entry point or of
+ * b200dpf_group_gen_queries_device that needs it, on that call's stream; every later call makes its own stream
+ * wait on that upload (a device-side wait, not a host one).
  * b200dpf_ctx_last_device_ms times the evaluation launches only (the gather and scatter are outside), and
  * b200dpf_ctx_last_launches counts them.
  * b200dpf_group_query_bytes: the size of one compact query; -1 on a null or non-grouped context.
@@ -296,6 +299,33 @@ enum { B200DPF_KEYS_WIRE = 0, B200DPF_KEYS_COMPACT = 1 };
 int64_t b200dpf_group_query_bytes(const b200dpf_ctx *ctx);
 int b200dpf_group_eval_queries_device(b200dpf_ctx *ctx, const void *keys_dev, int key_format, int64_t nqueries,
                                       int prf, void *out_dev, void *cuda_stream);
+
+/*
+ * The client's side of a query batch, on the GPU: both servers' queries for b200dpf_group_eval_queries_device,
+ * made from device-resident rows and seeds.  For load generators and benchmarks; works on every kind of grouped
+ * context, whose kind and bin sizes shape the keys.
+ *   alphas_dev: int64 [nqueries][nbins], the row of bin g that query q selects.  Any int64 is accepted: the key is
+ *               the one for the low log2(n_g) bits of alphas_dev[q][g], i.e. for row alpha mod n_g.
+ *   seeds_dev:  uint8 [nqueries][nbins][44], the entropy of each key (ChaCha20 key || nonce).  A real client
+ *               must take them from a CSPRNG; the keys are only as secret as these bytes.
+ *   out_a_dev, out_b_dev: the two servers' queries in key_format (16-byte aligned): int32 [nqueries][nbins][524]
+ *               (B200DPF_KEYS_WIRE) or uint8 [nqueries][b200dpf_group_query_bytes(ctx)] (B200DPF_KEYS_COMPACT).
+ * Key g of query q is bit for bit what b200dpf_gen_batch (_et, _xor: the context's kind) returns for
+ * (alphas[q][g] mod n_g, n_g, seeds[q][g]), and its compact form that key's b200dpf_key_pack (_et, _xor) bytes,
+ * so the outputs feed b200dpf_group_eval_queries_device unchanged.  A compact output is written only in the
+ * keys' own bytes; a wire key's unused slots are written as zero.
+ * The arguments are checked before anything is enqueued, in the order of b200dpf_group_eval_queries_device: a
+ * context that is not grouped is ESTATE; a null buffer, nqueries < 1, nqueries * nbins > 2^24, an unknown prf or
+ * key_format, or an output that is not 16-byte aligned is EINVAL.
+ * Everything is enqueued on cuda_stream with no host synchronisation.  The call writes only the caller's
+ * outputs: it does not join the context's one-operation-in-flight chain and leaves the cached plan of
+ * b200dpf_group_eval_queries_device alone.  Only the first of the two calls that needs the context's per-bin
+ * query layout uploads it, on its stream; every later call, on any stream, waits on the device for that upload.
+ * All four buffers must stay valid until the stream reaches the end of the call.
+ */
+int b200dpf_group_gen_queries_device(b200dpf_ctx *ctx, const int64_t *alphas_dev, const uint8_t *seeds_dev,
+                                     int64_t nqueries, int prf, int key_format, void *out_a_dev, void *out_b_dev,
+                                     void *cuda_stream);
 
 /*
  * Row updates of a live table (no counterpart in the reference, whose only way to change a row is a
@@ -482,6 +512,11 @@ int b200dpf_gen_et(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_le
 int b200dpf_gen_batch_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
                          int nthreads, int32_t *keys_a, int32_t *keys_b);
 
+/* b200dpf_gen_batch_et on a GPU, with the arguments and contract of b200dpf_gen_batch_gpu: bit-identical keys
+ * for the same seeds, outputs in host or device memory, n and every alpha checked before the device is opened. */
+int b200dpf_gen_batch_gpu_et(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
+                             int device, int32_t *keys_a, int32_t *keys_b);
+
 /* One server's share of every row on the CPU, natural order: out[i], i < n (n read from the key). */
 int b200dpf_eval_cpu_et(const int32_t *key, int prf, int32_t *out_n);
 
@@ -535,6 +570,10 @@ int b200dpf_gen_xor(int64_t alpha, int64_t n, const uint8_t *seed, size_t seed_l
  * 44 bytes; keys_a/keys_b: int32[count][524].  Identical keys for any nthreads. */
 int b200dpf_gen_batch_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
                           int nthreads, int32_t *keys_a, int32_t *keys_b);
+
+/* b200dpf_gen_batch_xor on a GPU, with the arguments and contract of b200dpf_gen_batch_gpu. */
+int b200dpf_gen_batch_gpu_xor(const int64_t *alphas, const uint8_t *seeds44, int64_t count, int64_t n, int prf,
+                              int device, int32_t *keys_a, int32_t *keys_b);
 
 /* One server's share bits of every row on the CPU, packed: bits[n / 32] in natural order, row i = bit
  * (i & 31) of bits[i >> 5] (leaf j gives words 4j .. 4j+3; n read from the key). */

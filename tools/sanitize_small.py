@@ -108,4 +108,27 @@ for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b2
         rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
         assert np.array_equal(rec, np.stack([tables[g][al] for g, al in zip(tiled, qalphas.reshape(-1))]))
     grp.close()
+# query batches generated on the GPU, one context per kind: the first call of the context generates (and uploads
+# the per-bin table), compact queries of the same 5 x 3 pairs as above, evaluated on the same stream
+qseeds = torch.from_numpy(np.frombuffer(bytes(range(44)) * nq * 3, np.uint8).copy()).cuda()
+qalphas_dev = torch.from_numpy(qalphas).cuda()
+for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b200dpf.gen_batch_et),
+                ({"xor": True}, b200dpf.gen_batch_xor)):
+    grp = b200dpf.GroupContext(tables, **kw)
+    qa, qb = [torch.empty(nq * grp.query_bytes, dtype=torch.uint8, device="cuda") for _ in range(2)]
+    outs = [torch.empty((nq, 3, 20), dtype=torch.int32, device="cuda") for _ in range(2)]
+    torch.cuda.synchronize()
+    grp.gen_queries_device(qalphas_dev.data_ptr(), qseeds.data_ptr(), nq, 2, qa.data_ptr(), qb.data_ptr(), stream.cuda_stream,
+                           compact=True)
+    for q, o in zip((qa, qb), outs):
+        grp.eval_queries_device(q.data_ptr(), nq, 2, o.data_ptr(), stream.cuda_stream, compact=True)
+    stream.synchronize()
+    ka = np.zeros((nq, 3, 524), np.int32)
+    for g in range(3):
+        ka[:, g] = gen(qalphas[:, g], tables[g].shape[0], bytes(range(44)) * nq, 2)[0]
+    assert np.array_equal(qa.cpu().numpy().reshape(nq, -1), grp.pack_queries(ka))
+    ga, gb = outs[0].cpu().numpy(), outs[1].cpu().numpy()
+    rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
+    assert np.array_equal(rec, np.stack([np.stack([tables[g][al] for g, al in enumerate(row)]) for row in qalphas]))
+    grp.close()
 print("sanitize run ok")
