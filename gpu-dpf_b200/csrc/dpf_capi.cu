@@ -118,30 +118,7 @@ constexpr size_t kKeyBytes = host::KEY_WORDS * sizeof(int32_t);   /* one key in 
 
 struct SmemLayoutCache;   /* per (prf, nv, mode) launch layouts, filled on first use */
 struct MultiState;        /* b200dpf_create_multi: per-device sub-contexts + worker threads */
-struct GroupQueries;      /* b200dpf_group_eval_queries_device: its cached plan and device lists */
-
-struct GroupBins {            /* b200dpf_group_create: many tables ("bins") behind one context */
-    std::vector<int64_t> n;
-    std::vector<int> depth;
-    std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
-    DeviceBuffer<GroupDesc> d_descs;   /* both hold at least 1,024 descriptors */
-    PinnedBuffer<GroupDesc> h_descs;
-    DeviceBuffer<WorkUnit> d_units;    /* modes that draw work units: the list; both hold at least 1,024 */
-    PinnedBuffer<WorkUnit> h_units;
-    std::vector<int64_t> perm;         /* sorted position -> caller's index, of the last evaluation */
-    DeviceBuffer<uint2> d_bin_info;    /* [nbins] (row_off, depth) for row updates, uploaded on first use */
-    /* b200dpf_group_eval_device: its own pinned staging, whose uploads (on the caller's stream) may still be
-     * pending when the call returns; ev_staged follows them, and the next call waits for it before it
-     * rewrites or regrows any of the three.  d_order: [nkeys] (caller's index, bin depth) by sorted position */
-    PinnedBuffer<GroupDesc> h_descs_dev;
-    PinnedBuffer<WorkUnit> h_units_dev;
-    PinnedBuffer<uint2> h_order;
-    DeviceBuffer<uint2> d_order;
-    cudaEvent_t ev_staged = nullptr;
-    bool staged_pending = false;
-    std::unique_ptr<GroupQueries> queries;   /* made on first use */
-    ~GroupBins();
-};
+struct GroupBins;         /* b200dpf_group_create: many tables ("bins") behind one context */
 
 struct b200dpf_ctx {
     std::unique_ptr<MultiState> multi;   /* non-null: this context only fans out to multi->sub[] */
@@ -503,48 +480,45 @@ struct EvalPlan {
     bool mac_tma; int mac_grid; uint32_t mac_ranges;
 };
 
-}  // namespace
-
-/* b200dpf_group_eval_queries_device: Q queries of one key per bin are sorted by bin by a fixed transpose
- * (sorted position g * Q + q holds key g of query q), so the plan, its device lists and the reordering depend
- * on Q alone.  They are kept from one call to the next, in lists no other entry point writes, and made again
- * when Q or the prf changes or an option is set (b200dpf_ctx_set_option and _set_subtree_log2 clear `valid`).
- * The pinned staging of the lists may still be read by their uploads when a call returns; ev_staged follows
- * those, and the next new shape waits for it before it rewrites or regrows the staging. */
-struct GroupQueries {
-    bool valid = false;
-    int64_t nq = 0;
-    int prf = -1;
+/* The plan of one evaluation on a grouped context and its launch lists, made on the host in pinned staging and
+ * uploaded on the caller's stream.  The uploads may still be pending when the call returns; ev_staged follows
+ * them, and plan() waits for it on the host before it rewrites or regrows the staging. */
+struct GroupLaunch {
     EvalPlan P;
-    int64_t nunits = 0;
-    PinnedBuffer<GroupDesc> h_descs;
+    int64_t nkeys = 0, nunits = 0;
+    PinnedBuffer<GroupDesc> h_descs;   /* the key groups' descriptors; all four lists hold at least 1,024 */
     DeviceBuffer<GroupDesc> d_descs;
-    PinnedBuffer<WorkUnit> h_units;
+    PinnedBuffer<WorkUnit> h_units;    /* modes that draw work units: the list */
     DeviceBuffer<WorkUnit> d_units;
-    PinnedBuffer<uint2> h_order;     /* [nq * nbins] (caller's index q * nbins + g, depth of bin g) by sorted position */
+    PinnedBuffer<uint2> h_order;       /* [nkeys] (caller's index, bin depth) by sorted position */
     DeviceBuffer<uint2> d_order;
-    /* The layout of one query, shared with b200dpf_group_gen_queries_device (group_query_bins): made and
-     * uploaded once, by whichever of the two entry points needs it first, and never rewritten.  ev_bins follows
-     * the upload; every stream that reads d_bins or d_te0 waits on it first. */
-    PinnedBuffer<uint2> h_bins;      /* [nbins] (uint4 offset of bin g's key in a compact query, depth of g) */
-    DeviceBuffer<uint2> d_bins;
-    PinnedBuffer<uint32_t> h_te0;    /* the key generator's AES table (global memory) */
-    DeviceBuffer<uint32_t> d_te0;
-    cudaEvent_t ev_bins = nullptr;   /* non-null once the uploads are enqueued */
-    uint64_t query_v = 0;            /* uint4 per compact query */
     cudaEvent_t ev_staged = nullptr;
     bool staged_pending = false;
-    ~GroupQueries()
-    {
-        if (ev_staged) cudaEventDestroy(ev_staged);
-        if (ev_bins) cudaEventDestroy(ev_bins);
-    }
+    ~GroupLaunch() { if (ev_staged) cudaEventDestroy(ev_staged); }
+    int plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, const int32_t *bins);
+    int upload(cudaStream_t stream, bool order);
 };
 
-GroupBins::~GroupBins()
-{
-    if (ev_staged) cudaEventDestroy(ev_staged);
-}
+}  // namespace
+
+struct GroupBins {
+    std::vector<int64_t> n;
+    std::vector<int> depth;
+    std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
+    /* made at create, never rewritten: [nbins] (row_off, depth) for row updates; [nbins] (uint4 offset of bin g's
+     * key in a compact query, depth of g), with query_v uint4 per query; the key generator's AES table */
+    DeviceBuffer<uint2> d_bin_info;
+    DeviceBuffer<uint2> d_bins;
+    uint64_t query_v = 0;
+    DeviceBuffer<uint32_t> d_te0;
+    GroupLaunch once;                  /* b200dpf_group_eval and _eval_device: planned by every call */
+    /* b200dpf_group_eval_queries_device: kept while nq, the prf and the options stay those of the call that made
+     * it (b200dpf_ctx_set_option and _set_subtree_log2 clear cached_valid) */
+    GroupLaunch cached;
+    int64_t cached_nq = 0;
+    int cached_prf = -1;
+    bool cached_valid = false;
+};
 
 namespace {
 
@@ -1644,7 +1618,7 @@ int b200dpf_ctx_last_launches(const b200dpf_ctx *c)
 /* The plans a grouped context keeps were made under its old options */
 static void options_changed(b200dpf_ctx *c)
 {
-    if (c->bins && c->bins->queries) c->bins->queries->valid = false;
+    if (c->bins) c->bins->cached_valid = false;
 }
 
 int b200dpf_ctx_set_subtree_log2(b200dpf_ctx *c, int s)
@@ -1984,6 +1958,7 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     rc = d_stage.reserve((size_t)n_max * entry_size * sizeof(int32_t));
     if (rc) return rc;
     uint64_t row0 = 0;
+    std::vector<uint2> bin_info, query_bins;
     for (int g = 0; g < nbins; g++) {
         /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows; a
          * leaf's 2^lane_bits rows stay adjacent */
@@ -1991,6 +1966,9 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         B->n.push_back(n[g]);
         B->depth.push_back(depth);
         B->row_off.push_back(row0);
+        bin_info.push_back(make_uint2((uint32_t)row0, (uint32_t)depth));
+        query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)depth));
+        B->query_v += b200dpf_key_packed_size(depth) / 16u;
         CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
         int32_t *dst = c->d_table.ptr + row0 * (uint64_t)c->entry_pad;
         CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, lane_bits, entry_size, c->entry_pad,
@@ -1998,6 +1976,15 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
         row0 += (uint64_t)n[g];
     }
+    const size_t bins_bytes = (size_t)nbins * sizeof(uint2);
+    rc = B->d_bin_info.reserve(bins_bytes);
+    if (!rc) rc = B->d_bins.reserve(bins_bytes);
+    if (!rc) rc = B->d_te0.reserve(256 * sizeof(uint32_t));
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(B->d_bin_info.ptr, bin_info.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(B->d_bins.ptr, query_bins.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(B->d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read them once the context is returned */
     *out = c.release();
     return B200DPF_OK;
 }
@@ -2020,22 +2007,31 @@ int b200dpf_group_create_xor(b200dpf_ctx **out, const int32_t *const *tables, co
     return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_XOR);
 }
 
-/* The argument checks of both grouped evaluations, before anything else */
-static int check_group_args(const b200dpf_ctx *c, const void *keys, const int32_t *bins, int64_t nkeys, int prf, const void *out)
+/* The argument checks every grouped entry point makes first, in this order: the context, its buffers (`bufs`: none
+ * is null), the count (nkeys keys or, with `queries`, nqueries queries of one key per bin), the prf and the
+ * key_format (the evaluations of a key list take wire keys). */
+static int check_group_args(const b200dpf_ctx *c, bool bufs, int64_t count, bool queries, int prf, int key_format)
 {
     if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
-    if (!keys || !bins || !out) return fail(B200DPF_EINVAL, "null buffer");
-    if (nkeys < 1 || nkeys > (int64_t)1 << 24) return fail(B200DPF_EINVAL, "nkeys=%lld out of range", (long long)nkeys);
+    if (!bufs) return fail(B200DPF_EINVAL, "null buffer");
+    const int per_query = queries ? (int)c->bins->n.size() : 1;
+    if (count < 1 || count > ((int64_t)1 << 24) / per_query)
+        return queries ? fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24",
+                              (long long)count, per_query)
+                       : fail(B200DPF_EINVAL, "nkeys=%lld out of range", (long long)count);
     if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
+    if (key_format != B200DPF_KEYS_WIRE && key_format != B200DPF_KEYS_COMPACT)
+        return fail(B200DPF_EINVAL, "unknown key_format %d", key_format);
     return B200DPF_OK;
 }
 
-/* Counting sort of the keys by bin (a key group must not mix bins): the keys of bin g go to sorted positions
- * count[g] .. count[g + 1], in the caller's order, and B->perm maps a sorted position to the caller's index.
- * Every bin id is checked and, given host `keys`, every key, key by key. */
-static int group_sort(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, std::vector<int64_t> *count_out)
+/* The counting sort of the keys by bin (a key group must not mix bins), up to its positions: the keys of bin g go to
+ * sorted positions count[g] .. count[g + 1], in the caller's order (GroupLaunch::plan places them).  Every bin id is
+ * checked and, given host `keys`, every key, key by key. */
+static int group_count(const b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys,
+                       std::vector<int64_t> *count_out)
 {
-    GroupBins *B = c->bins.get();
+    const GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
     std::vector<int64_t> &count = *count_out;
     count.assign((size_t)nbins + 1, 0);
@@ -2049,28 +2045,32 @@ static int group_sort(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, 
         count[(size_t)g + 1]++;
     }
     for (int g = 0; g < nbins; g++) count[(size_t)g + 1] += count[(size_t)g];
-    B->perm.assign((size_t)nkeys, 0);
-    std::vector<int64_t> next(count.begin(), count.end() - 1);
-    for (int64_t b = 0; b < nkeys; b++) B->perm[(size_t)(next[(size_t)bins[b]]++)] = b;
     return B200DPF_OK;
 }
 
-/* The plan of an evaluation of keys sorted by bin (bin g at positions count[g] .. count[g + 1]), with its key
- * groups' descriptors in h_descs and, for modes that draw work units, its units in h_units (*nunits of them);
- * the device lists d_descs and d_units grow to match. */
-static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, PinnedBuffer<GroupDesc> &h_descs,
-                      PinnedBuffer<WorkUnit> &h_units, DeviceBuffer<GroupDesc> &d_descs, DeviceBuffer<WorkUnit> &d_units,
-                      EvalPlan *out, int64_t *nunits_out)
+/* Plan an evaluation of keys sorted by bin (bin g at positions count[g] .. count[g + 1]) into the staging: the key
+ * groups' descriptors, for modes that draw work units their units, and the order list.  The keys come in the
+ * caller's order with key b in bin bins[b] (null: nkeys / nbins queries of one key per bin, key g of query q at
+ * caller's index q * nbins + g, so the sort is a fixed transpose).  The device lists grow to match. */
+int GroupLaunch::plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, const int32_t *bins)
 {
-    GroupBins *B = c->bins.get();
+    const GroupBins *B = c->bins.get();
     const int nbins = (int)B->n.size();
-    EvalPlan &P = *out;
+    if (!ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
+    if (staged_pending) {             /* the previous uploads read the staging rewritten below */
+        CUDA_TRY(cudaEventSynchronize(ev_staged));
+        staged_pending = false;
+    }
     int rc = plan_group_eval(c, prf, count, &P);
     if (rc) return rc;
+    nkeys = count.back();
     const int64_t ngroups = P.key_groups;
     const size_t descs_bytes = std::max<size_t>((size_t)ngroups, 1024) * sizeof(GroupDesc);
+    const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
     rc = h_descs.reserve(descs_bytes);
     if (!rc) rc = d_descs.reserve(descs_bytes);
+    if (!rc) rc = h_order.reserve(order_bytes);
+    if (!rc) rc = d_order.reserve(order_bytes);
     if (rc) return rc;
     {
         int64_t gi = 0;
@@ -2094,7 +2094,7 @@ static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
      * (units per block) unit times: whole-block units unless the launch holds fewer items than the grid
      * has warps, and then about items / blocks per unit, so that every block has work.  A key group with
      * fewer items than its unit size leaves the rest of its unit's warps idle. */
-    int64_t &nunits = *nunits_out = 0;
+    nunits = 0;
     if (mode_traits(P.mode).units) {
         int64_t items = 0;
         for (int64_t gi = 0; gi < ngroups; gi++) items += h_descs.ptr[gi].nsub;
@@ -2114,29 +2114,51 @@ static int group_plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
             }
         }
     }
+    if (bins) {
+        std::vector<int64_t> next(count.begin(), count.end() - 1);
+        for (int64_t b = 0; b < nkeys; b++)
+            h_order.ptr[next[(size_t)bins[b]]++] = make_uint2((uint32_t)b, (uint32_t)B->depth[(size_t)bins[b]]);
+    } else {
+        const int64_t nq = nkeys / nbins;
+        for (int g = 0; g < nbins; g++)
+            for (int64_t q = 0; q < nq; q++)
+                h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->depth[(size_t)g]);
+    }
     return B200DPF_OK;
 }
 
-/* Upload the descriptors and units of plan P (group_plan) into the device lists, on `stream`. */
-static int group_upload_lists(const EvalPlan &P, const GroupDesc *h_descs, const WorkUnit *h_units, int64_t nunits,
-                              GroupDesc *d_descs, WorkUnit *d_units, cudaStream_t stream)
+/* Upload the lists of the last plan on `stream` (the order list only if `order`), then record ev_staged. */
+int GroupLaunch::upload(cudaStream_t stream, bool order)
 {
-    CUDA_TRY(cudaMemcpyAsync(d_descs, h_descs, (size_t)P.key_groups * sizeof(GroupDesc), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(d_descs.ptr, h_descs.ptr, (size_t)P.key_groups * sizeof(GroupDesc), cudaMemcpyHostToDevice, stream));
     if (mode_traits(P.mode).units)
-        CUDA_TRY(cudaMemcpyAsync(d_units, h_units, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(d_units.ptr, h_units.ptr, (size_t)nunits * sizeof(WorkUnit), cudaMemcpyHostToDevice, stream));
+    if (order) CUDA_TRY(cudaMemcpyAsync(d_order.ptr, h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaEventRecord(ev_staged, stream));
+    staged_pending = true;
     return B200DPF_OK;
+}
+
+/* The evaluation by launch L of its keys, sorted by bin and compact in d_keys, into d_out in sorted order */
+static int group_launch(b200dpf_ctx *c, const GroupLaunch &L, int prf, cudaStream_t stream)
+{
+    const EvalJob J{c->d_keys.ptr, compact_layout(c->depth), L.nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
+                    L.d_descs.ptr, L.d_units.ptr, (uint32_t)L.nunits, true};
+    return launch_plan(c, J, L.P);
 }
 
 int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
 {
-    int rc = check_group_args(c, keys, bins, nkeys, prf, out);
+    int rc = check_group_args(c, keys && bins && out, nkeys, false, prf, B200DPF_KEYS_WIRE);
     if (rc) return rc;
-    GroupBins *B = c->bins.get();
     std::vector<int64_t> count;
-    rc = group_sort(c, keys, bins, nkeys, &count);
+    rc = group_count(c, keys, bins, nkeys, &count);
     if (rc) return rc;
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    GroupLaunch &L = c->bins->once;
+    rc = L.plan(c, prf, count, bins);
+    if (rc) return rc;
     /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
      * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
     const KeyLayout kl = compact_layout(c->depth);
@@ -2145,13 +2167,12 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     const size_t key_bytes = (size_t)nkeys * stride;
     rc = reserve_host_keys(c, key_bytes);
     if (rc) return rc;
+    const uint2 *order = L.h_order.ptr;
     {
         uint8_t *stage = reinterpret_cast<uint8_t *>(c->h_keys.ptr);
         auto pack_range = [&](int64_t p0, int64_t p1) {
-            for (int64_t pos = p0; pos < p1; pos++) {
-                const int64_t b = B->perm[(size_t)pos];
-                pack_compact(keys + b * host::KEY_WORDS, stage + (size_t)pos * stride, B->depth[(size_t)bins[b]], magic);
-            }
+            for (int64_t pos = p0; pos < p1; pos++)
+                pack_compact(keys + (size_t)order[pos].x * host::KEY_WORDS, stage + (size_t)pos * stride, (int)order[pos].y, magic);
         };
         const int nthr = (int)std::min<int64_t>(std::min<int64_t>(8, std::max(1u, std::thread::hardware_concurrency())), nkeys / 2048 + 1);
         std::vector<std::thread> pool;
@@ -2159,26 +2180,45 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
         pack_range(0, nkeys / nthr);
         for (auto &th : pool) th.join();
     }
-    EvalPlan P;
-    int64_t nunits = 0;
-    rc = group_plan(c, prf, count, B->h_descs, B->h_units, B->d_descs, B->d_units, &P, &nunits);
-    if (rc) return rc;
     const size_t out_elems = (size_t)nkeys * c->entry_size;
     rc = reserve_device_io(c, key_bytes, out_elems);
     if (!rc) rc = reserve_host_out(c, out_elems);
     if (!rc) rc = wait_last(c, c->stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_keys.ptr, c->h_keys.ptr, key_bytes, cudaMemcpyHostToDevice, c->stream));
-    rc = group_upload_lists(P, B->h_descs.ptr, B->h_units.ptr, nunits, B->d_descs.ptr, B->d_units.ptr, c->stream);
-    if (rc) return rc;
-    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, c->stream, true, false,
-                    B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
-    rc = launch_plan(c, J, P);
+    rc = L.upload(c->stream, false);
+    if (!rc) rc = group_launch(c, L, prf, c->stream);
     if (!rc) rc = download_out(c, c->h_out.ptr, true, out_elems);
     if (rc) return rc;
     for (int64_t pos = 0; pos < nkeys; pos++)       /* back to the caller's order */
-        std::memcpy(out + B->perm[(size_t)pos] * c->entry_size, c->h_out.ptr + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
+        std::memcpy(out + (size_t)order[pos].x * c->entry_size, c->h_out.ptr + pos * c->entry_size, sizeof(int32_t) * (size_t)c->entry_size);
     return B200DPF_OK;
+}
+
+/* The end of both device-resident grouped evaluations, on `stream` and after the context's last operation: launch
+ * L's lists go up if its caller just planned it (`upload`), a gather puts the caller's keys into bin order in
+ * d_keys (wire keys through the order list, compact queries through the per-bin table), the evaluation runs, and
+ * a scatter puts its results back into the caller's order in out_dev. */
+static int group_enqueue(b200dpf_ctx *c, GroupLaunch &L, bool upload, const void *keys_dev, int key_format, int prf,
+                         void *out_dev, cudaStream_t stream)
+{
+    const GroupBins *B = c->bins.get();
+    const KeyLayout kl = compact_layout(c->depth);
+    int rc = reserve_device_io(c, (size_t)L.nkeys * kl.stride_v * 16u, (size_t)L.nkeys * c->entry_size);
+    if (!rc) rc = wait_last(c, stream);
+    if (!rc && upload) rc = L.upload(stream, true);
+    if (rc) return rc;
+    uint32_t magic = 0;
+    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
+    if (key_format == B200DPF_KEYS_WIRE)
+        CUDA_TRY(launch_group_gather(keys_dev, L.d_order.ptr, L.nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
+    else
+        CUDA_TRY(launch_group_gather_queries(keys_dev, B->d_bins.ptr, L.nkeys, (uint32_t)(L.nkeys / (int64_t)B->n.size()),
+                                             B->query_v, magic, kl.stride_v, c->d_keys.ptr, stream));
+    rc = group_launch(c, L, prf, stream);
+    if (rc) return rc;
+    CUDA_TRY(launch_group_scatter(c->d_out.ptr, L.d_order.ptr, L.nkeys, c->entry_size, out_dev, stream));
+    return mark_last(c, stream);
 }
 
 /* The same evaluation from device keys into device results, enqueued on the caller's stream: the host sorts
@@ -2188,222 +2228,84 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
 int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_t *bins, int64_t nkeys, int prf,
                               void *out_dev, void *cuda_stream)
 {
-    int rc = check_group_args(c, keys_dev, bins, nkeys, prf, out_dev);
+    int rc = check_group_args(c, keys_dev && bins && out_dev, nkeys, false, prf, B200DPF_KEYS_WIRE);
     if (rc) return rc;
     if ((reinterpret_cast<uintptr_t>(keys_dev) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_dev) & 3u) != 0)
         return fail(B200DPF_EINVAL, "keys_dev must be 16-byte aligned and out_dev 4-byte aligned");
-    GroupBins *B = c->bins.get();
     std::vector<int64_t> count;
-    rc = group_sort(c, nullptr, bins, nkeys, &count);
+    rc = group_count(c, nullptr, bins, nkeys, &count);
     if (rc) return rc;
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!B->ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&B->ev_staged, cudaEventDisableTiming));
-    if (B->staged_pending) {             /* the previous call's uploads read the staging rewritten below */
-        CUDA_TRY(cudaEventSynchronize(B->ev_staged));
-        B->staged_pending = false;
-    }
-    EvalPlan P;
-    int64_t nunits = 0;
-    rc = group_plan(c, prf, count, B->h_descs_dev, B->h_units_dev, B->d_descs, B->d_units, &P, &nunits);
-    const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
-    if (!rc) rc = B->h_order.reserve(order_bytes);
-    if (!rc) rc = B->d_order.reserve(order_bytes);
-    if (rc) return rc;
-    for (int64_t pos = 0; pos < nkeys; pos++) {
-        const int64_t b = B->perm[(size_t)pos];
-        B->h_order.ptr[pos] = make_uint2((uint32_t)b, (uint32_t)B->depth[(size_t)bins[b]]);
-    }
-    const KeyLayout kl = compact_layout(c->depth);
-    rc = reserve_device_io(c, (size_t)nkeys * kl.stride_v * 16u, (size_t)nkeys * c->entry_size);
-    if (!rc) rc = wait_last(c, stream);
-    if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(B->d_order.ptr, B->h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-    rc = group_upload_lists(P, B->h_descs_dev.ptr, B->h_units_dev.ptr, nunits, B->d_descs.ptr, B->d_units.ptr, stream);
-    if (rc) return rc;
-    CUDA_TRY(cudaEventRecord(B->ev_staged, stream));
-    B->staged_pending = true;
-    uint32_t magic = 0;
-    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
-    CUDA_TRY(launch_group_gather(keys_dev, B->d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
-    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
-                    B->d_descs.ptr, B->d_units.ptr, (uint32_t)nunits, true};
-    rc = launch_plan(c, J, P);
-    if (rc) return rc;
-    CUDA_TRY(launch_group_scatter(c->d_out.ptr, B->d_order.ptr, nkeys, c->entry_size, out_dev, stream));
-    return mark_last(c, stream);
+    GroupLaunch &L = c->bins->once;
+    rc = L.plan(c, prf, count, bins);
+    return rc ? rc : group_enqueue(c, L, true, keys_dev, B200DPF_KEYS_WIRE, prf, out_dev, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 int64_t b200dpf_group_query_bytes(const b200dpf_ctx *c)
 {
-    if (!c || !c->bins) return -1;
-    int64_t bytes = 0;
-    for (int d : c->bins->depth) bytes += (int64_t)b200dpf_key_packed_size(d);
-    return bytes;
-}
-
-/* Make the plan of nq queries (one key per bin) in Qs, on the host from nq alone: bin g's keys are sorted
- * positions g * nq .. (g + 1) * nq.  The staging is rewritten only after the previous plan's uploads ran. */
-static int group_queries_plan(b200dpf_ctx *c, GroupQueries &Qs, int64_t nq, int prf)
-{
-    GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
-    const int64_t nkeys = nq * nbins;
-    Qs.valid = false;
-    if (!Qs.ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&Qs.ev_staged, cudaEventDisableTiming));
-    if (Qs.staged_pending) {
-        CUDA_TRY(cudaEventSynchronize(Qs.ev_staged));
-        Qs.staged_pending = false;
-    }
-    std::vector<int64_t> count((size_t)nbins + 1);
-    for (int g = 0; g <= nbins; g++) count[(size_t)g] = g * nq;
-    int rc = group_plan(c, prf, count, Qs.h_descs, Qs.h_units, Qs.d_descs, Qs.d_units, &Qs.P, &Qs.nunits);
-    const size_t order_bytes = std::max<size_t>((size_t)nkeys, 1024) * sizeof(uint2);
-    if (!rc) rc = Qs.h_order.reserve(order_bytes);
-    if (!rc) rc = Qs.d_order.reserve(order_bytes);
-    if (rc) return rc;
-    for (int g = 0; g < nbins; g++)
-        for (int64_t q = 0; q < nq; q++)
-            Qs.h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->depth[(size_t)g]);
-    return B200DPF_OK;
-}
-
-/* The query layout of GroupQueries (h_bins / d_bins, query_v) and the generator's AES table, for a call about to
- * read them on `stream`.  The first such call on the context makes them, enqueues their uploads on its stream and
- * records ev_bins after them; every call, that one included, makes its stream wait on ev_bins, so a stream that is not
- * the uploader's never reads the tables before they are complete. */
-static int group_query_bins(b200dpf_ctx *c, GroupQueries &Qs, cudaStream_t stream)
-{
-    if (!Qs.ev_bins) {
-        const GroupBins *B = c->bins.get();
-        const int nbins = (int)B->n.size();
-        int rc = Qs.h_bins.reserve((size_t)nbins * sizeof(uint2));
-        if (!rc) rc = Qs.d_bins.reserve((size_t)nbins * sizeof(uint2));
-        if (!rc) rc = Qs.h_te0.reserve(256 * sizeof(uint32_t));
-        if (!rc) rc = Qs.d_te0.reserve(256 * sizeof(uint32_t));
-        if (rc) return rc;
-        uint32_t off_v = 0;
-        for (int g = 0; g < nbins; g++) {
-            Qs.h_bins.ptr[g] = make_uint2(off_v, (uint32_t)B->depth[(size_t)g]);
-            off_v += (uint32_t)(b200dpf_key_packed_size(B->depth[(size_t)g]) / 16u);
-        }
-        Qs.query_v = off_v;
-        std::memcpy(Qs.h_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t));
-        cudaEvent_t ev = nullptr;
-        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        cudaError_t e = cudaMemcpyAsync(Qs.d_bins.ptr, Qs.h_bins.ptr, (size_t)nbins * sizeof(uint2), cudaMemcpyHostToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(Qs.d_te0.ptr, Qs.h_te0.ptr, 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, stream);
-        if (e == cudaSuccess) e = cudaEventRecord(ev, stream);
-        if (e != cudaSuccess) {
-            cudaEventDestroy(ev);
-            return fail(B200DPF_ECUDA, "query layout upload: %s", cudaGetErrorString(e));
-        }
-        Qs.ev_bins = ev;
-    }
-    CUDA_TRY(cudaStreamWaitEvent(stream, Qs.ev_bins, 0));
-    return B200DPF_OK;
+    return c && c->bins ? (int64_t)c->bins->query_v * 16 : -1;
 }
 
 /* b200dpf_group_eval_device for Q queries of one key per bin: the plan, its device lists and the reordering are
- * those of the previous call when Q, the prf and the options are (GroupQueries), and a call then only enqueues
- * the stream wait, the gather, the evaluation and the scatter. */
+ * those of the previous call when Q, the prf and the options are (GroupBins::cached), and a call then only
+ * enqueues the stream wait, the gather, the evaluation and the scatter. */
 int b200dpf_group_eval_queries_device(b200dpf_ctx *c, const void *keys_dev, int key_format, int64_t nqueries, int prf,
                                       void *out_dev, void *cuda_stream)
 {
-    if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
-    if (!keys_dev || !out_dev) return fail(B200DPF_EINVAL, "null buffer");
-    GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
-    if (nqueries < 1 || nqueries > ((int64_t)1 << 24) / nbins)
-        return fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24", (long long)nqueries, nbins);
-    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
-    if (key_format != B200DPF_KEYS_WIRE && key_format != B200DPF_KEYS_COMPACT)
-        return fail(B200DPF_EINVAL, "unknown key_format %d", key_format);
+    int rc = check_group_args(c, keys_dev && out_dev, nqueries, true, prf, key_format);
+    if (rc) return rc;
     if ((reinterpret_cast<uintptr_t>(keys_dev) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_dev) & 3u) != 0)
         return fail(B200DPF_EINVAL, "keys_dev must be 16-byte aligned and out_dev 4-byte aligned");
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!B->queries) B->queries.reset(new (std::nothrow) GroupQueries());
-    if (!B->queries) return fail(B200DPF_ENOMEM, "out of host memory");
-    GroupQueries &Qs = *B->queries;
-    const int64_t nkeys = nqueries * nbins;
-    const bool replan = !Qs.valid || Qs.nq != nqueries || Qs.prf != prf;
-    int rc = replan ? group_queries_plan(c, Qs, nqueries, prf) : B200DPF_OK;
-    const KeyLayout kl = compact_layout(c->depth);
-    if (!rc) rc = reserve_device_io(c, (size_t)nkeys * kl.stride_v * 16u, (size_t)nkeys * c->entry_size);
-    if (!rc) rc = wait_last(c, stream);
-    if (rc) return rc;
+    GroupBins *B = c->bins.get();
+    const bool replan = !B->cached_valid || B->cached_nq != nqueries || B->cached_prf != prf;
     if (replan) {
-        CUDA_TRY(cudaMemcpyAsync(Qs.d_order.ptr, Qs.h_order.ptr, (size_t)nkeys * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-        rc = group_upload_lists(Qs.P, Qs.h_descs.ptr, Qs.h_units.ptr, Qs.nunits, Qs.d_descs.ptr, Qs.d_units.ptr, stream);
-        if (rc) return rc;
-        CUDA_TRY(cudaEventRecord(Qs.ev_staged, stream));
-        Qs.staged_pending = true;
-        Qs.nq = nqueries;
-        Qs.prf = prf;
-        Qs.valid = true;
+        std::vector<int64_t> count(B->n.size() + 1);
+        for (size_t g = 0; g < count.size(); g++) count[g] = (int64_t)g * nqueries;
+        B->cached_valid = false;
+        rc = B->cached.plan(c, prf, count, nullptr);
     }
-    uint32_t magic = 0;
-    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
-    if (key_format == B200DPF_KEYS_WIRE) {
-        CUDA_TRY(launch_group_gather(keys_dev, Qs.d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
-    } else {
-        rc = group_query_bins(c, Qs, stream);
-        if (rc) return rc;
-        CUDA_TRY(launch_group_gather_queries(keys_dev, Qs.d_bins.ptr, nkeys, (uint32_t)nqueries, Qs.query_v, magic,
-                                             kl.stride_v, c->d_keys.ptr, stream));
+    if (!rc) rc = group_enqueue(c, B->cached, replan, keys_dev, key_format, prf, out_dev, reinterpret_cast<cudaStream_t>(cuda_stream));
+    if (!rc && replan) {
+        B->cached_nq = nqueries;
+        B->cached_prf = prf;
+        B->cached_valid = true;
     }
-    const EvalJob J{c->d_keys.ptr, kl, nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
-                    Qs.d_descs.ptr, Qs.d_units.ptr, (uint32_t)Qs.nunits, true};
-    rc = launch_plan(c, J, Qs.P);
-    if (rc) return rc;
-    CUDA_TRY(launch_group_scatter(c->d_out.ptr, Qs.d_order.ptr, nkeys, c->entry_size, out_dev, stream));
-    return mark_last(c, stream);
+    return rc;
 }
 
 /* The client's side of b200dpf_group_eval_queries_device: one keygen launch (one thread per (query, bin) pair,
- * dpf_keygen.cu) writes both servers' queries.  It reads only the query layout of the context, not its tables,
- * so it neither joins the one-operation-in-flight chain nor touches the cached plan. */
+ * dpf_keygen.cu) writes both servers' queries.  It reads only the per-bin tables of the context, not its tables of
+ * rows, so it neither joins the one-operation-in-flight chain nor touches the cached plan. */
 int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, const uint8_t *seeds_dev, int64_t nqueries,
                                      int prf, int key_format, void *out_a_dev, void *out_b_dev, void *cuda_stream)
 {
-    if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
-    if (!alphas_dev || !seeds_dev || !out_a_dev || !out_b_dev) return fail(B200DPF_EINVAL, "null buffer");
-    GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
-    if (nqueries < 1 || nqueries > ((int64_t)1 << 24) / nbins)
-        return fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24", (long long)nqueries, nbins);
-    if (prf < B200DPF_PRF_DUMMY || prf > B200DPF_PRF_AES128) return fail(B200DPF_EINVAL, "unknown prf id %d", prf);
-    if (key_format != B200DPF_KEYS_WIRE && key_format != B200DPF_KEYS_COMPACT)
-        return fail(B200DPF_EINVAL, "unknown key_format %d", key_format);
+    const int rc = check_group_args(c, alphas_dev && seeds_dev && out_a_dev && out_b_dev, nqueries, true, prf, key_format);
+    if (rc) return rc;
     if (((reinterpret_cast<uintptr_t>(out_a_dev) | reinterpret_cast<uintptr_t>(out_b_dev)) & 15u) != 0)
         return fail(B200DPF_EINVAL, "out_a_dev and out_b_dev must be 16-byte aligned");
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!B->queries) B->queries.reset(new (std::nothrow) GroupQueries());
-    if (!B->queries) return fail(B200DPF_ENOMEM, "out of host memory");
-    GroupQueries &Qs = *B->queries;
-    const int rc = group_query_bins(c, Qs, stream);
-    if (rc) return rc;
+    const GroupBins *B = c->bins.get();
+    const int nbins = (int)B->n.size();
     const host::KindInfo &k = host::kKinds[c->kind];
     KeygenParams p{};
     p.alphas = alphas_dev;
     p.seeds44 = seeds_dev;
     p.count = nqueries * nbins;
     p.lane_bits = k.lane_bits;
-    p.bins = Qs.d_bins.ptr;
+    p.bins = B->d_bins.ptr;
     p.nq = (uint32_t)nqueries;
     p.nbins = (uint32_t)nbins;
-    p.query_v = Qs.query_v;
+    p.query_v = B->query_v;
     p.compact = key_format == B200DPF_KEYS_COMPACT;
     std::memcpy(&p.magic, k.magic, 4);
-    p.te0 = Qs.d_te0.ptr;
+    p.te0 = B->d_te0.ptr;
     p.out_a = static_cast<uint4 *>(out_a_dev);
     p.out_b = static_cast<uint4 *>(out_b_dev);
-    CUDA_TRY(launch_keygen(prf, k.group, p, stream));
+    CUDA_TRY(launch_keygen(prf, k.group, p, reinterpret_cast<cudaStream_t>(cuda_stream)));
     return B200DPF_OK;
 }
 
@@ -2601,13 +2503,6 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     if (count == 0) return B200DPF_OK;
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
-    if (!B->d_bin_info.ptr) {
-        std::vector<uint2> info((size_t)nbins);
-        for (int g = 0; g < nbins; g++) info[(size_t)g] = make_uint2((uint32_t)B->row_off[(size_t)g], (uint32_t)B->depth[(size_t)g]);
-        rc = B->d_bin_info.reserve(info.size() * sizeof(uint2));
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpy(B->d_bin_info.ptr, info.data(), info.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    }
     rc = update_host_enqueue(c, indices, bins, rows, count);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(c->stream));

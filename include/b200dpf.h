@@ -248,9 +248,10 @@ int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bin
  * Ordering: the call joins the context's one-operation-in-flight chain (see "Threading" above), so it is
  * ordered against earlier and later b200dpf_group_eval, b200dpf_group_eval_device and
  * b200dpf_group_update_rows calls on any stream.
- * Host staging: the sort order, descriptors and work units go up from pinned buffers the context reuses.
- * A call never waits for its own work, but before it rewrites that staging it waits on the host until
- * the PREVIOUS b200dpf_group_eval_device call's uploads (not its kernels) have run.
+ * Host staging: the sort order, descriptors and work units go up from pinned buffers the context reuses
+ * (b200dpf_group_eval plans into them too). A call never waits for its own work, but before it rewrites that
+ * staging it waits on the host until the PREVIOUS b200dpf_group_eval_device call's uploads (not its kernels)
+ * have run; b200dpf_group_eval waits for them the same way.
  * b200dpf_ctx_last_device_ms times the evaluation launches only (as for b200dpf_group_eval: the key gather
  * and result scatter are outside), and b200dpf_ctx_last_launches counts them.
  */
@@ -288,9 +289,8 @@ int b200dpf_group_bins(const b200dpf_ctx *ctx);
  * nothing and never waits on the host: it only enqueues a stream wait, the key gather, the evaluation and the
  * result scatter.  A call with a new shape plans again and uploads the plan from pinned staging; before it
  * rewrites that staging it waits on the host until the previous new shape's uploads (not its kernels) have run.
- * The per-bin layout of a compact query is uploaded once, by the first call of this entry point or of
- * b200dpf_group_gen_queries_device that needs it, on that call's stream; every later call makes its own stream
- * wait on that upload (a device-side wait, not a host one).
+ * The per-bin layout of a compact query is made and uploaded when the context is created, so no call waits for
+ * it.
  * b200dpf_ctx_last_device_ms times the evaluation launches only (the gather and scatter are outside), and
  * b200dpf_ctx_last_launches counts them.
  * b200dpf_group_query_bytes: the size of one compact query; -1 on a null or non-grouped context.
@@ -319,8 +319,8 @@ int b200dpf_group_eval_queries_device(b200dpf_ctx *ctx, const void *keys_dev, in
  * key_format, or an output that is not 16-byte aligned is EINVAL.
  * Everything is enqueued on cuda_stream with no host synchronisation.  The call writes only the caller's
  * outputs: it does not join the context's one-operation-in-flight chain and leaves the cached plan of
- * b200dpf_group_eval_queries_device alone.  Only the first of the two calls that needs the context's per-bin
- * query layout uploads it, on its stream; every later call, on any stream, waits on the device for that upload.
+ * b200dpf_group_eval_queries_device alone.  The per-bin query layout and the AES table it reads are made when
+ * the context is created, so it never waits, on the host or on the device, for anything of the context.
  * All four buffers must stay valid until the stream reaches the end of the call.
  */
 int b200dpf_group_gen_queries_device(b200dpf_ctx *ctx, const int64_t *alphas_dev, const uint8_t *seeds_dev,
