@@ -131,4 +131,32 @@ for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b2
     rec = ga ^ gb if kw.get("xor") else (ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32)
     assert np.array_equal(rec, np.stack([np.stack([tables[g][al] for g, al in enumerate(row)]) for row in qalphas]))
     grp.close()
+# 4095 columns, one short of the widest entry: the leaf-cache pass and 64 MAC slices by both MAC kernels (the
+# last slice 63 columns wide), an XOR-shared plain context (256 passes of 16 columns), and a grouped context
+n, e = 1024, 4095
+table = rng.randint(-2**31, 2**31, size=(n, e), dtype=np.int64).astype(np.int32)
+alphas = rng.randint(0, n, size=40)
+ka, kb = b200dpf.gen_batch(alphas, n, np.arange(40) + 3, 2)
+ctx = b200dpf.Context(table)
+for mac_tma in (1, 0):
+    ctx.set_option("mac_tma", mac_tma)
+    a, b = ctx.eval(ka, 2), ctx.eval(kb, 2)
+    assert ctx.last_launches == 1 + 64
+    assert np.array_equal((a.astype(np.uint32) - b.astype(np.uint32)).astype(np.int32), table[alphas])
+ctx.close()
+ka, kb = b200dpf.gen_batch_xor(alphas[:5], n, bytes(range(44)) * 5, 3)
+ctx = b200dpf.Context(table, xor=True)
+assert np.array_equal(ctx.eval(ka, 3) ^ ctx.eval(kb, 3), table[alphas[:5]])
+ctx.close()
+tables = [table[:256], table[:64]]
+bins = np.array([0, 1, 1, 0, 1] * 4, np.int32)
+alphas = np.array([rng.randint(0, tables[g].shape[0]) for g in bins], np.int64)
+ka, kb = np.zeros((len(bins), 524), np.int32), np.zeros((len(bins), 524), np.int32)
+for g in range(2):
+    sel = np.nonzero(bins == g)[0]
+    ka[sel], kb[sel] = b200dpf.gen_batch_et(alphas[sel], tables[g].shape[0], bytes(range(44)) * len(sel), 1)
+grp = b200dpf.GroupContext(tables, early_termination=True)
+ga, gb = grp.eval(ka, bins, 1), grp.eval(kb, bins, 1)
+assert np.array_equal((ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32), table[alphas])
+grp.close()
 print("sanitize run ok")
