@@ -62,8 +62,8 @@ def test_gen_secure(oracle):
     assert np.any(cw_top[1:] != 0)
     with pytest.raises(b200dpf.B200DPFError, match="44 bytes"):
         b200dpf.gen_secure(5, 1024, b"short", 3)
-    # RFC 8439 section 2.3.2 keystream block check of the DRBG is implicit in determinism; the
-    # construction's correctness is what matters for the protocol and is checked above.
+    # the exact keys (the DRBG against RFC 8439's vectors, the construction against the reference's keys) are
+    # checked in tests/test_keygen_ref_host.py
 
 
 def test_eval_cpu_matches_golden_and_oracle(oracle, golden):
