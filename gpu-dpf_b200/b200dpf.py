@@ -32,6 +32,8 @@ SYMBOLS = [
     "b200dpf_create_xor", "b200dpf_group_create_xor",
     "b200dpf_group_query_bytes", "b200dpf_group_eval_queries_device",
     "b200dpf_gen_batch_gpu_et", "b200dpf_gen_batch_gpu_xor", "b200dpf_group_gen_queries_device",
+    "b200dpf_trimmed_domain", "b200dpf_trimmed_alpha", "b200dpf_create_trimmed", "b200dpf_group_create_trimmed",
+    "b200dpf_ctx_trimmed", "b200dpf_ctx_table_rows",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -41,6 +43,8 @@ KINDS = {
     "_et": (2, 29, "early-terminated"),
     "_xor": (7, 24, "XOR-shared"),
 }
+# the kind ids of b200dpf_create_trimmed and b200dpf_group_create_trimmed (B200DPF_KIND_*), by suffix
+KIND_IDS = {"": 0, "_et": 1, "_xor": 2}
 
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
 _i64p = np.ctypeslib.ndpointer(dtype=np.int64, flags="C_CONTIGUOUS")
@@ -112,6 +116,15 @@ def load():
     L.b200dpf_ctx_rows_per_leaf.argtypes = [C.c_void_p]
     for kind in ("_et", "_xor"):
         getattr(L, "b200dpf_group_create" + kind).argtypes = L.b200dpf_group_create.argtypes
+    L.b200dpf_trimmed_domain.argtypes = [C.c_int64, C.c_int]
+    L.b200dpf_trimmed_domain.restype = C.c_int64
+    L.b200dpf_trimmed_alpha.argtypes = [C.c_int64, C.c_int64, C.c_int]
+    L.b200dpf_trimmed_alpha.restype = C.c_int64
+    L.b200dpf_create_trimmed.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int]
+    L.b200dpf_group_create_trimmed.argtypes = L.b200dpf_group_create.argtypes + [C.c_int]
+    L.b200dpf_ctx_trimmed.argtypes = [C.c_void_p]
+    L.b200dpf_ctx_table_rows.argtypes = [C.c_void_p]
+    L.b200dpf_ctx_table_rows.restype = C.c_int64
     return L
 
 
@@ -310,13 +323,38 @@ def key_unpack_xor(packed):
     return _key_unpack("_xor", packed)
 
 
+def _kind_id(kind):
+    if kind in KIND_IDS:
+        return KIND_IDS[kind]
+    if kind in KIND_IDS.values():
+        return kind
+    raise ValueError("unknown key kind %r (one of %s or 0, 1, 2)" % (kind, sorted(KIND_IDS)))
+
+
+def trimmed_domain(n, kind=""):
+    """the n of the keys a trimmed table of n rows takes (b200dpf_trimmed_domain); kind: "", "_et", "_xor" or its id"""
+    N = lib().b200dpf_trimmed_domain(int(n), _kind_id(kind))
+    if N < 0:
+        raise ValueError("trimmed_domain: n=%d outside [1, 2^31]" % n)
+    return N
+
+
+def trimmed_alpha(row, n, kind=""):
+    """the key index of row `row` of a trimmed table of n rows (b200dpf_trimmed_alpha)"""
+    a = lib().b200dpf_trimmed_alpha(int(row), int(n), _kind_id(kind))
+    if a < 0:
+        raise ValueError("trimmed_alpha: row %d of n=%d out of range" % (row, n))
+    return a
+
+
 class Context:
     """One table (or one entry-range shard of it) resident on one GPU.  early_termination=True makes a
     context for early-terminated keys (b200dpf_create_et): four table rows per tree leaf.  xor=True makes
     one for XOR-shared keys (b200dpf_create_xor): 128 rows per leaf, and results that XOR (not add) to
-    the selected row."""
+    the selected row.  trimmed=True makes a trimmed context (b200dpf_create_trimmed) of the kind: any number of
+    rows, row r reached by a key for trimmed_alpha(r, n) over trimmed_domain(n) rows, update_rows by row number."""
 
-    def __init__(self, table, device=0, shard_rank=0, shard_count=1, early_termination=False, xor=False):
+    def __init__(self, table, device=0, shard_rank=0, shard_count=1, early_termination=False, xor=False, trimmed=False):
         if xor and early_termination:
             raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
         table = np.ascontiguousarray(table, np.int32)
@@ -324,6 +362,12 @@ class Context:
         self.n, self.entry_size = table.shape
         self.handle = C.c_void_p()
         self.kind = "_xor" if xor else "_et" if early_termination else ""
+        if trimmed:
+            if (shard_rank, shard_count) != (0, 1):
+                raise ValueError("a trimmed context holds the whole table: no shards")
+            _check(lib().b200dpf_create_trimmed(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n,
+                                                self.entry_size, device, KIND_IDS[self.kind]), "b200dpf_create_trimmed")
+            return
         name = "b200dpf_create" + self.kind
         _check(getattr(lib(), name)(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
                                     device, shard_rank, shard_count), name)
@@ -422,6 +466,15 @@ class Context:
     def rows_per_leaf(self):
         return lib().b200dpf_ctx_rows_per_leaf(self.handle)
 
+    @property
+    def trimmed(self):
+        return lib().b200dpf_ctx_trimmed(self.handle) == 1
+
+    @property
+    def table_rows(self):
+        """rows of the device table, padding included (b200dpf_ctx_table_rows)"""
+        return lib().b200dpf_ctx_table_rows(self.handle)
+
     def close(self):
         if self.handle:
             lib().b200dpf_destroy(self.handle)
@@ -439,9 +492,10 @@ class GroupContext(Context):
     (b200dpf_group_create / b200dpf_group_eval).  early_termination=True makes the context for
     early-terminated keys (b200dpf_group_create_et): bins of >= 8 rows, four rows per tree leaf.  xor=True
     makes it for XOR-shared keys (b200dpf_group_create_xor): bins of >= 256 rows, 128 rows per tree leaf,
-    and results that XOR (not add) to the selected row."""
+    and results that XOR (not add) to the selected row.  trimmed=True makes a trimmed grouped context
+    (b200dpf_group_create_trimmed) of the kind: bins of any size, numbered as on a trimmed Context."""
 
-    def __init__(self, tables, device=0, early_termination=False, xor=False):
+    def __init__(self, tables, device=0, early_termination=False, xor=False, trimmed=False):
         if xor and early_termination:
             raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
         self.tables = [np.ascontiguousarray(t, np.int32) for t in tables]
@@ -452,6 +506,11 @@ class GroupContext(Context):
         ptrs = (C.c_void_p * len(self.tables))(*[t.ctypes.data for t in self.tables])
         self.handle = C.c_void_p()
         self.kind = "_xor" if xor else "_et" if early_termination else ""
+        self._trimmed = trimmed        # what pack_queries needs besides the kind and the bin sizes
+        if trimmed:
+            _check(lib().b200dpf_group_create_trimmed(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size,
+                                                      device, KIND_IDS[self.kind]), "b200dpf_group_create_trimmed")
+            return
         name = "b200dpf_group_create" + self.kind
         _check(getattr(lib(), name)(C.byref(self.handle), ptrs, sizes, len(self.tables), self.entry_size, device), name)
 
@@ -513,7 +572,9 @@ class GroupContext(Context):
         if keys.ndim != 3 or keys.shape[1:] != (nbins, KEY_WORDS):
             raise ValueError("pack_queries: keys must be int32 [Q, %d, %d], got shape %s" % (nbins, KEY_WORDS, keys.shape))
         lane_bits = KINDS[self.kind][0]
-        sizes = [lib().b200dpf_key_packed_size(t.shape[0].bit_length() - 1 - lane_bits) for t in self.tables]
+        trimmed = getattr(self, "_trimmed", False)
+        domains = [trimmed_domain(t.shape[0], self.kind) if trimmed else t.shape[0] for t in self.tables]
+        sizes = [lib().b200dpf_key_packed_size(n.bit_length() - 1 - lane_bits) for n in domains]
         out = np.empty((keys.shape[0], sum(sizes)), np.uint8)
         for q in range(keys.shape[0]):
             off = 0

@@ -138,6 +138,11 @@ struct b200dpf_ctx {
      * frontier count leaves. */
     int kind = host::KIND_STANDARD;
     int lane_bits() const { return host::kKinds[kind].lane_bits; }
+    /* trimmed (b200dpf_create_trimmed, b200dpf_group_create_trimmed): row r is device row r, at leaf position
+     * r >> lane_bits of a tree over trimmed_domain(n) rows, and the device table (n_local rows; per bin on a
+     * grouped context) is zero-padded to a multiple of 2^trim_log2 rows only.  n is the live rows. */
+    bool trimmed = false;
+    int trim_log2 = 0;
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
     DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
@@ -396,6 +401,34 @@ constexpr KindOps kKindOps[host::KIND_COUNT] = {
     {MODE_FUSED_XOR, MODE_EXPAND_XOR, MODE_GROUPED_XOR, 4, false, false, 2, 4, "b200dpf_gen_xor"},
 };
 
+/* Trimmed tables (DESIGN.md section 11).  Row r of an n-row table sits at leaf position r >> lane_bits of a tree
+ * over N = trimmed_domain(n) rows (the next power of two, at least the kind's n_min), so the live rows are a
+ * prefix of the leaf positions and the work items past it are never issued.  The device table is padded with
+ * zero rows to a multiple of 2^trim_log2 rows, where one granule is N/128 rows on a large table (the padding is
+ * then below N/128 < n/64) and never less than one work item of the smallest size the launch planner keeps for
+ * the kind: 64 leaves of standard and early-terminated keys, 1 leaf pair of XOR-shared ones (whose leaves are
+ * 128 rows of work).  Every issued item lies inside the padded rows. */
+bool trim_args_ok(int64_t n, int kind) { return kind >= 0 && kind < host::KIND_COUNT && n >= 1 && n <= ((int64_t)1 << 31); }
+
+int64_t trimmed_domain_of(int64_t n, int kind)
+{
+    return std::max<int64_t>((int64_t)1 << ilog2(n), host::kKinds[kind].n_min);
+}
+
+int trim_log2_of(int64_t n, int kind)
+{
+    const int log_n = ilog2(trimmed_domain_of(n, kind));
+    const int item_leaves_log2 = kKindOps[kind].leaf_items ? 1 : 6;
+    return std::min(log_n, std::max(log_n - 7, host::kKinds[kind].lane_bits + item_leaves_log2));
+}
+
+int64_t trimmed_alpha_of(int64_t row, int64_t n, int kind)
+{
+    const int b = host::kKinds[kind].lane_bits;
+    const int d = ilog2(trimmed_domain_of(n, kind)) - b;
+    return ((int64_t)bitrev_host((uint32_t)(row >> b), d) << b) | (row & (((int64_t)1 << b) - 1));
+}
+
 /* "a standard", "an early-terminated", "an XOR-shared": the article of a kind's name */
 inline const char *article(int kind) { return kind == host::KIND_STANDARD ? "a" : "an"; }
 
@@ -427,6 +460,9 @@ int check_key(int kind, int64_t n, const int32_t *key, int64_t b, int bin)
     return fail(B200DPF_EINVAL, "key %lld is not %s %s key for n=%lld (its n: %lld)", (long long)b, article(kind), k.name,
                 (long long)n, (long long)kn);
 }
+
+/* The n of the keys a context (or its bin of `depth` leaf levels) takes: its rows, or trimmed_domain(rows) */
+int64_t key_rows(const b200dpf_ctx *c, int depth) { return (int64_t)1 << (depth + c->lane_bits()); }
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
 {
@@ -505,10 +541,14 @@ struct GroupBins {
     std::vector<int64_t> n;
     std::vector<int> depth;
     std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
-    /* made at create, never rewritten: [nbins] (row_off, depth) for row updates; [nbins] (uint4 offset of bin g's
-     * key in a compact query, depth of g), with query_v uint4 per query; the key generator's AES table */
+    std::vector<int64_t> rows;         /* its rows in d_table: n, or on a trimmed context n padded (trim_log2_of) */
+    std::vector<int> room;             /* log2 leaves of the largest work item inside them: depth, or less if trimmed */
+    /* made at create, never rewritten: [nbins] (row_off, depth) for row updates ((row_off, n) if trimmed); [nbins]
+     * (uint4 offset of bin g's key in a compact query, depth of g), with query_v uint4 per query; trimmed: [nbins]
+     * n for the key generator; the key generator's AES table */
     DeviceBuffer<uint2> d_bin_info;
     DeviceBuffer<uint2> d_bins;
+    DeviceBuffer<uint32_t> d_bin_rows;
     uint64_t query_v = 0;
     DeviceBuffer<uint32_t> d_te0;
     GroupLaunch once;                  /* b200dpf_group_eval and _eval_device: planned by every call */
@@ -529,8 +569,8 @@ template <class Items> int shrink_s(int s, int s_floor, int64_t wanted, Items it
     return s;
 }
 
-/* The work-item size of a key group of a bin of `depth` levels on a grouped context */
-int group_s(const EvalPlan &P, int depth) { return std::max(1, std::min(depth, P.s_group)); }
+/* The work-item size of a key group of bin g on a grouped context */
+int group_s(const EvalPlan &P, const GroupBins &B, int g) { return std::max(1, std::min(B.room[(size_t)g], P.s_group)); }
 
 /* The fields of EvalParams that every launch of job J on layout L shares; the others are zero. */
 void fill_common(const b200dpf_ctx *c, const SmemLayout &L, const EvalJob &J, const EvalPlan &P, EvalParams *p)
@@ -617,7 +657,7 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         const int s_floor = ops.leaf_items ? 1 : want_frontier ? 3 : 5;
         const int64_t items_per_warp = ops.leaf_items ? ops.leaf_items : want_frontier ? 24 : 6;
         s = shrink_s(std::min(c->depth_local, std::min(L.s_max, s_cap)), s_floor, items_per_warp * warps, [&](int t) {
-            return (((int64_t)1 << (c->depth_local - t)) * key_groups) >> (5 - kpw_log2);
+            return ((c->n_local >> (t + c->lane_bits())) * key_groups) >> (5 - kpw_log2);
         });
     }
     if (s < 1) s = 1;
@@ -632,6 +672,17 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
             P.tile_bytes = 0;
             rc = smem_layout(c, prf, P.nv, P.mode, &L);
             if (rc) return rc;
+        }
+    }
+    if (c->trimmed) {
+        /* a ticket (2^(s + spw_log2) leaves) must not reach past the padded rows: smaller items first (down to
+         * one leaf pair), then fewer subtrees per warp.  Lanes of a key quad trade leaf values by SHFL, so every
+         * lane of an issued ticket runs; the padding is what keeps its rows inside the table. */
+        const int room = c->trim_log2 - c->lane_bits();
+        s = std::max(1, std::min(s, room - (5 - kpw_log2)));
+        if (5 - kpw_log2 > room - s) {
+            kpw_log2 = 5 - (room - s);
+            key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
         }
     }
     const int rel = c->depth_local - s;           /* tree levels between the shard root and the items */
@@ -706,7 +757,7 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         P.smem = (size_t)P.off_tile + P.tile_bytes;
     }
     fill_phase(L, s, &P.main);
-    P.main.nsub = (uint32_t)1 << rel;
+    P.main.nsub = (uint32_t)(c->n_local >> (s + c->lane_bits()));   /* 2^rel, or the items over a trimmed table's rows */
     P.main.sub_first = (uint32_t)c->shard_rank << rel;
     if (f_rel > 0) {
         P.main.front_shift = rel - f_rel;
@@ -768,13 +819,14 @@ int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, 
         const int64_t items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
         P.s_group = shrink_s(P.s_group, s_floor, items_wanted, [&](int t) {
             int64_t items = 0;
-            for (int g = 0; g < nbins; g++) items += groups_of(g) << std::max(0, B->depth[(size_t)g] - t);
+            for (int g = 0; g < nbins; g++)
+                items += groups_of(g) * (B->rows[(size_t)g] >> (std::min(B->room[(size_t)g], t) + c->lane_bits()));
             return items;
         });
     }
     P.s = 1;
     for (int g = 0; g < nbins; g++)
-        if (count[(size_t)g + 1] > count[(size_t)g]) P.s = std::max(P.s, group_s(P, B->depth[(size_t)g]));
+        if (count[(size_t)g + 1] > count[(size_t)g]) P.s = std::max(P.s, group_s(P, *B, g));
     /* per pass: one ticket counter per key group, or the one unit counter */
     P.pass_counters = mode_traits(P.mode).units ? 1u : (size_t)P.key_groups;
     P.smem = smem_bytes(L, P.s);
@@ -1318,19 +1370,31 @@ int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key)
 
 }  // extern "C"
 
-/* b200dpf_create, b200dpf_create_et and b200dpf_create_xor: a context for keys of `kind` */
+/* Staged rows [rows][cols] to device rows [rows][stride] in the same order (a trimmed table): the permutation of
+ * launch_permute_table with every row in one leaf of 2^31 rows, which leaves the order as it is */
+static cudaError_t copy_rows(const int32_t *stage, int32_t *table, int64_t rows, int cols, int stride, int sm_count,
+                             cudaStream_t stream)
+{
+    return launch_permute_table(stage, table, (uint64_t)rows, 0, 31, cols, stride, sm_count, stream);
+}
+
+/* b200dpf_create, b200dpf_create_et, b200dpf_create_xor and (`trimmed`) b200dpf_create_trimmed: a context for keys
+ * of `kind` */
 static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int shard_rank,
-                       int shard_count, int kind)
+                       int shard_count, int kind, bool trimmed = false)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!table) return fail(B200DPF_EINVAL, "null table");
+    if (kind < 0 || kind >= host::KIND_COUNT) return fail(B200DPF_EINVAL, "unknown key kind %d", kind);
     const int lane_bits = host::kKinds[kind].lane_bits;
     const int64_t n_min = host::kKinds[kind].n_min;
-    if (n < n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0)
+    if (trimmed && !trim_args_ok(n, kind))
+        return fail(B200DPF_EINVAL, "table size n=%lld out of range [1, 2^31]", (long long)n);
+    if (!trimmed && (n < n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0))
         return fail(B200DPF_EINVAL, "table size n=%lld must be a power of two in [%lld, 2^31]", (long long)n, (long long)n_min);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
-    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 || (int64_t)shard_count > n / n_min ||
+    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 || (!trimmed && (int64_t)shard_count > n / n_min) ||
         shard_rank < 0 || shard_rank >= shard_count)
         return fail(B200DPF_EINVAL, "bad shard %d of %d for n=%lld", shard_rank, shard_count, (long long)n);
 
@@ -1340,7 +1404,7 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     if (rc) return rc;
     c->n = n;
     c->kind = kind;
-    c->depth = ilog2(n) - lane_bits;   /* the tree is over leaves */
+    c->depth = ilog2(trimmed ? trimmed_domain_of(n, kind) : n) - lane_bits;   /* the tree is over leaves */
     c->entry_size = entry_size;
     /* rows padded to what one pass reads: 16, 32 or a multiple of 64 int32 */
     c->entry_pad = entry_size <= 16 ? 16 : (entry_size <= 32 ? 32 : ((entry_size + 63) & ~63));
@@ -1349,6 +1413,11 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     c->shard_bits = ilog2(shard_count);
     c->n_local = n / shard_count;
     c->depth_local = c->depth - c->shard_bits;
+    if (trimmed) {
+        c->trimmed = true;
+        c->trim_log2 = trim_log2_of(n, kind);
+        c->n_local = (n + ((int64_t)1 << c->trim_log2) - 1) >> c->trim_log2 << c->trim_log2;
+    }
 
     /* Table: gather this shard's rows (natural indices j*G + bitrev_g(rank)),
      * then permute on the device into breadth-first leaf order, padded to
@@ -1369,7 +1438,7 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
         cudaGetLastError();
     }
     const size_t row_bytes = (size_t)entry_size * sizeof(int32_t);
-    const size_t stage_bytes = (size_t)c->n_local * row_bytes;
+    const size_t stage_bytes = (size_t)n / shard_count * row_bytes;
     const size_t leaf_bytes = row_bytes << lane_bits;            /* one leaf's rows */
     const int64_t leaves_local = c->n_local >> lane_bits;
     const size_t table_bytes = (size_t)c->n_local * (size_t)c->entry_pad * sizeof(int32_t);
@@ -1401,8 +1470,9 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, lane_bits, entry_size,
-                                  c->entry_pad, c->sm_count, c->stream));
+    if (trimmed) CUDA_TRY(copy_rows(d_stage.ptr, c->d_table.ptr, n, entry_size, c->entry_pad, c->sm_count, c->stream));
+    else CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, lane_bits, entry_size,
+                                       c->entry_pad, c->sm_count, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     d_stage.release();
 
@@ -1444,7 +1514,21 @@ int b200dpf_create_xor(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     return create_impl(out, table, n, entry_size, device, shard_rank, shard_count, host::KIND_XOR);
 }
 
+int b200dpf_create_trimmed(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int kind)
+{
+    return create_impl(out, table, n, entry_size, device, 0, 1, kind, true);
+}
+
 int b200dpf_ctx_rows_per_leaf(const b200dpf_ctx *c) { return c ? 1 << c->lane_bits() : -1; }
+
+int b200dpf_ctx_trimmed(const b200dpf_ctx *c) { return c ? (c->trimmed ? 1 : 0) : -1; }
+
+int64_t b200dpf_trimmed_domain(int64_t n, int kind) { return trim_args_ok(n, kind) ? trimmed_domain_of(n, kind) : -1; }
+
+int64_t b200dpf_trimmed_alpha(int64_t row, int64_t n, int kind)
+{
+    return trim_args_ok(n, kind) && row >= 0 && row < n ? trimmed_alpha_of(row, n, kind) : -1;
+}
 
 int b200dpf_destroy(b200dpf_ctx *c)
 {
@@ -1488,7 +1572,7 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     int rc = check_eval_args(c, keys, nkeys, prf, out);
     if (rc) return rc;
     for (int64_t b = 0; b < nkeys; b++)
-        if ((rc = check_key(c->kind, c->n, keys + b * host::KEY_WORDS, b, -1))) return rc;
+        if ((rc = check_key(c->kind, key_rows(c, c->depth), keys + b * host::KEY_WORDS, b, -1))) return rc;
     if (!is_pinned_host(keys)) {
         /* pageable keys have to be staged by the CPU anyway: stage only their live 32 + 64*depth bytes
          * (44 % of a key at n = 2^14, 63 % at 2^20) and let the DMA of a chunk overlap the next one */
@@ -1527,7 +1611,7 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
         for (int64_t b = b0; b < b1; b++) {
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
-            if (validate && (rc = check_key(c->kind, c->n, keys[b], b, -1))) return rc;
+            if (validate && (rc = check_key(c->kind, key_rows(c, c->depth), keys[b], b, -1))) return rc;
             pack_compact(keys[b], stage + (size_t)b * stride, c->depth, host::kKinds[c->kind].magic);
         }
         if (!c->multi)
@@ -1600,6 +1684,7 @@ int b200dpf_expand_device(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, i
     if (rc) return rc;
     if (c->multi) return fail(B200DPF_ESTATE, "multi-device contexts take host buffers (b200dpf_eval / b200dpf_eval_packed)");
     if (c->shard_count != 1) return fail(B200DPF_ESTATE, "expand needs an unsharded context");
+    if (c->trimmed) return fail(B200DPF_ESTATE, "expand needs a context that is not trimmed");
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
     return run_pipeline(c, keys_dev, reference_layout(), nkeys, prf, MODE_EXPAND, shares_dev,
@@ -1917,22 +2002,28 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
 /* b200dpf_group_create, _et and _xor: a grouped context for keys of `kind`.  n and the row
  * offsets count rows, the depths (per bin and the context's deepest) leaves. */
 static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
-                             int device, int kind)
+                             int device, int kind, bool trimmed = false)
 {
     if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
     *out = nullptr;
     if (!tables || !n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
+    if (kind < 0 || kind >= host::KIND_COUNT) return fail(B200DPF_EINVAL, "unknown key kind %d", kind);
     const int lane_bits = host::kKinds[kind].lane_bits;
     const int64_t n_min = host::kKinds[kind].n_min;
-    int64_t n_max = 0, rows = 0;
+    int64_t n_max = 0, rows = 0, stage_rows = 0;
     for (int g = 0; g < nbins; g++) {
         if (!tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
-        if (n[g] < n_min || n[g] > ((int64_t)1 << 31) || (n[g] & (n[g] - 1)) != 0)
+        if (trimmed && !trim_args_ok(n[g], kind))
+            return fail(B200DPF_EINVAL, "bin %d: size n=%lld out of range [1, 2^31]", g, (long long)n[g]);
+        if (!trimmed && (n[g] < n_min || n[g] > ((int64_t)1 << 31) || (n[g] & (n[g] - 1)) != 0))
             return fail(B200DPF_EINVAL, "bin %d: size n=%lld must be a power of two in [%lld, 2^31]", g, (long long)n[g],
                         (long long)n_min);
-        n_max = std::max(n_max, n[g]);
-        rows += n[g];
+        const int64_t domain = trimmed ? trimmed_domain_of(n[g], kind) : n[g];
+        const int gran = trimmed ? trim_log2_of(n[g], kind) : ilog2(n[g]);
+        n_max = std::max(n_max, domain);
+        rows += (n[g] + ((int64_t)1 << gran) - 1) >> gran << gran;
+        stage_rows = std::max(stage_rows, n[g]);   /* the largest bin's live rows */
     }
     std::optional<DeviceGuard> guard;
     std::unique_ptr<b200dpf_ctx> c;
@@ -1941,9 +2032,10 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     c->bins.reset(new (std::nothrow) GroupBins());
     if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
     GroupBins *B = c->bins.get();
-    c->n = n_max;                      /* the launch plan (shared memory for correction words) is sized by the deepest bin */
+    c->n = stage_rows;                 /* b200dpf_ctx_n: the largest bin's rows */
     c->kind = kind;
-    c->depth = ilog2(n_max) - lane_bits;
+    c->trimmed = trimmed;
+    c->depth = ilog2(n_max) - lane_bits;   /* the launch plan (shared memory for correction words) is sized by the deepest bin */
     c->entry_size = entry_size;
     c->entry_pad = (entry_size + 15) & ~15;       /* 16 columns per pass */
     c->n_local = n_max;
@@ -1955,34 +2047,44 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
     DeviceBuffer<int32_t> d_stage;
-    rc = d_stage.reserve((size_t)n_max * entry_size * sizeof(int32_t));
+    rc = d_stage.reserve((size_t)stage_rows * entry_size * sizeof(int32_t));
     if (rc) return rc;
     uint64_t row0 = 0;
     std::vector<uint2> bin_info, query_bins;
+    std::vector<uint32_t> bin_rows;
     for (int g = 0; g < nbins; g++) {
         /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows; a
-         * leaf's 2^lane_bits rows stay adjacent */
-        const int depth = ilog2(n[g]) - lane_bits;
+         * leaf's 2^lane_bits rows stay adjacent.  A trimmed bin keeps the caller's row order. */
+        const int depth = ilog2(trimmed ? trimmed_domain_of(n[g], kind) : n[g]) - lane_bits;
+        const int gran = trimmed ? trim_log2_of(n[g], kind) : depth + lane_bits;
         B->n.push_back(n[g]);
         B->depth.push_back(depth);
         B->row_off.push_back(row0);
-        bin_info.push_back(make_uint2((uint32_t)row0, (uint32_t)depth));
+        B->rows.push_back((n[g] + ((int64_t)1 << gran) - 1) >> gran << gran);
+        B->room.push_back(gran - lane_bits);
+        bin_info.push_back(make_uint2((uint32_t)row0, trimmed ? (uint32_t)n[g] : (uint32_t)depth));
         query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)depth));
+        bin_rows.push_back((uint32_t)n[g]);
         B->query_v += b200dpf_key_packed_size(depth) / 16u;
         CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
         int32_t *dst = c->d_table.ptr + row0 * (uint64_t)c->entry_pad;
-        CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, lane_bits, entry_size, c->entry_pad,
-                                      c->sm_count, c->stream));
+        if (trimmed) CUDA_TRY(copy_rows(d_stage.ptr, dst, n[g], entry_size, c->entry_pad, c->sm_count, c->stream));
+        else CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, lane_bits, entry_size, c->entry_pad,
+                                           c->sm_count, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
-        row0 += (uint64_t)n[g];
+        row0 += (uint64_t)B->rows.back();
     }
     const size_t bins_bytes = (size_t)nbins * sizeof(uint2);
     rc = B->d_bin_info.reserve(bins_bytes);
     if (!rc) rc = B->d_bins.reserve(bins_bytes);
+    if (!rc && trimmed) rc = B->d_bin_rows.reserve((size_t)nbins * sizeof(uint32_t));
     if (!rc) rc = B->d_te0.reserve(256 * sizeof(uint32_t));
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(B->d_bin_info.ptr, bin_info.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_bins.ptr, query_bins.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
+    if (trimmed)
+        CUDA_TRY(cudaMemcpyAsync(B->d_bin_rows.ptr, bin_rows.data(), (size_t)nbins * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                 c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read them once the context is returned */
     *out = c.release();
@@ -2005,6 +2107,12 @@ int b200dpf_group_create_xor(b200dpf_ctx **out, const int32_t *const *tables, co
                              int device)
 {
     return group_create_impl(out, tables, n, nbins, entry_size, device, host::KIND_XOR);
+}
+
+int b200dpf_group_create_trimmed(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                                 int device, int kind)
+{
+    return group_create_impl(out, tables, n, nbins, entry_size, device, kind, true);
 }
 
 /* The argument checks every grouped entry point makes first, in this order: the context, its buffers (`bufs`: none
@@ -2039,7 +2147,7 @@ static int group_count(const b200dpf_ctx *c, const int32_t *keys, const int32_t 
         const int g = bins[b];
         if (g < 0 || g >= nbins) return fail(B200DPF_EINVAL, "key %lld: bin %d out of range [0,%d)", (long long)b, g, nbins);
         if (keys) {
-            const int rc = check_key(c->kind, B->n[(size_t)g], keys + b * host::KEY_WORDS, b, g);
+            const int rc = check_key(c->kind, key_rows(c, B->depth[(size_t)g]), keys + b * host::KEY_WORDS, b, g);
             if (rc) return rc;
         }
         count[(size_t)g + 1]++;
@@ -2076,14 +2184,14 @@ int GroupLaunch::plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
         int64_t gi = 0;
         for (int g = 0; g < nbins; g++) {
             const int depth = B->depth[(size_t)g];
-            const int s = group_s(P, depth);
+            const int s = group_s(P, *B, g);
             for (int64_t k = count[(size_t)g]; k < count[(size_t)g + 1]; k += 32, gi++) {
                 GroupDesc &d = h_descs.ptr[gi];
                 d.key_first = (uint32_t)k;
                 d.nkeys = (uint32_t)std::min<int64_t>(32, count[(size_t)g + 1] - k);
                 d.depth = depth;
                 d.s = s;
-                d.nsub = (uint32_t)1 << (depth - s);
+                d.nsub = (uint32_t)(B->rows[(size_t)g] >> (s + c->lane_bits()));   /* 2^(depth - s) unless trimmed */
                 d.pad = 0;
                 d.table_off_v = B->row_off[(size_t)g] * (uint64_t)(c->entry_pad / 4);
             }
@@ -2297,6 +2405,7 @@ int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, 
     p.count = nqueries * nbins;
     p.lane_bits = k.lane_bits;
     p.bins = B->d_bins.ptr;
+    p.bin_rows = B->d_bin_rows.ptr;   /* null unless trimmed */
     p.nq = (uint32_t)nqueries;
     p.nbins = (uint32_t)nbins;
     p.query_v = B->query_v;
@@ -2332,7 +2441,7 @@ size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 /* rows of the device table; also the skip marker of the update kernels (larger than every position) */
 uint64_t update_table_rows(const b200dpf_ctx *c)
 {
-    return c->bins ? c->bins->row_off.back() + (uint64_t)c->bins->n.back() : (uint64_t)c->n_local;
+    return c->bins ? c->bins->row_off.back() + (uint64_t)c->bins->rows.back() : (uint64_t)c->n_local;
 }
 
 /* Grow the scratch for `count` rows (staged: the inputs are copied into it) and order everything that
@@ -2371,6 +2480,7 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     std::memset(&u, 0, sizeof u);
     u.idx = idx;
     u.bins = bins;
+    u.identity = c->trimmed;
     if (bins) {
         u.bin_info = c->bins->d_bin_info.ptr;
         u.nbins = (int)c->bins->n.size();
@@ -2524,6 +2634,13 @@ double b200dpf_ctx_last_device_ms(b200dpf_ctx *c)
 }
 
 int b200dpf_group_bins(const b200dpf_ctx *c) { return (c && c->bins) ? (int)c->bins->n.size() : 0; }
+
+int64_t b200dpf_ctx_table_rows(const b200dpf_ctx *c)
+{
+    if (!c) return -1;
+    if (c->multi) return (int64_t)update_table_rows(c->multi->sub[0]);
+    return (int64_t)update_table_rows(c);
+}
 
 
 int b200dpf_ctx_read_timing(b200dpf_ctx *c, uint64_t *stamps, int max_blocks, int *nblocks)

@@ -24,6 +24,7 @@
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <functional>
 #include <vector>
 
 #include "b200dpf.h"
@@ -231,8 +232,8 @@ std::vector<void *> eval_init_multi(const at::Tensor &table, const std::vector<i
 
 /* batch PIR: many tables ("bins") of one entry size behind one context, for keys of one kind
  * (b200dpf_group_create, _et or _xor, named `what` in messages) */
-std::vector<void *> group_init_with(const std::vector<at::Tensor> &tables, int device,
-                                    int (*create)(b200dpf_ctx **, const int32_t *const *, const int64_t *, int, int, int),
+using GroupCreate = std::function<int(b200dpf_ctx **, const int32_t *const *, const int64_t *, int, int, int)>;
+std::vector<void *> group_init_with(const std::vector<at::Tensor> &tables, int device, const GroupCreate &create,
                                     const char *what)
 {
     TORCH_CHECK(!tables.empty(), what, ": no tables");
@@ -263,6 +264,41 @@ std::vector<void *> group_init_et(const std::vector<at::Tensor> &tables, int dev
 std::vector<void *> group_init_xor(const std::vector<at::Tensor> &tables, int device)
 {
     return group_init_with(tables, device, b200dpf_group_create_xor, "group_init_xor");
+}
+
+/* trimmed tables of any row count, for keys of `kind` (B200DPF_KIND_*): b200dpf_create_trimmed and
+ * b200dpf_group_create_trimmed; row r is reached by a key for trimmed_alpha(r, n, kind) over trimmed_domain(n, kind) */
+Ctx eval_init_trimmed(const at::Tensor &table, int device, int kind)
+{
+    TORCH_CHECK(table.dim() == 2, "eval_init_trimmed: table must be [num_entries, entry_size]");
+    at::Tensor t = table.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    check(b200dpf_create_trimmed(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), device, kind), "eval_init_trimmed");
+    return {static_cast<void *>(ctx)};
+}
+
+std::vector<void *> group_init_trimmed(const std::vector<at::Tensor> &tables, int device, int kind)
+{
+    return group_init_with(
+        tables, device,
+        [kind](b200dpf_ctx **c, const int32_t *const *t, const int64_t *n, int nbins, int e, int d) {
+            return b200dpf_group_create_trimmed(c, t, n, nbins, e, d, kind);
+        },
+        "group_init_trimmed");
+}
+
+int64_t trimmed_domain(int64_t n, int kind)
+{
+    const int64_t v = b200dpf_trimmed_domain(n, kind);
+    TORCH_CHECK(v >= 0, "trimmed_domain: n=", n, " outside [1, 2^31] or unknown kind ", kind);
+    return v;
+}
+
+int64_t trimmed_alpha(int64_t row, int64_t n, int kind)
+{
+    const int64_t v = b200dpf_trimmed_alpha(row, n, kind);
+    TORCH_CHECK(v >= 0, "trimmed_alpha: row ", row, " of n=", n, " out of range, or unknown kind ", kind);
+    return v;
 }
 
 /* keys int32 [B,524], bins int32/int64 [B] -> int32 [B, E]: key b evaluated on table bins[b] */
@@ -572,6 +608,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
           py::arg("device") = 0);
     m.def("group_init_xor", &group_init_xor, "batch PIR for XOR-shared keys (128 rows per leaf, XOR results)",
           py::arg("tables"), py::arg("device") = 0);
+    m.def("eval_init_trimmed", &eval_init_trimmed, "eval_init for a table of any row count (trimmed context)",
+          py::arg("table"), py::arg("device") = 0, py::arg("kind") = 0);
+    m.def("group_init_trimmed", &group_init_trimmed, "batch PIR over bins of any row count (trimmed context)",
+          py::arg("tables"), py::arg("device") = 0, py::arg("kind") = 0);
+    m.def("trimmed_domain", &trimmed_domain, "n of the keys a trimmed table of n rows takes", py::arg("n"), py::arg("kind") = 0);
+    m.def("trimmed_alpha", &trimmed_alpha, "key index of row `row` of a trimmed n-row table", py::arg("row"), py::arg("n"),
+          py::arg("kind") = 0);
+    m.def("table_rows", [](const std::vector<void *> &b) { return b200dpf_ctx_table_rows(ctx_of(b)); },
+          "rows of the context's device table, padding included");
     m.def("group_eval", &group_eval, "batch PIR: evaluate (bin, key) pairs in one launch");
     m.def("group_eval_device", &group_eval_device, "batch PIR from device keys into device results, enqueued on a stream",
           py::arg("keys_ptr"), py::arg("bins"), py::arg("nkeys"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"),

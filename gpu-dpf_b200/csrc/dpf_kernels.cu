@@ -1014,9 +1014,14 @@ __global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, u
             const int32_t g = u.bins[j];
             if (g >= 0 && g < u.nbins) {
                 const uint2 info = u.bin_info[g];
-                if (i >= 0 && i < ((int64_t)1 << (info.y + u.lane_bits)))
+                if (u.identity) {
+                    if (i >= 0 && i < (int64_t)info.y) p = info.x + (uint32_t)i;
+                } else if (i >= 0 && i < ((int64_t)1 << (info.y + u.lane_bits))) {
                     p = info.x + ((bitrev_bits(leaf, (int)info.y) << u.lane_bits) | lane);
+                }
             }
+        } else if (u.identity) {
+            if (i >= 0 && i < u.n) p = (uint32_t)i;
         } else if (i >= 0 && i < u.n && (leaf & u.own_mask) == u.own_val) {
             p = (bitrev_bits(leaf >> u.shift, u.depth) << u.lane_bits) | lane;
         }

@@ -23,7 +23,8 @@ struct PhaseParams {
     int walk_steps;           /* walk steps from the start node to the subtree root     */
     int level_base;           /* level of the subtree's bottom expansion (0 = leaves)   */
     uint32_t sub_first;       /* breadth-first index of the shard's first 2^s-subtree   */
-    uint32_t nsub;            /* number of 2^s-subtrees in this shard                   */
+    uint32_t nsub;            /* number of 2^s-subtrees issued in this shard: all of them, or on
+                                 a trimmed context those over its padded table rows        */
     uint32_t *counters;       /* [key_groups] tickets, zero at phase start; one ticket =
                                  32/kpw consecutive subtrees for the group's kpw keys   */
     int stack_split;          /* pending-sibling stack levels [0, split) live in the lo
@@ -38,7 +39,8 @@ struct GroupDesc {
     uint32_t nkeys;           /* 1..32                                                      */
     int32_t depth;            /* log2 of the bin's table size (MODE_GROUPED_ET, _XOR: of its leaves) */
     int32_t s;                /* log2 leaves per work item for this group                   */
-    uint32_t nsub;            /* work items (2^s-leaf subtrees) = 2^(depth - s)             */
+    uint32_t nsub;            /* work items (2^s-leaf subtrees): 2^(depth - s), or on a trimmed
+                                 context those over the bin's padded rows                   */
     uint32_t pad;
     uint64_t table_off_v;     /* bin's first row, in uint4 units from EvalParams::table     */
 };
@@ -256,6 +258,10 @@ struct KeygenParams {
     int64_t count;
     int depth, lane_bits;      /* depth: flat batches only */
     const uint2 *bins;         /* query batches: [nbins] (uint4 offset of the key in a compact query, depth) */
+    /* query batches of a trimmed context: [nbins] live rows n_g.  Key g of query q is then for row
+     * alphas[q][g] mod n_g (non-negative), placed at index (bitrev_depth(r >> lane_bits) << lane_bits) |
+     * (r & (2^lane_bits - 1)) of the tree's domain, as b200dpf_trimmed_alpha; null: the low bits of alpha */
+    const uint32_t *bin_rows;
     uint32_t nq, nbins;
     uint64_t query_v;          /* uint4 per compact query */
     int compact;
@@ -301,11 +307,15 @@ cudaError_t launch_group_gather_queries(const void *queries, const uint2 *bins, 
  *                  skip unless 0 <= i < 2^(bin_info[g].y + lane_bits);
  *                  else bin_info[g].x + (bitrev_{bin_info[g].y}(v) << lane_bits | (i & (2^lane_bits - 1)))
  *                                                                     (grouped context)
+ * With `identity` (trimmed contexts, which store row i at device row i) the index is the row number and
+ *   bins == null   skip unless 0 <= i < n; else i
+ *   bins != null   skip unless 0 <= i < bin_info[g].y (the bin's rows); else bin_info[g].x + i
  * Skipped entries are never written. */
 struct UpdateParams {
-    const int64_t *idx;       /* [count] natural indices                                      */
+    const int64_t *idx;       /* [count] natural indices (trimmed contexts: row numbers)      */
     const int32_t *bins;      /* [count] bin ids, or null                                     */
-    const uint2 *bin_info;    /* [nbins] (first row, depth)                                   */
+    const uint2 *bin_info;    /* [nbins] (first row, depth), trimmed: (first row, rows)       */
+    int identity;
     int nbins;
     const int32_t *rows;      /* [count][cols] new rows                                       */
     int64_t count;            /* <= 2^31 - 1                                                  */

@@ -168,18 +168,26 @@ __global__ void __launch_bounds__(64, 1) keygen_kernel(const KeygenParams p)
     int64_t idx = k;   /* of the key's alpha and seed, and of the key pair in a wire-format output */
     int depth = p.depth;
     uint64_t off_v = (uint64_t)k * 131u;
+    uint32_t rows = 0;   /* trimmed query batches: the bin's live rows */
     if (p.bins) {
         const uint32_t g = (uint32_t)(k / p.nq), q = (uint32_t)(k - (int64_t)g * p.nq);
         const uint2 b = p.bins[g];
         idx = (int64_t)q * p.nbins + g;
         depth = (int)b.y;
         off_v = p.compact ? (uint64_t)q * p.query_v + b.x : (uint64_t)idx * 131u;
+        if (p.bin_rows) rows = p.bin_rows[g];
     }
     const KeyOut out{p.out_a + off_v, p.out_b + off_v, p.compact != 0};
 
     /* the key for the low depth + lane_bits bits of alpha: its leaf, and the payload at level 0 (beta = 1,
      * dpf_wrapper.cu:53; early-terminated: lane alpha & 3 of the leaf; XOR-shared: bit alpha & 127) */
-    const uint64_t a_row = (uint64_t)p.alphas[idx];
+    uint64_t a_row = (uint64_t)p.alphas[idx];
+    if (rows != 0) {   /* row r = alpha mod n_g of a trimmed bin sits at leaf position r >> lane_bits */
+        int64_t r = p.alphas[idx] % (int64_t)rows;
+        if (r < 0) r += rows;
+        const uint64_t leaf = __brev((uint32_t)((uint64_t)r >> p.lane_bits)) >> (32 - depth);
+        a_row = (leaf << p.lane_bits) | ((uint64_t)r & ((1u << p.lane_bits) - 1u));
+    }
     const uint64_t alpha = (a_row & ((((uint64_t)1) << (depth + p.lane_bits)) - 1u)) >> p.lane_bits;
     u128 beta[32];
     beta[0] = GROUP == GROUP_LANES32 ? (u128)1 << (32 * (a_row & 3u)) : GROUP == GROUP_XOR128 ? (u128)1 << (a_row & 127u) : (u128)1;

@@ -41,13 +41,14 @@ except ImportError as exc:  # fail loudly: there is no Python/CPU stand-in for t
 # What DPF does differently per kind of key (include/b200dpf.h): the dpf_cpp functions, whether explicit seeds
 # are ChaCha20-DRBG bytes only (at least 44 per key) or may also select the reference's 32-bit mt19937
 # generator, and the name in messages.  `gen` / `gen_batch` are the ChaCha20-DRBG generators.
-_Kind = collections.namedtuple("_Kind", "name drbg_only gen gen_batch eval_cpu eval_init pack")
+# `id` is the kind's B200DPF_KIND_* (the trimmed contexts' kind argument).
+_Kind = collections.namedtuple("_Kind", "name drbg_only gen gen_batch eval_cpu eval_init pack id")
 _STANDARD = _Kind("standard", False, dpf_cpp.gen_secure, dpf_cpp.gen_batch_secure, dpf_cpp.eval_cpu,
-                  dpf_cpp.eval_init_sharded, dpf_cpp.key_pack)
+                  dpf_cpp.eval_init_sharded, dpf_cpp.key_pack, 0)
 _EARLY_TERMINATED = _Kind("early-terminated", True, dpf_cpp.gen_et, dpf_cpp.gen_batch_et, dpf_cpp.eval_cpu_et,
-                          dpf_cpp.eval_init_et, dpf_cpp.key_pack_et)
+                          dpf_cpp.eval_init_et, dpf_cpp.key_pack_et, 1)
 _XOR_SHARED = _Kind("XOR-shared", True, dpf_cpp.gen_xor, dpf_cpp.gen_batch_xor, dpf_cpp.eval_cpu_xor,
-                    dpf_cpp.eval_init_xor, dpf_cpp.key_pack_xor)
+                    dpf_cpp.eval_init_xor, dpf_cpp.key_pack_xor, 2)
 
 
 class DPF(object):
@@ -70,7 +71,7 @@ class DPF(object):
     }
 
     def __init__(self, prf=None, device=0, shard=(0, 1), allow_non_pow2=False, devices=None, axis="auto",
-                 early_termination=False, xor=False):
+                 early_termination=False, xor=False, trim=False):
         # devices: None (one GPU: `device`), "all", or a list of device ids -- one process drives them all
         # (b200dpf_create_multi); axis "auto" | "entries" | "keys".  B200DPF_DEVICES / B200DPF_AXIS in the
         # environment set the defaults, so an unchanged `dpf.DPF()` caller (benchmark.py) can scale too.
@@ -111,6 +112,15 @@ class DPF(object):
             raise Exception("xor=True has no multi-device variant: use one device per DPF "
                             "(DPF(device=d, shard=(rank, count), xor=True))")
         self.kind = _XOR_SHARED if self.xor else _EARLY_TERMINATED if self.early_termination else _STANDARD
+        # trim: tables of any row count without padding to a power of two (include/b200dpf.h,
+        # b200dpf_create_trimmed).  Row k is reached by an ordinary key of the kind for index
+        # trimmed_alpha(k, n) over trimmed_domain(n) rows, which gen / gen_batch make from k and n.
+        self.trim = bool(trim)
+        if self.trim and self.devices:
+            raise Exception("trim=True has no multi-device variant: a trimmed table lives on one GPU (DPF(device=d, trim=True))")
+        if self.trim and self.shard != (0, 1):
+            raise Exception("trim=True has no sharded variant: a trimmed context holds the whole table")
+        self._trim_order = None
 
     # ---- client -----------------------------------------------------------
     def gen(self, k, n, seed=None, secure=None):
@@ -135,6 +145,11 @@ class DPF(object):
             secure = seed is None
         if seed is None:
             seed = os.urandom(128)
+        if self.trim:
+            if not 0 <= k < n:
+                raise Exception("k (%d), the selected row, must be in [0, n) with n (%d) the number of rows in the table" % (k, n))
+            return (self.kind.gen if secure else dpf_cpp.gen)(dpf_cpp.trimmed_alpha(k, n, self.kind.id),
+                                                              dpf_cpp.trimmed_domain(n, self.kind.id), seed, self.prf_method)
         if n & (n - 1) != 0 and not self.allow_non_pow2:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
         if k >= n:
@@ -146,10 +161,16 @@ class DPF(object):
         """Keys for many indices at once: two int32 [B, 524] tensors (multi-threaded keygen).
         seeds=None: ChaCha20-DRBG keys from os.urandom entropy (44 bytes per key); explicit integer
         seeds select the reference's 32-bit mt19937 generator (deterministic, for tests).  With
-        early_termination or xor, explicit seeds are bytes: 44 per key, concatenated."""
+        early_termination or xor, explicit seeds are bytes: 44 per key, concatenated.  With trim, n is any row
+        count and each index a row < n."""
+        idx = torch.as_tensor(list(indices), dtype=torch.int64)
+        if self.trim:
+            if idx.numel() and not (0 <= int(idx.min()) and int(idx.max()) < n):
+                raise Exception("indices must be rows in [0, n) with n (%d) the number of rows in the table" % n)
+            idx = torch.as_tensor([dpf_cpp.trimmed_alpha(int(r), n, self.kind.id) for r in idx], dtype=torch.int64)
+            n = dpf_cpp.trimmed_domain(n, self.kind.id)
         if n & (n - 1) != 0:
             raise Exception("Table num entries (%d) must be a power of two" % (n))
-        idx = torch.as_tensor(list(indices), dtype=torch.int64)
         if self.kind.drbg_only:
             if seeds is None:
                 seeds = os.urandom(44 * idx.numel())
@@ -171,17 +192,28 @@ class DPF(object):
             return self._eval_cpu_xor(keys, one_hot_only)
         eval_one = self.kind.eval_cpu
         if one_hot_only:
-            return torch.stack([eval_one(k, self.prf_method) for k in keys])
+            return self._rows(torch.stack([eval_one(k, self.prf_method) for k in keys]))
         if self.table is None:
             raise Exception("Must call `eval_init` before `eval_cpu` with one_hot_only=False")
-        one_hots = torch.stack([eval_one(k, self.prf_method) for k in keys])
+        one_hots = self._rows(torch.stack([eval_one(k, self.prf_method) for k in keys]))
         return torch.matmul(one_hots, self.table)
+
+    def _rows(self, shares):
+        """Share vectors [B, domain] in row order: with trim, column r is the share of row r (index trimmed_alpha(r))."""
+        if not self.trim:
+            return shares
+        if self.table is None:
+            raise Exception("Must call `eval_init` before `eval_cpu` with trim=True: the row order depends on the table size")
+        if self._trim_order is None:
+            n = self.table.shape[0]
+            self._trim_order = torch.as_tensor([dpf_cpp.trimmed_alpha(r, n, self.kind.id) for r in range(n)], dtype=torch.int64)
+        return shares[:, self._trim_order]
 
     def _eval_cpu_xor(self, keys, one_hot_only):
         shifts = torch.arange(32, dtype=torch.int32)
         # packed words [B, n/32] -> bits [B, n]: row i is bit (i & 31) of word i >> 5
         bits = torch.stack([(self.kind.eval_cpu(k, self.prf_method).view(-1, 1) >> shifts) & 1 for k in keys])
-        bits = bits.reshape(len(keys), -1)
+        bits = self._rows(bits.reshape(len(keys), -1))
         if one_hot_only:
             return bits
         if self.table is None:
@@ -200,13 +232,14 @@ class DPF(object):
         if self.buffers is not None:
             dpf_cpp.eval_free(self.buffers)
             self.buffers = None
-        if table.shape[0] < 128:
+        if table.shape[0] < (1 if self.trim else 128):
             raise Exception("Table (%d) must have at least 128 elements" % table.shape[0])
         # the caller's row count: with allow_non_pow2 the rows beyond it are zero padding that updates may not touch
         self.table_rows = table.shape[0]
         # eval_cpu reads self.table; update_rows copies it before the first write, never writing the caller's tensor
         self._table_is_callers = True
-        if table.shape[0] & (table.shape[0] - 1) != 0:
+        self._trim_order = None
+        if table.shape[0] & (table.shape[0] - 1) != 0 and not self.trim:
             if not self.allow_non_pow2:
                 raise Exception("Table num entries (%d) must be a power of two" % (table.shape[0]))
             table = _pad_rows_to_pow2(table)
@@ -214,14 +247,16 @@ class DPF(object):
         self.table = table
         self.table_num_entries = table.shape[0]
         self.table_effective_entry_size = table.shape[1]
-        if self.devices:      # standard keys only: __init__ refuses the other kinds with devices
+        if self.trim:
+            self.buffers = dpf_cpp.eval_init_trimmed(table, self.device, self.kind.id)
+        elif self.devices:    # standard keys only: __init__ refuses the other kinds with devices
             self.buffers = dpf_cpp.eval_init_multi(table, self.devices, {"auto": 0, "entries": 1, "keys": 2}[self.axis])
         else:
             self.buffers = self.kind.eval_init(table, self.device, self.shard[0], self.shard[1])
 
     def update_rows(self, indices, rows):
         """Replace rows of the uploaded table in place: table[indices[j]] := rows[j] for natural indices (the
-        numbering keys use); when an index repeats, its last row wins.  `rows` [count, entry_size] is cast to
+        numbering keys use; with trim, row numbers); when an index repeats, its last row wins.  `rows` [count, entry_size] is cast to
         int32 like eval_init's table.  Only the touched rows move: no re-upload, and `buffers` stays valid.
 
         CPU tensors (or lists) are applied synchronously.  CUDA tensors on the context's device are applied on
@@ -359,6 +394,9 @@ class DPF(object):
         With xor the share bits come packed: int32 [B, n / 32], row i = bit (i & 31) of word i >> 5."""
         if self.buffers is None:
             raise Exception("Must call `eval_init` before `expand_gpu_device`")
+        if self.trim:
+            raise Exception("expand_gpu_device has no trim=True variant: use eval_cpu(keys, one_hot_only=True) for share vectors "
+                            "in row order")
         assert keys_dev.is_cuda and keys_dev.dtype == torch.int32 and keys_dev.is_contiguous()
         if out_dev is None:
             out_dev = torch.empty((keys_dev.shape[0], self.table_num_entries // (32 if self.xor else 1)), dtype=torch.int32,
@@ -397,6 +435,9 @@ class BinnedDPF(DPF):
         d.eval_init([bin0, bin1, ...])           # tables [n_g, entry_size], power-of-two n_g >= 2
         k1, k2 = d.gen_in_bin(g, index)          # keys for entry `index` of bin g
         shares = d.eval_gpu(keys, bins)          # int32 [len(keys), entry_size]
+
+    With trim=True the bins may have any size n_g >= 1 (b200dpf_group_create_trimmed): gen_in_bin(g, index) makes
+    the key of row `index` of bin g, and gen_queries_device maps its rows the same way.
     """
 
     def __init__(self, *args, **kwargs):
@@ -414,13 +455,16 @@ class BinnedDPF(DPF):
             self.buffers = None
         tables = list(tables)
         for t in tables:
-            if t.shape[0] & (t.shape[0] - 1) != 0 or t.shape[0] < 2:
+            if self.trim and t.shape[0] < 1:
+                raise Exception("Table num entries (%d) must be at least 1" % (t.shape[0]))
+            if not self.trim and (t.shape[0] & (t.shape[0] - 1) != 0 or t.shape[0] < 2):
                 raise Exception("Table num entries (%d) must be a power of two" % (t.shape[0]))
         self.bin_sizes = [int(t.shape[0]) for t in tables]
         self.table = None
         self.table_num_entries = sum(self.bin_sizes)
         self.table_effective_entry_size = tables[0].shape[1]
-        self.buffers = dpf_cpp.group_init(tables, self.device)
+        self.buffers = (dpf_cpp.group_init_trimmed(tables, self.device, self.kind.id) if self.trim
+                        else dpf_cpp.group_init(tables, self.device))
 
     def gen_in_bin(self, g, k, seed=None, secure=False):
         return self.gen(k, self.bin_sizes[g], seed=seed, secure=secure)

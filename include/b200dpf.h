@@ -604,6 +604,73 @@ int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key);
 int b200dpf_create_xor(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size,
                        int device, int shard_rank, int shard_count);
 
+/* ------------------------------------------------------------------------------------------- */
+/* Trimmed tables: any row count, no padding to a power of two (DESIGN.md section 11).          */
+/* ------------------------------------------------------------------------------------------- */
+/*
+ * The contexts above need a power-of-two row count; padding a table with zero rows up to one costs as
+ * much device memory and evaluation work as real rows.  A trimmed context takes a table of any n rows,
+ * 1 <= n <= 2^31, for keys of any kind, and numbers rows so that the live rows come first in the tree:
+ * row r sits at leaf position r >> b (b = log2 rows per leaf: 0 standard, 2 early-terminated, 7
+ * XOR-shared), so the work past the last live row is never issued.  The client reaches row r with an
+ * ordinary key of the kind (b200dpf_gen_secure, _gen_et, _gen_xor and their batched and GPU forms), made
+ * for n = b200dpf_trimmed_domain(n) rows and alpha = b200dpf_trimmed_alpha(r, n, kind); keygen, the key
+ * formats and packing are unchanged.  The result is then, with share_b the key's CPU share vector over
+ * the domain (b200dpf_eval_cpu, _et, _xor):
+ *   out[b][e] = sum over r < n of share_b[trimmed_alpha(r)] * table[r][e]  mod 2^32   (XOR-shared: XOR)
+ * so the two servers' results reconstruct table[r] for the key of row r.
+ *
+ * Padding bound: the device table holds b200dpf_ctx_table_rows = n rounded up to a multiple of 2^g rows
+ * (per bin on a grouped context), with N = b200dpf_trimmed_domain(n) and
+ *   g = min(log2 N, max(log2 N - 7, b + m)),   m = 6 for standard and early-terminated keys, 1 for XOR-shared,
+ * so the padding is below max(N / 128, 2^(b + m)) rows: under n / 64 (1.6 %) once n > 2^(b + m + 7), and at
+ * most 63 rows (standard), 255 (early-terminated) or 255 (XOR-shared) on a bin that small.  Work items are
+ * sized so that none reaches past those rows.
+ */
+enum { B200DPF_KIND_STANDARD = 0, B200DPF_KIND_ET = 1, B200DPF_KIND_XOR = 2 };
+
+/* The key domain of a trimmed n-row table: the next power of two >= n, at least the kind's smallest key
+ * (2 standard, 8 early-terminated, 256 XOR-shared).  -1 for n outside [1, 2^31] or an unknown kind. */
+int64_t b200dpf_trimmed_domain(int64_t n, int kind);
+
+/* The key index of row `row` of a trimmed n-row table: bitrev_d(row >> b) << b | (row & (2^b - 1)), with
+ * d = log2(b200dpf_trimmed_domain(n, kind)) - b.  -1 for n outside [1, 2^31], an unknown kind or a row
+ * outside [0, n).  Distinct rows have distinct indices in [0, trimmed_domain). */
+int64_t b200dpf_trimmed_alpha(int64_t row, int64_t n, int kind);
+
+/*
+ * A trimmed context of `kind` (B200DPF_KIND_*) on device `device`.  table: int32 [n][entry_size] in row
+ * order, host or device memory, 1 <= n <= 2^31, entry_size as b200dpf_create.  On it b200dpf_eval,
+ * _eval_gather, _eval_packed (the kind's compact keys), _host_staging, _eval_device, _eval_device_acc, the
+ * option setters, timing and introspection work as on a context of the kind, taking only keys of the kind
+ * for n = b200dpf_trimmed_domain(n) rows (any other key is EINVAL on the host paths, before anything is
+ * copied).  b200dpf_update_rows and _update_rows_device take ROW numbers r: the host path is EINVAL for
+ * r outside [0, n), the device path skips such entries.  b200dpf_ctx_n is n.  b200dpf_expand_device is
+ * ESTATE.  There is no sharded or multi-device trimmed context.
+ */
+int b200dpf_create_trimmed(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size, int device,
+                           int kind);
+
+/*
+ * A trimmed grouped (batch-PIR) context: bins of any size n[g] in [1, 2^31], each numbered as above.
+ * b200dpf_group_eval, _group_eval_device, _group_eval_queries_device (both formats), _group_query_bytes and
+ * _group_update_rows (row numbers, EINVAL for r >= n[g]) work as on a grouped context of the kind; the key
+ * of bin g is for b200dpf_trimmed_domain(n[g]) rows.  b200dpf_group_gen_queries_device makes key (q, g)
+ * for row alphas[q][g] mod n[g] (a non-negative modulo), i.e. the key b200dpf_gen_batch_secure (_et, _xor)
+ * returns for (b200dpf_trimmed_alpha(row, n[g], kind), b200dpf_trimmed_domain(n[g], kind)); its compact
+ * form is that key's b200dpf_key_pack (_et, _xor) bytes.
+ */
+int b200dpf_group_create_trimmed(b200dpf_ctx **ctx, const int32_t *const *tables, const int64_t *n, int nbins,
+                                 int entry_size, int device, int kind);
+
+/* 1 on a trimmed context, 0 on any other, -1 for null. */
+int b200dpf_ctx_trimmed(const b200dpf_ctx *ctx);
+
+/* Rows of the context's device table, padding included (on a grouped context all bins together; on a
+ * multi-device context one device's); -1 for null.  A context that is not trimmed pads nothing: n (a
+ * shard: n / shard_count). */
+int64_t b200dpf_ctx_table_rows(const b200dpf_ctx *ctx);
+
 #ifdef __cplusplus
 }
 #endif
