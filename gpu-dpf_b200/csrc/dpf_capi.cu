@@ -59,13 +59,6 @@ int ilog2(int64_t v)
     return b;
 }
 
-uint32_t bitrev_host(uint32_t v, int bits)
-{
-    uint32_t r = 0;
-    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
-    return r;
-}
-
 struct DeviceGuard {
     int prev = -1;
     bool ok = false;
@@ -143,6 +136,7 @@ struct b200dpf_ctx {
      * grouped context) is zero-padded to a multiple of 2^trim_log2 rows only.  n is the live rows. */
     bool trimmed = false;
     int trim_log2 = 0;
+    RowPlacement place{};             /* where this table's (or shard's) rows live in d_table; not used when grouped */
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
     DeviceBuffer<int32_t> d_keys;     /* whole wire-format keys */
@@ -425,8 +419,7 @@ int trim_log2_of(int64_t n, int kind)
 int64_t trimmed_alpha_of(int64_t row, int64_t n, int kind)
 {
     const int b = host::kKinds[kind].lane_bits;
-    const int d = ilog2(trimmed_domain_of(n, kind)) - b;
-    return ((int64_t)bitrev_host((uint32_t)(row >> b), d) << b) | (row & (((int64_t)1 << b) - 1));
+    return (int64_t)trimmed_alpha((uint64_t)row, ilog2(trimmed_domain_of(n, kind)) - b, b);
 }
 
 /* "a standard", "an early-terminated", "an XOR-shared": the article of a kind's name */
@@ -543,12 +536,11 @@ struct GroupBins {
     std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
     std::vector<int64_t> rows;         /* its rows in d_table: n, or on a trimmed context n padded (trim_log2_of) */
     std::vector<int> room;             /* log2 leaves of the largest work item inside them: depth, or less if trimmed */
-    /* made at create, never rewritten: [nbins] (row_off, depth) for row updates ((row_off, n) if trimmed); [nbins]
-     * (uint4 offset of bin g's key in a compact query, depth of g), with query_v uint4 per query; trimmed: [nbins]
-     * n for the key generator; the key generator's AES table */
-    DeviceBuffer<uint2> d_bin_info;
+    /* made at create, never rewritten: [nbins] the bins' placements, for row updates and the key generator; [nbins]
+     * (uint4 offset of bin g's key in a compact query, depth of g), with query_v uint4 per query; the key generator's
+     * AES table */
+    DeviceBuffer<RowPlacement> d_place;
     DeviceBuffer<uint2> d_bins;
-    DeviceBuffer<uint32_t> d_bin_rows;
     uint64_t query_v = 0;
     DeviceBuffer<uint32_t> d_te0;
     GroupLaunch once;                  /* b200dpf_group_eval and _eval_device: planned by every call */
@@ -1370,14 +1362,6 @@ int b200dpf_key_unpack_xor(const uint8_t *in, size_t in_len, int32_t *key)
 
 }  // extern "C"
 
-/* Staged rows [rows][cols] to device rows [rows][stride] in the same order (a trimmed table): the permutation of
- * launch_permute_table with every row in one leaf of 2^31 rows, which leaves the order as it is */
-static cudaError_t copy_rows(const int32_t *stage, int32_t *table, int64_t rows, int cols, int stride, int sm_count,
-                             cudaStream_t stream)
-{
-    return launch_permute_table(stage, table, (uint64_t)rows, 0, 31, cols, stride, sm_count, stream);
-}
-
 /* b200dpf_create, b200dpf_create_et, b200dpf_create_xor and (`trimmed`) b200dpf_create_trimmed: a context for keys
  * of `kind` */
 static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int device, int shard_rank,
@@ -1418,12 +1402,11 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
         c->trim_log2 = trim_log2_of(n, kind);
         c->n_local = (n + ((int64_t)1 << c->trim_log2) - 1) >> c->trim_log2 << c->trim_log2;
     }
+    c->place = RowPlacement{0, (uint32_t)n, lane_bits, trimmed ? (int)PLACE_IDENTITY : c->depth_local,
+                            (uint32_t)shard_count - 1u, bitrev((uint32_t)shard_rank, c->shard_bits), c->shard_bits};
 
-    /* Table: gather this shard's rows (natural indices j*G + bitrev_g(rank)),
-     * then permute on the device into breadth-first leaf order, padded to
-     * 64-byte rows.  dpf_wrapper.cu:103-115 does the analogous reorder on the
-     * host with one ATen call per element.  On an early-terminated context the
-     * same is done to runs of 2^lane_bits rows, one leaf each. */
+    /* Table: gather this shard's rows, then place them on the device (RowPlacement), padded to 64-byte
+     * rows.  dpf_wrapper.cu:103-115 does the analogous reorder on the host with one ATen call per element. */
     {   /* a device-resident table may still be being written on the caller's stream (e.g. a dtype
          * cast enqueued just before this call): our copy runs on a private non-blocking stream,
          * so wait for the producing device first */
@@ -1448,8 +1431,8 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     cudaError_t e = cudaSuccess;
     if (shard_count == 1) {
         e = cudaMemcpyAsync(d_stage.ptr, table, stage_bytes, cudaMemcpyDefault, c->stream);
-    } else {
-        const int32_t *src = table + ((size_t)bitrev_host((uint32_t)shard_rank, c->shard_bits) << lane_bits) * entry_size;
+    } else {   /* the shard's leaves, own_val + k * shard_count for k = 0, 1, ..., in order */
+        const int32_t *src = table + ((size_t)c->place.own_val << lane_bits) * entry_size;
         cudaPointerAttributes attr;
         const bool on_device = cudaPointerGetAttributes(&attr, table) == cudaSuccess &&
                                (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
@@ -1470,9 +1453,7 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    if (trimmed) CUDA_TRY(copy_rows(d_stage.ptr, c->d_table.ptr, n, entry_size, c->entry_pad, c->sm_count, c->stream));
-    else CUDA_TRY(launch_permute_table(d_stage.ptr, c->d_table.ptr, (uint64_t)c->n_local, c->depth_local, lane_bits, entry_size,
-                                       c->entry_pad, c->sm_count, c->stream));
+    CUDA_TRY(launch_fill_table(d_stage.ptr, c->d_table.ptr, c->place, entry_size, c->entry_pad, c->sm_count, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     d_stage.release();
 
@@ -2050,11 +2031,10 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     rc = d_stage.reserve((size_t)stage_rows * entry_size * sizeof(int32_t));
     if (rc) return rc;
     uint64_t row0 = 0;
-    std::vector<uint2> bin_info, query_bins;
-    std::vector<uint32_t> bin_rows;
+    std::vector<RowPlacement> place;
+    std::vector<uint2> query_bins;
     for (int g = 0; g < nbins; g++) {
-        /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), 64-byte rows; a
-         * leaf's 2^lane_bits rows stay adjacent.  A trimmed bin keeps the caller's row order. */
+        /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), or trimmed in row order */
         const int depth = ilog2(trimmed ? trimmed_domain_of(n[g], kind) : n[g]) - lane_bits;
         const int gran = trimmed ? trim_log2_of(n[g], kind) : depth + lane_bits;
         B->n.push_back(n[g]);
@@ -2062,29 +2042,21 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         B->row_off.push_back(row0);
         B->rows.push_back((n[g] + ((int64_t)1 << gran) - 1) >> gran << gran);
         B->room.push_back(gran - lane_bits);
-        bin_info.push_back(make_uint2((uint32_t)row0, trimmed ? (uint32_t)n[g] : (uint32_t)depth));
+        place.push_back(RowPlacement{row0, (uint32_t)n[g], lane_bits, trimmed ? (int)PLACE_IDENTITY : depth, 0, 0, 0});
         query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)depth));
-        bin_rows.push_back((uint32_t)n[g]);
         B->query_v += b200dpf_key_packed_size(depth) / 16u;
         CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
-        int32_t *dst = c->d_table.ptr + row0 * (uint64_t)c->entry_pad;
-        if (trimmed) CUDA_TRY(copy_rows(d_stage.ptr, dst, n[g], entry_size, c->entry_pad, c->sm_count, c->stream));
-        else CUDA_TRY(launch_permute_table(d_stage.ptr, dst, (uint64_t)n[g], depth, lane_bits, entry_size, c->entry_pad,
-                                           c->sm_count, c->stream));
+        CUDA_TRY(launch_fill_table(d_stage.ptr, c->d_table.ptr, place.back(), entry_size, c->entry_pad, c->sm_count, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
         row0 += (uint64_t)B->rows.back();
     }
-    const size_t bins_bytes = (size_t)nbins * sizeof(uint2);
-    rc = B->d_bin_info.reserve(bins_bytes);
+    const size_t bins_bytes = (size_t)nbins * sizeof(uint2), place_bytes = (size_t)nbins * sizeof(RowPlacement);
+    rc = B->d_place.reserve(place_bytes);
     if (!rc) rc = B->d_bins.reserve(bins_bytes);
-    if (!rc && trimmed) rc = B->d_bin_rows.reserve((size_t)nbins * sizeof(uint32_t));
     if (!rc) rc = B->d_te0.reserve(256 * sizeof(uint32_t));
     if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(B->d_bin_info.ptr, bin_info.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(B->d_place.ptr, place.data(), place_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_bins.ptr, query_bins.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
-    if (trimmed)
-        CUDA_TRY(cudaMemcpyAsync(B->d_bin_rows.ptr, bin_rows.data(), (size_t)nbins * sizeof(uint32_t), cudaMemcpyHostToDevice,
-                                 c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read them once the context is returned */
     *out = c.release();
@@ -2405,7 +2377,7 @@ int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, 
     p.count = nqueries * nbins;
     p.lane_bits = k.lane_bits;
     p.bins = B->d_bins.ptr;
-    p.bin_rows = B->d_bin_rows.ptr;   /* null unless trimmed */
+    p.bin_place = B->d_place.ptr;
     p.nq = (uint32_t)nqueries;
     p.nbins = (uint32_t)nbins;
     p.query_v = B->query_v;
@@ -2480,20 +2452,14 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     std::memset(&u, 0, sizeof u);
     u.idx = idx;
     u.bins = bins;
-    u.identity = c->trimmed;
     if (bins) {
-        u.bin_info = c->bins->d_bin_info.ptr;
+        u.bin_place = c->bins->d_place.ptr;
         u.nbins = (int)c->bins->n.size();
     }
+    u.place = c->place;
     u.rows = rows;
     u.count = count;
-    u.n = c->n;
-    u.own_mask = (uint32_t)c->shard_count - 1u;
-    u.own_val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
-    u.shift = c->shard_bits;
-    u.depth = c->depth_local;
     u.table_rows = (uint32_t)update_table_rows(c);
-    u.lane_bits = c->lane_bits();
     u.table = c->d_table.ptr;
     u.cols = c->entry_size;
     u.stride = c->entry_pad;
@@ -2515,9 +2481,8 @@ int update_host_enqueue(b200dpf_ctx *c, const int64_t *idx, const int32_t *bins,
     std::vector<int64_t> own_idx;
     std::vector<int32_t> own_rows;
     if (c->shard_count > 1) {             /* a shard copies only its own rows */
-        const uint32_t mask = (uint32_t)c->shard_count - 1u, val = bitrev_host((uint32_t)c->shard_rank, c->shard_bits);
         for (int64_t j = 0; j < count; j++)
-            if (((uint32_t)(idx[j] >> c->lane_bits()) & mask) == val) {
+            if (c->place.owns(idx[j])) {
                 own_idx.push_back(idx[j]);
                 own_rows.insert(own_rows.end(), rows + j * c->entry_size, rows + (j + 1) * c->entry_size);
             }

@@ -448,6 +448,18 @@ DPF_HD Seed expand_one(const TA &ta, const Seed &parent, uint32_t pos)
     return aes128_one(ta, parent, pos);
 }
 
+/* The low `bits` bits of v in reverse order, bits in [0, 32]; 0 when bits = 0. */
+DPF_HD uint32_t bitrev(uint32_t v, int bits)
+{
+#if DPF_DEVICE_CODE
+    return bits ? __brev(v) >> (32 - bits) : 0u;
+#else
+    uint32_t r = 0;
+    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
+    return r;
+#endif
+}
+
 /* ---- tree traversal ------------------------------------------------------ */
 /*
  * Tree conventions (dpf_base/dpf.h:362-377, EvaluateFlat): the root consumes

@@ -362,12 +362,6 @@ struct CpuEnv {
     Seed pop(int h) const { return stack[h]; }
     void leaf_prefetch(uint32_t) {}
     void node_pair(uint32_t, const Seed &, const Seed &) {}
-    static uint32_t bitrev(uint32_t v, int bits)
-    {
-        uint32_t r = 0;
-        for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
-        return r;
-    }
     void leaf_pair(uint32_t local_pos, uint32_t v0, uint32_t v1)
     {
         /* position p holds index bitrev_depth(p) */

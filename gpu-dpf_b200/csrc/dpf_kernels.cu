@@ -982,50 +982,37 @@ __global__ void probe_smem_kernel(uint32_t *out)
     if (threadIdx.x == 0) *out = (uint32_t)__cvta_generic_to_shared(g_dyn_smem);
 }
 
-__device__ __forceinline__ uint32_t bitrev_bits(uint32_t v, int bits) { return bits ? __brev(v) >> (32 - bits) : 0u; }
-
-/* runs of 2^lane_bits rows (one leaf) move together: table[q] = stage[(bitrev_bits(q >> lane_bits) << lane_bits)
- * | (q & (2^lane_bits - 1))] */
-__global__ void permute_table_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table,
-                                     uint64_t rows, int bits, int lane_bits, int cols, int stride)
+/* table[P.first + q][c] = the stage's copy of natural row P.natural_row(q), for q < rows, c < cols.  The stage holds
+ * P's own rows in natural order, a shard's leaf v at stage leaf v >> P.shift. */
+__global__ void fill_table_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table, const RowPlacement P,
+                                  uint64_t rows, int cols, int stride)
 {
     const uint64_t total = rows * (uint64_t)cols;
-    const uint64_t lane_mask = (1u << lane_bits) - 1u;
+    const uint64_t lane_mask = (1u << P.lane_bits) - 1u;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t q = i / (uint64_t)cols;
         const int c = (int)(i - q * (uint64_t)cols);
-        const uint64_t src = ((uint64_t)bitrev_bits((uint32_t)(q >> lane_bits), bits) << lane_bits) | (q & lane_mask);
-        table[q * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
+        const uint64_t r = (uint64_t)P.natural_row(q);
+        const uint64_t src = ((r >> (P.lane_bits + P.shift)) << P.lane_bits) | (r & lane_mask);
+        table[(P.first + q) * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
     }
 }
 
-/* row update, step 1: natural index -> table row (the mapping documented on UpdateParams) or the skip
- * marker, occurrence number j */
+/* row update, step 1: natural row -> device row (UpdateParams) or the skip marker, occurrence number j */
 __global__ void __launch_bounds__(256) update_map_kernel(const UpdateParams u, uint32_t *__restrict__ pos,
                                                          uint32_t *__restrict__ ord)
 {
-    const uint32_t lane_mask = (1u << u.lane_bits) - 1u;
     for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < u.count; j += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = u.idx[j];
-        const uint32_t leaf = (uint32_t)(i >> u.lane_bits), lane = (uint32_t)i & lane_mask;
-        uint32_t p = u.table_rows;
+        RowPlacement P = u.place;
+        bool in_range = true;
         if (u.bins) {
             const int32_t g = u.bins[j];
-            if (g >= 0 && g < u.nbins) {
-                const uint2 info = u.bin_info[g];
-                if (u.identity) {
-                    if (i >= 0 && i < (int64_t)info.y) p = info.x + (uint32_t)i;
-                } else if (i >= 0 && i < ((int64_t)1 << (info.y + u.lane_bits))) {
-                    p = info.x + ((bitrev_bits(leaf, (int)info.y) << u.lane_bits) | lane);
-                }
-            }
-        } else if (u.identity) {
-            if (i >= 0 && i < u.n) p = (uint32_t)i;
-        } else if (i >= 0 && i < u.n && (leaf & u.own_mask) == u.own_val) {
-            p = (bitrev_bits(leaf >> u.shift, u.depth) << u.lane_bits) | lane;
+            in_range = g >= 0 && g < u.nbins;
+            if (in_range) P = u.bin_place[g];
         }
-        pos[j] = p;
+        pos[j] = in_range && P.owns(i) ? (uint32_t)P.device_row(i) : u.table_rows;
         ord[j] = (uint32_t)j;
     }
 }
@@ -1210,14 +1197,15 @@ cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t wo
     return cudaGetLastError();
 }
 
-cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits, int lane_bits,
-                                 int cols, int stride, int sm_count, cudaStream_t stream)
+cudaError_t launch_fill_table(const int32_t *stage, int32_t *table, const RowPlacement &P, int cols, int stride,
+                              int sm_count, cudaStream_t stream)
 {
+    const uint64_t rows = (uint64_t)P.n >> P.shift;   /* the rows P owns: n, or n / 2^shift of a shard */
     const uint64_t total = rows * (uint64_t)cols;
     const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
     int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
     if (grid < 1) grid = 1;
-    permute_table_kernel<<<grid, 256, 0, stream>>>(stage, table, rows, bits, lane_bits, cols, stride);
+    fill_table_kernel<<<grid, 256, 0, stream>>>(stage, table, P, rows, cols, stride);
     return cudaGetLastError();
 }
 

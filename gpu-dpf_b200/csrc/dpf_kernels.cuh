@@ -11,6 +11,53 @@
 
 namespace b200dpf {
 
+/* RowPlacement::depth of a trimmed table or bin, which keeps the caller's row order */
+enum { PLACE_IDENTITY = -1 };
+
+/* Where the rows of one table live in the device table of its context: a whole table, one shard of one (an entry
+ * range, DESIGN.md section 5) or one bin of a grouped context.  Table creation, row updates and the key generator all
+ * read it from here.  Natural row i is row i & (2^lane_bits - 1) of leaf v = i >> lane_bits; a leaf's rows stay
+ * adjacent.
+ *   owns(i)        0 <= i < n and (v & own_mask) == own_val.  Shard r of G = 2^shift owns the leaves under tree node r
+ *                  of level `shift`, those with bitrev(v mod G, shift) = r (own_mask = G - 1, own_val = bitrev(r, shift));
+ *                  any other placement has no shards (mask, value and shift 0).
+ *   device_row(i)  first + (bitrev(v >> shift, depth) << lane_bits | (i & (2^lane_bits - 1))): breadth-first leaf order
+ *                  over the depth leaf levels below the shard's root, the order the evaluation kernels walk the tree in.
+ *                  A trimmed table or bin (depth = PLACE_IDENTITY) stores row i at device row first + i.
+ *   natural_row(q) the natural row held by device row first + q, the inverse of device_row. */
+struct RowPlacement {
+    uint64_t first;           /* first device row */
+    uint32_t n;               /* live rows: natural rows [0, n) */
+    int lane_bits;            /* log2 rows per leaf: 0, 2 (early-terminated keys) or 7 (XOR-shared keys) */
+    int depth;                /* width of the leaf bit reversal, or PLACE_IDENTITY */
+    uint32_t own_mask, own_val;
+    int shift;                /* log2 shards */
+
+    DPF_HD bool owns(int64_t i) const
+    {
+        return i >= 0 && i < (int64_t)n && ((uint32_t)(i >> lane_bits) & own_mask) == own_val;
+    }
+    DPF_HD uint64_t device_row(int64_t i) const
+    {
+        if (depth == PLACE_IDENTITY) return first + (uint64_t)i;
+        const uint32_t leaf = bitrev((uint32_t)(i >> lane_bits) >> shift, depth);
+        return first + (((uint64_t)leaf << lane_bits) | ((uint32_t)i & ((1u << lane_bits) - 1u)));
+    }
+    DPF_HD int64_t natural_row(uint64_t q) const
+    {
+        if (depth == PLACE_IDENTITY) return (int64_t)q;
+        const uint32_t leaf = bitrev((uint32_t)(q >> lane_bits), depth) << shift | own_val;
+        return ((int64_t)leaf << lane_bits) | (int64_t)(q & ((1u << lane_bits) - 1u));
+    }
+};
+
+/* The key index of row r of a trimmed table whose tree has `depth` leaf levels (b200dpf_trimmed_alpha): r sits at leaf
+ * position r >> lane_bits, which the key reaches as leaf bitrev(r >> lane_bits, depth). */
+DPF_HD uint64_t trimmed_alpha(uint64_t r, int depth, int lane_bits)
+{
+    return ((uint64_t)bitrev((uint32_t)(r >> lane_bits), depth) << lane_bits) | (r & ((1u << lane_bits) - 1u));
+}
+
 /* One traversal phase of a launch: which subtrees the work items are, where an item starts and
  * which ticket counters hand the items out. */
 struct PhaseParams {
@@ -258,10 +305,9 @@ struct KeygenParams {
     int64_t count;
     int depth, lane_bits;      /* depth: flat batches only */
     const uint2 *bins;         /* query batches: [nbins] (uint4 offset of the key in a compact query, depth) */
-    /* query batches of a trimmed context: [nbins] live rows n_g.  Key g of query q is then for row
-     * alphas[q][g] mod n_g (non-negative), placed at index (bitrev_depth(r >> lane_bits) << lane_bits) |
-     * (r & (2^lane_bits - 1)) of the tree's domain, as b200dpf_trimmed_alpha; null: the low bits of alpha */
-    const uint32_t *bin_rows;
+    /* query batches: [nbins] the bins' placements.  Key g of query q of a trimmed bin (depth PLACE_IDENTITY) is for
+     * row alphas[q][g] mod n (non-negative), at index trimmed_alpha of it; of any other bin for the low bits of alpha */
+    const RowPlacement *bin_place;
     uint32_t nq, nbins;
     uint64_t query_v;          /* uint4 per compact query */
     int compact;
@@ -274,12 +320,12 @@ cudaError_t launch_keygen(int prf, int group, const KeygenParams &p, cudaStream_
 /* Maximum dynamic shared memory the evaluation kernel may be given. */
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
-/* table[q][c] = stage[(bitrev_bits(q >> lane_bits) << lane_bits) | (q & (2^lane_bits - 1))][c] for
- * q < rows, c < cols: rows move in runs of 2^lane_bits (one leaf; 4 on early-terminated contexts),
- * rows = 2^(bits + lane_bits).  Padded columns [cols, stride) are left untouched (pre-zeroed).  The
- * grid-stride helpers take the device's SM count to cap their grids at a few waves. */
-cudaError_t launch_permute_table(const int32_t *stage, int32_t *table, uint64_t rows, int bits, int lane_bits,
-                                 int cols, int stride, int sm_count, cudaStream_t stream);
+/* Table creation: device row P.device_row(i) of `table` := stage row i for every row i that P owns, the stage
+ * holding P's own rows, [rows][cols], in natural order (a shard's leaf v at stage leaf v >> P.shift).  Padded columns
+ * [cols, stride) are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM count to cap their
+ * grids at a few waves. */
+cudaError_t launch_fill_table(const int32_t *stage, int32_t *table, const RowPlacement &P, int cols, int stride,
+                              int sm_count, cudaStream_t stream);
 
 /* Device-resident grouped evaluation (dpf_group_io.cu), one warp per key, no host synchronisation.
  * order[pos] = (the caller's index of the key at bin-sorted position pos, the depth of its bin).
@@ -297,34 +343,18 @@ cudaError_t launch_group_scatter(const int32_t *sorted, const uint2 *order, int6
 cudaError_t launch_group_gather_queries(const void *queries, const uint2 *bins, int64_t nkeys, uint32_t nq, uint64_t query_v,
                                         uint32_t magic, uint32_t stride_v, void *compact, cudaStream_t stream);
 
-/* Row update of a live table (b200dpf_update_rows*): table row position(idx[j]) := rows[j] for
- * j < count, the last occurrence of a position winning.  Natural index i is row i & (2^lane_bits - 1)
- * of leaf v = i >> lane_bits, and its position is
- *   bins == null   skip unless 0 <= i < n and (v & own_mask) == own_val;
- *                  else bitrev_depth(v >> shift) << lane_bits | (i & (2^lane_bits - 1))
- *                                                                     (whole table or one shard)
- *   bins != null   bin g = bins[j] (skip unless 0 <= g < nbins; .y = the bin's leaf depth);
- *                  skip unless 0 <= i < 2^(bin_info[g].y + lane_bits);
- *                  else bin_info[g].x + (bitrev_{bin_info[g].y}(v) << lane_bits | (i & (2^lane_bits - 1)))
- *                                                                     (grouped context)
- * With `identity` (trimmed contexts, which store row i at device row i) the index is the row number and
- *   bins == null   skip unless 0 <= i < n; else i
- *   bins != null   skip unless 0 <= i < bin_info[g].y (the bin's rows); else bin_info[g].x + i
- * Skipped entries are never written. */
+/* Row update of a live table (b200dpf_update_rows*): device row P.device_row(idx[j]) := rows[j] for j < count, the
+ * last occurrence of a device row winning.  P is bin_place[bins[j]] on a grouped context, else `place`; entry j is
+ * skipped, never written, when bins[j] is not in [0, nbins) or P does not own idx[j]. */
 struct UpdateParams {
-    const int64_t *idx;       /* [count] natural indices (trimmed contexts: row numbers)      */
+    const int64_t *idx;       /* [count] natural rows                                         */
     const int32_t *bins;      /* [count] bin ids, or null                                     */
-    const uint2 *bin_info;    /* [nbins] (first row, depth), trimmed: (first row, rows)       */
-    int identity;
+    const RowPlacement *bin_place;   /* [nbins] the bins' placements                          */
     int nbins;
+    RowPlacement place;       /* the context's own placement (bins == null)                   */
     const int32_t *rows;      /* [count][cols] new rows                                       */
     int64_t count;            /* <= 2^31 - 1                                                  */
-    int64_t n;
-    uint32_t own_mask, own_val;
-    int shift, depth;
-    uint32_t table_rows;      /* rows of the device table: the skip marker, larger than every position */
-    int lane_bits;            /* log2 rows per leaf: 0, or 2 on an early-terminated context
-                                 (it fills the alignment gap before `table`)                      */
+    uint32_t table_rows;      /* rows of the device table: the skip marker, larger than every device row */
     int32_t *table;           /* [table_rows][stride], 64-byte rows; pad columns are not touched */
     int cols, stride;
 };

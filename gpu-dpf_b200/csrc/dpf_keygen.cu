@@ -175,18 +175,17 @@ __global__ void __launch_bounds__(64, 1) keygen_kernel(const KeygenParams p)
         idx = (int64_t)q * p.nbins + g;
         depth = (int)b.y;
         off_v = p.compact ? (uint64_t)q * p.query_v + b.x : (uint64_t)idx * 131u;
-        if (p.bin_rows) rows = p.bin_rows[g];
+        if (p.bin_place[g].depth == PLACE_IDENTITY) rows = p.bin_place[g].n;
     }
     const KeyOut out{p.out_a + off_v, p.out_b + off_v, p.compact != 0};
 
     /* the key for the low depth + lane_bits bits of alpha: its leaf, and the payload at level 0 (beta = 1,
      * dpf_wrapper.cu:53; early-terminated: lane alpha & 3 of the leaf; XOR-shared: bit alpha & 127) */
     uint64_t a_row = (uint64_t)p.alphas[idx];
-    if (rows != 0) {   /* row r = alpha mod n_g of a trimmed bin sits at leaf position r >> lane_bits */
+    if (rows != 0) {   /* row r = alpha mod n_g of a trimmed bin */
         int64_t r = p.alphas[idx] % (int64_t)rows;
         if (r < 0) r += rows;
-        const uint64_t leaf = __brev((uint32_t)((uint64_t)r >> p.lane_bits)) >> (32 - depth);
-        a_row = (leaf << p.lane_bits) | ((uint64_t)r & ((1u << p.lane_bits) - 1u));
+        a_row = trimmed_alpha((uint64_t)r, depth, p.lane_bits);
     }
     const uint64_t alpha = (a_row & ((((uint64_t)1) << (depth + p.lane_bits)) - 1u)) >> p.lane_bits;
     u128 beta[32];
