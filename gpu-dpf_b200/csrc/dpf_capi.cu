@@ -107,6 +107,15 @@ template <class T> using PinnedBuffer = Buffer<T, true>;
 
 constexpr size_t kKeyBytes = host::KEY_WORDS * sizeof(int32_t);   /* one key in the wire format */
 
+/* The shape of one table or bin, made by table_shape.  Its keys are made for 2^(depth + lane_bits) rows. */
+struct TableShape {
+    int64_t n;          /* live rows */
+    int depth;          /* leaf levels of the key tree */
+    int64_t rows;       /* rows of the device table, padding included */
+    int room;           /* log2 leaves of the largest work item inside those rows: depth, or less if trimmed */
+    uint64_t first;     /* first device row */
+};
+
 }  // namespace
 
 struct SmemLayoutCache;   /* per (prf, nv, mode) launch layouts, filled on first use */
@@ -118,24 +127,22 @@ struct b200dpf_ctx {
     std::unique_ptr<GroupBins> bins;     /* non-null: grouped (batch-PIR) context, use b200dpf_group_eval */
     std::unique_ptr<SmemLayoutCache> layouts;
     int device = 0;
-    int64_t n = 0;
-    int depth = 0;
+    TableShape shape{};      /* the whole table's; grouped: the largest bin's n, the deepest bin's depth, all bins' rows */
     int entry_size = 0;
     int entry_pad = 0;       /* row length in int32: 16, 32 or a multiple of 64     */
     int shard_rank = 0, shard_count = 1, shard_bits = 0;
-    int64_t n_local = 0;
-    int depth_local = 0;
+    /* this shard's part of the table: the tree below the shard root and the rows of d_table */
+    int depth_local() const { return shape.depth - shard_bits; }
+    int64_t rows_local() const { return shape.rows >> shard_bits; }
     /* the kind of key the context takes (host::KindInfo): standard, early-terminated (b200dpf_create_et) or
-     * XOR-shared (b200dpf_create_xor).  A leaf carries 2^lane_bits() table rows: n, n_local, the table, the
-     * leaf cache and the results count rows; depth, depth_local, the shards, the work items and the
-     * frontier count leaves. */
+     * XOR-shared (b200dpf_create_xor).  A leaf carries 2^lane_bits() table rows: the shape's n and rows, the
+     * table, the leaf cache and the results count rows; depths, the shards, the work items and the frontier
+     * count leaves. */
     int kind = host::KIND_STANDARD;
     int lane_bits() const { return host::kKinds[kind].lane_bits; }
     /* trimmed (b200dpf_create_trimmed, b200dpf_group_create_trimmed): row r is device row r, at leaf position
-     * r >> lane_bits of a tree over trimmed_domain(n) rows, and the device table (n_local rows; per bin on a
-     * grouped context) is zero-padded to a multiple of 2^trim_log2 rows only.  n is the live rows. */
+     * r >> lane_bits of a tree over trimmed_domain(n) rows (table_shape) */
     bool trimmed = false;
-    int trim_log2 = 0;
     RowPlacement place{};             /* where this table's (or shard's) rows live in d_table; not used when grouped */
     DeviceBuffer<int32_t> d_table;
     cudaStream_t stream = nullptr;
@@ -262,7 +269,7 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
     budget &= ~15;
     L->budget = budget;
 
-    L->meta_cw = (uint32_t)c->depth * 4u * 32u * 16u;
+    L->meta_cw = (uint32_t)c->shape.depth * 4u * 32u * 16u;
     const uint32_t kMetaSmall = 512u + 512u + 16u;
     const uint32_t meta = L->meta_cw + kMetaSmall;
     L->level_bytes = (uint32_t)L->threads * 16u;
@@ -283,7 +290,7 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
             L->off_meta = 0; a_used = L->meta_cw;
             L->off_small = b_off; b_used = kMetaSmall;
         }
-        else return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->depth);
+        else return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->shape.depth);
         a_used = (a_used + 15u) & ~15u;
         b_used = (b_used + 15u) & ~15u;
         L->off_lo = b_off + b_used;
@@ -295,7 +302,7 @@ int smem_layout_compute(b200dpf_ctx *c, int prf, int nv, int mode, SmemLayout *L
         L->off_meta = 0;
         L->off_small = L->meta_cw;
         L->off_lo = (meta + 15u) & ~15u;
-        if ((int64_t)budget < (int64_t)L->off_lo) return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->depth);
+        if ((int64_t)budget < (int64_t)L->off_lo) return fail(B200DPF_EINVAL, "depth %d needs more shared memory than available", c->shape.depth);
         L->cap_lo = (int)(((uint32_t)budget - L->off_lo) / L->level_bytes);
         L->off_hi = L->off_lo;
         L->cap_hi = 0;
@@ -397,11 +404,7 @@ constexpr KindOps kKindOps[host::KIND_COUNT] = {
 
 /* Trimmed tables (DESIGN.md section 11).  Row r of an n-row table sits at leaf position r >> lane_bits of a tree
  * over N = trimmed_domain(n) rows (the next power of two, at least the kind's n_min), so the live rows are a
- * prefix of the leaf positions and the work items past it are never issued.  The device table is padded with
- * zero rows to a multiple of 2^trim_log2 rows, where one granule is N/128 rows on a large table (the padding is
- * then below N/128 < n/64) and never less than one work item of the smallest size the launch planner keeps for
- * the kind: 64 leaves of standard and early-terminated keys, 1 leaf pair of XOR-shared ones (whose leaves are
- * 128 rows of work).  Every issued item lies inside the padded rows. */
+ * prefix of the leaf positions and the work items past it are never issued. */
 bool trim_args_ok(int64_t n, int kind) { return kind >= 0 && kind < host::KIND_COUNT && n >= 1 && n <= ((int64_t)1 << 31); }
 
 int64_t trimmed_domain_of(int64_t n, int kind)
@@ -409,17 +412,40 @@ int64_t trimmed_domain_of(int64_t n, int kind)
     return std::max<int64_t>((int64_t)1 << ilog2(n), host::kKinds[kind].n_min);
 }
 
-int trim_log2_of(int64_t n, int kind)
-{
-    const int log_n = ilog2(trimmed_domain_of(n, kind));
-    const int item_leaves_log2 = kKindOps[kind].leaf_items ? 1 : 6;
-    return std::min(log_n, std::max(log_n - 7, host::kKinds[kind].lane_bits + item_leaves_log2));
-}
-
 int64_t trimmed_alpha_of(int64_t row, int64_t n, int kind)
 {
     const int b = host::kKinds[kind].lane_bits;
     return (int64_t)trimmed_alpha((uint64_t)row, ilog2(trimmed_domain_of(n, kind)) - b, b);
+}
+
+/* The shape of a table of n rows (bin < 0) or of bin `bin` for keys of `kind` (valid), or EINVAL for an n out of
+ * range: a power of two in [n_min, 2^31], or when trimmed any n in [1, 2^31].  The device table is padded with
+ * zero rows to a multiple of 2^g rows (one granule).  Untrimmed, that is the whole table.  Trimmed, one granule is
+ * N/128 rows on a large table (the padding is then below N/128 < n/64) and never less than one work item of the
+ * smallest size the launch planner keeps for the kind: 64 leaves of standard and early-terminated keys, 1 leaf
+ * pair of XOR-shared ones (whose leaves are 128 rows of work).  Every issued item lies inside the padded rows. */
+int table_shape(int64_t n, int kind, bool trimmed, int bin, TableShape *t)
+{
+    const host::KindInfo &k = host::kKinds[kind];
+    if (trimmed ? !trim_args_ok(n, kind) : (n < k.n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0)) {
+        char where[32] = "table";
+        if (bin >= 0) snprintf(where, sizeof where, "bin %d:", bin);
+        if (trimmed) return fail(B200DPF_EINVAL, "%s size n=%lld out of range [1, 2^31]", where, (long long)n);
+        return fail(B200DPF_EINVAL, "%s size n=%lld must be a power of two in [%lld, 2^31]", where, (long long)n,
+                    (long long)k.n_min);
+    }
+    const int log_n = ilog2(trimmed ? trimmed_domain_of(n, kind) : n);
+    const int item_leaves_log2 = kKindOps[kind].leaf_items ? 1 : 6;
+    const int g = trimmed ? std::min(log_n, std::max(log_n - 7, k.lane_bits + item_leaves_log2)) : log_n;
+    *t = TableShape{n, log_n - k.lane_bits, (n + ((int64_t)1 << g) - 1) >> g << g, g - k.lane_bits, 0};
+    return B200DPF_OK;
+}
+
+/* Where the rows of shape t live on the device, for shard `rank` of 2^shard_bits */
+RowPlacement place_of(const TableShape &t, int lane_bits, bool trimmed, int rank, int shard_bits)
+{
+    return RowPlacement{t.first, (uint32_t)t.n, lane_bits, trimmed ? (int)PLACE_IDENTITY : t.depth - shard_bits,
+                        (1u << shard_bits) - 1u, bitrev((uint32_t)rank, shard_bits), shard_bits};
 }
 
 /* "a standard", "an early-terminated", "an XOR-shared": the article of a kind's name */
@@ -432,10 +458,13 @@ int fail_not_kind(int kind, const char *name)
     return fail(B200DPF_EINVAL, "%s: not an %s key", name, host::kKinds[kind].name);
 }
 
-/* Key number `b` of a batch (null: none) must be a key of `kind` for the n rows of the context's table, or
- * of its bin `bin` (>= 0).  Only a refused key is decoded twice. */
-int check_key(int kind, int64_t n, const int32_t *key, int64_t b, int bin)
+/* Key number `b` of a batch (null: none) must be a key of the context's kind for its table, or its bin `bin` (>= 0),
+ * of shape t: for n = 2^(t.depth + lane_bits) rows, the table's rows or trimmed_domain(rows).  Only a refused key is
+ * decoded twice. */
+int check_key(const b200dpf_ctx *c, const TableShape &t, const int32_t *key, int64_t b, int bin)
 {
+    const int kind = c->kind;
+    const int64_t n = (int64_t)1 << (t.depth + c->lane_bits());
     const int64_t kn = key ? host::key_n(key, kind) : -1;
     if (kn == n) return B200DPF_OK;
     const int other = key ? host::key_kind(key) : -1;
@@ -453,9 +482,6 @@ int check_key(int kind, int64_t n, const int32_t *key, int64_t b, int bin)
     return fail(B200DPF_EINVAL, "key %lld is not %s %s key for n=%lld (its n: %lld)", (long long)b, article(kind), k.name,
                 (long long)n, (long long)kn);
 }
-
-/* The n of the keys a context (or its bin of `depth` leaf levels) takes: its rows, or trimmed_domain(rows) */
-int64_t key_rows(const b200dpf_ctx *c, int depth) { return (int64_t)1 << (depth + c->lane_bits()); }
 
 void fill_phase(const SmemLayout &L, int s, PhaseParams *ph)
 {
@@ -531,11 +557,7 @@ struct GroupLaunch {
 }  // namespace
 
 struct GroupBins {
-    std::vector<int64_t> n;
-    std::vector<int> depth;
-    std::vector<uint64_t> row_off;     /* first row of the bin in d_table */
-    std::vector<int64_t> rows;         /* its rows in d_table: n, or on a trimmed context n padded (trim_log2_of) */
-    std::vector<int> room;             /* log2 leaves of the largest work item inside them: depth, or less if trimmed */
+    std::vector<TableShape> shape;     /* [nbins] */
     /* made at create, never rewritten: [nbins] the bins' placements, for row updates and the key generator; [nbins]
      * (uint4 offset of bin g's key in a compact query, depth of g), with query_v uint4 per query; the key generator's
      * AES table */
@@ -562,7 +584,7 @@ template <class Items> int shrink_s(int s, int s_floor, int64_t wanted, Items it
 }
 
 /* The work-item size of a key group of bin g on a grouped context */
-int group_s(const EvalPlan &P, const GroupBins &B, int g) { return std::max(1, std::min(B.room[(size_t)g], P.s_group)); }
+int group_s(const EvalPlan &P, const GroupBins &B, int g) { return std::max(1, std::min(B.shape[(size_t)g].room, P.s_group)); }
 
 /* The fields of EvalParams that every launch of job J on layout L shares; the others are zero. */
 void fill_common(const b200dpf_ctx *c, const SmemLayout &L, const EvalJob &J, const EvalPlan &P, EvalParams *p)
@@ -570,13 +592,13 @@ void fill_common(const b200dpf_ctx *c, const SmemLayout &L, const EvalJob &J, co
     std::memset(p, 0, sizeof *p);
     p->keys = reinterpret_cast<const uint4 *>(J.keys);
     p->key_stride_v = J.kl.stride_v; p->key_root_v = J.kl.root_v; p->key_compact = J.kl.compact;
-    p->depth = c->depth;
+    p->depth = c->shape.depth;
     p->nkeys = (int)J.nkeys; p->kpw_log2 = P.kpw_log2; p->key_groups = (int)P.key_groups;
     p->groups = J.groups; p->units = J.units; p->nunits = J.nunits;
     p->table = reinterpret_cast<const uint4 *>(c->d_table.ptr);
     p->row_stride_v = (uint32_t)c->entry_pad / 4u;
     p->out_stride = (uint32_t)c->entry_size;
-    p->n = (uint64_t)c->n;
+    p->n = (uint64_t)c->shape.n;
     p->off_cw = L.off_meta;
     p->off_cwlo = L.off_small;
     p->off_root = p->off_cwlo + 512u;
@@ -633,7 +655,7 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
      * tail. */
     const bool want_frontier = K.frontier != 0;
     if (K.subtree_log2 > 0) {
-        s = std::min(K.subtree_log2, std::min(c->depth_local, L.s_max));
+        s = std::min(K.subtree_log2, std::min(c->depth_local(), L.s_max));
     } else {
         /* B=512 E=16, frontier on, 1x H100 SXM 80 GB at a 400 W power limit, DPFs/s (run-to-run
          * spread about 3 %); the automatic choice is within the spread of the best fixed s:
@@ -648,8 +670,8 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
          *   n=2^20: auto 0.971; s=1 0.989, 2 0.980, 3 0.971, 4 0.975, 5 0.975, 6 0.973 */
         const int s_floor = ops.leaf_items ? 1 : want_frontier ? 3 : 5;
         const int64_t items_per_warp = ops.leaf_items ? ops.leaf_items : want_frontier ? 24 : 6;
-        s = shrink_s(std::min(c->depth_local, std::min(L.s_max, s_cap)), s_floor, items_per_warp * warps, [&](int t) {
-            return ((c->n_local >> (t + c->lane_bits())) * key_groups) >> (5 - kpw_log2);
+        s = shrink_s(std::min(c->depth_local(), std::min(L.s_max, s_cap)), s_floor, items_per_warp * warps, [&](int t) {
+            return ((c->rows_local() >> (t + c->lane_bits())) * key_groups) >> (5 - kpw_log2);
         });
     }
     if (s < 1) s = 1;
@@ -670,14 +692,14 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         /* a ticket (2^(s + spw_log2) leaves) must not reach past the padded rows: smaller items first (down to
          * one leaf pair), then fewer subtrees per warp.  Lanes of a key quad trade leaf values by SHFL, so every
          * lane of an issued ticket runs; the padding is what keeps its rows inside the table. */
-        const int room = c->trim_log2 - c->lane_bits();
+        const int room = c->shape.room;
         s = std::max(1, std::min(s, room - (5 - kpw_log2)));
         if (5 - kpw_log2 > room - s) {
             kpw_log2 = 5 - (room - s);
             key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
         }
     }
-    const int rel = c->depth_local - s;           /* tree levels between the shard root and the items */
+    const int rel = c->depth_local() - s;           /* tree levels between the shard root and the items */
     if (5 - kpw_log2 > rel) {                     /* not enough subtrees to split a warp that far */
         kpw_log2 = 5 - rel;
         key_groups = (nkeys + ((int64_t)1 << kpw_log2) - 1) >> kpw_log2;
@@ -734,9 +756,9 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         fill_phase(LF, s_top, &P.top);
         P.top.nsub = (uint32_t)1 << (f_rel - s_top);
         P.top.sub_first = (uint32_t)c->shard_rank << (f_rel - s_top);
-        P.top.walk_first_level = c->depth - 1;
+        P.top.walk_first_level = c->shape.depth - 1;
         P.top.walk_steps = c->shard_bits + f_rel - s_top;
-        P.top.level_base = c->depth_local - f_rel;
+        P.top.level_base = c->depth_local() - f_rel;
         P.smem_top = smem_bytes(LF, s_top);
         P.nfront = (uint32_t)1 << f_rel;
     }
@@ -749,15 +771,15 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         P.smem = (size_t)P.off_tile + P.tile_bytes;
     }
     fill_phase(L, s, &P.main);
-    P.main.nsub = (uint32_t)(c->n_local >> (s + c->lane_bits()));   /* 2^rel, or the items over a trimmed table's rows */
+    P.main.nsub = (uint32_t)(c->rows_local() >> (s + c->lane_bits()));   /* 2^rel, or the items over a trimmed table's rows */
     P.main.sub_first = (uint32_t)c->shard_rank << rel;
     if (f_rel > 0) {
         P.main.front_shift = rel - f_rel;
-        P.main.walk_first_level = c->depth_local - f_rel - 1;
+        P.main.walk_first_level = c->depth_local() - f_rel - 1;
         P.main.walk_steps = rel - f_rel;
     } else {
-        P.main.walk_first_level = c->depth - 1;
-        P.main.walk_steps = c->depth - s;
+        P.main.walk_first_level = c->shape.depth - 1;
+        P.main.walk_steps = c->shape.depth - s;
     }
     if (P.one_launch) {
         const uint64_t items = (uint64_t)key_groups * (uint64_t)(P.top.nsub >> spw_log2);
@@ -769,7 +791,7 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
     /* ---- wide entries: the leaf-caching pass, then the MAC-only passes ---- */
     if (P.leaf_cache) {
         P.mode = ops.mode_fused;                   /* the kind's fused kernel, on the layout planned above */
-        P.leaf_cache_bytes = (size_t)key_groups * 32u * (size_t)c->n_local * sizeof(uint32_t);
+        P.leaf_cache_bytes = (size_t)key_groups * 32u * (size_t)c->rows_local() * sizeof(uint32_t);
         P.mac_tma = K.mac_tma != 0;
         /* register-staged variant: 8 warps per block */
         const int64_t mac_warps = (int64_t)c->sm_count * 2 * 8;
@@ -778,8 +800,8 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
         const int64_t kg_blocks = (key_groups + 7) / 8;
         const int64_t tr = std::max<int64_t>(1, (2 * (int64_t)c->sm_count + kg_blocks - 1) / kg_blocks);
         P.mac_grid = P.mac_tma ? c->sm_count : c->sm_count * 2;
-        P.mac_ranges = (uint32_t)(P.mac_tma ? std::min<int64_t>(tr, std::max<int64_t>(1, c->n_local / 256))
-                                            : std::min<int64_t>(ranges, std::max<int64_t>(1, c->n_local / 64)));
+        P.mac_ranges = (uint32_t)(P.mac_tma ? std::min<int64_t>(tr, std::max<int64_t>(1, c->rows_local() / 256))
+                                            : std::min<int64_t>(ranges, std::max<int64_t>(1, c->rows_local() / 64)));
     }
     return B200DPF_OK;
 }
@@ -793,7 +815,7 @@ int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, 
 {
     const GroupBins *B = c->bins.get();
     const KindOps &ops = kKindOps[c->kind];
-    const int nbins = (int)B->n.size();
+    const int nbins = (int)B->shape.size();
     EvalPlan &P = *out = EvalPlan{};
     const SmemLayout &L = P.L;
     P.grouped = P.one_launch = true;
@@ -812,7 +834,7 @@ int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, 
         P.s_group = shrink_s(P.s_group, s_floor, items_wanted, [&](int t) {
             int64_t items = 0;
             for (int g = 0; g < nbins; g++)
-                items += groups_of(g) * (B->rows[(size_t)g] >> (std::min(B->room[(size_t)g], t) + c->lane_bits()));
+                items += groups_of(g) * (B->shape[(size_t)g].rows >> (std::min(B->shape[(size_t)g].room, t) + c->lane_bits()));
             return items;
         });
     }
@@ -912,7 +934,7 @@ int launch_plan(b200dpf_ctx *c, const EvalJob &J, const EvalPlan &P)
         rc = launch_main();
     } else {
         p.out = reinterpret_cast<uint32_t *>(J.out);
-        if (P.leaf_cache) { p.leaf_cache = c->d_leaf_cache.ptr; p.n_local = (uint64_t)c->n_local; }
+        if (P.leaf_cache) { p.leaf_cache = c->d_leaf_cache.ptr; p.n_local = (uint64_t)c->rows_local(); }
         for (int pass = 0; pass < P.passes && rc == B200DPF_OK; pass++) {
             p.col_off_v = (uint32_t)(pass * P.nv);
             p.col_off = (uint32_t)(pass * 4 * P.nv);
@@ -935,7 +957,7 @@ int launch_plan(b200dpf_ctx *c, const EvalJob &J, const EvalPlan &P)
         std::memset(&m, 0, sizeof m);
         m.leaf_cache = p.leaf_cache; m.table = p.table; m.row_stride_v = p.row_stride_v;
         m.out = p.out; m.out_stride = p.out_stride;
-        m.nkeys = (int)J.nkeys; m.key_groups = (int)P.key_groups; m.n_local = (uint64_t)c->n_local;
+        m.nkeys = (int)J.nkeys; m.key_groups = (int)P.key_groups; m.n_local = (uint64_t)c->rows_local();
         m.ranges_per_group = P.mac_ranges;
         for (int blk = 0; blk * 64 < c->entry_size; blk++) {       /* 64-column slices of the rows */
             m.col_off_v = (uint32_t)(blk * 16); m.col_off = (uint32_t)(blk * 64);
@@ -952,7 +974,7 @@ int launch_plan(b200dpf_ctx *c, const EvalJob &J, const EvalPlan &P)
 }
 
 /*
- * One evaluation on a plain context.  Wide entries whose leaf cache (nkeys x n_local x 4 bytes) would
+ * One evaluation on a plain context.  Wide entries whose leaf cache (nkeys x rows_local x 4 bytes) would
  * exceed the cap are evaluated in batch chunks that fit -- the cache is what makes columns beyond the
  * first 16 cost a MAC pass instead of a tree expansion, so shrinking the chunk beats dropping the cache.
  */
@@ -961,7 +983,7 @@ int run_pipeline(b200dpf_ctx *c, const void *keys_dev, const KeyLayout &kl, int6
 {
     const b200dpf_ctx::Knobs &K = c->knobs;
     const bool wide = mode_main == MODE_FUSED && c->entry_pad > 32 && nkeys >= 17 && K.leaf_cache != 0 && kKindOps[c->kind].leaf_cache;
-    const size_t per_group = 32u * (size_t)c->n_local * sizeof(uint32_t);
+    const size_t per_group = 32u * (size_t)c->rows_local() * sizeof(uint32_t);
     const size_t cap = (size_t)std::max(K.leaf_cache_mb, 1) << 20;
     /* not a cached evaluation, or one key group alone overflows the cap (re-expand per 64 columns): one chunk */
     const bool cached = wide && per_group <= cap;
@@ -1065,6 +1087,54 @@ int ctx_open(int device, bool read_env, std::optional<DeviceGuard> *guard, std::
     CUDA_TRY(probe_dynamic_smem_base(&c->smem_base, c->stream));
     CUDA_TRY(upload_aes_table(host::aes_te0()));
     *out = std::move(c);
+    return B200DPF_OK;
+}
+
+/* Fill the device rows of placement P from `src`, the caller's table of P.n rows in host or device memory, and wait
+ * (the stage is then free for the next table): stage P's own rows in natural order (a shard gathers its leaves
+ * own_val + k * 2^shift, k = 0, 1, ...), then place them in d_table, padded to 64-byte rows.  dpf_wrapper.cu:103-115
+ * does the analogous reorder on the host with one ATen call per element. */
+int upload_table(b200dpf_ctx *c, const int32_t *src, const RowPlacement &P, DeviceBuffer<int32_t> *stage)
+{
+    cudaPointerAttributes attr;
+    const bool on_device = cudaPointerGetAttributes(&attr, src) == cudaSuccess &&
+                           (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+    cudaGetLastError();
+    if (on_device) {   /* it may still be being written on the caller's stream (e.g. a dtype cast enqueued just before
+                        * this call): our copy runs on a private non-blocking stream, so wait for its device first */
+        if (attr.device != c->device) cudaSetDevice(attr.device);
+        const cudaError_t es = cudaDeviceSynchronize();
+        if (attr.device != c->device) cudaSetDevice(c->device);
+        CUDA_TRY(es);
+    }
+    const size_t row_bytes = (size_t)c->entry_size * sizeof(int32_t);
+    const int64_t rows = (int64_t)P.n >> P.shift;
+    const size_t stage_bytes = (size_t)rows * row_bytes;
+    int rc = stage->reserve(stage_bytes);
+    if (rc) return rc;
+    cudaError_t e = cudaSuccess;
+    if (P.shift == 0) {
+        e = cudaMemcpyAsync(stage->ptr, src, stage_bytes, cudaMemcpyDefault, c->stream);
+    } else {
+        const int shards = 1 << P.shift;
+        const size_t leaf_bytes = row_bytes << P.lane_bits;
+        const int64_t leaves = rows >> P.lane_bits;
+        const int32_t *own = src + ((size_t)P.own_val << P.lane_bits) * c->entry_size;
+        if (on_device) {
+            e = cudaMemcpy2DAsync(stage->ptr, leaf_bytes, own, leaf_bytes * shards, leaf_bytes, (size_t)leaves, cudaMemcpyDefault,
+                                  c->stream);
+        } else {
+            std::vector<int32_t> gathered((size_t)rows * c->entry_size);
+            const size_t leaf_words = (size_t)c->entry_size << P.lane_bits;
+            for (int64_t j = 0; j < leaves; j++)
+                std::memcpy(gathered.data() + (size_t)j * leaf_words, own + (size_t)j * shards * leaf_words, leaf_bytes);
+            e = cudaMemcpyAsync(stage->ptr, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        }
+    }
+    CUDA_TRY(e);
+    CUDA_TRY(launch_fill_table(stage->ptr, c->d_table.ptr, P, c->entry_size, c->entry_pad, c->sm_count, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
     return B200DPF_OK;
 }
 
@@ -1371,90 +1441,36 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     *out = nullptr;
     if (!table) return fail(B200DPF_EINVAL, "null table");
     if (kind < 0 || kind >= host::KIND_COUNT) return fail(B200DPF_EINVAL, "unknown key kind %d", kind);
-    const int lane_bits = host::kKinds[kind].lane_bits;
-    const int64_t n_min = host::kKinds[kind].n_min;
-    if (trimmed && !trim_args_ok(n, kind))
-        return fail(B200DPF_EINVAL, "table size n=%lld out of range [1, 2^31]", (long long)n);
-    if (!trimmed && (n < n_min || n > ((int64_t)1 << 31) || (n & (n - 1)) != 0))
-        return fail(B200DPF_EINVAL, "table size n=%lld must be a power of two in [%lld, 2^31]", (long long)n, (long long)n_min);
+    TableShape shape;
+    int rc = table_shape(n, kind, trimmed, -1, &shape);
+    if (rc) return rc;
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
-    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 || (!trimmed && (int64_t)shard_count > n / n_min) ||
-        shard_rank < 0 || shard_rank >= shard_count)
+    if (shard_count < 1 || (shard_count & (shard_count - 1)) != 0 ||
+        (!trimmed && (int64_t)shard_count > n / host::kKinds[kind].n_min) || shard_rank < 0 || shard_rank >= shard_count)
         return fail(B200DPF_EINVAL, "bad shard %d of %d for n=%lld", shard_rank, shard_count, (long long)n);
 
     std::optional<DeviceGuard> guard;
     std::unique_ptr<b200dpf_ctx> c;
-    int rc = ctx_open(device, true, &guard, &c);
+    rc = ctx_open(device, true, &guard, &c);
     if (rc) return rc;
-    c->n = n;
+    c->shape = shape;
     c->kind = kind;
-    c->depth = ilog2(trimmed ? trimmed_domain_of(n, kind) : n) - lane_bits;   /* the tree is over leaves */
+    c->trimmed = trimmed;
     c->entry_size = entry_size;
     /* rows padded to what one pass reads: 16, 32 or a multiple of 64 int32 */
     c->entry_pad = entry_size <= 16 ? 16 : (entry_size <= 32 ? 32 : ((entry_size + 63) & ~63));
     c->shard_rank = shard_rank;
     c->shard_count = shard_count;
     c->shard_bits = ilog2(shard_count);
-    c->n_local = n / shard_count;
-    c->depth_local = c->depth - c->shard_bits;
-    if (trimmed) {
-        c->trimmed = true;
-        c->trim_log2 = trim_log2_of(n, kind);
-        c->n_local = (n + ((int64_t)1 << c->trim_log2) - 1) >> c->trim_log2 << c->trim_log2;
-    }
-    c->place = RowPlacement{0, (uint32_t)n, lane_bits, trimmed ? (int)PLACE_IDENTITY : c->depth_local,
-                            (uint32_t)shard_count - 1u, bitrev((uint32_t)shard_rank, c->shard_bits), c->shard_bits};
+    c->place = place_of(shape, c->lane_bits(), trimmed, shard_rank, c->shard_bits);
 
-    /* Table: gather this shard's rows, then place them on the device (RowPlacement), padded to 64-byte
-     * rows.  dpf_wrapper.cu:103-115 does the analogous reorder on the host with one ATen call per element. */
-    {   /* a device-resident table may still be being written on the caller's stream (e.g. a dtype
-         * cast enqueued just before this call): our copy runs on a private non-blocking stream,
-         * so wait for the producing device first */
-        cudaPointerAttributes attr;
-        if (cudaPointerGetAttributes(&attr, table) == cudaSuccess &&
-            (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)) {
-            if (attr.device != device) cudaSetDevice(attr.device);
-            const cudaError_t es = cudaDeviceSynchronize();
-            if (attr.device != device) cudaSetDevice(device);
-            CUDA_TRY(es);
-        }
-        cudaGetLastError();
-    }
-    const size_t row_bytes = (size_t)entry_size * sizeof(int32_t);
-    const size_t stage_bytes = (size_t)n / shard_count * row_bytes;
-    const size_t leaf_bytes = row_bytes << lane_bits;            /* one leaf's rows */
-    const int64_t leaves_local = c->n_local >> lane_bits;
-    const size_t table_bytes = (size_t)c->n_local * (size_t)c->entry_pad * sizeof(int32_t);
-    DeviceBuffer<int32_t> d_stage;
-    rc = d_stage.reserve(stage_bytes);
-    if (rc) return rc;
-    cudaError_t e = cudaSuccess;
-    if (shard_count == 1) {
-        e = cudaMemcpyAsync(d_stage.ptr, table, stage_bytes, cudaMemcpyDefault, c->stream);
-    } else {   /* the shard's leaves, own_val + k * shard_count for k = 0, 1, ..., in order */
-        const int32_t *src = table + ((size_t)c->place.own_val << lane_bits) * entry_size;
-        cudaPointerAttributes attr;
-        const bool on_device = cudaPointerGetAttributes(&attr, table) == cudaSuccess &&
-                               (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
-        cudaGetLastError();
-        if (on_device) {
-            e = cudaMemcpy2DAsync(d_stage.ptr, leaf_bytes, src, leaf_bytes * shard_count, leaf_bytes, (size_t)leaves_local,
-                                  cudaMemcpyDefault, c->stream);
-        } else {
-            std::vector<int32_t> gathered((size_t)c->n_local * entry_size);
-            const size_t leaf_words = (size_t)entry_size << lane_bits;
-            for (int64_t j = 0; j < leaves_local; j++)
-                std::memcpy(gathered.data() + (size_t)j * leaf_words, src + (size_t)j * shard_count * leaf_words, leaf_bytes);
-            e = cudaMemcpyAsync(d_stage.ptr, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        }
-    }
-    CUDA_TRY(e);
+    const size_t table_bytes = (size_t)c->rows_local() * (size_t)c->entry_pad * sizeof(int32_t);
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    CUDA_TRY(launch_fill_table(d_stage.ptr, c->d_table.ptr, c->place, entry_size, c->entry_pad, c->sm_count, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    DeviceBuffer<int32_t> d_stage;
+    rc = upload_table(c.get(), table, c->place, &d_stage);
+    if (rc) return rc;
     d_stage.release();
 
     /* Like the reference's eval_init (dpf_wrapper.cu:120-129), set up everything a default batch
@@ -1553,7 +1569,7 @@ int b200dpf_eval(b200dpf_ctx *c, const int32_t *keys, int64_t nkeys, int prf, in
     int rc = check_eval_args(c, keys, nkeys, prf, out);
     if (rc) return rc;
     for (int64_t b = 0; b < nkeys; b++)
-        if ((rc = check_key(c->kind, key_rows(c, c->depth), keys + b * host::KEY_WORDS, b, -1))) return rc;
+        if ((rc = check_key(c, c->shape, keys + b * host::KEY_WORDS, b, -1))) return rc;
     if (!is_pinned_host(keys)) {
         /* pageable keys have to be staged by the CPU anyway: stage only their live 32 + 64*depth bytes
          * (44 % of a key at n = 2^14, 63 % at 2^20) and let the DMA of a chunk overlap the next one */
@@ -1572,7 +1588,7 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
     b200dpf_ctx *c0 = c->multi ? multi_first(c) : c;
     DeviceGuard guard(c0->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c0->device);
-    const size_t stride = b200dpf_key_packed_size(c->depth);
+    const size_t stride = b200dpf_key_packed_size(c->shape.depth);
     const size_t key_bytes = (size_t)nkeys * stride;
     int rc = reserve_host_keys(c0, key_bytes);
     if (rc) return rc;
@@ -1592,15 +1608,15 @@ static int eval_gather_impl(b200dpf_ctx *c, const int32_t *const *keys, int64_t 
         for (int64_t b = b0; b < b1; b++) {
             /* validated here, while the key's cache lines are being read anyway (one pass over 512 scattered
              * 2 KiB keys instead of two); copies already issued for earlier chunks are harmless on failure */
-            if (validate && (rc = check_key(c->kind, key_rows(c, c->depth), keys[b], b, -1))) return rc;
-            pack_compact(keys[b], stage + (size_t)b * stride, c->depth, host::kKinds[c->kind].magic);
+            if (validate && (rc = check_key(c, c->shape, keys[b], b, -1))) return rc;
+            pack_compact(keys[b], stage + (size_t)b * stride, c->shape.depth, host::kKinds[c->kind].magic);
         }
         if (!c->multi)
             CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(c->d_keys.ptr) + (size_t)b0 * stride, stage + (size_t)b0 * stride,
                                      (size_t)(b1 - b0) * stride, cudaMemcpyHostToDevice, c->stream));
     }
-    if (c->multi) return multi_eval_host(c, stage, stride, compact_layout(c->depth), nkeys, prf, out);
-    return eval_tail(c, compact_layout(c->depth), nkeys, prf, out);
+    if (c->multi) return multi_eval_host(c, stage, stride, compact_layout(c->shape.depth), nkeys, prf, out);
+    return eval_tail(c, compact_layout(c->shape.depth), nkeys, prf, out);
 }
 
 int b200dpf_eval_gather(b200dpf_ctx *c, const int32_t *const *keys, int64_t nkeys, int prf, int32_t *out)
@@ -1614,15 +1630,15 @@ int b200dpf_eval_packed(b200dpf_ctx *c, const uint8_t *packed, int64_t nkeys, in
 {
     int rc = check_eval_args(c, packed, nkeys, prf, out);
     if (rc) return rc;
-    const size_t stride = b200dpf_key_packed_size(c->depth);
+    const size_t stride = b200dpf_key_packed_size(c->shape.depth);
     for (int64_t b = 0; b < nkeys; b++) {
         const uint8_t *k = packed + (size_t)b * stride;
-        if (std::memcmp(k, host::kKinds[c->kind].magic, 4) != 0 || k[4] != (uint8_t)c->depth)
+        if (std::memcmp(k, host::kKinds[c->kind].magic, 4) != 0 || k[4] != (uint8_t)c->shape.depth)
             return fail(B200DPF_EINVAL, "packed key %lld: bad header or depth %d, table has depth %d (n=%lld)", (long long)b,
-                        (int)k[4], c->depth, (long long)c->n);
+                        (int)k[4], c->shape.depth, (long long)c->shape.n);
     }
-    if (c->multi) return multi_eval_host(c, packed, stride, compact_layout(c->depth), nkeys, prf, out);
-    return eval_host(c, packed, (size_t)nkeys * stride, compact_layout(c->depth), nkeys, prf, out);
+    if (c->multi) return multi_eval_host(c, packed, stride, compact_layout(c->shape.depth), nkeys, prf, out);
+    return eval_host(c, packed, (size_t)nkeys * stride, compact_layout(c->shape.depth), nkeys, prf, out);
 }
 
 int b200dpf_host_staging(b200dpf_ctx *c, int64_t nkeys, int32_t **keys_pinned)
@@ -1672,7 +1688,7 @@ int b200dpf_expand_device(b200dpf_ctx *c, const void *keys_dev, int64_t nkeys, i
                         reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
-int64_t b200dpf_ctx_n(const b200dpf_ctx *c) { return c ? c->n : -1; }
+int64_t b200dpf_ctx_n(const b200dpf_ctx *c) { return c ? c->shape.n : -1; }
 int b200dpf_ctx_entry_size(const b200dpf_ctx *c) { return c ? c->entry_size : -1; }
 int b200dpf_ctx_device(const b200dpf_ctx *c) { return c ? c->device : -1; }
 int b200dpf_ctx_last_launches(const b200dpf_ctx *c)
@@ -1941,8 +1957,6 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
     if (root) root->multi.reset(new (std::nothrow) MultiState());
     if (!root || !root->multi) return fail(B200DPF_ENOMEM, "out of host memory");
     MultiState *M = root->multi.get();
-    root->n = n;
-    root->depth = ilog2(n);
     root->entry_size = entry_size;
     root->device = devices[0];
     M->ndev = ndev;
@@ -1958,6 +1972,7 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
         if (rc) return rc;     /* message already set by b200dpf_create; the root destroys the sub-contexts made */
         M->sub.push_back(c);
     }
+    root->shape = M->sub[0]->shape;     /* the whole table's */
     /* device 0 reads the other shards' partial results in place: NVLink peer mappings */
     M->peer = axis == B200DPF_AXIS_ENTRIES && ndev > 1;
     if (M->peer) {
@@ -1990,21 +2005,17 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     if (!tables || !n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
     if (kind < 0 || kind >= host::KIND_COUNT) return fail(B200DPF_EINVAL, "unknown key kind %d", kind);
-    const int lane_bits = host::kKinds[kind].lane_bits;
-    const int64_t n_min = host::kKinds[kind].n_min;
-    int64_t n_max = 0, rows = 0, stage_rows = 0;
+    std::vector<TableShape> shape((size_t)nbins);
+    TableShape all{};                   /* the context's (b200dpf_ctx::shape) */
     for (int g = 0; g < nbins; g++) {
         if (!tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
-        if (trimmed && !trim_args_ok(n[g], kind))
-            return fail(B200DPF_EINVAL, "bin %d: size n=%lld out of range [1, 2^31]", g, (long long)n[g]);
-        if (!trimmed && (n[g] < n_min || n[g] > ((int64_t)1 << 31) || (n[g] & (n[g] - 1)) != 0))
-            return fail(B200DPF_EINVAL, "bin %d: size n=%lld must be a power of two in [%lld, 2^31]", g, (long long)n[g],
-                        (long long)n_min);
-        const int64_t domain = trimmed ? trimmed_domain_of(n[g], kind) : n[g];
-        const int gran = trimmed ? trim_log2_of(n[g], kind) : ilog2(n[g]);
-        n_max = std::max(n_max, domain);
-        rows += (n[g] + ((int64_t)1 << gran) - 1) >> gran << gran;
-        stage_rows = std::max(stage_rows, n[g]);   /* the largest bin's live rows */
+        TableShape &t = shape[(size_t)g];
+        const int rc = table_shape(n[g], kind, trimmed, g, &t);
+        if (rc) return rc;
+        t.first = (uint64_t)all.rows;
+        all.n = std::max(all.n, t.n);
+        all.depth = std::max(all.depth, t.depth);   /* the launch plan (shared memory for correction words) is sized by it */
+        all.rows += t.rows;
     }
     std::optional<DeviceGuard> guard;
     std::unique_ptr<b200dpf_ctx> c;
@@ -2013,42 +2024,31 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     c->bins.reset(new (std::nothrow) GroupBins());
     if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
     GroupBins *B = c->bins.get();
-    c->n = stage_rows;                 /* b200dpf_ctx_n: the largest bin's rows */
+    B->shape = std::move(shape);
+    c->shape = all;
     c->kind = kind;
     c->trimmed = trimmed;
-    c->depth = ilog2(n_max) - lane_bits;   /* the launch plan (shared memory for correction words) is sized by the deepest bin */
     c->entry_size = entry_size;
     c->entry_pad = (entry_size + 15) & ~15;       /* 16 columns per pass */
-    c->n_local = n_max;
-    c->depth_local = c->depth;
     CUDA_TRY(cudaMemsetAsync(c->d_gridbar.ptr, 0, sizeof(uint32_t), c->stream));
     if (!c->coop_ok) return fail(B200DPF_ECUDA, "grouped evaluation needs cooperative launch support");
-    const size_t table_bytes = (size_t)rows * (size_t)c->entry_pad * sizeof(int32_t);
+    const size_t table_bytes = (size_t)all.rows * (size_t)c->entry_pad * sizeof(int32_t);
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    DeviceBuffer<int32_t> d_stage;
-    rc = d_stage.reserve((size_t)stage_rows * entry_size * sizeof(int32_t));
+    DeviceBuffer<int32_t> d_stage;     /* every bin's: the largest one's */
+    rc = d_stage.reserve((size_t)all.n * entry_size * sizeof(int32_t));
     if (rc) return rc;
-    uint64_t row0 = 0;
     std::vector<RowPlacement> place;
     std::vector<uint2> query_bins;
     for (int g = 0; g < nbins; g++) {
         /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), or trimmed in row order */
-        const int depth = ilog2(trimmed ? trimmed_domain_of(n[g], kind) : n[g]) - lane_bits;
-        const int gran = trimmed ? trim_log2_of(n[g], kind) : depth + lane_bits;
-        B->n.push_back(n[g]);
-        B->depth.push_back(depth);
-        B->row_off.push_back(row0);
-        B->rows.push_back((n[g] + ((int64_t)1 << gran) - 1) >> gran << gran);
-        B->room.push_back(gran - lane_bits);
-        place.push_back(RowPlacement{row0, (uint32_t)n[g], lane_bits, trimmed ? (int)PLACE_IDENTITY : depth, 0, 0, 0});
-        query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)depth));
-        B->query_v += b200dpf_key_packed_size(depth) / 16u;
-        CUDA_TRY(cudaMemcpyAsync(d_stage.ptr, tables[g], (size_t)n[g] * entry_size * sizeof(int32_t), cudaMemcpyDefault, c->stream));
-        CUDA_TRY(launch_fill_table(d_stage.ptr, c->d_table.ptr, place.back(), entry_size, c->entry_pad, c->sm_count, c->stream));
-        CUDA_TRY(cudaStreamSynchronize(c->stream));    /* the staging buffer is reused */
-        row0 += (uint64_t)B->rows.back();
+        const TableShape &t = B->shape[(size_t)g];
+        place.push_back(place_of(t, c->lane_bits(), trimmed, 0, 0));
+        query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)t.depth));
+        B->query_v += b200dpf_key_packed_size(t.depth) / 16u;
+        rc = upload_table(c.get(), tables[g], place.back(), &d_stage);
+        if (rc) return rc;
     }
     const size_t bins_bytes = (size_t)nbins * sizeof(uint2), place_bytes = (size_t)nbins * sizeof(RowPlacement);
     rc = B->d_place.reserve(place_bytes);
@@ -2094,7 +2094,7 @@ static int check_group_args(const b200dpf_ctx *c, bool bufs, int64_t count, bool
 {
     if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
     if (!bufs) return fail(B200DPF_EINVAL, "null buffer");
-    const int per_query = queries ? (int)c->bins->n.size() : 1;
+    const int per_query = queries ? (int)c->bins->shape.size() : 1;
     if (count < 1 || count > ((int64_t)1 << 24) / per_query)
         return queries ? fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%d) <= 2^24",
                               (long long)count, per_query)
@@ -2112,14 +2112,14 @@ static int group_count(const b200dpf_ctx *c, const int32_t *keys, const int32_t 
                        std::vector<int64_t> *count_out)
 {
     const GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
+    const int nbins = (int)B->shape.size();
     std::vector<int64_t> &count = *count_out;
     count.assign((size_t)nbins + 1, 0);
     for (int64_t b = 0; b < nkeys; b++) {
         const int g = bins[b];
         if (g < 0 || g >= nbins) return fail(B200DPF_EINVAL, "key %lld: bin %d out of range [0,%d)", (long long)b, g, nbins);
         if (keys) {
-            const int rc = check_key(c->kind, key_rows(c, B->depth[(size_t)g]), keys + b * host::KEY_WORDS, b, g);
+            const int rc = check_key(c, B->shape[(size_t)g], keys + b * host::KEY_WORDS, b, g);
             if (rc) return rc;
         }
         count[(size_t)g + 1]++;
@@ -2135,7 +2135,7 @@ static int group_count(const b200dpf_ctx *c, const int32_t *keys, const int32_t 
 int GroupLaunch::plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, const int32_t *bins)
 {
     const GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
+    const int nbins = (int)B->shape.size();
     if (!ev_staged) CUDA_TRY(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
     if (staged_pending) {             /* the previous uploads read the staging rewritten below */
         CUDA_TRY(cudaEventSynchronize(ev_staged));
@@ -2155,17 +2155,17 @@ int GroupLaunch::plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
     {
         int64_t gi = 0;
         for (int g = 0; g < nbins; g++) {
-            const int depth = B->depth[(size_t)g];
+            const TableShape &t = B->shape[(size_t)g];
             const int s = group_s(P, *B, g);
             for (int64_t k = count[(size_t)g]; k < count[(size_t)g + 1]; k += 32, gi++) {
                 GroupDesc &d = h_descs.ptr[gi];
                 d.key_first = (uint32_t)k;
                 d.nkeys = (uint32_t)std::min<int64_t>(32, count[(size_t)g + 1] - k);
-                d.depth = depth;
+                d.depth = t.depth;
                 d.s = s;
-                d.nsub = (uint32_t)(B->rows[(size_t)g] >> (s + c->lane_bits()));   /* 2^(depth - s) unless trimmed */
+                d.nsub = (uint32_t)(t.rows >> (s + c->lane_bits()));   /* 2^(depth - s) unless trimmed */
                 d.pad = 0;
-                d.table_off_v = B->row_off[(size_t)g] * (uint64_t)(c->entry_pad / 4);
+                d.table_off_v = t.first * (uint64_t)(c->entry_pad / 4);
             }
         }
     }
@@ -2197,12 +2197,12 @@ int GroupLaunch::plan(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count
     if (bins) {
         std::vector<int64_t> next(count.begin(), count.end() - 1);
         for (int64_t b = 0; b < nkeys; b++)
-            h_order.ptr[next[(size_t)bins[b]]++] = make_uint2((uint32_t)b, (uint32_t)B->depth[(size_t)bins[b]]);
+            h_order.ptr[next[(size_t)bins[b]]++] = make_uint2((uint32_t)b, (uint32_t)B->shape[(size_t)bins[b]].depth);
     } else {
         const int64_t nq = nkeys / nbins;
         for (int g = 0; g < nbins; g++)
             for (int64_t q = 0; q < nq; q++)
-                h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->depth[(size_t)g]);
+                h_order.ptr[g * nq + q] = make_uint2((uint32_t)(q * nbins + g), (uint32_t)B->shape[(size_t)g].depth);
     }
     return B200DPF_OK;
 }
@@ -2222,7 +2222,7 @@ int GroupLaunch::upload(cudaStream_t stream, bool order)
 /* The evaluation by launch L of its keys, sorted by bin and compact in d_keys, into d_out in sorted order */
 static int group_launch(b200dpf_ctx *c, const GroupLaunch &L, int prf, cudaStream_t stream)
 {
-    const EvalJob J{c->d_keys.ptr, compact_layout(c->depth), L.nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
+    const EvalJob J{c->d_keys.ptr, compact_layout(c->shape.depth), L.nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
                     L.d_descs.ptr, L.d_units.ptr, (uint32_t)L.nunits, true};
     return launch_plan(c, J, L.P);
 }
@@ -2241,7 +2241,7 @@ int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins,
     if (rc) return rc;
     /* keys travel in the compact layout, one stride for all bins (that of the deepest): a key for a
      * 2^10-entry bin has 672 live bytes of its 2096 (early-terminated: 544) */
-    const KeyLayout kl = compact_layout(c->depth);
+    const KeyLayout kl = compact_layout(c->shape.depth);
     const char *magic = host::kKinds[c->kind].magic;
     const size_t stride = (size_t)kl.stride_v * 16u;
     const size_t key_bytes = (size_t)nkeys * stride;
@@ -2283,7 +2283,7 @@ static int group_enqueue(b200dpf_ctx *c, GroupLaunch &L, bool upload, const void
                          void *out_dev, cudaStream_t stream)
 {
     const GroupBins *B = c->bins.get();
-    const KeyLayout kl = compact_layout(c->depth);
+    const KeyLayout kl = compact_layout(c->shape.depth);
     int rc = reserve_device_io(c, (size_t)L.nkeys * kl.stride_v * 16u, (size_t)L.nkeys * c->entry_size);
     if (!rc) rc = wait_last(c, stream);
     if (!rc && upload) rc = L.upload(stream, true);
@@ -2293,7 +2293,7 @@ static int group_enqueue(b200dpf_ctx *c, GroupLaunch &L, bool upload, const void
     if (key_format == B200DPF_KEYS_WIRE)
         CUDA_TRY(launch_group_gather(keys_dev, L.d_order.ptr, L.nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
     else
-        CUDA_TRY(launch_group_gather_queries(keys_dev, B->d_bins.ptr, L.nkeys, (uint32_t)(L.nkeys / (int64_t)B->n.size()),
+        CUDA_TRY(launch_group_gather_queries(keys_dev, B->d_bins.ptr, L.nkeys, (uint32_t)(L.nkeys / (int64_t)B->shape.size()),
                                              B->query_v, magic, kl.stride_v, c->d_keys.ptr, stream));
     rc = group_launch(c, L, prf, stream);
     if (rc) return rc;
@@ -2342,7 +2342,7 @@ int b200dpf_group_eval_queries_device(b200dpf_ctx *c, const void *keys_dev, int 
     GroupBins *B = c->bins.get();
     const bool replan = !B->cached_valid || B->cached_nq != nqueries || B->cached_prf != prf;
     if (replan) {
-        std::vector<int64_t> count(B->n.size() + 1);
+        std::vector<int64_t> count(B->shape.size() + 1);
         for (size_t g = 0; g < count.size(); g++) count[g] = (int64_t)g * nqueries;
         B->cached_valid = false;
         rc = B->cached.plan(c, prf, count, nullptr);
@@ -2369,7 +2369,7 @@ int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, 
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
     const GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
+    const int nbins = (int)B->shape.size();
     const host::KindInfo &k = host::kKinds[c->kind];
     KeygenParams p{};
     p.alphas = alphas_dev;
@@ -2410,18 +2410,12 @@ struct UpdateLayout {
 
 size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
-/* rows of the device table; also the skip marker of the update kernels (larger than every position) */
-uint64_t update_table_rows(const b200dpf_ctx *c)
-{
-    return c->bins ? c->bins->row_off.back() + (uint64_t)c->bins->rows.back() : (uint64_t)c->n_local;
-}
-
 /* Grow the scratch for `count` rows (staged: the inputs are copied into it) and order everything that
  * follows on `stream` after the context's previous evaluation or update: the update writes the table
  * those read, and the scratch is the previous update's. */
 int update_begin(b200dpf_ctx *c, int64_t count, bool staged, bool with_bins, cudaStream_t stream, UpdateLayout *L)
 {
-    const uint64_t rows = update_table_rows(c);
+    const uint64_t rows = (uint64_t)c->rows_local();
     if (rows >= 0xffffffffull) return fail(B200DPF_EINVAL, "table of %llu rows too large for row updates", (unsigned long long)rows);
     L->end_bit = 1;
     while (L->end_bit < 32 && (rows >> L->end_bit) != 0) L->end_bit++;
@@ -2454,12 +2448,12 @@ int update_run(b200dpf_ctx *c, const UpdateLayout &L, const int64_t *idx, const 
     u.bins = bins;
     if (bins) {
         u.bin_place = c->bins->d_place.ptr;
-        u.nbins = (int)c->bins->n.size();
+        u.nbins = (int)c->bins->shape.size();
     }
     u.place = c->place;
     u.rows = rows;
     u.count = count;
-    u.table_rows = (uint32_t)update_table_rows(c);
+    u.table_rows = (uint32_t)c->rows_local();
     u.table = c->d_table.ptr;
     u.cols = c->entry_size;
     u.stride = c->entry_pad;
@@ -2523,9 +2517,9 @@ int b200dpf_update_rows(b200dpf_ctx *c, const int64_t *indices, const int32_t *r
     if (c->bins) return fail(B200DPF_ESTATE, "grouped context: use b200dpf_group_update_rows");
     if (!c->d_table.ptr && !c->multi) return fail(B200DPF_ESTATE, "context has no table");
     for (int64_t j = 0; j < count; j++)
-        if (indices[j] < 0 || indices[j] >= c->n)
+        if (indices[j] < 0 || indices[j] >= c->shape.n)
             return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld)", (long long)j, (long long)indices[j],
-                        (long long)c->n);
+                        (long long)c->shape.n);
     if (count == 0) return B200DPF_OK;
     std::vector<b200dpf_ctx *> subs = c->multi ? c->multi->sub : std::vector<b200dpf_ctx *>{c};
     /* every device's copies and kernels are issued before the first synchronisation */
@@ -2567,13 +2561,13 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     if (!c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
     if (count > 0 && !bins) return fail(B200DPF_EINVAL, "null buffer");
     GroupBins *B = c->bins.get();
-    const int nbins = (int)B->n.size();
+    const int nbins = (int)B->shape.size();
     for (int64_t j = 0; j < count; j++) {
         if (bins[j] < 0 || bins[j] >= nbins)
             return fail(B200DPF_EINVAL, "update %lld: bin %d out of range [0,%d)", (long long)j, bins[j], nbins);
-        if (indices[j] < 0 || indices[j] >= B->n[(size_t)bins[j]])
+        if (indices[j] < 0 || indices[j] >= B->shape[(size_t)bins[j]].n)
             return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld) of bin %d", (long long)j,
-                        (long long)indices[j], (long long)B->n[(size_t)bins[j]], bins[j]);
+                        (long long)indices[j], (long long)B->shape[(size_t)bins[j]].n, bins[j]);
     }
     if (count == 0) return B200DPF_OK;
     DeviceGuard guard(c->device);
@@ -2598,13 +2592,12 @@ double b200dpf_ctx_last_device_ms(b200dpf_ctx *c)
     return (double)ms;
 }
 
-int b200dpf_group_bins(const b200dpf_ctx *c) { return (c && c->bins) ? (int)c->bins->n.size() : 0; }
+int b200dpf_group_bins(const b200dpf_ctx *c) { return (c && c->bins) ? (int)c->bins->shape.size() : 0; }
 
 int64_t b200dpf_ctx_table_rows(const b200dpf_ctx *c)
 {
     if (!c) return -1;
-    if (c->multi) return (int64_t)update_table_rows(c->multi->sub[0]);
-    return (int64_t)update_table_rows(c);
+    return (c->multi ? c->multi->sub[0] : c)->rows_local();
 }
 
 

@@ -467,8 +467,13 @@ at::Tensor eval_gpu_compact(const at::Tensor &packed, int64_t nkeys, const std::
     b200dpf_ctx *ctx = ctx_of(buffers);
     TORCH_CHECK(packed.device().is_cpu() && packed.scalar_type() == at::kByte && packed.is_contiguous(),
                 "eval_gpu_compact: packed keys must be a contiguous CPU uint8 tensor");
+    /* the keys' n: the table's rows, or on a trimmed context trimmed_domain(rows) for the context's kind */
+    const int per_leaf = b200dpf_ctx_rows_per_leaf(ctx);
+    int64_t n = b200dpf_ctx_n(ctx);
+    if (b200dpf_ctx_trimmed(ctx) == 1)
+        n = b200dpf_trimmed_domain(n, per_leaf == 1 ? B200DPF_KIND_STANDARD : per_leaf == 4 ? B200DPF_KIND_ET : B200DPF_KIND_XOR);
     int depth = 0;   /* of the tree: over leaves, which are rows_per_leaf rows each */
-    for (int64_t n = b200dpf_ctx_n(ctx) / b200dpf_ctx_rows_per_leaf(ctx); n > 1; n >>= 1) depth++;
+    for (n /= per_leaf; n > 1; n >>= 1) depth++;
     TORCH_CHECK(nkeys >= 1 && (int64_t)packed.numel() == nkeys * (int64_t)b200dpf_key_packed_size(depth),
                 "eval_gpu_compact: expected ", nkeys, " keys of ", b200dpf_key_packed_size(depth), " bytes");
     at::Tensor result = torch::empty({nkeys, (int64_t)b200dpf_ctx_entry_size(ctx)}, at::kInt);

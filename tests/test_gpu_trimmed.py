@@ -174,6 +174,14 @@ def test_paths(kind):
         assert np.array_equal(acc.cpu().numpy(), twice)
     finally:
         ctx.close()
+    # the dpf_cpp binding: packed keys are sized by the key domain, not by the live rows
+    import dpf
+    d = dpf.DPF(prf=prf, trim=True, early_termination=kind == "et", xor=kind == "xor")
+    try:
+        d.eval_init(torch.from_numpy(table))
+        assert np.array_equal(d.eval_gpu_compact(d.pack_keys(torch.from_numpy(ka))).numpy(), want)
+    finally:
+        d.close()
 
 
 # ---- row updates by row number -----------------------------------------------------------------------------
