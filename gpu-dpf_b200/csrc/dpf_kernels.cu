@@ -1042,10 +1042,11 @@ __global__ void __launch_bounds__(256) update_scatter_kernel(const int32_t *__re
     }
 }
 
-/* An instantiated evaluation kernel: its entry point, and the dynamic shared memory size last configured
- * for it on each device (bytes + 1, 0 = never).  Function attributes are per device and sticky, so
- * they are set once per (device, size); contexts on different host threads may race there, hence the
- * atomics (a duplicate set is harmless). */
+/* An instantiated evaluation kernel: its entry point, and whether its attributes are set on each device
+ * (1 = set, 0 = never).  Function attributes belong to the (kernel, device) pair for the whole process, not
+ * to one context, so the dynamic shared-memory ceiling is set once, to the most the kernel can take
+ * (eval_max_smem), and every launch passes its own size below it.  Contexts on different host threads may
+ * race to set it; they all write the same values, so a duplicate set is harmless. */
 struct EvalKernel {
     const void *fn;
     std::atomic<int> *configured;   /* [64] */
@@ -1105,6 +1106,20 @@ EvalKernel find_eval_kernel(int prf, int nv, int mode)
     }
 }
 
+/* The most dynamic shared memory one block of kernel `fn` may take on the current device: the opt-in limit
+ * less the kernel's static shared memory */
+cudaError_t kernel_max_smem(const void *fn, int *bytes)
+{
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, fn);
+    if (e != cudaSuccess) return e;
+    int dev = 0, optin = 0;
+    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+    if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
+    *bytes = optin - (int)a.sharedSizeBytes;
+    return cudaSuccess;
+}
+
 }  // namespace
 
 cudaError_t probe_dynamic_smem_base(uint32_t *base, cudaStream_t stream)
@@ -1134,13 +1149,17 @@ cudaError_t launch_eval(int prf, int nv, int mode, const EvalParams &p, int grid
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64 || k.configured[dev].load(std::memory_order_acquire) != (int)smem + 1) {
-        e = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (dev < 0 || dev >= 64 || !k.configured[dev].load(std::memory_order_acquire)) {
+        /* the ceiling, not this launch's size: a smaller value set by another thread between its check and its
+         * launch would make that launch fail */
+        int max_smem = 0;
+        if ((e = kernel_max_smem(k.fn, &max_smem)) != cudaSuccess) return e;
+        e = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
         if (e != cudaSuccess) return e;
         /* the kernels live in shared memory; L1 only sees broadcast table rows */
         e = cudaFuncSetAttribute(k.fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) k.configured[dev].store((int)smem + 1, std::memory_order_release);
+        if (dev >= 0 && dev < 64) k.configured[dev].store(1, std::memory_order_release);
     }
     const dim3 block((unsigned)eval_block_shape(prf, nv, mode).threads);
     void *args[] = {const_cast<EvalParams *>(&p)};
@@ -1153,20 +1172,14 @@ cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes)
 {
     const EvalKernel k = find_eval_kernel(prf, nv, mode);
     if (k.fn == nullptr) return cudaErrorInvalidValue;
-    cudaFuncAttributes a;
-    cudaError_t e = cudaFuncGetAttributes(&a, k.fn);
-    if (e != cudaSuccess) return e;
-    int dev = 0, optin = 0;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-    if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
-    *bytes = optin - (int)a.sharedSizeBytes;
-    return cudaSuccess;
+    return kernel_max_smem(k.fn, bytes);
 }
 
 cudaError_t launch_mac_tma(const MacParams &p, int grid, cudaStream_t stream)
 {
     typedef MacTmaShape<16> S;
     auto kern = dpf_mac_tma_kernel<16>;
+    /* every launch takes the same S::SMEM, so every thread that sets the attribute writes the same value */
     static std::atomic<int> configured[64];
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);

@@ -29,6 +29,14 @@
  * come from one host thread at a time.  Evaluations enqueued on DIFFERENT streams through the
  * *_device entry points are ordered by the library (each waits for the context's previous
  * evaluation).  Use one context per concurrent stream of work; contexts are independent.
+ * Tested (tests/test_gpu_concurrency.py, tests/test_concurrency_host.py): independent contexts of
+ * every kind, plain, trimmed and grouped, used from any host threads of one device at once, while
+ * other threads create and destroy contexts and generate keys; one context used by several threads
+ * in turn, each enqueueing on its own stream without synchronising before it hands over; and the
+ * ordering across streams, including calls whose larger batches grow the context's scratch while
+ * earlier calls may still run, row updates and accumulating calls.  The host entry points (key
+ * generation, host evaluation, key packing) may be called from any number of threads, and
+ * b200dpf_last_error reports the calling thread's last failure.
  */
 #ifndef B200DPF_H
 #define B200DPF_H

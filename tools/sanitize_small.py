@@ -159,4 +159,31 @@ grp = b200dpf.GroupContext(tables, early_termination=True)
 ga, gb = grp.eval(ka, bins, 1), grp.eval(kb, bins, 1)
 assert np.array_equal((ga.astype(np.uint32) - gb.astype(np.uint32)).astype(np.int32), table[alphas])
 grp.close()
+# one context, calls rotating over three streams with no host synchronisation between them: each larger batch
+# grows the counters, tree-top tickets, frontier and (at 40 columns) the leaf cache while earlier calls may still
+# run, so memcheck sees any use of scratch after it was freed; a row update on a fourth stream sits in the chain
+n, e = 1024, 40
+table = rng.randint(-2**31, 2**31, size=(n, e), dtype=np.int64).astype(np.int32)
+alphas = rng.randint(0, n, size=600).astype(np.int64)
+ka, kb = b200dpf.gen_batch_secure(alphas, n, bytes(range(44)) * 600, 2)
+ctx = b200dpf.Context(table)
+ctx.set_option("leaf_cache_mb", 1)
+want = ctx.eval(ka, 2)
+streams = [torch.cuda.Stream() for _ in range(4)]
+keys = torch.from_numpy(ka).cuda()
+batches = (1, 5, 33, 200, 600, 17)
+outs = [torch.empty((b, e), dtype=torch.int32, device="cuda") for b in batches]
+upd_idx = torch.from_numpy(np.array([alphas[0]], np.int64)).cuda()
+upd_row = torch.from_numpy(table[alphas[0]][None].copy()).cuda()         # rewrites a row with its own value
+torch.cuda.synchronize()
+for i, (b, o) in enumerate(zip(batches, outs)):
+    ctx.eval_device(keys.data_ptr(), b, 2, o.data_ptr(), stream=streams[i % 3].cuda_stream)
+    if i == 3:
+        ctx.update_rows_device(upd_idx.data_ptr(), upd_row.data_ptr(), 1, stream=streams[3].cuda_stream)
+torch.cuda.synchronize()
+for b, o in zip(batches, outs):
+    assert np.array_equal(o.cpu().numpy(), want[:b])
+rec = (want.astype(np.uint32) - ctx.eval(kb, 2).astype(np.uint32)).astype(np.int32)
+assert np.array_equal(rec, table[alphas])
+ctx.close()
 print("sanitize run ok")
