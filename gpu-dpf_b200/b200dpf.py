@@ -34,6 +34,7 @@ SYMBOLS = [
     "b200dpf_gen_batch_gpu_et", "b200dpf_gen_batch_gpu_xor", "b200dpf_group_gen_queries_device",
     "b200dpf_trimmed_domain", "b200dpf_trimmed_alpha", "b200dpf_create_trimmed", "b200dpf_group_create_trimmed",
     "b200dpf_ctx_trimmed", "b200dpf_ctx_table_rows",
+    "b200dpf_group_eval_device_bins", "b200dpf_group_plan_lists",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -85,6 +86,10 @@ def load():
     L.b200dpf_group_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _i64p, C.c_int, C.c_int, C.c_int]
     L.b200dpf_group_eval.argtypes = [C.c_void_p, _i32p, _i32p, C.c_int64, C.c_int, _i32p]
     L.b200dpf_group_eval_device.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
+    L.b200dpf_group_eval_device_bins.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p]
+    L.b200dpf_group_plan_lists.argtypes = [C.c_void_p, C.c_int, _i64p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_int64]
     L.b200dpf_group_bins.argtypes = [C.c_void_p]
     L.b200dpf_group_query_bytes.argtypes = [C.c_void_p]
     L.b200dpf_group_query_bytes.restype = C.c_int64
@@ -533,6 +538,30 @@ class GroupContext(Context):
         bins = np.ascontiguousarray(bins, np.int32).reshape(-1)
         _check(lib().b200dpf_group_eval_device(self.handle, C.c_void_p(keys_ptr), bins, len(bins), prf,
                                                C.c_void_p(out_ptr), C.c_void_p(stream)), "b200dpf_group_eval_device")
+
+    def eval_device_bins(self, keys_ptr, bins_ptr, nkeys, prf, out_ptr, bad_ptr=0, stream=0):
+        """eval_device with the bins in device memory too (int32 [nkeys] at bins_ptr), planned on the GPU and
+        enqueued on `stream` without any host wait.  A key whose bin is outside [0, nbins) gets a zero row; if
+        bad_ptr is not 0, the int64 there receives the number of such keys."""
+        _check(lib().b200dpf_group_eval_device_bins(self.handle, C.c_void_p(keys_ptr), C.c_void_p(bins_ptr), nkeys, prf,
+                                                    C.c_void_p(out_ptr), C.c_void_p(bad_ptr or None), C.c_void_p(stream)),
+               "b200dpf_group_eval_device_bins")
+
+    def plan_lists(self, device_planned):
+        """for tests: the lists of the last plan, made on the device by eval_device_bins (device_planned=True) or on the
+        host by eval / eval_device: (counts, descs, units, order) with counts = (key groups, work units, keys, keys
+        whose bin is out of range), descs uint32 [K, 8], units uint32 [U, 4], order uint32 [nkeys, 2]"""
+        counts = np.zeros(4, np.int64)
+        empty = np.zeros(8, np.uint32)
+        which = 0 if device_planned else 1
+        _check(lib().b200dpf_group_plan_lists(self.handle, which, counts, empty.ctypes.data, 0, empty.ctypes.data, 0,
+                                              empty.ctypes.data, 0), "b200dpf_group_plan_lists")
+        descs = np.zeros((max(int(counts[0]), 1), 8), np.uint32)
+        units = np.zeros((max(int(counts[1]), 1), 4), np.uint32)
+        order = np.zeros((max(int(counts[2]), 1), 2), np.uint32)
+        _check(lib().b200dpf_group_plan_lists(self.handle, which, counts, descs.ctypes.data, int(counts[0]), units.ctypes.data,
+                                              int(counts[1]), order.ctypes.data, int(counts[2])), "b200dpf_group_plan_lists")
+        return counts, descs[:counts[0]], units[:counts[1]], order[:counts[2]]
 
     @property
     def query_bytes(self):

@@ -388,6 +388,7 @@ inline void pack_compact(const int32_t *key, uint8_t *dst, int depth, const char
 struct KindOps {
     int mode_fused, mode_expand;
     int mode_grouped;
+    int mode_grouped_dev;   /* the grouped mode of lists planned on the device (b200dpf_group_eval_device_bins) */
     int max_nv;             /* fused passes: at most 4 * max_nv columns (early-terminated 32, XOR-shared 16) */
     bool leaf_cache;        /* wide entries may cache leaves (XOR-shared: a further 16 columns re-walk the tree) */
     bool tma_rows;          /* the B200DPF_TMA_ROWS variant exists */
@@ -397,9 +398,9 @@ struct KindOps {
     const char *gen;        /* the generator of the kind's keys, in messages */
 };
 constexpr KindOps kKindOps[host::KIND_COUNT] = {
-    {MODE_FUSED, MODE_EXPAND, MODE_GROUPED, 16, true, true, 0, 0, "b200dpf_gen"},
-    {MODE_FUSED_ET, MODE_EXPAND_ET, MODE_GROUPED_ET, 8, true, false, 0, 0, "b200dpf_gen_et"},
-    {MODE_FUSED_XOR, MODE_EXPAND_XOR, MODE_GROUPED_XOR, 4, false, false, 2, 4, "b200dpf_gen_xor"},
+    {MODE_FUSED, MODE_EXPAND, MODE_GROUPED, MODE_GROUPED_DEV, 16, true, true, 0, 0, "b200dpf_gen"},
+    {MODE_FUSED_ET, MODE_EXPAND_ET, MODE_GROUPED_ET, MODE_GROUPED_ET_DEV, 8, true, false, 0, 0, "b200dpf_gen_et"},
+    {MODE_FUSED_XOR, MODE_EXPAND_XOR, MODE_GROUPED_XOR, MODE_GROUPED_XOR_DEV, 4, false, false, 2, 4, "b200dpf_gen_xor"},
 };
 
 /* Trimmed tables (DESIGN.md section 11).  Row r of an n-row table sits at leaf position r >> lane_bits of a tree
@@ -503,6 +504,7 @@ struct EvalJob {
     /* grouped contexts: the key groups' descriptors and work units; `timed`: ev_t0 / ev_t1 bracket the launches */
     const GroupDesc *groups; const WorkUnit *units; uint32_t nunits;
     bool timed;
+    const uint32_t *counts;   /* modes whose counts are on the device: EvalParams::dev_counts */
 };
 
 /*
@@ -554,6 +556,24 @@ struct GroupLaunch {
     int upload(cudaStream_t stream, bool order);
 };
 
+/* The lists of b200dpf_group_eval_device_bins, planned on the device (dpf_group_plan.cu) into buffers of their own,
+ * and the host half of their plan, which needs no key counts.  The host half is kept while nkeys, the prf and the
+ * options stay those of the call that made it (b200dpf_ctx_set_option and _set_subtree_log2 clear `valid`). */
+struct DevicePlanned {
+    EvalPlan P;               /* key_groups: a bound of the key groups; s: the largest s a group can be given */
+    int64_t nkeys = 0;
+    int64_t units_bound = 0;
+    int prf = -1;
+    bool valid = false;
+    GroupPlanParams gp{};     /* without the caller's bins and bad-key word */
+    DeviceBuffer<uint32_t> d_hist, d_sort, d_counts;   /* d_sort: keys in, keys out, values in, values out */
+    DeviceBuffer<void> d_temp;
+    DeviceBuffer<uint4> d_bin_first;
+    DeviceBuffer<uint2> d_order;
+    DeviceBuffer<GroupDesc> d_descs;
+    DeviceBuffer<WorkUnit> d_units;
+};
+
 }  // namespace
 
 struct GroupBins {
@@ -565,6 +585,7 @@ struct GroupBins {
     DeviceBuffer<uint2> d_bins;
     uint64_t query_v = 0;
     DeviceBuffer<uint32_t> d_te0;
+    DeviceBuffer<GroupBinInfo> d_bin_info;   /* made at create, never rewritten: [nbins] what the device planner reads */
     GroupLaunch once;                  /* b200dpf_group_eval and _eval_device: planned by every call */
     /* b200dpf_group_eval_queries_device: kept while nq, the prf and the options stay those of the call that made
      * it (b200dpf_ctx_set_option and _set_subtree_log2 clear cached_valid) */
@@ -572,6 +593,7 @@ struct GroupBins {
     int64_t cached_nq = 0;
     int cached_prf = -1;
     bool cached_valid = false;
+    DevicePlanned device_planned;      /* b200dpf_group_eval_device_bins */
 };
 
 namespace {
@@ -594,7 +616,7 @@ void fill_common(const b200dpf_ctx *c, const SmemLayout &L, const EvalJob &J, co
     p->key_stride_v = J.kl.stride_v; p->key_root_v = J.kl.root_v; p->key_compact = J.kl.compact;
     p->depth = c->shape.depth;
     p->nkeys = (int)J.nkeys; p->kpw_log2 = P.kpw_log2; p->key_groups = (int)P.key_groups;
-    p->groups = J.groups; p->units = J.units; p->nunits = J.nunits;
+    p->groups = J.groups; p->units = J.units; p->nunits = J.nunits; p->dev_counts = J.counts;
     p->table = reinterpret_cast<const uint4 *>(c->d_table.ptr);
     p->row_stride_v = (uint32_t)c->entry_pad / 4u;
     p->out_stride = (uint32_t)c->entry_size;
@@ -806,6 +828,28 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
     return B200DPF_OK;
 }
 
+/* The part of a grouped plan that needs no key counts: the mode, the passes, the shared-memory layout and the grid
+ * (which depend on the kernel alone, not on s), and s_group before shrink_s.  Automatic s (`shrink`) shrinks it from
+ * there down to *s_floor while the launch has fewer than *items_wanted work items. */
+int plan_group_base(b200dpf_ctx *c, int prf, int mode, EvalPlan *out, bool *shrink, int *s_floor, int64_t *items_wanted)
+{
+    const KindOps &ops = kKindOps[c->kind];
+    EvalPlan &P = *out = EvalPlan{};
+    const SmemLayout &L = P.L;
+    P.grouped = P.one_launch = true;
+    P.mode = mode;
+    P.nv = 4; P.passes = c->entry_pad / 16;     /* 16 columns per pass */
+    P.kpw_log2 = 5;
+    int rc = smem_layout(c, prf, P.nv, P.mode, &P.L);
+    if (rc) return rc;
+    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
+    P.s_group = std::min(c->knobs.subtree_log2 > 0 ? c->knobs.subtree_log2 : 6, L.s_max);
+    *shrink = c->knobs.subtree_log2 <= 0;
+    *s_floor = ops.leaf_items ? 1 : 3;
+    *items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
+    return B200DPF_OK;
+}
+
 /* The plan of one evaluation on a grouped context, whose bin-sorted keys of bin g are at positions
  * count[g] .. count[g + 1].  Key groups and their work-item size: big items amortise the root-to-subtree
  * walk every item pays (there is no frontier: bins are small), small items keep every warp busy.  Leaves
@@ -814,23 +858,17 @@ int plan_eval(b200dpf_ctx *c, const EvalJob &J, EvalPlan *out)
 int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, EvalPlan *out)
 {
     const GroupBins *B = c->bins.get();
-    const KindOps &ops = kKindOps[c->kind];
     const int nbins = (int)B->shape.size();
-    EvalPlan &P = *out = EvalPlan{};
+    EvalPlan &P = *out;
     const SmemLayout &L = P.L;
-    P.grouped = P.one_launch = true;
-    P.mode = ops.mode_grouped;
-    P.nv = 4; P.passes = c->entry_pad / 16;     /* 16 columns per pass */
-    P.kpw_log2 = 5;
-    int rc = smem_layout(c, prf, P.nv, P.mode, &P.L);
+    bool shrink = false;
+    int s_floor = 0;
+    int64_t items_wanted = 0;
+    int rc = plan_group_base(c, prf, kKindOps[c->kind].mode_grouped, out, &shrink, &s_floor, &items_wanted);
     if (rc) return rc;
-    const int64_t warps = (int64_t)L.grid * (L.threads / 32);
     auto groups_of = [&](int g) { return (count[(size_t)g + 1] - count[(size_t)g] + 31) / 32; };
     for (int g = 0; g < nbins; g++) P.key_groups += groups_of(g);
-    P.s_group = std::min(c->knobs.subtree_log2 > 0 ? c->knobs.subtree_log2 : 6, L.s_max);
-    if (c->knobs.subtree_log2 <= 0) {
-        const int s_floor = ops.leaf_items ? 1 : 3;
-        const int64_t items_wanted = (ops.leaf_items ? ops.leaf_items : 2) * warps;
+    if (shrink) {
         P.s_group = shrink_s(P.s_group, s_floor, items_wanted, [&](int t) {
             int64_t items = 0;
             for (int g = 0; g < nbins; g++)
@@ -845,6 +883,86 @@ int plan_group_eval(b200dpf_ctx *c, int prf, const std::vector<int64_t> &count, 
     P.pass_counters = mode_traits(P.mode).units ? 1u : (size_t)P.key_groups;
     P.smem = smem_bytes(L, P.s);
     fill_phase(L, P.s, &P.main);
+    return B200DPF_OK;
+}
+
+/* The host half of the plan of b200dpf_group_eval_device_bins for nkeys keys: plan_group_base, bounds of the lists
+ * the device half writes, and their buffers.  The rest (the counts, s_group, every group's s, the lists) is
+ * computed on the device from the bins by launch_group_plan. */
+int plan_group_device(b200dpf_ctx *c, int prf, int64_t nkeys, DevicePlanned *D)
+{
+    GroupBins *B = c->bins.get();
+    const int nbins = (int)B->shape.size();
+    EvalPlan &P = D->P;
+    const SmemLayout &L = P.L;
+    D->valid = false;
+    bool shrink = false;
+    int s_floor = 0;
+    int64_t items_wanted = 0;
+    int rc = plan_group_base(c, prf, kKindOps[c->kind].mode_grouped_dev, &P, &shrink, &s_floor, &items_wanted);
+    if (rc) return rc;
+    /* every key group but the last of its bin holds 32 keys: at most nkeys / 32 full groups, and one partial group
+     * per bin that has keys */
+    P.key_groups = nkeys / 32 + std::min<int64_t>(nbins, nkeys);
+    /* shared memory for the largest s a group can be given (group_s <= max(1, s_group)); a group's own s only picks
+     * its items.  L.grid and the block shape come from the kernel alone, so they do not depend on s. */
+    P.s = std::max(1, P.s_group);
+    P.pass_counters = mode_traits(P.mode).units ? 1u : (size_t)P.key_groups;
+    P.smem = smem_bytes(L, P.s);
+    fill_phase(L, P.s, &P.main);
+    /* Work units (GroupLaunch::plan): a key group of nsub items is cut into ceil(nsub / per_unit) units, per_unit =
+     * clamp(ceil(items / grid), 1, W) with W warps per block and `items` the sum of every group's nsub.  So units
+     * <= key groups + items / per_unit.  While per_unit < W, per_unit >= items / grid and items / per_unit <= grid;
+     * at per_unit = W, items / W <= key groups * nsub_max / W, nsub_max being the most items a bin's group can
+     * have (at s = 1). */
+    const bool units = mode_traits(P.mode).units;
+    const int unit_cap = L.threads / 32;
+    D->units_bound = 0;
+    if (units) {
+        int64_t nsub_max = 1;
+        for (const TableShape &t : B->shape) nsub_max = std::max<int64_t>(nsub_max, t.rows >> (1 + c->lane_bits()));
+        D->units_bound = P.key_groups + std::max<int64_t>(L.grid, (P.key_groups * nsub_max + unit_cap - 1) / unit_cap);
+    }
+    GroupPlanParams &g = D->gp;
+    g = GroupPlanParams{};
+    g.nkeys = nkeys;
+    g.nbins = nbins;
+    g.bin_info = B->d_bin_info.ptr;
+    g.lane_bits = c->lane_bits();
+    g.s_start = P.s_group;
+    g.shrink = shrink ? 1 : 0;
+    g.s_floor = s_floor;
+    g.items_wanted = items_wanted;
+    g.units = units ? 1 : 0;
+    g.grid = L.grid;
+    g.unit_cap = unit_cap;
+    g.end_bit = ilog2((int64_t)nbins + 1);     /* sort keys 0 .. nbins, nbins for a key outside every bin */
+    CUDA_TRY(group_plan_temp_bytes(nkeys, g.end_bit, &g.temp_bytes));
+    g.descs_cap = P.key_groups;
+    g.units_cap = D->units_bound;
+    rc = D->d_hist.reserve(((size_t)nbins + 1) * sizeof(uint32_t));
+    if (!rc) rc = D->d_counts.reserve(4 * sizeof(uint32_t));
+    if (!rc) rc = D->d_bin_first.reserve((size_t)nbins * sizeof(uint4));
+    if (!rc) rc = D->d_sort.reserve(4 * (size_t)nkeys * sizeof(uint32_t));
+    if (!rc) rc = D->d_temp.reserve(std::max<size_t>(g.temp_bytes, 1));
+    if (!rc) rc = D->d_order.reserve((size_t)nkeys * sizeof(uint2));
+    if (!rc) rc = D->d_descs.reserve((size_t)P.key_groups * sizeof(GroupDesc));
+    if (!rc && units) rc = D->d_units.reserve((size_t)D->units_bound * sizeof(WorkUnit));
+    if (rc) return rc;
+    g.hist = D->d_hist.ptr;
+    g.keys_in = D->d_sort.ptr;
+    g.keys_out = g.keys_in + nkeys;
+    g.vals_in = g.keys_out + nkeys;
+    g.vals_out = g.vals_in + nkeys;
+    g.temp = D->d_temp.ptr;
+    g.bin_first = D->d_bin_first.ptr;
+    g.order = D->d_order.ptr;
+    g.descs = D->d_descs.ptr;
+    g.units_out = D->d_units.ptr;
+    g.counts = D->d_counts.ptr;
+    D->nkeys = nkeys;
+    D->prf = prf;
+    D->valid = true;
     return B200DPF_OK;
 }
 
@@ -1700,7 +1818,10 @@ int b200dpf_ctx_last_launches(const b200dpf_ctx *c)
 /* The plans a grouped context keeps were made under its old options */
 static void options_changed(b200dpf_ctx *c)
 {
-    if (c->bins) c->bins->cached_valid = false;
+    if (c->bins) {
+        c->bins->cached_valid = false;
+        c->bins->device_planned.valid = false;
+    }
 }
 
 int b200dpf_ctx_set_subtree_log2(b200dpf_ctx *c, int s)
@@ -2041,22 +2162,27 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     if (rc) return rc;
     std::vector<RowPlacement> place;
     std::vector<uint2> query_bins;
+    std::vector<GroupBinInfo> info;
     for (int g = 0; g < nbins; g++) {
         /* each bin in its own breadth-first leaf order (bit reversal over ITS depth), or trimmed in row order */
         const TableShape &t = B->shape[(size_t)g];
         place.push_back(place_of(t, c->lane_bits(), trimmed, 0, 0));
+        info.push_back(GroupBinInfo{t.first * (uint64_t)(c->entry_pad / 4), (uint32_t)t.rows, t.depth, t.room, 0u});
         query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)t.depth));
         B->query_v += b200dpf_key_packed_size(t.depth) / 16u;
         rc = upload_table(c.get(), tables[g], place.back(), &d_stage);
         if (rc) return rc;
     }
     const size_t bins_bytes = (size_t)nbins * sizeof(uint2), place_bytes = (size_t)nbins * sizeof(RowPlacement);
+    const size_t info_bytes = (size_t)nbins * sizeof(GroupBinInfo);
     rc = B->d_place.reserve(place_bytes);
     if (!rc) rc = B->d_bins.reserve(bins_bytes);
+    if (!rc) rc = B->d_bin_info.reserve(info_bytes);
     if (!rc) rc = B->d_te0.reserve(256 * sizeof(uint32_t));
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(B->d_place.ptr, place.data(), place_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_bins.ptr, query_bins.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(B->d_bin_info.ptr, info.data(), info_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read them once the context is returned */
     *out = c.release();
@@ -2219,12 +2345,19 @@ int GroupLaunch::upload(cudaStream_t stream, bool order)
     return B200DPF_OK;
 }
 
-/* The evaluation by launch L of its keys, sorted by bin and compact in d_keys, into d_out in sorted order */
+/* The evaluation by plan P of nkeys keys, sorted by bin and compact in d_keys, into d_out in sorted order: the key
+ * groups' descriptors, the work units (nunits of them, or a bound of them when `counts` holds their counts) */
+static int group_launch_lists(b200dpf_ctx *c, const EvalPlan &P, int64_t nkeys, const GroupDesc *descs, const WorkUnit *units,
+                              uint32_t nunits, const uint32_t *counts, int prf, cudaStream_t stream)
+{
+    const EvalJob J{c->d_keys.ptr, compact_layout(c->shape.depth), nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
+                    descs, units, nunits, true, counts};
+    return launch_plan(c, J, P);
+}
+
 static int group_launch(b200dpf_ctx *c, const GroupLaunch &L, int prf, cudaStream_t stream)
 {
-    const EvalJob J{c->d_keys.ptr, compact_layout(c->shape.depth), L.nkeys, prf, MODE_FUSED, c->d_out.ptr, stream, true, false,
-                    L.d_descs.ptr, L.d_units.ptr, (uint32_t)L.nunits, true};
-    return launch_plan(c, J, L.P);
+    return group_launch_lists(c, L.P, L.nkeys, L.d_descs.ptr, L.d_units.ptr, (uint32_t)L.nunits, nullptr, prf, stream);
 }
 
 int b200dpf_group_eval(b200dpf_ctx *c, const int32_t *keys, const int32_t *bins, int64_t nkeys, int prf, int32_t *out)
@@ -2320,6 +2453,77 @@ int b200dpf_group_eval_device(b200dpf_ctx *c, const void *keys_dev, const int32_
     GroupLaunch &L = c->bins->once;
     rc = L.plan(c, prf, count, bins);
     return rc ? rc : group_enqueue(c, L, true, keys_dev, B200DPF_KEYS_WIRE, prf, out_dev, reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+/* The same evaluation with the bins in device memory too: the host half of the plan (plan_group_device) is kept per
+ * (nkeys, prf, options), and a call enqueues the device half (launch_group_plan: histogram, sort, plan, lists), the
+ * gather, the evaluation in the mode whose counts are on the device, and the scatter.  Keys whose bin is out of
+ * range sort to a tail no key group covers; the launch clears d_out, so the scatter gives them zero rows. */
+int b200dpf_group_eval_device_bins(b200dpf_ctx *c, const void *keys_dev, const int32_t *bins_dev, int64_t nkeys, int prf,
+                                   void *out_dev, int64_t *bad_dev, void *cuda_stream)
+{
+    int rc = check_group_args(c, keys_dev && bins_dev && out_dev, nkeys, false, prf, B200DPF_KEYS_WIRE);
+    if (rc) return rc;
+    if ((reinterpret_cast<uintptr_t>(keys_dev) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_dev) & 3u) != 0)
+        return fail(B200DPF_EINVAL, "keys_dev must be 16-byte aligned and out_dev 4-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(bins_dev) & 3u) != 0 || (reinterpret_cast<uintptr_t>(bad_dev) & 7u) != 0)
+        return fail(B200DPF_EINVAL, "bins_dev must be 4-byte aligned and bad_dev 8-byte aligned");
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    const cudaStream_t stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    DevicePlanned &D = c->bins->device_planned;
+    if (!D.valid || D.nkeys != nkeys || D.prf != prf) rc = plan_group_device(c, prf, nkeys, &D);
+    const KeyLayout kl = compact_layout(c->shape.depth);
+    if (!rc) rc = reserve_device_io(c, (size_t)nkeys * kl.stride_v * 16u, (size_t)nkeys * c->entry_size);
+    if (!rc) rc = wait_last(c, stream);
+    if (rc) return rc;
+    GroupPlanParams gp = D.gp;
+    gp.bins = bins_dev;
+    gp.bad = bad_dev;
+    CUDA_TRY(launch_group_plan(gp, c->sm_count, stream));
+    uint32_t magic = 0;
+    std::memcpy(&magic, host::kKinds[c->kind].magic, 4);
+    CUDA_TRY(launch_group_gather(keys_dev, D.d_order.ptr, nkeys, magic, kl.stride_v, c->d_keys.ptr, stream));
+    rc = group_launch_lists(c, D.P, nkeys, D.d_descs.ptr, D.d_units.ptr, (uint32_t)D.units_bound, D.d_counts.ptr, prf, stream);
+    if (rc) return rc;
+    CUDA_TRY(launch_group_scatter(c->d_out.ptr, D.d_order.ptr, nkeys, c->entry_size, out_dev, stream));
+    return mark_last(c, stream);
+}
+
+/* The lists of a grouped context's last plan, for tests: which = 0, those b200dpf_group_eval_device_bins made on the
+ * device (read after the context's last operation); which = 1, those b200dpf_group_eval or _eval_device made on the
+ * host.  counts = (key groups, work units, keys, keys out of range); up to the caps of entries are copied. */
+int b200dpf_group_plan_lists(b200dpf_ctx *c, int which, int64_t *counts, void *descs, int64_t descs_cap, void *units,
+                             int64_t units_cap, void *order, int64_t order_cap)
+{
+    if (!c || !c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
+    if (!counts || !descs || !units || !order || which < 0 || which > 1 || descs_cap < 0 || units_cap < 0 || order_cap < 0)
+        return fail(B200DPF_EINVAL, "bad arguments");
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    GroupBins *B = c->bins.get();
+    if (which == 0) {
+        const DevicePlanned &D = B->device_planned;
+        if (!D.valid) return fail(B200DPF_ESTATE, "no b200dpf_group_eval_device_bins call to read");
+        if (c->has_last) CUDA_TRY(cudaEventSynchronize(c->ev_done));
+        uint32_t n[4];
+        CUDA_TRY(cudaMemcpy(n, D.d_counts.ptr, sizeof n, cudaMemcpyDeviceToHost));
+        counts[0] = n[0]; counts[1] = n[1]; counts[2] = D.nkeys; counts[3] = n[2];
+        if (std::min<int64_t>(n[0], descs_cap) > 0)
+            CUDA_TRY(cudaMemcpy(descs, D.d_descs.ptr, (size_t)std::min<int64_t>(n[0], descs_cap) * sizeof(GroupDesc), cudaMemcpyDeviceToHost));
+        if (std::min<int64_t>(n[1], units_cap) > 0)
+            CUDA_TRY(cudaMemcpy(units, D.d_units.ptr, (size_t)std::min<int64_t>(n[1], units_cap) * sizeof(WorkUnit), cudaMemcpyDeviceToHost));
+        if (std::min<int64_t>(D.nkeys, order_cap) > 0)
+            CUDA_TRY(cudaMemcpy(order, D.d_order.ptr, (size_t)std::min<int64_t>(D.nkeys, order_cap) * sizeof(uint2), cudaMemcpyDeviceToHost));
+        return B200DPF_OK;
+    }
+    const GroupLaunch &L = B->once;
+    if (!L.h_descs.ptr) return fail(B200DPF_ESTATE, "no b200dpf_group_eval or _eval_device call to read");
+    counts[0] = L.P.key_groups; counts[1] = L.nunits; counts[2] = L.nkeys; counts[3] = 0;
+    std::memcpy(descs, L.h_descs.ptr, (size_t)std::min<int64_t>(L.P.key_groups, descs_cap) * sizeof(GroupDesc));
+    if (L.nunits) std::memcpy(units, L.h_units.ptr, (size_t)std::min<int64_t>(L.nunits, units_cap) * sizeof(WorkUnit));
+    std::memcpy(order, L.h_order.ptr, (size_t)std::min<int64_t>(L.nkeys, order_cap) * sizeof(uint2));
+    return B200DPF_OK;
 }
 
 int64_t b200dpf_group_query_bytes(const b200dpf_ctx *c)

@@ -335,6 +335,18 @@ void group_eval_device(int64_t keys_ptr, const at::Tensor &bins, int64_t nkeys, 
           "group_eval_device");
 }
 
+/* the same with the bins in device memory too (b200dpf_group_eval_device_bins): int32 [nkeys] at bins_ptr, planned on
+ * the GPU; a key whose bin is out of range gets a zero row, and their number goes to the int64 at bad_ptr if it is not
+ * 0.  Enqueued on the stream handle passed as an integer, with no host wait. */
+void group_eval_device_bins(int64_t keys_ptr, int64_t bins_ptr, int64_t nkeys, const std::vector<void *> &buffers, int prf,
+                            int64_t out_ptr, int64_t bad_ptr, int64_t stream)
+{
+    check(b200dpf_group_eval_device_bins(ctx_of(buffers), reinterpret_cast<const void *>(keys_ptr),
+                                         reinterpret_cast<const int32_t *>(bins_ptr), nkeys, prf, reinterpret_cast<void *>(out_ptr),
+                                         reinterpret_cast<int64_t *>(bad_ptr), reinterpret_cast<void *>(stream)),
+          "group_eval_device_bins");
+}
+
 /* batch-PIR queries of one key per bin (b200dpf_group_eval_queries_device): device keys at keys_ptr, int32
  * [nqueries, nbins, 524], or with `compact` uint8 [nqueries, group_query_bytes] compact queries, into device
  * results int32 [nqueries, nbins, E] at out_ptr, enqueued on the stream handle passed as an integer */
@@ -626,6 +638,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("group_eval_device", &group_eval_device, "batch PIR from device keys into device results, enqueued on a stream",
           py::arg("keys_ptr"), py::arg("bins"), py::arg("nkeys"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"),
           py::arg("stream"));
+    m.def("group_eval_device_bins", &group_eval_device_bins,
+          "batch PIR from device keys and device bins into device results, planned on the GPU, enqueued on a stream",
+          py::arg("keys_ptr"), py::arg("bins_ptr"), py::arg("nkeys"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"),
+          py::arg("bad_ptr"), py::arg("stream"));
     m.def("group_eval_queries_device", &group_eval_queries_device,
           "batch PIR: queries of one key per bin from device memory into device results, enqueued on a stream",
           py::arg("keys_ptr"), py::arg("nqueries"), py::arg("buffers"), py::arg("prf"), py::arg("out_ptr"), py::arg("stream"),

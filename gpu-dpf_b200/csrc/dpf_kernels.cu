@@ -502,8 +502,12 @@ __device__ __forceinline__ void run_phase(const EvalParams &p, const PhaseParams
     }
 
     uint32_t taken = 0;
-    for (int j = 0; j < p.key_groups; j++) {
-        const int kg = (int)((blockIdx.x + (unsigned)j) % (unsigned)p.key_groups);
+    /* the key groups: those the device planned (read once), or p.key_groups */
+    int dev_groups = 0;
+    if constexpr (M.counts_on_device) dev_groups = (int)p.dev_counts[0];
+    auto key_groups = [&]() { return M.counts_on_device ? dev_groups : p.key_groups; };
+    for (int j = 0; j < key_groups(); j++) {
+        const int kg = (int)((blockIdx.x + (unsigned)j) % (unsigned)key_groups());
 
         /* what this key group evaluates: the context's one table, or (grouped) its own bin */
         int g_depth = p.depth, g_s = ph.s, g_walk_first = ph.walk_first_level, g_walk_steps = ph.walk_steps;
@@ -680,6 +684,8 @@ __device__ __forceinline__ void run_units(const EvalParams &p, const PhaseParams
     env.leaf_out = nullptr;
     env.key_valid = true;
 
+    uint32_t dev_units = 0;
+    if constexpr (M.counts_on_device) dev_units = p.dev_counts[1];
     uint32_t loaded = 0xffffffffu;        /* the key group in shared memory (block-uniform) */
     for (uint32_t i = 0;; i++) {
         /* the two slots take turns: slot i & 1 is written again at draw i + 2, and every thread has read it
@@ -687,7 +693,7 @@ __device__ __forceinline__ void run_units(const EvalParams &p, const PhaseParams
         if (tid == 0) draw_s[i & 1] = atomicAdd(ph.counters, 1u);
         __syncthreads();                  /* also: every warp is done with the previous unit */
         const uint32_t u = draw_s[i & 1];
-        if (u >= p.nunits) break;
+        if (u >= (M.counts_on_device ? dev_units : p.nunits)) break;
         const WorkUnit unit = p.units[u];
         const GroupDesc g = p.groups[unit.group];
         const int key_first = (int)g.key_first, key_last = (int)(g.key_first + g.nkeys) - 1;
@@ -1078,6 +1084,9 @@ EvalKernel eval_kernel_of(int nv, int mode)
         case MODE_FUSED_XOR: return eval_kernel<PRF, 4, MODE_FUSED_XOR>();
         case MODE_EXPAND_XOR: return eval_kernel<PRF, 4, MODE_EXPAND_XOR>();
         case MODE_GROUPED_XOR: return eval_kernel<PRF, 4, MODE_GROUPED_XOR>();
+        case MODE_GROUPED_DEV: return eval_kernel<PRF, 4, MODE_GROUPED_DEV>();
+        case MODE_GROUPED_ET_DEV: return eval_kernel<PRF, 4, MODE_GROUPED_ET_DEV>();
+        case MODE_GROUPED_XOR_DEV: return eval_kernel<PRF, 4, MODE_GROUPED_XOR_DEV>();
         case MODE_FUSED_TMA:       /* AES: no shared memory left beside the tables */
             if constexpr (PRF != PRF_AES128) return eval_kernel<PRF, 4, MODE_FUSED_TMA>();
             break;

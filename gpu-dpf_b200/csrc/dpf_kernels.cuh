@@ -166,13 +166,19 @@ struct EvalParams {
     /* modes that draw work units: the list, drawn through main.counters[0] (one counter per pass) */
     const WorkUnit *units;
     uint32_t nunits;
+    /* modes whose counts are on the device (ModeTraits::counts_on_device): [0] the key groups of `groups`, [1] the
+     * work units of `units`, written by the plan kernels (dpf_group_plan.cu).  key_groups and nunits above are then
+     * only bounds of those lists */
+    const uint32_t *dev_counts;
 };
 
 /* Kernel modes: the MODE of dpf_eval_kernel<PRF, NV, MODE>.  Each is a combination of the properties
  * of ModeTraits, and mode_traits below is the one place that says which. */
 enum { MODE_FUSED = 0, MODE_EXPAND = 1, MODE_FRONTIER = 2, MODE_GROUPED = 3, MODE_FUSED_TMA = 4,
        MODE_FUSED_ET = 5, MODE_EXPAND_ET = 6, MODE_FUSED_COLSPLIT = 7, MODE_GROUPED_ET = 8,
-       MODE_FUSED_XOR = 9, MODE_EXPAND_XOR = 10, MODE_GROUPED_XOR = 11, MODE_COUNT = 12 };
+       MODE_FUSED_XOR = 9, MODE_EXPAND_XOR = 10, MODE_GROUPED_XOR = 11,
+       /* the grouped modes with their key-group and work-unit counts on the device (b200dpf_group_eval_device_bins) */
+       MODE_GROUPED_DEV = 12, MODE_GROUPED_ET_DEV = 13, MODE_GROUPED_XOR_DEV = 14, MODE_COUNT = 15 };
 
 /* The group a mode's result lives in (ModeTraits::result). */
 enum { RESULT_ADD,        /* Z/2^32: out[key][col] = sum of share * row, red.global.add */
@@ -207,24 +213,30 @@ struct ModeTraits {
     /* the main phase draws work units (EvalParams::units, one per block and draw) instead of walking
      * every key group's tickets: a block touches only the key groups it draws units of */
     bool units;
+    /* grouped: the main phase takes its key-group count (units: its work-unit count) from EvalParams::dev_counts, read
+     * once per phase, instead of from key_groups (nunits), which is then a bound: the lists were planned on the device */
+    bool counts_on_device;
 };
 
 __host__ __device__ constexpr ModeTraits mode_traits(int mode)
 {
-    switch (mode) {                            /* feeds           row_load        row_shift grouped result   units */
-    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false, RESULT_ADD, false};
-    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false, RESULT_ADD, false};
-    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false, RESULT_ADD, false};
-    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD, false};
-    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false, RESULT_ADD, false};
-    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false, RESULT_ADD, false};
-    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false, RESULT_ADD, false};
-    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false, RESULT_ADD, false};
-    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD, false};
-    case MODE_FUSED_XOR:      return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, false, RESULT_XOR, false};
-    case MODE_EXPAND_XOR:     return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 7, false, RESULT_XOR, false};
-    case MODE_GROUPED_XOR:    return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, true,  RESULT_XOR, true};
-    default:                  return ModeTraits{-1, -1, 0, false, RESULT_ADD, false};
+    switch (mode) {                            /* feeds           row_load        row_shift grouped result   units  counts_on_device */
+    case MODE_FUSED:          return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, false, RESULT_ADD, false, false};
+    case MODE_EXPAND:         return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 0, false, RESULT_ADD, false, false};
+    case MODE_FRONTIER:       return ModeTraits{FEEDS_FRONTIER, ROWS_BROADCAST, 0, false, RESULT_ADD, false, false};
+    case MODE_GROUPED:        return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD, false, false};
+    case MODE_FUSED_TMA:      return ModeTraits{FEEDS_MAC,      ROWS_STAGED,    0, false, RESULT_ADD, false, false};
+    case MODE_FUSED_ET:       return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, false, RESULT_ADD, false, false};
+    case MODE_EXPAND_ET:      return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 2, false, RESULT_ADD, false, false};
+    case MODE_FUSED_COLSPLIT: return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  0, false, RESULT_ADD, false, false};
+    case MODE_GROUPED_ET:     return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD, false, false};
+    case MODE_FUSED_XOR:      return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, false, RESULT_XOR, false, false};
+    case MODE_EXPAND_XOR:     return ModeTraits{FEEDS_SHARES,   ROWS_BROADCAST, 7, false, RESULT_XOR, false, false};
+    case MODE_GROUPED_XOR:    return ModeTraits{FEEDS_MAC,      ROWS_COLSPLIT,  7, true,  RESULT_XOR, true,  false};
+    case MODE_GROUPED_DEV:    return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 0, true,  RESULT_ADD, false, true};
+    case MODE_GROUPED_ET_DEV: return ModeTraits{FEEDS_MAC,      ROWS_BROADCAST, 2, true,  RESULT_ADD, false, true};
+    case MODE_GROUPED_XOR_DEV: return ModeTraits{FEEDS_MAC,     ROWS_COLSPLIT,  7, true,  RESULT_XOR, true,  true};
+    default:                  return ModeTraits{-1, -1, 0, false, RESULT_ADD, false, false};
     }
 }
 
@@ -317,6 +329,14 @@ struct KeygenParams {
 };
 cudaError_t launch_keygen(int prf, int group, const KeygenParams &p, cudaStream_t stream);
 
+/* The device-planned grouped modes are their parents in every other property, so they take their parents' block
+ * shapes: the host plans their grid and shared memory before it knows any count */
+static_assert(eval_block_shape(PRF_AES128, 4, MODE_GROUPED_DEV).threads == eval_block_shape(PRF_AES128, 4, MODE_GROUPED).threads &&
+              eval_block_shape(PRF_AES128, 4, MODE_GROUPED_ET_DEV).threads == eval_block_shape(PRF_AES128, 4, MODE_GROUPED_ET).threads &&
+              eval_block_shape(PRF_AES128, 4, MODE_GROUPED_XOR_DEV).threads == eval_block_shape(PRF_AES128, 4, MODE_GROUPED_XOR).threads &&
+              eval_block_shape(PRF_CHACHA20, 4, MODE_GROUPED_XOR_DEV).threads == eval_block_shape(PRF_CHACHA20, 4, MODE_GROUPED_XOR).threads,
+              "a device-planned grouped mode has its parent's block shape");
+
 /* Maximum dynamic shared memory the evaluation kernel may be given. */
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
@@ -342,6 +362,56 @@ cudaError_t launch_group_scatter(const int32_t *sorted, const uint2 *order, int6
  * its header rewritten to (magic, depth, 0, 0), stride_v uint4 apart: the bytes pack_compact writes. */
 cudaError_t launch_group_gather_queries(const void *queries, const uint2 *bins, int64_t nkeys, uint32_t nq, uint64_t query_v,
                                         uint32_t magic, uint32_t stride_v, void *compact, cudaStream_t stream);
+
+/* One bin of a grouped context as the device planner sees it, made at create and never rewritten. */
+struct GroupBinInfo {
+    uint64_t table_off_v;     /* the bin's first row, in uint4 units from the table (GroupDesc::table_off_v) */
+    uint32_t rows;            /* rows of its device table, padding included                               */
+    int32_t depth;            /* leaf levels of its key tree                                             */
+    int32_t room;             /* log2 leaves of the largest work item inside its rows                    */
+    uint32_t pad;
+};
+
+/* The plan of a grouped evaluation made on the device from a device-resident bin list
+ * (b200dpf_group_eval_device_bins, dpf_group_plan.cu).  The host fills what needs no key counts; the kernels
+ * compute, from the counts, the lists GroupLaunch::plan makes on the host for the same bins:
+ *   histogram : hist[g] = keys of bin g, hist[nbins] = keys whose bin is outside [0, nbins)
+ *   sort      : a stable radix sort of (bin, caller's index), out-of-range keys as bin nbins, so they form a tail
+ *               no key group covers; order[pos] = (caller's index, bin depth, 0 for the tail)
+ *   plan      : one block: s_group by shrink_s, per bin its first sorted key, key group and work unit
+ *               (bin_first[g] = (key, group, unit, s)); counts = (key groups, work units, out-of-range keys,
+ *               items per unit); *bad = counts[2] when bad is not null
+ *   emit      : descs[k] for k < counts[0] in bin order and, for modes that draw work units, units[u] for
+ *               u < counts[1] in group-major order */
+struct GroupPlanParams {
+    const int32_t *bins;      /* [nkeys] the caller's bin ids */
+    int64_t nkeys;
+    int nbins;
+    const GroupBinInfo *bin_info;   /* [nbins] */
+    int lane_bits;
+    int s_start;              /* s_group before shrink_s: min(subtree_log2 knob or 6, s_max) */
+    int shrink;               /* automatic s: shrink from s_start down to s_floor while the launch has fewer items than wanted */
+    int s_floor;
+    int64_t items_wanted;
+    int units;                /* the mode draws work units (ModeTraits::units) */
+    int grid, unit_cap;       /* work units: items per unit = clamp(ceil(items / grid), 1, unit_cap) */
+    int end_bit;              /* bits of a sort key: bins 0 .. nbins */
+    uint32_t *hist;           /* [nbins + 1], cleared by launch_group_plan */
+    uint32_t *keys_in, *keys_out, *vals_in, *vals_out;   /* [nkeys] sort buffers */
+    void *temp;
+    size_t temp_bytes;        /* group_plan_temp_bytes */
+    uint4 *bin_first;         /* [nbins] */
+    uint2 *order;             /* [nkeys] */
+    GroupDesc *descs;         /* [key-group bound] */
+    WorkUnit *units_out;      /* [work-unit bound] */
+    int64_t descs_cap, units_cap;
+    uint32_t *counts;         /* [4] */
+    int64_t *bad;             /* or null */
+};
+/* Bytes of temporary storage the sort of `nkeys` keys below 2^end_bit needs. */
+cudaError_t group_plan_temp_bytes(int64_t nkeys, int end_bit, size_t *bytes);
+/* Enqueue the histogram, the sort, the plan and the emission on `stream`; no host synchronisation. */
+cudaError_t launch_group_plan(const GroupPlanParams &p, int sm_count, cudaStream_t stream);
 
 /* Row update of a live table (b200dpf_update_rows*): device row P.device_row(idx[j]) := rows[j] for j < count, the
  * last occurrence of a device row winning.  P is bin_place[bins[j]] on a grouped context, else `place`; entry j is

@@ -505,6 +505,37 @@ class BinnedDPF(DPF):
                                   self.prf_method, out_dev.data_ptr(), stream)
         return out_dev
 
+    def eval_gpu_device_bins(self, keys_dev, bins_dev, out_dev=None, bad_dev=None):
+        """eval_gpu_device with the bins on the device too: keys_dev int32 [B, 524] and bins_dev int32 [B] CUDA
+        tensors -> int32 [B, entry_size] CUDA tensor (out_dev, if given, is filled), planned on the GPU and enqueued
+        on the current torch stream without any host wait.  A key whose bin is outside [0, nbins) gets a zero row;
+        bad_dev, an int64 [1] CUDA tensor if given, receives the number of such keys."""
+        name = "BinnedDPF.eval_gpu_device_bins"
+        if not (isinstance(keys_dev, torch.Tensor) and keys_dev.is_cuda and keys_dev.dtype == torch.int32
+                and keys_dev.is_contiguous() and keys_dev.dim() == 2 and keys_dev.shape[1] == 524
+                and keys_dev.device.index == self.device):
+            raise Exception("%s: keys_dev must be a contiguous int32 [B, 524] tensor on cuda:%d" % (name, self.device))
+        if not (isinstance(bins_dev, torch.Tensor) and bins_dev.is_cuda and bins_dev.dtype == torch.int32
+                and bins_dev.is_contiguous() and tuple(bins_dev.shape) == (keys_dev.shape[0],)
+                and bins_dev.device == keys_dev.device):
+            raise Exception("%s: bins_dev must be a contiguous int32 [%d] tensor on %s (one bin per key)"
+                            % (name, keys_dev.shape[0], keys_dev.device))
+        if bad_dev is not None and not (isinstance(bad_dev, torch.Tensor) and bad_dev.is_cuda and bad_dev.dtype == torch.int64
+                                        and bad_dev.numel() == 1 and bad_dev.device == keys_dev.device):
+            raise Exception("%s: bad_dev must be an int64 [1] tensor on %s" % (name, keys_dev.device))
+        if self.buffers is None:
+            raise Exception("%s: must call `eval_init` first" % name)
+        shape = (keys_dev.shape[0], self.table_effective_entry_size)
+        if out_dev is None:
+            out_dev = torch.empty(shape, dtype=torch.int32, device=keys_dev.device)
+        elif not (isinstance(out_dev, torch.Tensor) and out_dev.is_cuda and out_dev.dtype == torch.int32
+                  and out_dev.is_contiguous() and out_dev.device == keys_dev.device and tuple(out_dev.shape) == shape):
+            raise Exception("%s: out_dev must be a contiguous int32 [%d, %d] tensor on %s" % ((name,) + shape + (keys_dev.device,)))
+        stream = torch.cuda.current_stream(keys_dev.device).cuda_stream
+        dpf_cpp.group_eval_device_bins(keys_dev.data_ptr(), bins_dev.data_ptr(), keys_dev.shape[0], self.buffers, self.prf_method,
+                                       out_dev.data_ptr(), 0 if bad_dev is None else bad_dev.data_ptr(), stream)
+        return out_dev
+
     def eval_queries_device(self, keys_dev, out_dev=None):
         """Batch-PIR queries of one key per bin, device-resident and asynchronous: keys_dev is a CUDA tensor of
         Q queries, either int32 [Q, nbins, 524] wire-format keys (key g of a query for bin g) or uint8

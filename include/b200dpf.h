@@ -265,6 +265,45 @@ int b200dpf_group_eval(b200dpf_ctx *ctx, const int32_t *keys, const int32_t *bin
  */
 int b200dpf_group_eval_device(b200dpf_ctx *ctx, const void *keys_dev, const int32_t *bins, int64_t nkeys, int prf,
                               void *out_dev, void *cuda_stream);
+
+/*
+ * b200dpf_group_eval_device with the bin list in device memory too, planned on the GPU, for any mix of (bin, key)
+ * pairs on every kind of grouped context, trimmed ones included.
+ *   keys_dev: int32 [nkeys][524] (16-byte aligned), as for b200dpf_group_eval_device.
+ *   bins_dev: int32 [nkeys] in device memory (4-byte aligned): key b is evaluated on bin bins_dev[b].
+ *   out_dev:  int32 [nkeys][entry_size] (4-byte aligned).  out_dev[b] is bit for bit what b200dpf_group_eval_device
+ *             returns for key b with the same bins on the host.  A key whose bin is outside [0, nbins) gets a zero
+ *             row; the other keys' rows do not change.
+ *   bad_dev:  NULL, or int64 in device memory (8-byte aligned) that receives the number of keys whose bin is out of
+ *             range (written, not accumulated).
+ * The arguments are checked as by b200dpf_group_eval_device, before anything is enqueued: a context that is not
+ * grouped is ESTATE; a null buffer, nkeys outside [1, 2^24], an unknown prf or a misaligned buffer is EINVAL.  The
+ * bin ids are not checked on the host (they are never read there), and the keys are not validated: a key's depth
+ * comes from its bin.  Every buffer must stay valid until the stream reaches the end of the evaluation.
+ * No host wait: the call enqueues everything on cuda_stream and returns.  The sort by bin, the key groups, their
+ * work-item sizes, descriptors and work units, and the order list are computed on the device, into lists only this
+ * entry point uses; the host does work that does not grow with nkeys.  The only exception is device scratch that
+ * grows (an allocation) when nkeys grows past every earlier call's.  The host half of the plan is kept while nkeys,
+ * prf and the context's options (b200dpf_ctx_set_option, b200dpf_ctx_set_subtree_log2) stay those of its previous call.
+ * Ordering: the call joins the context's one-operation-in-flight chain (see "Threading" above), so it is ordered
+ * against every other grouped evaluation and row update of the context, on any stream.  Its launches are not for
+ * CUDA-graph capture: each cooperative launch's grid-barrier target is computed on the host.
+ * b200dpf_ctx_last_device_ms times the evaluation launches only (the plan kernels, gather and scatter are outside),
+ * and b200dpf_ctx_last_launches counts them.
+ */
+int b200dpf_group_eval_device_bins(b200dpf_ctx *ctx, const void *keys_dev, const int32_t *bins_dev, int64_t nkeys,
+                                   int prf, void *out_dev, int64_t *bad_dev, void *cuda_stream);
+/*
+ * For tests: the lists of a grouped context's last plan.  which = 0: those b200dpf_group_eval_device_bins made on the
+ * device (this waits for the context's last operation); which = 1: those the last b200dpf_group_eval or
+ * b200dpf_group_eval_device made on the host.  counts receives (key groups, work units, keys, keys whose bin is out of
+ * range); descs (32 bytes each: key_first, nkeys, depth, s, nsub, 0 as 32-bit words, then the bin's first row in
+ * 16-byte units as 64 bits), units (4 x uint32: group, first item, items, 0) and order (2 x uint32: the caller's index
+ * of the key at each sorted position, its bin's depth) receive up to their caps' entries.  ESTATE when there is no
+ * such plan.
+ */
+int b200dpf_group_plan_lists(b200dpf_ctx *ctx, int which, int64_t *counts, void *descs, int64_t descs_cap, void *units,
+                             int64_t units_cap, void *order, int64_t order_cap);
 int b200dpf_group_bins(const b200dpf_ctx *ctx);
 
 /*

@@ -186,4 +186,35 @@ for b, o in zip(batches, outs):
 rec = (want.astype(np.uint32) - ctx.eval(kb, 2).astype(np.uint32)).astype(np.int32)
 assert np.array_equal(rec, table[alphas])
 ctx.close()
+# grouped evaluation from device-resident bins, planned on the GPU, one context per kind: histogram, sort, plan and
+# list kernels, then the gather, evaluation and scatter; out-of-range bins mixed in, and a larger second batch that
+# grows the plan's scratch while the first may still run
+tables = [rng.randint(-2**31, 2**31, size=(m, 20), dtype=np.int64).astype(np.int32) for m in (256, 4096, 1024)]
+bins = np.array([0, 1, 2, 1, 1, 2, 1] * 7, np.int32)
+alphas = np.array([rng.randint(0, tables[g].shape[0]) for g in bins], np.int64)
+for kw, gen in (({}, b200dpf.gen_batch_secure), ({"early_termination": True}, b200dpf.gen_batch_et),
+                ({"xor": True}, b200dpf.gen_batch_xor)):
+    grp = b200dpf.GroupContext(tables, **kw)
+    ka, kb = np.zeros((len(bins), 524), np.int32), np.zeros((len(bins), 524), np.int32)
+    for g in range(3):
+        sel = np.nonzero(bins == g)[0]
+        ka[sel], kb[sel] = gen(alphas[sel], tables[g].shape[0], bytes(range(44)) * len(sel), 3)
+    with_bad = bins.copy()
+    with_bad[[3, 10, 20]] = [-1, 3, 99]
+    keys = [torch.from_numpy(k).cuda() for k in (ka, kb, ka)]
+    bins_dev = [torch.from_numpy(b).cuda() for b in (bins[:20], bins, with_bad)]
+    outs = [torch.empty((len(b), 20), dtype=torch.int32, device="cuda") for b in bins_dev]
+    bad = torch.full((3,), -1, dtype=torch.int64, device="cuda")
+    torch.cuda.synchronize()
+    for i, (k, b, o) in enumerate(zip(keys, bins_dev, outs)):
+        grp.eval_device_bins(k.data_ptr(), b.data_ptr(), len(b), 3, o.data_ptr(), bad[i:].data_ptr(), stream.cuda_stream)
+    stream.synchronize()
+    want_a, want_b = grp.eval(ka, bins, 3), grp.eval(kb, bins, 3)
+    assert bad.cpu().tolist() == [0, 0, 3]
+    assert np.array_equal(outs[0].cpu().numpy(), want_a[:20]) and np.array_equal(outs[1].cpu().numpy(), want_b)
+    good = np.setdiff1d(np.arange(len(bins)), [3, 10, 20])
+    assert np.array_equal(outs[2].cpu().numpy()[good], want_a[good]) and not outs[2].cpu().numpy()[[3, 10, 20]].any()
+    rec = want_a ^ want_b if kw.get("xor") else (want_a.astype(np.uint32) - want_b.astype(np.uint32)).astype(np.int32)
+    assert np.array_equal(rec, np.stack([tables[g][al] for g, al in zip(bins, alphas)]))
+    grp.close()
 print("sanitize run ok")
