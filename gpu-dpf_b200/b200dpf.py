@@ -35,6 +35,8 @@ SYMBOLS = [
     "b200dpf_trimmed_domain", "b200dpf_trimmed_alpha", "b200dpf_create_trimmed", "b200dpf_group_create_trimmed",
     "b200dpf_ctx_trimmed", "b200dpf_ctx_table_rows",
     "b200dpf_group_eval_device_bins", "b200dpf_group_plan_lists",
+    "b200dpf_batchcode_create", "b200dpf_batchcode_layout", "b200dpf_batchcode_locate", "b200dpf_batchcode_plan",
+    "b200dpf_batchcode_plan_device", "b200dpf_batchcode_update_rows",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -130,6 +132,13 @@ def load():
     L.b200dpf_ctx_trimmed.argtypes = [C.c_void_p]
     L.b200dpf_ctx_table_rows.argtypes = [C.c_void_p]
     L.b200dpf_ctx_table_rows.restype = C.c_int64
+    L.b200dpf_batchcode_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_int,
+                                           C.c_int]
+    L.b200dpf_batchcode_layout.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int), C.POINTER(C.c_uint64)]
+    L.b200dpf_batchcode_locate.argtypes = [C.c_int64, C.c_int, C.c_uint64, C.c_int64, _i32p, _i64p]
+    L.b200dpf_batchcode_plan.argtypes = [C.c_int64, C.c_int, C.c_uint64, _i64p, C.c_int64, C.c_int, _i64p, _i32p]
+    L.b200dpf_batchcode_plan_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200dpf_batchcode_update_rows.argtypes = [C.c_void_p, _i64p, _i32p, C.c_int64]
     return L
 
 
@@ -523,6 +532,11 @@ class GroupContext(Context):
     def nbins(self):
         return lib().b200dpf_group_bins(self.handle)
 
+    @property
+    def bin_rows(self):
+        """the live rows of each bin"""
+        return [t.shape[0] for t in self.tables]
+
     def eval(self, keys, bins, prf):
         keys = np.ascontiguousarray(keys, np.int32).reshape(-1, KEY_WORDS)
         bins = np.ascontiguousarray(bins, np.int32)
@@ -597,12 +611,12 @@ class GroupContext(Context):
         queries: each query its keys' compact forms (key_pack of the context's kind) back to back.  A key that
         is not of the context's kind, or not for its bin's size, raises."""
         keys = np.ascontiguousarray(keys, np.int32)
-        nbins = len(self.tables)
+        nbins = len(self.bin_rows)
         if keys.ndim != 3 or keys.shape[1:] != (nbins, KEY_WORDS):
             raise ValueError("pack_queries: keys must be int32 [Q, %d, %d], got shape %s" % (nbins, KEY_WORDS, keys.shape))
         lane_bits = KINDS[self.kind][0]
         trimmed = getattr(self, "_trimmed", False)
-        domains = [trimmed_domain(t.shape[0], self.kind) if trimmed else t.shape[0] for t in self.tables]
+        domains = [trimmed_domain(rows, self.kind) if trimmed else rows for rows in self.bin_rows]
         sizes = [lib().b200dpf_key_packed_size(n.bit_length() - 1 - lane_bits) for n in domains]
         out = np.empty((keys.shape[0], sum(sizes)), np.uint8)
         for q in range(keys.shape[0]):
@@ -623,3 +637,74 @@ class GroupContext(Context):
         assert bins.shape == indices.shape
         rows = np.ascontiguousarray(rows, np.int32).reshape(len(indices), self.entry_size)
         _check(lib().b200dpf_group_update_rows(self.handle, bins, indices, rows, len(indices)), "b200dpf_group_update_rows")
+
+
+def _layout_args(n, nbins, seed):
+    return int(n), int(nbins), int(seed) & 0xFFFFFFFFFFFFFFFF
+
+
+def batchcode_locate(n, nbins, seed, row):
+    """(bins, rows): the bin and the in-bin row of copies 0, 1, 2 of `row` in the batch-code layout (n, nbins, seed)
+    (b200dpf_batchcode_locate); host only"""
+    bins = np.zeros(3, np.int32)
+    rows = np.zeros(3, np.int64)
+    _check(lib().b200dpf_batchcode_locate(*_layout_args(n, nbins, seed), int(row), bins, rows), "b200dpf_batchcode_locate")
+    return bins, rows
+
+
+def batchcode_plan(n, nbins, seed, wanted):
+    """the client's plan of queries of k wanted rows (b200dpf_batchcode_plan): wanted int64 [Q, k] -> (alphas int64
+    [Q, nbins], the in-bin row to query in each bin; slots int32 [Q, k], the bin answering wanted row i or -1)"""
+    wanted = np.ascontiguousarray(wanted, np.int64)
+    if wanted.ndim != 2:
+        raise ValueError("batchcode_plan: wanted must be [Q, k], got shape %s" % (wanted.shape,))
+    alphas = np.zeros((wanted.shape[0], max(int(nbins), 0)), np.int64)
+    slots = np.zeros(wanted.shape, np.int32)
+    _check(lib().b200dpf_batchcode_plan(*_layout_args(n, nbins, seed), wanted, wanted.shape[0], wanted.shape[1], alphas, slots),
+           "b200dpf_batchcode_plan")
+    return alphas, slots
+
+
+class BatchCodeContext(GroupContext):
+    """One table of n rows stored as a batch code (b200dpf_batchcode_create): every row in 3 of nbins trimmed bins, so a
+    query of one key per bin retrieves any k rows the client's plan (batchcode_plan) places.  The kinds as for
+    GroupContext; every GroupContext evaluation works on it.  Rows change through update_rows, all three copies at once."""
+
+    def __init__(self, table, nbins, seed, device=0, early_termination=False, xor=False):
+        if xor and early_termination:
+            raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
+        table = np.ascontiguousarray(table, np.int32)
+        if table.ndim != 2:
+            raise ValueError("BatchCodeContext: table must be [n, entry_size], got shape %s" % (table.shape,))
+        self.n, self.entry_size = table.shape
+        self.kind = "_xor" if xor else "_et" if early_termination else ""
+        self._trimmed = True
+        self.handle = C.c_void_p()
+        _check(lib().b200dpf_batchcode_create(C.byref(self.handle), table.ctypes.data_as(C.c_void_p), self.n, self.entry_size,
+                                              int(nbins), int(seed) & 0xFFFFFFFFFFFFFFFF, device, KIND_IDS[self.kind]),
+               "b200dpf_batchcode_create")
+
+    @property
+    def layout(self):
+        """(n, nbins, seed): the public parameters a client plans with (b200dpf_batchcode_layout)"""
+        n, nbins, seed = C.c_int64(), C.c_int(), C.c_uint64()
+        _check(lib().b200dpf_batchcode_layout(self.handle, C.byref(n), C.byref(nbins), C.byref(seed)), "b200dpf_batchcode_layout")
+        return n.value, nbins.value, seed.value
+
+    @property
+    def bin_rows(self):
+        """the rows of each bin: 3 m_j, m_j = ceil((n - j) / nbins)"""
+        n, nbins, _ = self.layout
+        return [3 * ((n - j + nbins - 1) // nbins) for j in range(nbins)]
+
+    def plan_device(self, wanted_ptr, nqueries, k, alphas_ptr, slots_ptr, stream=0):
+        """batchcode_plan on the GPU from device buffers (wanted int64 [nqueries, k] into alphas int64 [nqueries,
+        nbins] and slots int32 [nqueries, k]), enqueued on `stream` with no host wait"""
+        _check(lib().b200dpf_batchcode_plan_device(self.handle, C.c_void_p(wanted_ptr), nqueries, k, C.c_void_p(alphas_ptr),
+                                                   C.c_void_p(slots_ptr), C.c_void_p(stream)), "b200dpf_batchcode_plan_device")
+
+    def update_rows(self, indices, rows):
+        """table[indices[j]] := rows[j] in all three copies (last occurrence wins); synchronous"""
+        indices = np.ascontiguousarray(indices, np.int64).reshape(-1)
+        rows = np.ascontiguousarray(rows, np.int32).reshape(len(indices), self.entry_size)
+        _check(lib().b200dpf_batchcode_update_rows(self.handle, indices, rows, len(indices)), "b200dpf_batchcode_update_rows")

@@ -594,6 +594,9 @@ struct GroupBins {
     int cached_prf = -1;
     bool cached_valid = false;
     DevicePlanned device_planned;      /* b200dpf_group_eval_device_bins */
+    /* a batch-code context (b200dpf_batchcode_create): the layout its bins follow.  Its rows change only three
+     * copies at a time (b200dpf_batchcode_update_rows), so b200dpf_group_update_rows refuses it. */
+    std::optional<BatchCodeLayout> batch;
 };
 
 namespace {
@@ -1208,27 +1211,39 @@ int ctx_open(int device, bool read_env, std::optional<DeviceGuard> *guard, std::
     return B200DPF_OK;
 }
 
-/* Fill the device rows of placement P from `src`, the caller's table of P.n rows in host or device memory, and wait
- * (the stage is then free for the next table): stage P's own rows in natural order (a shard gathers its leaves
- * own_val + k * 2^shift, k = 0, 1, ...), then place them in d_table, padded to 64-byte rows.  dpf_wrapper.cu:103-115
- * does the analogous reorder on the host with one ATen call per element. */
-int upload_table(b200dpf_ctx *c, const int32_t *src, const RowPlacement &P, DeviceBuffer<int32_t> *stage)
+/* Whether `src` is device memory (then *src_device is its device), after waiting for that device: the caller's table
+ * may still be being written there. */
+int wait_source(const b200dpf_ctx *c, const void *src, bool *on_device, int *src_device)
 {
     cudaPointerAttributes attr;
-    const bool on_device = cudaPointerGetAttributes(&attr, src) == cudaSuccess &&
-                           (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+    *on_device = cudaPointerGetAttributes(&attr, src) == cudaSuccess &&
+                 (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
     cudaGetLastError();
-    if (on_device) {   /* it may still be being written on the caller's stream (e.g. a dtype cast enqueued just before
+    *src_device = *on_device ? attr.device : -1;
+    if (*on_device) {  /* it may still be being written on the caller's stream (e.g. a dtype cast enqueued just before
                         * this call): our copy runs on a private non-blocking stream, so wait for its device first */
         if (attr.device != c->device) cudaSetDevice(attr.device);
         const cudaError_t es = cudaDeviceSynchronize();
         if (attr.device != c->device) cudaSetDevice(c->device);
         CUDA_TRY(es);
     }
+    return B200DPF_OK;
+}
+
+/* Fill the device rows of placement P from `src`, the caller's table of P.n rows in host or device memory, and wait
+ * (the stage is then free for the next table): stage P's own rows in natural order (a shard gathers its leaves
+ * own_val + k * 2^shift, k = 0, 1, ...), then place them in d_table, padded to 64-byte rows.  dpf_wrapper.cu:103-115
+ * does the analogous reorder on the host with one ATen call per element. */
+int upload_table(b200dpf_ctx *c, const int32_t *src, const RowPlacement &P, DeviceBuffer<int32_t> *stage)
+{
+    bool on_device;
+    int src_device;
+    int rc = wait_source(c, src, &on_device, &src_device);
+    if (rc) return rc;
     const size_t row_bytes = (size_t)c->entry_size * sizeof(int32_t);
     const int64_t rows = (int64_t)P.n >> P.shift;
     const size_t stage_bytes = (size_t)rows * row_bytes;
-    int rc = stage->reserve(stage_bytes);
+    rc = stage->reserve(stage_bytes);
     if (rc) return rc;
     cudaError_t e = cudaSuccess;
     if (P.shift == 0) {
@@ -2116,20 +2131,20 @@ int b200dpf_create_multi(b200dpf_ctx **out, const int32_t *table, int64_t n, int
 /* ------------------------------------------------------------------------------------------- */
 /* Grouped evaluation: the batch-PIR front end (SURVEY.md section 8(f) rank 4).                  */
 /* ------------------------------------------------------------------------------------------- */
-/* b200dpf_group_create, _et and _xor: a grouped context for keys of `kind`.  n and the row
- * offsets count rows, the depths (per bin and the context's deepest) leaves. */
-static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
-                             int device, int kind, bool trimmed = false)
+/* The context every grouped create function starts from: bins of n[g] rows for keys of `kind`, their shapes,
+ * placements and per-bin tables on the device (enqueued on the context's stream), and a zeroed device table, current
+ * while `guard` lives.  `tables` (null: not checked) are the bins' sources.  n and the row offsets count rows, the
+ * depths (per bin and the context's deepest) leaves. */
+static int group_open(const int32_t *const *tables, const int64_t *n, int nbins, int entry_size, int device, int kind,
+                      bool trimmed, std::optional<DeviceGuard> *guard, std::unique_ptr<b200dpf_ctx> *out)
 {
-    if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
-    *out = nullptr;
-    if (!tables || !n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
+    if (!n || nbins < 1 || nbins > (1 << 20)) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
     if (entry_size < 1 || entry_size > 4096) return fail(B200DPF_EINVAL, "entry_size=%d out of range [1,4096]", entry_size);
     if (kind < 0 || kind >= host::KIND_COUNT) return fail(B200DPF_EINVAL, "unknown key kind %d", kind);
     std::vector<TableShape> shape((size_t)nbins);
     TableShape all{};                   /* the context's (b200dpf_ctx::shape) */
     for (int g = 0; g < nbins; g++) {
-        if (!tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
+        if (tables && !tables[g]) return fail(B200DPF_EINVAL, "bin %d: null table", g);
         TableShape &t = shape[(size_t)g];
         const int rc = table_shape(n[g], kind, trimmed, g, &t);
         if (rc) return rc;
@@ -2138,9 +2153,8 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         all.depth = std::max(all.depth, t.depth);   /* the launch plan (shared memory for correction words) is sized by it */
         all.rows += t.rows;
     }
-    std::optional<DeviceGuard> guard;
-    std::unique_ptr<b200dpf_ctx> c;
-    int rc = ctx_open(device, false, &guard, &c);     /* grouped contexts keep the default knobs */
+    std::unique_ptr<b200dpf_ctx> &c = *out;
+    int rc = ctx_open(device, false, guard, &c);     /* grouped contexts keep the default knobs */
     if (rc) return rc;
     c->bins.reset(new (std::nothrow) GroupBins());
     if (!c->bins) return fail(B200DPF_ENOMEM, "out of host memory");
@@ -2157,9 +2171,6 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    DeviceBuffer<int32_t> d_stage;     /* every bin's: the largest one's */
-    rc = d_stage.reserve((size_t)all.n * entry_size * sizeof(int32_t));
-    if (rc) return rc;
     std::vector<RowPlacement> place;
     std::vector<uint2> query_bins;
     std::vector<GroupBinInfo> info;
@@ -2170,8 +2181,6 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
         info.push_back(GroupBinInfo{t.first * (uint64_t)(c->entry_pad / 4), (uint32_t)t.rows, t.depth, t.room, 0u});
         query_bins.push_back(make_uint2((uint32_t)B->query_v, (uint32_t)t.depth));
         B->query_v += b200dpf_key_packed_size(t.depth) / 16u;
-        rc = upload_table(c.get(), tables[g], place.back(), &d_stage);
-        if (rc) return rc;
     }
     const size_t bins_bytes = (size_t)nbins * sizeof(uint2), place_bytes = (size_t)nbins * sizeof(RowPlacement);
     const size_t info_bytes = (size_t)nbins * sizeof(GroupBinInfo);
@@ -2184,7 +2193,30 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     CUDA_TRY(cudaMemcpyAsync(B->d_bins.ptr, query_bins.data(), bins_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_bin_info.ptr, info.data(), info_bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(B->d_te0.ptr, host::aes_te0(), 256 * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read them once the context is returned */
+    /* the staging above is pageable: every copy has been taken from it when cudaMemcpyAsync returns */
+    return B200DPF_OK;
+}
+
+/* b200dpf_group_create, _et, _xor and _trimmed: a grouped context for keys of `kind`, each bin uploaded from its
+ * caller's table. */
+static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, const int64_t *n, int nbins, int entry_size,
+                             int device, int kind, bool trimmed = false)
+{
+    if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
+    *out = nullptr;
+    if (!tables) return fail(B200DPF_EINVAL, "bad bin list (nbins=%d)", nbins);
+    std::optional<DeviceGuard> guard;
+    std::unique_ptr<b200dpf_ctx> c;
+    int rc = group_open(tables, n, nbins, entry_size, device, kind, trimmed, &guard, &c);
+    if (rc) return rc;
+    DeviceBuffer<int32_t> d_stage;     /* every bin's: the largest one's */
+    rc = d_stage.reserve((size_t)c->shape.n * entry_size * sizeof(int32_t));
+    if (rc) return rc;
+    for (int g = 0; g < nbins; g++) {
+        rc = upload_table(c.get(), tables[g], place_of(c->bins->shape[(size_t)g], c->lane_bits(), trimmed, 0, 0), &d_stage);
+        if (rc) return rc;
+    }
+    CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read the per-bin tables once the context is returned */
     *out = c.release();
     return B200DPF_OK;
 }
@@ -2595,6 +2627,158 @@ int b200dpf_group_gen_queries_device(b200dpf_ctx *c, const int64_t *alphas_dev, 
 }
 
 /* ------------------------------------------------------------------------------------------- */
+/* Batch codes: any k rows of one table per query (DESIGN.md section 13).                        */
+/* ------------------------------------------------------------------------------------------- */
+/* The layout of an n-row table in nbins bins (BatchCodeLayout), or EINVAL */
+static int batchcode_layout_of(int64_t n, int nbins, uint64_t seed, BatchCodeLayout *L)
+{
+    if (n < 1 || n > ((int64_t)1 << 31)) return fail(B200DPF_EINVAL, "table size n=%lld out of range [1, 2^31]", (long long)n);
+    if (nbins < 1 || nbins > (1 << 20) || nbins > n)
+        return fail(B200DPF_EINVAL, "nbins=%d out of range [1, min(n, 2^20)] (n=%lld)", nbins, (long long)n);
+    int bits = 2;
+    while (bits < 64 && ((int64_t)1 << bits) < n) bits += 2;
+    *L = BatchCodeLayout{(uint64_t)n, seed, (uint32_t)nbins, bits / 2};
+    if (BATCHCODE_COPIES * L->per_copy(0) > ((uint64_t)1 << 31))
+        return fail(B200DPF_EINVAL, "bin 0 would hold %llu rows, more than 2^31: use more bins",
+                    (unsigned long long)(BATCHCODE_COPIES * L->per_copy(0)));
+    return B200DPF_OK;
+}
+
+/* The batch-code layout of a context, or ESTATE */
+static int batchcode_of(const b200dpf_ctx *c, const BatchCodeLayout **L)
+{
+    if (!c || !c->bins || !c->bins->batch) return fail(B200DPF_ESTATE, "not a batch-code context (b200dpf_batchcode_create)");
+    *L = &*c->bins->batch;
+    return B200DPF_OK;
+}
+
+/* The argument checks both planners make: k wanted rows per query, nqueries queries of one key per bin */
+static int check_plan_args(const BatchCodeLayout &L, bool bufs, int64_t nqueries, int k)
+{
+    if (!bufs) return fail(B200DPF_EINVAL, "null buffer");
+    if (k < 1 || k > BATCHCODE_MAX_K) return fail(B200DPF_EINVAL, "k=%d out of range [1, %d]", k, (int)BATCHCODE_MAX_K);
+    if (nqueries < 1 || nqueries > ((int64_t)1 << 24) / (int64_t)L.nbins)
+        return fail(B200DPF_EINVAL, "nqueries=%lld out of range: 1 <= nqueries * nbins (%u) <= 2^24", (long long)nqueries, L.nbins);
+    return B200DPF_OK;
+}
+
+/* Write the copies of rows [0, n) of `table` into the bins of c (placements already on the device), from the caller's
+ * buffer if it is on c's device, else through a bounded stage in chunks, and wait. */
+static int batchcode_fill(b200dpf_ctx *c, const int32_t *table, const BatchCodeLayout &L)
+{
+    bool on_device;
+    int src_device;
+    int rc = wait_source(c, table, &on_device, &src_device);
+    if (rc) return rc;
+    const size_t row_bytes = (size_t)c->entry_size * sizeof(int32_t);
+    DeviceBuffer<int32_t> stage;
+    if (on_device && src_device == c->device) {
+        CUDA_TRY(launch_batchcode_scatter(table, 0, L.n, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_size, c->entry_pad,
+                                          c->stream));
+    } else {
+        constexpr size_t kStageBytes = (size_t)64 << 20;
+        const uint64_t chunk = std::min<uint64_t>(L.n, std::max<size_t>(1, kStageBytes / row_bytes));
+        rc = stage.reserve((size_t)chunk * row_bytes);
+        if (rc) return rc;
+        for (uint64_t r0 = 0; r0 < L.n; r0 += chunk) {     /* one stream: a chunk's copy waits for the previous scatter */
+            const uint64_t rows = std::min<uint64_t>(chunk, L.n - r0);
+            CUDA_TRY(cudaMemcpyAsync(stage.ptr, table + r0 * (uint64_t)c->entry_size, (size_t)rows * row_bytes, cudaMemcpyDefault,
+                                     c->stream));
+            CUDA_TRY(launch_batchcode_scatter(stage.ptr, r0, rows, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_size,
+                                              c->entry_pad, c->stream));
+        }
+    }
+    CUDA_TRY(cudaStreamSynchronize(c->stream));       /* before the stage is freed; any stream may read the table after */
+    return B200DPF_OK;
+}
+
+int b200dpf_batchcode_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int nbins, uint64_t layout_seed,
+                             int device, int kind)
+{
+    if (!out) return fail(B200DPF_EINVAL, "null ctx out pointer");
+    *out = nullptr;
+    if (!table) return fail(B200DPF_EINVAL, "null table");
+    BatchCodeLayout L;
+    int rc = batchcode_layout_of(n, nbins, layout_seed, &L);
+    if (rc) return rc;
+    std::vector<int64_t> rows((size_t)nbins);
+    for (int j = 0; j < nbins; j++) rows[(size_t)j] = (int64_t)(BATCHCODE_COPIES * L.per_copy((uint32_t)j));
+    std::optional<DeviceGuard> guard;
+    std::unique_ptr<b200dpf_ctx> c;
+    rc = group_open(nullptr, rows.data(), nbins, entry_size, device, kind, true, &guard, &c);
+    if (!rc) rc = batchcode_fill(c.get(), table, L);
+    if (rc) return rc;
+    c->bins->batch = L;
+    *out = c.release();
+    return B200DPF_OK;
+}
+
+int b200dpf_batchcode_layout(const b200dpf_ctx *c, int64_t *n, int *nbins, uint64_t *seed)
+{
+    const BatchCodeLayout *L = nullptr;
+    const int rc = batchcode_of(c, &L);
+    if (rc) return rc;
+    if (!n || !nbins || !seed) return fail(B200DPF_EINVAL, "null buffer");
+    *n = (int64_t)L->n;
+    *nbins = (int)L->nbins;
+    *seed = L->seed;
+    return B200DPF_OK;
+}
+
+int b200dpf_batchcode_locate(int64_t n, int nbins, uint64_t seed, int64_t row, int32_t *bins3, int64_t *rows3)
+{
+    BatchCodeLayout L;
+    const int rc = batchcode_layout_of(n, nbins, seed, &L);
+    if (rc) return rc;
+    if (!bins3 || !rows3) return fail(B200DPF_EINVAL, "null buffer");
+    if (row < 0 || row >= n) return fail(B200DPF_EINVAL, "row %lld out of range [0, %lld)", (long long)row, (long long)n);
+    for (int c = 0; c < BATCHCODE_COPIES; c++) {
+        uint32_t bin;
+        uint64_t r;
+        L.locate(c, (uint64_t)row, &bin, &r);
+        bins3[c] = (int32_t)bin;
+        rows3[c] = (int64_t)r;
+    }
+    return B200DPF_OK;
+}
+
+int b200dpf_batchcode_plan(int64_t n, int nbins, uint64_t seed, const int64_t *wanted, int64_t nqueries, int k, int64_t *alphas,
+                           int32_t *slots)
+{
+    BatchCodeLayout L;
+    int rc = batchcode_layout_of(n, nbins, seed, &L);
+    if (!rc) rc = check_plan_args(L, wanted && alphas && slots, nqueries, k);
+    if (rc) return rc;
+    for (int64_t j = 0; j < nqueries * k; j++)
+        if (wanted[j] < 0 || wanted[j] >= n)
+            return fail(B200DPF_EINVAL, "query %lld: wanted row %lld out of range [0, %lld)", (long long)(j / k), (long long)wanted[j],
+                        (long long)n);
+    gen_parallel(nqueries, nqueries >= 64 ? 0 : 1, [&](int64_t q) {
+        batchcode_plan_query(L, wanted + q * k, k, alphas + q * (int64_t)nbins, slots + q * k);
+        return false;
+    });
+    return B200DPF_OK;
+}
+
+/* The planner of b200dpf_batchcode_plan, one thread per query, in the caller's buffers only: it neither joins the
+ * context's one-operation-in-flight chain nor reads anything of the context on the device. */
+int b200dpf_batchcode_plan_device(b200dpf_ctx *c, const int64_t *wanted_dev, int64_t nqueries, int k, int64_t *alphas_dev,
+                                  int32_t *slots_dev, void *cuda_stream)
+{
+    const BatchCodeLayout *L = nullptr;
+    int rc = batchcode_of(c, &L);
+    if (!rc) rc = check_plan_args(*L, wanted_dev && alphas_dev && slots_dev, nqueries, k);
+    if (rc) return rc;
+    if (((reinterpret_cast<uintptr_t>(wanted_dev) | reinterpret_cast<uintptr_t>(alphas_dev)) & 7u) != 0 ||
+        (reinterpret_cast<uintptr_t>(slots_dev) & 3u) != 0)
+        return fail(B200DPF_EINVAL, "wanted_dev and alphas_dev must be 8-byte aligned and slots_dev 4-byte aligned");
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    CUDA_TRY(launch_batchcode_plan(*L, wanted_dev, nqueries, k, alphas_dev, slots_dev, reinterpret_cast<cudaStream_t>(cuda_stream)));
+    return B200DPF_OK;
+}
+
+/* ------------------------------------------------------------------------------------------- */
 /* Row updates of a live table.                                                                  */
 /* ------------------------------------------------------------------------------------------- */
 }  // extern "C"
@@ -2763,6 +2947,8 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     int rc = check_update_args(c, indices, rows, count);
     if (rc) return rc;
     if (!c->bins) return fail(B200DPF_ESTATE, "not a grouped context (b200dpf_group_create)");
+    if (c->bins->batch)
+        return fail(B200DPF_ESTATE, "batch-code context: one copy of a row cannot change alone, use b200dpf_batchcode_update_rows");
     if (count > 0 && !bins) return fail(B200DPF_EINVAL, "null buffer");
     GroupBins *B = c->bins.get();
     const int nbins = (int)B->shape.size();
@@ -2777,6 +2963,43 @@ int b200dpf_group_update_rows(b200dpf_ctx *c, const int32_t *bins, const int64_t
     DeviceGuard guard(c->device);
     if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
     rc = update_host_enqueue(c, indices, bins, rows, count);
+    if (rc) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return B200DPF_OK;
+}
+
+/* All three copies of each row, through the grouped update path: entry j becomes entries 3j, 3j + 1, 3j + 2, one per
+ * copy, so the last occurrence of a row still wins in every copy. */
+int b200dpf_batchcode_update_rows(b200dpf_ctx *c, const int64_t *indices, const int32_t *rows, int64_t count)
+{
+    const BatchCodeLayout *L = nullptr;
+    int rc = batchcode_of(c, &L);
+    if (!rc) rc = check_update_args(c, indices, rows, count);
+    if (rc) return rc;
+    if (count > kMaxUpdateCount / BATCHCODE_COPIES)
+        return fail(B200DPF_EINVAL, "update count=%lld out of range [0, (2^31 - 1) / 3]", (long long)count);
+    for (int64_t j = 0; j < count; j++)
+        if (indices[j] < 0 || (uint64_t)indices[j] >= L->n)
+            return fail(B200DPF_EINVAL, "update %lld: index %lld out of range [0, %lld)", (long long)j, (long long)indices[j],
+                        (long long)L->n);
+    if (count == 0) return B200DPF_OK;
+    const size_t E = (size_t)c->entry_size;
+    std::vector<int32_t> bins3((size_t)count * BATCHCODE_COPIES);
+    std::vector<int64_t> idx3(bins3.size());
+    std::vector<int32_t> rows3(bins3.size() * E);
+    for (int64_t j = 0; j < count; j++)
+        for (int k = 0; k < BATCHCODE_COPIES; k++) {
+            const size_t e = (size_t)j * BATCHCODE_COPIES + k;
+            uint32_t bin;
+            uint64_t row;
+            L->locate(k, (uint64_t)indices[j], &bin, &row);
+            bins3[e] = (int32_t)bin;
+            idx3[e] = (int64_t)row;
+            std::memcpy(rows3.data() + e * E, rows + (size_t)j * E, E * sizeof(int32_t));
+        }
+    DeviceGuard guard(c->device);
+    if (!guard.ok) return fail(B200DPF_ECUDA, "cudaSetDevice(%d) failed", c->device);
+    rc = update_host_enqueue(c, idx3.data(), bins3.data(), rows3.data(), (int64_t)bins3.size());
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     return B200DPF_OK;

@@ -413,6 +413,81 @@ void group_update_rows(const at::Tensor &bins, const at::Tensor &indices, const 
           "group_update_rows");
 }
 
+/* batch codes (b200dpf_batchcode_*): one table [n, E] (CPU or CUDA tensor) in nbins bins of three copies per row */
+std::vector<void *> batchcode_init(const at::Tensor &table, int nbins, uint64_t seed, int device, int kind)
+{
+    TORCH_CHECK(table.dim() == 2, "batchcode_init: table must be [num_entries, entry_size]");
+    at::Tensor t = table.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    {
+        py::gil_scoped_release nogil;
+        check(b200dpf_batchcode_create(&ctx, t.data_ptr<int32_t>(), t.size(0), (int)t.size(1), nbins, seed, device, kind),
+              "batchcode_init");
+    }
+    return {static_cast<void *>(ctx)};
+}
+
+/* (n, nbins, layout seed) of a batch-code context */
+py::tuple batchcode_layout(const std::vector<void *> &buffers)
+{
+    int64_t n = 0;
+    int nbins = 0;
+    uint64_t seed = 0;
+    check(b200dpf_batchcode_layout(ctx_of(buffers), &n, &nbins, &seed), "batchcode_layout");
+    return py::make_tuple(n, nbins, seed);
+}
+
+/* ([bin of copy c], [in-bin row of copy c]) for c = 0, 1, 2 */
+py::tuple batchcode_locate(int64_t n, int nbins, uint64_t seed, int64_t row)
+{
+    int32_t bins[3];
+    int64_t rows[3];
+    check(b200dpf_batchcode_locate(n, nbins, seed, row, bins, rows), "batchcode_locate");
+    return py::make_tuple(std::vector<int32_t>(bins, bins + 3), std::vector<int64_t>(rows, rows + 3));
+}
+
+/* the host plan: wanted int64 [Q, k] CPU tensor -> (alphas int64 [Q, nbins], slots int32 [Q, k]) */
+std::vector<at::Tensor> batchcode_plan(int64_t n, int nbins, uint64_t seed, const at::Tensor &wanted)
+{
+    TORCH_CHECK(wanted.device().is_cpu() && wanted.scalar_type() == at::kLong && wanted.dim() == 2 && wanted.is_contiguous(),
+                "batchcode_plan: wanted must be a contiguous CPU int64 tensor [Q, k]");
+    at::Tensor alphas = torch::empty({wanted.size(0), (int64_t)std::max(nbins, 0)}, at::kLong);
+    at::Tensor slots = torch::empty({wanted.size(0), wanted.size(1)}, at::kInt);
+    {
+        py::gil_scoped_release nogil;
+        check(b200dpf_batchcode_plan(n, nbins, seed, wanted.data_ptr<int64_t>(), wanted.size(0), (int)wanted.size(1),
+                                     alphas.data_ptr<int64_t>(), slots.data_ptr<int32_t>()),
+              "batchcode_plan");
+    }
+    return {alphas, slots};
+}
+
+/* the device plan (b200dpf_batchcode_plan_device): wanted int64 [nqueries, k] at wanted_ptr, into alphas int64
+ * [nqueries, nbins] at alphas_ptr and slots int32 [nqueries, k] at slots_ptr, enqueued on the stream handle passed as
+ * an integer */
+void batchcode_plan_device(int64_t wanted_ptr, int64_t nqueries, int k, const std::vector<void *> &buffers, int64_t alphas_ptr,
+                           int64_t slots_ptr, int64_t stream)
+{
+    check(b200dpf_batchcode_plan_device(ctx_of(buffers), reinterpret_cast<const int64_t *>(wanted_ptr), nqueries, k,
+                                        reinterpret_cast<int64_t *>(alphas_ptr), reinterpret_cast<int32_t *>(slots_ptr),
+                                        reinterpret_cast<void *>(stream)),
+          "batchcode_plan_device");
+}
+
+/* table row indices[j] := rows[j] in all three copies; CPU tensors, synchronous */
+void batchcode_update_rows(const at::Tensor &indices, const at::Tensor &rows, const std::vector<void *> &buffers)
+{
+    b200dpf_ctx *ctx = ctx_of(buffers);
+    TORCH_CHECK(indices.device().is_cpu() && indices.scalar_type() == at::kLong && indices.dim() == 1 && indices.is_contiguous(),
+                "batchcode_update_rows: indices must be a contiguous CPU int64 tensor [count]");
+    TORCH_CHECK(rows.device().is_cpu() && rows.scalar_type() == at::kInt && rows.dim() == 2 && rows.is_contiguous() &&
+                    rows.size(0) == indices.size(0) && rows.size(1) == b200dpf_ctx_entry_size(ctx),
+                "batchcode_update_rows: rows must be a contiguous CPU int32 tensor [count, entry_size]");
+    py::gil_scoped_release nogil;
+    check(b200dpf_batchcode_update_rows(ctx, indices.data_ptr<int64_t>(), rows.data_ptr<int32_t>(), indices.size(0)),
+          "batchcode_update_rows");
+}
+
 /* "all" / "" -> every visible device; "0,2,3" -> that list */
 std::vector<int> parse_devices(const std::string &spec)
 {
@@ -658,6 +733,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("update_rows_device", &update_rows_device, "row update from device buffers, enqueued on a stream",
           py::arg("idx_ptr"), py::arg("rows_ptr"), py::arg("count"), py::arg("buffers"), py::arg("stream"));
     m.def("group_update_rows", &group_update_rows, "batch PIR: row indices[j] of bin bins[j] := rows[j]");
+    m.def("batchcode_init", &batchcode_init, "batch code: one table in nbins bins, three copies per row", py::arg("table"),
+          py::arg("nbins"), py::arg("seed"), py::arg("device") = 0, py::arg("kind") = 0);
+    m.def("batchcode_layout", &batchcode_layout, "(n, nbins, layout seed) of a batch-code context");
+    m.def("batchcode_locate", &batchcode_locate, "(bins, in-bin rows) of the three copies of a row", py::arg("n"),
+          py::arg("nbins"), py::arg("seed"), py::arg("row"));
+    m.def("batchcode_plan", &batchcode_plan, "the client's plan: wanted [Q, k] -> (alphas [Q, nbins], slots [Q, k])",
+          py::arg("n"), py::arg("nbins"), py::arg("seed"), py::arg("wanted"));
+    m.def("batchcode_plan_device", &batchcode_plan_device, "the client's plan on the GPU, from and into device buffers",
+          py::arg("wanted_ptr"), py::arg("nqueries"), py::arg("k"), py::arg("buffers"), py::arg("alphas_ptr"),
+          py::arg("slots_ptr"), py::arg("stream") = 0);
+    m.def("batchcode_update_rows", &batchcode_update_rows, "batch code: table row indices[j] := rows[j] in all three copies");
     m.def("parse_devices", &parse_devices, "'all' or '0,1,2' -> device list");
     m.def("device_count", [](const std::vector<void *> &b) { return b200dpf_ctx_device_count(ctx_of(b)); });
     m.def("axis", [](const std::vector<void *> &b) { return b200dpf_ctx_axis(ctx_of(b)); });

@@ -58,6 +58,133 @@ DPF_HD uint64_t trimmed_alpha(uint64_t r, int depth, int lane_bits)
     return ((uint64_t)bitrev((uint32_t)(r >> lane_bits), depth) << lane_bits) | (r & ((1u << lane_bits) - 1u));
 }
 
+/* Batch-code layout (b200dpf_batchcode_create, DESIGN.md section 13): every row of an n-row table has three copies in
+ * nbins trimmed bins, each copy placed by its own keyed permutation of [0, n).  Table creation, row updates, the host
+ * planner and the device planner all place rows through this one definition; include/b200dpf.h states it in full. */
+enum { BATCHCODE_COPIES = 3, BATCHCODE_ROUNDS = 4, BATCHCODE_MAX_K = 4096 };
+
+/* The SplitMix64 finalizer */
+DPF_HD uint64_t batchcode_mix(uint64_t z)
+{
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    return z ^ (z >> 31);
+}
+
+struct BatchCodeLayout {
+    uint64_t n;               /* rows of the table, [1, 2^31] */
+    uint64_t seed;            /* the public layout seed */
+    uint32_t nbins;           /* B, [1, min(n, 2^20)] */
+    int half;                 /* h: the Feistel network is over 2h >= max(2, ceil(log2 n)) bits */
+
+    /* One pass of the balanced Feistel network of copy c over [0, 2^2h): x = (L, R) of h bits each, and each round
+     * maps (L, R) to (R, L ^ F(round, R)) with F(i, R) = mix(seed ^ mix((c * 8 + i) << 32 | R)) mod 2^h. */
+    DPF_HD uint64_t feistel(int copy, uint64_t x) const
+    {
+        const uint64_t mask = ((uint64_t)1 << half) - 1;
+        uint64_t l = x >> half, r = x & mask;
+        for (int round = 0; round < BATCHCODE_ROUNDS; round++) {
+            const uint64_t f = batchcode_mix(seed ^ batchcode_mix((uint64_t)(copy * 8 + round) << 32 | r)) & mask;
+            const uint64_t t = l ^ f;
+            l = r;
+            r = t;
+        }
+        return l << half | r;
+    }
+    /* pi_c(r): the Feistel network applied until the value is below n (cycle walking), a permutation of [0, n) */
+    DPF_HD uint64_t perm(int copy, uint64_t r) const
+    {
+        uint64_t x = r;
+        do x = feistel(copy, x); while (x >= n);
+        return x;
+    }
+    /* m_j: the x in [0, n) with x mod B = j.  Bin j holds 3 m_j rows. */
+    DPF_HD uint64_t per_copy(uint32_t j) const { return (n - j + nbins - 1) / nbins; }
+    DPF_HD uint32_t bin_of(int copy, uint64_t r) const { return (uint32_t)(perm(copy, r) % nbins); }
+    /* copy c of row r: bin x mod B, row c m_j + x / B of that bin, for x = pi_c(r) */
+    DPF_HD void locate(int copy, uint64_t r, uint32_t *bin, uint64_t *row) const
+    {
+        const uint64_t x = perm(copy, r);
+        *bin = (uint32_t)(x % nbins);
+        *row = (uint64_t)copy * per_copy(*bin) + x / nbins;
+    }
+};
+
+/*
+ * The plan of one query of k wanted rows (b200dpf_batchcode_plan): Kuhn's augmenting paths over the wanted rows in
+ * order, trying copies 0, 1, 2 in order, a row that repeats a placed earlier row sharing its bin.  Rows outside
+ * [0, n) are not placed.  It runs in the caller's outputs: while the matching is built, state[v] (v < nbins) holds
+ * the wanted row matched to bin v plus one (bits 0..15, 0 for none), that row's copy (bits 16..17) and the root of
+ * the last search that visited v plus one (bits 32..47); slots[u] holds the row and copy (plus one, and in bits
+ * 16..17) a search came from to reach row u.  At the end state becomes the alphas (bin v's in-bin row to query, 0
+ * for a bin no row uses) and slots the bin answering each wanted row, or -1.  The host and the device run this same
+ * code, so their plans agree bit for bit.
+ */
+DPF_HD void batchcode_plan_query(const BatchCodeLayout &L, const int64_t *wanted, int k, int64_t *state, int32_t *slots)
+{
+    const int64_t n = (int64_t)L.n;
+    for (uint32_t v = 0; v < L.nbins; v++) state[v] = 0;
+    for (int i = 0; i < k; i++) {
+        const int64_t r = wanted[i];
+        if (r < 0 || r >= n) continue;
+        bool placed = false;        /* an earlier occurrence of r holds one of r's bins */
+        for (int c = 0; c < BATCHCODE_COPIES; c++) {
+            const int m = (int)(state[L.bin_of(c, (uint64_t)r)] & 0xffff);
+            placed |= m != 0 && wanted[m - 1] == r;
+        }
+        if (placed) continue;       /* (an earlier occurrence that was not placed fails again: no augmenting path appears) */
+        const int64_t stamp = (int64_t)(i + 1) << 32;
+        int u = i, c = 0;
+        for (;;) {
+            if (c == BATCHCODE_COPIES) {              /* row u has no way out: back to the row that reached it */
+                if (u == i) break;
+                const int32_t p = slots[u];
+                u = (p & 0xffff) - 1;
+                c = (p >> 16) + 1;
+                continue;
+            }
+            const uint32_t v = L.bin_of(c, (uint64_t)wanted[u]);
+            const int64_t s = state[v];
+            if ((s & ((int64_t)0xffff << 32)) == stamp) {
+                c++;
+                continue;
+            }
+            state[v] = (s & 0xffffffff) | stamp;
+            const int w = (int)(s & 0xffff) - 1;
+            if (w >= 0) {                              /* bin v is taken: try to move its row w */
+                slots[w] = (u + 1) | (c << 16);
+                u = w;
+                c = 0;
+                continue;
+            }
+            for (;;) {                                 /* an augmenting path: every row on it takes the bin it tried */
+                const uint32_t b = L.bin_of(c, (uint64_t)wanted[u]);
+                state[b] = (state[b] & ~(int64_t)0xffffffff) | (int64_t)((u + 1) | (c << 16));
+                if (u == i) break;
+                const int32_t p = slots[u];
+                u = (p & 0xffff) - 1;
+                c = p >> 16;
+            }
+            break;
+        }
+    }
+    for (int i = 0; i < k; i++) {
+        const int64_t r = wanted[i];
+        int32_t slot = -1;
+        for (int c = 0; r >= 0 && r < n && c < BATCHCODE_COPIES && slot < 0; c++) {
+            const uint32_t v = L.bin_of(c, (uint64_t)r);
+            const int m = (int)(state[v] & 0xffff);
+            if (m != 0 && wanted[m - 1] == r) slot = (int32_t)v;
+        }
+        slots[i] = slot;
+    }
+    for (uint32_t v = 0; v < L.nbins; v++) {
+        const int m = (int)(state[v] & 0xffff);
+        const int c = (int)((state[v] >> 16) & 3);
+        state[v] = m == 0 ? 0 : (int64_t)((uint64_t)c * L.per_copy(v) + L.perm(c, (uint64_t)wanted[m - 1]) / L.nbins);
+    }
+}
+
 /* One traversal phase of a launch: which subtrees the work items are, where an item starts and
  * which ticket counters hand the items out. */
 struct PhaseParams {
@@ -440,5 +567,15 @@ cudaError_t update_temp_bytes(int64_t count, int end_bit, size_t *bytes);
 /* map -> stable radix sort of (position, occurrence) -> one warp per surviving row; enqueued on
  * `stream`, no host synchronisation. */
 cudaError_t launch_update_rows(const UpdateParams &u, const UpdateWork &w, int end_bit, int sm_count, cudaStream_t stream);
+
+/* Batch-code contexts (dpf_batchcode.cu).
+ *   scatter: rows [first, first + count) of the table, src holding them [count][cols]: copy c of row r goes to device row
+ *            place[bin].first + in-bin row of L.locate(c, r), columns [0, cols) of a stride-int32 row.  One warp per row.
+ *   plan   : batchcode_plan_query for each of nq queries, one thread each: wanted [nq][k] -> alphas [nq][nbins], slots
+ *            [nq][k]. */
+cudaError_t launch_batchcode_scatter(const int32_t *src, uint64_t first, uint64_t count, const BatchCodeLayout &L,
+                                     const RowPlacement *place, int32_t *table, int cols, int stride, cudaStream_t stream);
+cudaError_t launch_batchcode_plan(const BatchCodeLayout &L, const int64_t *wanted, int64_t nq, int k, int64_t *alphas,
+                                  int32_t *slots, cudaStream_t stream);
 
 }  // namespace b200dpf

@@ -626,6 +626,130 @@ class BinnedDPF(DPF):
             len(self.bin_sizes), self.table_num_entries, self.table_effective_entry_size, self.prf_method_string)
 
 
+class BatchCodeDPF(BinnedDPF):
+    """Any k rows of one table per query (include/b200dpf.h, b200dpf_batchcode_create): the server stores every row in
+    3 of `nbins` bins, the client places its k rows in distinct bins (plan) and sends one key per bin, and the answers
+    of the bins that hold the wanted rows reconstruct them.  With nbins about 1.5 k, every row is placed with high
+    probability; a row that is not has slot -1 and found False.  Every kind of key (early_termination, xor).
+
+        d = BatchCodeDPF(DPF.PRF_AES128, 0, nbins=48)
+        d.eval_init(table)                                   # [n, entry_size]
+        qa, qb, slots = d.gen_queries(wanted)                # wanted [Q, k] rows; keys int32 [Q, nbins, 524]
+        rows, found = d.reconstruct(d.eval_queries_device(qa.cuda()), d.eval_queries_device(qb.cuda()), slots)
+
+    `seed` is the public layout seed (None: random).  gen_in_bin, eval_gpu and the other BinnedDPF evaluations work on
+    the bins as on a trimmed BinnedDPF."""
+
+    def __init__(self, prf=None, device=0, nbins=None, seed=None, early_termination=False, xor=False):
+        if nbins is None or int(nbins) < 1:
+            raise Exception("BatchCodeDPF needs nbins >= 1 (about 1.5 times the rows wanted per query)")
+        DPF.__init__(self, prf, device, early_termination=early_termination, xor=xor, trim=True)
+        self.nbins = int(nbins)
+        self.seed = int.from_bytes(os.urandom(8), "little") if seed is None else int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.n = None
+
+    def use_layout(self, n):
+        """Plan for a table of n rows without holding it: a client knows (n, nbins, seed), not the table.  eval_init
+        does this too."""
+        self.n = int(n)
+        self.bin_sizes = [3 * ((self.n - j + self.nbins - 1) // self.nbins) for j in range(self.nbins)]
+
+    def eval_init(self, table):
+        if self.buffers is not None:
+            dpf_cpp.eval_free(self.buffers)
+            self.buffers = None
+        table = torch.as_tensor(table)
+        if table.dim() != 2:
+            raise Exception("BatchCodeDPF.eval_init: table must be [n, entry_size]")
+        self.buffers = dpf_cpp.batchcode_init(table, self.nbins, self.seed, self.device, self.kind.id)
+        self.use_layout(table.shape[0])
+        self.table = None
+        self.table_num_entries = self.n
+        self.table_effective_entry_size = int(table.shape[1])
+
+    def _wanted(self, wanted, name):
+        if self.n is None:
+            raise Exception("BatchCodeDPF.%s: must call `eval_init` (or `use_layout`) first" % name)
+        w = torch.as_tensor(wanted)
+        if w.is_floating_point() or w.is_complex() or w.dtype == torch.bool or w.dim() not in (1, 2):
+            raise Exception("BatchCodeDPF.%s: wanted must be an integer tensor [Q, k] (or [k] for one query)" % name)
+        return w.reshape(1, -1) if w.dim() == 1 else w
+
+    def plan(self, wanted):
+        """The client's plan (b200dpf_batchcode_plan) of wanted rows [Q, k]: (alphas int64 [Q, nbins], the in-bin row
+        to query in each bin; slots int32 [Q, k], the bin that answers each wanted row, or -1)."""
+        w = self._wanted(wanted, "plan").to(torch.int64).cpu().contiguous()
+        return tuple(dpf_cpp.batchcode_plan(self.n, self.nbins, self.seed, w))
+
+    def gen_queries(self, wanted, seeds=None):
+        """The host client: both servers' queries for wanted rows [Q, k], as int32 [Q, nbins, 524] wire-format keys
+        (key g of query q for bin g, made by the kind's ChaCha20-DRBG keygen for trimmed_alpha(row, bin size)), and
+        the slots of plan.  seeds: 44 bytes per key, Q * nbins keys in query-major order (None: os.urandom)."""
+        alphas, slots = self.plan(wanted)
+        nq = alphas.shape[0]
+        if seeds is None:
+            seeds = os.urandom(44 * nq * self.nbins)
+        if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * nq * self.nbins:
+            raise Exception("BatchCodeDPF.gen_queries: seeds must be bytes, 44 per key (%d keys)" % (nq * self.nbins))
+        qa = torch.zeros((nq, self.nbins, 524), dtype=torch.int32)
+        qb = torch.zeros_like(qa)
+        for size in sorted(set(self.bin_sizes)):         # the bins of one size share a key domain
+            bins = [g for g in range(self.nbins) if self.bin_sizes[g] == size]
+            idx = torch.as_tensor([dpf_cpp.trimmed_alpha(int(alphas[q, g]), size, self.kind.id)
+                                   for q in range(nq) for g in bins], dtype=torch.int64)
+            sd = b"".join(seeds[44 * (q * self.nbins + g):44 * (q * self.nbins + g + 1)] for q in range(nq) for g in bins)
+            ka, kb = self.kind.gen_batch(idx, dpf_cpp.trimmed_domain(size, self.kind.id), sd, self.prf_method, 0)
+            qa[:, bins] = ka.reshape(nq, len(bins), 524)
+            qb[:, bins] = kb.reshape(nq, len(bins), 524)
+        return qa, qb, slots
+
+    def gen_queries_device(self, wanted_dev, seeds_dev=None, compact=True):
+        """The device client for load generators: the plan of wanted_dev (an int64 [Q, k] CUDA tensor) on the GPU
+        (b200dpf_batchcode_plan_device), then the keys on the GPU (BinnedDPF.gen_queries_device) from its alphas,
+        all enqueued on the current torch stream.  Returns (qa, qb, slots): the two servers' queries in the format of
+        `compact` and the slots int32 [Q, k] CUDA tensor, bit for bit those of plan."""
+        name = "BatchCodeDPF.gen_queries_device"
+        if self.buffers is None:
+            raise Exception("%s: must call `eval_init` first" % name)
+        if not (isinstance(wanted_dev, torch.Tensor) and wanted_dev.is_cuda and wanted_dev.dtype == torch.int64
+                and wanted_dev.is_contiguous() and wanted_dev.dim() == 2 and wanted_dev.device.index == self.device):
+            raise Exception("%s: wanted_dev must be a contiguous int64 [Q, k] tensor on cuda:%d" % (name, self.device))
+        nq, k = wanted_dev.shape
+        alphas = torch.empty((nq, self.nbins), dtype=torch.int64, device=wanted_dev.device)
+        slots = torch.empty((nq, k), dtype=torch.int32, device=wanted_dev.device)
+        stream = torch.cuda.current_stream(wanted_dev.device).cuda_stream
+        dpf_cpp.batchcode_plan_device(wanted_dev.data_ptr(), nq, k, self.buffers, alphas.data_ptr(), slots.data_ptr(), stream)
+        qa, qb = BinnedDPF.gen_queries_device(self, alphas, seeds_dev, compact)
+        return qa, qb, slots
+
+    def reconstruct(self, out_a, out_b, slots):
+        """The wanted rows from both servers' answers (int32 [Q, nbins, entry_size], as eval_queries_device returns
+        them) and the plan's slots [Q, k]: (rows int32 [Q, k, entry_size], found bool [Q, k]).  A row is a - b mod 2^32
+        (XOR-shared keys: a ^ b) of its bin's answers; an unplaced row is zero and not found."""
+        slots = torch.as_tensor(slots).to(device=out_a.device, dtype=torch.int64)
+        if out_a.dim() != 3 or out_a.shape != out_b.shape or slots.dim() != 2 or slots.shape[0] != out_a.shape[0]:
+            raise Exception("BatchCodeDPF.reconstruct: answers must be [Q, nbins, entry_size] and slots [Q, k]")
+        found = slots >= 0
+        idx = slots.clamp(min=0).unsqueeze(-1).expand(-1, -1, out_a.shape[2])
+        a, b = torch.gather(out_a, 1, idx), torch.gather(out_b, 1, idx)
+        rows = a ^ b if self.xor else a - b          # int32 wraps: the difference mod 2^32
+        return rows * found.unsqueeze(-1).to(rows.dtype), found
+
+    def update_rows(self, indices, rows):
+        """Replace table rows in all three copies: row indices[j] := rows[j] (last occurrence wins); synchronous.  An
+        index out of range raises, and nothing is applied."""
+        if self.buffers is None:
+            raise Exception("Must call `eval_init` before `update_rows`")
+        idx, rows = _update_args(indices, rows, self.table_effective_entry_size)
+        dpf_cpp.batchcode_update_rows(idx.to(torch.int64).cpu().contiguous(), rows.to(torch.int32).cpu().contiguous(), self.buffers)
+
+    def __repr__(self):
+        if self.buffers is None:
+            return "BatchCodeDPF(_uninitialized_, nbins=%d, prf_method=%s)" % (self.nbins, self.prf_method_string)
+        return "BatchCodeDPF(entries=%d, nbins=%d, entry_size=%d, prf_method=%s)" % (
+            self.n, self.nbins, self.table_effective_entry_size, self.prf_method_string)
+
+
 def _next_pow2(n):
     return 1 << max(1, (n - 1).bit_length())
 

@@ -413,7 +413,8 @@ int b200dpf_update_rows_device(b200dpf_ctx *ctx, const int64_t *indices_dev, con
                                void *cuda_stream);
 
 /* Grouped (batch-PIR) context: row indices[j] of bin bins[j] := rows[j].  Host buffers, synchronous.  A
- * bin id outside [0, nbins) or an index >= n[bin] is EINVAL, and nothing is applied. */
+ * bin id outside [0, nbins) or an index >= n[bin] is EINVAL, and nothing is applied.  ESTATE on a batch-code
+ * context (b200dpf_batchcode_create), whose rows change in all three copies at once (b200dpf_batchcode_update_rows). */
 int b200dpf_group_update_rows(b200dpf_ctx *ctx, const int32_t *bins, const int64_t *indices, const int32_t *rows,
                               int64_t count);
 
@@ -712,6 +713,85 @@ int b200dpf_group_create_trimmed(b200dpf_ctx **ctx, const int32_t *const *tables
 
 /* 1 on a trimmed context, 0 on any other, -1 for null. */
 int b200dpf_ctx_trimmed(const b200dpf_ctx *ctx);
+
+/* ------------------------------------------------------------------------------------------- */
+/* Batch codes: any k rows of one table per query (DESIGN.md section 13).                       */
+/* ------------------------------------------------------------------------------------------- */
+/*
+ * A probabilistic batch code (Angel et al., "PIR with compressed queries and amortized query processing", 2018): the
+ * server stores every row of an n-row table in 3 of nbins bins; a client that wants k rows assigns them to distinct
+ * bins (a bipartite matching) and sends one key per bin.  With nbins about 1.5 k every row is placed with high
+ * probability, and the server's work is 3n rows per query instead of k n for k separate queries.
+ *
+ * Layout.  Parameters: n rows (1 <= n <= 2^31), nbins = B (1 <= B <= min(n, 2^20)) and a public 64-bit layout_seed.
+ *   mix(z)       the SplitMix64 finalizer on 64-bit words: z ^= z >> 30; z *= 0xbf58476d1ce4e5b9; z ^= z >> 27;
+ *                z *= 0x94d049bb133111eb; z ^= z >> 31.
+ *   h            the smallest h >= 1 with 2^(2h) >= n (so 2h >= max(2, ceil(log2 n))).
+ *   F_c(x)       copy c's balanced Feistel network over 2h bits: L = x >> h, R = x mod 2^h; for rounds i = 0, 1, 2, 3:
+ *                (L, R) := (R, L ^ (mix(layout_seed ^ mix(((c * 8 + i) << 32) | R)) mod 2^h)); then x = (L << h) | R.
+ *   pi_c(r)      x = F_c(r), repeated (x = F_c(x)) until x < n: cycle walking makes pi_c a permutation of [0, n).
+ *   m_j          ceil((n - j) / B), the x in [0, n) with x mod B = j.
+ *   copy c of r  (c = 0, 1, 2) with x = pi_c(r): bin j = x mod B, row c * m_j + floor(x / B) of that bin.
+ * Bin j holds exactly 3 m_j rows, every one a copy of a table row; 3 m_0 (the largest) must be <= 2^31.  The bins are
+ * those of a trimmed grouped context (b200dpf_group_create_trimmed), so a client reaches row t of bin j with the key of
+ * its kind for (b200dpf_trimmed_alpha(t, 3 m_j, kind), b200dpf_trimmed_domain(3 m_j, kind)).  A client locates a row's
+ * copies from (n, B, layout_seed) alone.
+ *
+ * Privacy.  Every query carries exactly one key for every bin, whichever rows it wants; a bin no wanted row uses gets a
+ * key for its row 0, which its key hides like any other row.  The layout and its seed are public and depend on no
+ * query.  The plan -- which wanted row went to which bin, and which rows could not be placed -- stays with the client:
+ * the server sees keys only.
+ */
+
+/* A batch-code context of `kind` (B200DPF_KIND_*) on `device`: a trimmed grouped context with the nbins bins of the
+ * layout above, of 3 m_j rows each.  table: int32 [n][entry_size], host or device memory; entry_size as b200dpf_create.
+ * The bins are written into the context's device table by a scatter kernel, one table row to its three copies; a host
+ * table goes up in chunks of at most 64 MiB, and no other copy of the replicated table is made.  b200dpf_group_eval,
+ * _group_eval_device, _group_eval_device_bins, _group_eval_queries_device, _group_gen_queries_device, _group_query_bytes,
+ * the option setters, timing and introspection work on it as on any trimmed grouped context of the kind.
+ * b200dpf_group_update_rows returns ESTATE on it (one copy of a row cannot change alone): use
+ * b200dpf_batchcode_update_rows.  EINVAL for n, nbins or a bin size out of range, as above. */
+int b200dpf_batchcode_create(b200dpf_ctx **ctx, const int32_t *table, int64_t n, int entry_size, int nbins,
+                             uint64_t layout_seed, int device, int kind);
+
+/* The public parameters of a batch-code context, which a client needs: n, nbins and layout_seed.  ESTATE on any other
+ * context. */
+int b200dpf_batchcode_layout(const b200dpf_ctx *ctx, int64_t *n, int *nbins, uint64_t *layout_seed);
+
+/* Host only, no context: bins3[c] and rows3[c] receive the bin and the in-bin row of copy c = 0, 1, 2 of `row`.  EINVAL
+ * for a layout out of range or a row outside [0, n). */
+int b200dpf_batchcode_locate(int64_t n, int nbins, uint64_t layout_seed, int64_t row, int32_t *bins3, int64_t *rows3);
+
+/*
+ * The client's plan of nqueries queries of k wanted rows each, in host memory.
+ *   wanted: int64 [nqueries][k], rows in [0, n) (any other is EINVAL before anything is written).
+ *   alphas: int64 [nqueries][nbins] receives the in-bin row to query in each bin (0 in a bin no wanted row uses).
+ *   slots:  int32 [nqueries][k] receives the bin whose answer is wanted row i, or -1 when it could not be placed.
+ * Per query, a maximum matching of the wanted rows to distinct bins: Kuhn's augmenting paths, started from the wanted
+ * rows in order, a search from row u trying its copies 0, 1, 2 in order (depth first, each bin visited at most once
+ * per search, a taken bin tried by moving its row along its own copies).  A row that repeats an earlier wanted row of
+ * the same query shares that row's slot (and is -1 with it).  Deterministic: the same arguments give the same bytes.
+ * Limits: 1 <= k <= 4096, 1 <= nqueries, nqueries * nbins <= 2^24; the layout as for b200dpf_batchcode_create.
+ */
+int b200dpf_batchcode_plan(int64_t n, int nbins, uint64_t layout_seed, const int64_t *wanted, int64_t nqueries, int k,
+                           int64_t *alphas, int32_t *slots);
+
+/* The same plan on the context's GPU for load generators, one thread per query, in device buffers (wanted_dev and
+ * alphas_dev 8-byte aligned, slots_dev 4-byte aligned): alphas_dev and slots_dev are bit for bit what
+ * b200dpf_batchcode_plan writes, except that a wanted row outside [0, n) gets slot -1 instead of failing the call.  The
+ * matching is built in alphas_dev and slots_dev themselves, so no scratch grows with nqueries.  alphas_dev feeds
+ * b200dpf_group_gen_queries_device unchanged.  Enqueued on cuda_stream with no host wait; it writes only the caller's
+ * buffers and, like b200dpf_group_gen_queries_device, does not join the context's one-operation-in-flight chain.
+ * ESTATE on a context that is not a batch code; EINVAL for the limits of b200dpf_batchcode_plan, a null or misaligned
+ * buffer. */
+int b200dpf_batchcode_plan_device(b200dpf_ctx *ctx, const int64_t *wanted_dev, int64_t nqueries, int k, int64_t *alphas_dev,
+                                  int32_t *slots_dev, void *cuda_stream);
+
+/* Row updates of a batch-code context: table row indices[j] := rows[j] in all three copies, the last occurrence of a row
+ * winning.  Host buffers, synchronous, ordered against evaluations as b200dpf_group_update_rows is (it takes the same
+ * path, three entries per row).  An index outside [0, n), a negative count or more than (2^31 - 1) / 3 rows is EINVAL
+ * before anything is applied; ESTATE on any other context. */
+int b200dpf_batchcode_update_rows(b200dpf_ctx *ctx, const int64_t *indices, const int32_t *rows, int64_t count);
 
 /* Rows of the context's device table, padding included (on a grouped context all bins together; on a
  * multi-device context one device's); -1 for null.  A context that is not trimmed pads nothing: n (a
