@@ -37,6 +37,8 @@ SYMBOLS = [
     "b200dpf_group_eval_device_bins", "b200dpf_group_plan_lists",
     "b200dpf_batchcode_create", "b200dpf_batchcode_layout", "b200dpf_batchcode_locate", "b200dpf_batchcode_plan",
     "b200dpf_batchcode_plan_device", "b200dpf_batchcode_update_rows",
+    "b200dpf_kwpir_create", "b200dpf_kwpir_layout", "b200dpf_kwpir_build_stats", "b200dpf_kwpir_locate",
+    "b200dpf_kwpir_plan_device", "b200dpf_kwpir_update", "b200dpf_kwpir_tags",
 ]
 
 # The kinds of key, by the suffix of their entry points: log2 table rows per leaf, maximum depth, name.  A key
@@ -52,6 +54,7 @@ KIND_IDS = {"": 0, "_et": 1, "_xor": 2}
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
 _i64p = np.ctypeslib.ndpointer(dtype=np.int64, flags="C_CONTIGUOUS")
 _u32p = np.ctypeslib.ndpointer(dtype=np.uint32, flags="C_CONTIGUOUS")
+_u64p = np.ctypeslib.ndpointer(dtype=np.uint64, flags="C_CONTIGUOUS")
 
 
 class B200DPFError(RuntimeError):
@@ -139,6 +142,15 @@ def load():
     L.b200dpf_batchcode_plan.argtypes = [C.c_int64, C.c_int, C.c_uint64, _i64p, C.c_int64, C.c_int, _i64p, _i32p]
     L.b200dpf_batchcode_plan_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b200dpf_batchcode_update_rows.argtypes = [C.c_void_p, _i64p, _i32p, C.c_int64]
+    L.b200dpf_kwpir_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_uint64,
+                                       C.c_int, C.c_int]
+    L.b200dpf_kwpir_layout.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_uint64),
+                                       C.POINTER(C.c_int)]
+    L.b200dpf_kwpir_build_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double)]
+    L.b200dpf_kwpir_locate.argtypes = [C.c_int64, C.c_uint64, _u64p, C.c_int64, _i64p]
+    L.b200dpf_kwpir_plan_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    L.b200dpf_kwpir_update.argtypes = [C.c_void_p, _u64p, _i32p, C.c_int64]
+    L.b200dpf_kwpir_tags.argtypes = [C.c_void_p, _u64p]
     return L
 
 
@@ -708,3 +720,74 @@ class BatchCodeContext(GroupContext):
         indices = np.ascontiguousarray(indices, np.int64).reshape(-1)
         rows = np.ascontiguousarray(rows, np.int32).reshape(len(indices), self.entry_size)
         _check(lib().b200dpf_batchcode_update_rows(self.handle, indices, rows, len(indices)), "b200dpf_batchcode_update_rows")
+
+
+def kwpir_locate(m, seed, keywords):
+    """the in-bin rows int64 [Q, 3] to query for keywords [Q] in the keyword-PIR layout (m, seed): row c of keyword j is
+    h_c(keywords[j]) (b200dpf_kwpir_locate); host only"""
+    keywords = np.ascontiguousarray(keywords, np.uint64).reshape(-1)
+    rows = np.zeros((len(keywords), 3), np.int64)
+    _check(lib().b200dpf_kwpir_locate(int(m), int(seed) & 0xFFFFFFFFFFFFFFFF, keywords, len(keywords), rows), "b200dpf_kwpir_locate")
+    return rows
+
+
+class KeywordContext(GroupContext):
+    """(keyword, value) items in a cuckoo hash table of three trimmed bins of m slots (b200dpf_kwpir_create): a query of
+    one key per bin, for the keyword's rows kwpir_locate gives, returns the value with its tag.  keywords: uint64 [n],
+    values: int32 [n, value_size]; bins of value_size + 2 columns.  The kinds as for GroupContext; every GroupContext
+    evaluation works on it.  Values change through update.  Raises B200DPFError "... failed (-5)" (EFULL) when the
+    placement does not finish with this seed (dpf.KeywordDPF retries further seeds)."""
+
+    def __init__(self, keywords, values, m, seed, device=0, early_termination=False, xor=False):
+        if xor and early_termination:
+            raise ValueError("a context takes one kind of key: pass xor=True or early_termination=True, not both")
+        keywords = np.ascontiguousarray(keywords, np.uint64).reshape(-1)
+        values = np.ascontiguousarray(values, np.int32)
+        if values.ndim != 2 or values.shape[0] != len(keywords):
+            raise ValueError("KeywordContext: values must be [n, value_size] with one row per keyword, got shape %s" % (values.shape,))
+        self.n, self.value_size = values.shape
+        self.entry_size = self.value_size + 2
+        self.kind = "_xor" if xor else "_et" if early_termination else ""
+        self._trimmed = True
+        self.handle = C.c_void_p()
+        _check(lib().b200dpf_kwpir_create(C.byref(self.handle), keywords.ctypes.data_as(C.c_void_p), values.ctypes.data_as(C.c_void_p),
+                                          self.n, self.value_size, int(m), int(seed) & 0xFFFFFFFFFFFFFFFF, device, KIND_IDS[self.kind]),
+               "b200dpf_kwpir_create")
+
+    @property
+    def layout(self):
+        """(n, m, seed, value_size): the public parameters a client locates with (b200dpf_kwpir_layout)"""
+        n, m, seed, e = C.c_int64(), C.c_int64(), C.c_uint64(), C.c_int()
+        _check(lib().b200dpf_kwpir_layout(self.handle, C.byref(n), C.byref(m), C.byref(seed), C.byref(e)), "b200dpf_kwpir_layout")
+        return n.value, m.value, seed.value, e.value
+
+    @property
+    def build_stats(self):
+        """(rounds, ms): the rounds the placement took and their device time (b200dpf_kwpir_build_stats)"""
+        rounds, ms = C.c_int(), C.c_double()
+        _check(lib().b200dpf_kwpir_build_stats(self.handle, C.byref(rounds), C.byref(ms)), "b200dpf_kwpir_build_stats")
+        return rounds.value, ms.value
+
+    @property
+    def bin_rows(self):
+        """the rows of each bin: m"""
+        return [self.layout[1]] * 3
+
+    def tags(self):
+        """uint64 [3, m]: the tag stored in every slot, keyword + 1 or 0 for an empty slot (b200dpf_kwpir_tags)"""
+        out = np.zeros((3, self.layout[1]), np.uint64)
+        _check(lib().b200dpf_kwpir_tags(self.handle, out), "b200dpf_kwpir_tags")
+        return out
+
+    def plan_device(self, keywords_ptr, nqueries, alphas_ptr, stream=0):
+        """kwpir_locate on the GPU from device buffers (keywords uint64 [nqueries] into alphas int64 [nqueries, 3]),
+        enqueued on `stream` with no host wait"""
+        _check(lib().b200dpf_kwpir_plan_device(self.handle, C.c_void_p(keywords_ptr), nqueries, C.c_void_p(alphas_ptr),
+                                               C.c_void_p(stream)), "b200dpf_kwpir_plan_device")
+
+    def update(self, keywords, values):
+        """the value of keywords[j] := values[j] (last occurrence wins); synchronous.  A keyword not in the table raises,
+        and nothing is applied."""
+        keywords = np.ascontiguousarray(keywords, np.uint64).reshape(-1)
+        values = np.ascontiguousarray(values, np.int32).reshape(len(keywords), self.value_size)
+        _check(lib().b200dpf_kwpir_update(self.handle, keywords, values, len(keywords)), "b200dpf_kwpir_update")

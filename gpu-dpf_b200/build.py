@@ -22,7 +22,7 @@ LIB = os.path.join(HERE, "libb200dpf.so")
 EXT = os.path.join(HERE, "dpf_cpp" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 
 LIB_SOURCES = ["dpf_kernels.cu", "dpf_capi.cu", "dpf_keygen.cu", "dpf_group_io.cu", "dpf_group_plan.cu", "dpf_batchcode.cu",
-               "dpf_host.cpp"]
+               "dpf_kwpir.cu", "dpf_host.cpp"]
 # this script is a dependency too: its flags (the target architecture among them) shape both binaries
 LIB_DEPS = LIB_SOURCES + ["dpf_core.cuh", "dpf_kernels.cuh", "dpf_host.h", os.path.join(INCLUDE, "b200dpf.h"),
                           os.path.abspath(__file__)]

@@ -488,6 +488,95 @@ void batchcode_update_rows(const at::Tensor &indices, const at::Tensor &rows, co
           "batchcode_update_rows");
 }
 
+/* keyword PIR (b200dpf_kwpir_*): keywords int64 [n] (the uint64 keywords' bits) and values [n, E], CPU or CUDA tensors.
+ * An empty buffer list when the placement does not finish (B200DPF_EFULL), so the caller can retry another seed; any
+ * other failure raises. */
+std::vector<void *> kwpir_init(const at::Tensor &keywords, const at::Tensor &values, int64_t m, uint64_t seed, int device, int kind)
+{
+    TORCH_CHECK(keywords.dim() == 1 && keywords.scalar_type() == at::kLong, "kwpir_init: keywords must be an int64 tensor [n]");
+    TORCH_CHECK(values.dim() == 2 && values.size(0) == keywords.size(0), "kwpir_init: values must be [n, value_size]");
+    at::Tensor k = keywords.contiguous();
+    at::Tensor v = values.to(at::kInt).contiguous();
+    b200dpf_ctx *ctx = nullptr;
+    int rc;
+    {
+        py::gil_scoped_release nogil;
+        rc = b200dpf_kwpir_create(&ctx, reinterpret_cast<const uint64_t *>(k.data_ptr<int64_t>()), v.data_ptr<int32_t>(), k.size(0),
+                                  (int)v.size(1), m, seed, device, kind);
+    }
+    if (rc == B200DPF_EFULL) return {};
+    check(rc, "kwpir_init");
+    return {static_cast<void *>(ctx)};
+}
+
+/* (n, m, layout seed, value size) of a keyword-PIR context */
+py::tuple kwpir_layout(const std::vector<void *> &buffers)
+{
+    int64_t n = 0, m = 0;
+    uint64_t seed = 0;
+    int value_size = 0;
+    check(b200dpf_kwpir_layout(ctx_of(buffers), &n, &m, &seed, &value_size), "kwpir_layout");
+    return py::make_tuple(n, m, seed, value_size);
+}
+
+/* (rounds, placement device ms) of a keyword-PIR context's build */
+py::tuple kwpir_build_stats(const std::vector<void *> &buffers)
+{
+    int rounds = 0;
+    double ms = 0;
+    check(b200dpf_kwpir_build_stats(ctx_of(buffers), &rounds, &ms), "kwpir_build_stats");
+    return py::make_tuple(rounds, ms);
+}
+
+/* the host locator: keywords int64 [Q] CPU tensor -> rows int64 [Q, 3] */
+at::Tensor kwpir_locate(int64_t m, uint64_t seed, const at::Tensor &keywords)
+{
+    TORCH_CHECK(keywords.device().is_cpu() && keywords.scalar_type() == at::kLong && keywords.dim() == 1 && keywords.is_contiguous(),
+                "kwpir_locate: keywords must be a contiguous CPU int64 tensor [Q]");
+    at::Tensor rows = torch::empty({keywords.size(0), 3}, at::kLong);
+    check(b200dpf_kwpir_locate(m, seed, reinterpret_cast<const uint64_t *>(keywords.data_ptr<int64_t>()), keywords.size(0),
+                               rows.data_ptr<int64_t>()),
+          "kwpir_locate");
+    return rows;
+}
+
+/* the device locator (b200dpf_kwpir_plan_device): keywords [nqueries] at keywords_ptr into alphas int64 [nqueries, 3] at
+ * alphas_ptr, enqueued on the stream handle passed as an integer */
+void kwpir_plan_device(int64_t keywords_ptr, int64_t nqueries, const std::vector<void *> &buffers, int64_t alphas_ptr, int64_t stream)
+{
+    check(b200dpf_kwpir_plan_device(ctx_of(buffers), reinterpret_cast<const uint64_t *>(keywords_ptr), nqueries,
+                                    reinterpret_cast<int64_t *>(alphas_ptr), reinterpret_cast<void *>(stream)),
+          "kwpir_plan_device");
+}
+
+/* the value of keywords[j] := values[j]; CPU tensors, synchronous */
+void kwpir_update(const at::Tensor &keywords, const at::Tensor &values, const std::vector<void *> &buffers)
+{
+    b200dpf_ctx *ctx = ctx_of(buffers);
+    TORCH_CHECK(keywords.device().is_cpu() && keywords.scalar_type() == at::kLong && keywords.dim() == 1 && keywords.is_contiguous(),
+                "kwpir_update: keywords must be a contiguous CPU int64 tensor [count]");
+    TORCH_CHECK(values.device().is_cpu() && values.scalar_type() == at::kInt && values.dim() == 2 && values.is_contiguous() &&
+                    values.size(0) == keywords.size(0) && values.size(1) == b200dpf_ctx_entry_size(ctx) - 2,
+                "kwpir_update: values must be a contiguous CPU int32 tensor [count, value_size]");
+    py::gil_scoped_release nogil;
+    check(b200dpf_kwpir_update(ctx, reinterpret_cast<const uint64_t *>(keywords.data_ptr<int64_t>()), values.data_ptr<int32_t>(),
+                               keywords.size(0)),
+          "kwpir_update");
+}
+
+/* every slot's stored tag, int64 [3, m] (the uint64 tags' bits; 0 = empty) */
+at::Tensor kwpir_tags(const std::vector<void *> &buffers)
+{
+    b200dpf_ctx *ctx = ctx_of(buffers);
+    int64_t n = 0, m = 0;
+    uint64_t seed = 0;
+    int value_size = 0;
+    check(b200dpf_kwpir_layout(ctx, &n, &m, &seed, &value_size), "kwpir_tags");
+    at::Tensor tags = torch::empty({3, m}, at::kLong);
+    check(b200dpf_kwpir_tags(ctx, reinterpret_cast<uint64_t *>(tags.data_ptr<int64_t>())), "kwpir_tags");
+    return tags;
+}
+
 /* "all" / "" -> every visible device; "0,2,3" -> that list */
 std::vector<int> parse_devices(const std::string &spec)
 {
@@ -744,6 +833,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
           py::arg("wanted_ptr"), py::arg("nqueries"), py::arg("k"), py::arg("buffers"), py::arg("alphas_ptr"),
           py::arg("slots_ptr"), py::arg("stream") = 0);
     m.def("batchcode_update_rows", &batchcode_update_rows, "batch code: table row indices[j] := rows[j] in all three copies");
+    m.def("kwpir_init", &kwpir_init, "keyword PIR: (keyword, value) items placed in 3 tables of m slots; [] if placement fails",
+          py::arg("keywords"), py::arg("values"), py::arg("m"), py::arg("seed"), py::arg("device") = 0, py::arg("kind") = 0);
+    m.def("kwpir_layout", &kwpir_layout, "(n, m, layout seed, value size) of a keyword-PIR context");
+    m.def("kwpir_build_stats", &kwpir_build_stats, "(rounds, placement device ms) of a keyword-PIR context's build");
+    m.def("kwpir_locate", &kwpir_locate, "the in-bin rows [Q, 3] of keywords [Q]", py::arg("m"), py::arg("seed"), py::arg("keywords"));
+    m.def("kwpir_plan_device", &kwpir_plan_device, "the in-bin rows on the GPU, from and into device buffers", py::arg("keywords_ptr"),
+          py::arg("nqueries"), py::arg("buffers"), py::arg("alphas_ptr"), py::arg("stream") = 0);
+    m.def("kwpir_update", &kwpir_update, "keyword PIR: the value of keywords[j] := values[j]");
+    m.def("kwpir_tags", &kwpir_tags, "every slot's stored tag [3, m] (keyword + 1, 0 = empty)");
     m.def("parse_devices", &parse_devices, "'all' or '0,1,2' -> device list");
     m.def("device_count", [](const std::vector<void *> &b) { return b200dpf_ctx_device_count(ctx_of(b)); });
     m.def("axis", [](const std::vector<void *> &b) { return b200dpf_ctx_axis(ctx_of(b)); });

@@ -185,6 +185,27 @@ DPF_HD void batchcode_plan_query(const BatchCodeLayout &L, const int64_t *wanted
     }
 }
 
+/* Keyword-PIR layout (b200dpf_kwpir_create, DESIGN.md section 14): n (keyword, value) items in a cuckoo hash table of
+ * three tables (bins) of m slots; an item sits in one of its three candidate slots, its row the value then the tag
+ * w + 1 in two columns.  Table creation, row updates and both locators place keywords through this one definition;
+ * include/b200dpf.h states it in full. */
+enum { KWPIR_TABLES = 3, KWPIR_MAX_ROUNDS = 1024, KWPIR_MAX_VALUE = 4094 };
+
+struct KeywordLayout {
+    uint64_t n;               /* items, [1, 2^30] */
+    uint64_t m;               /* slots per table, [ceil(n / 3), 2^31] */
+    uint64_t seed;            /* the public layout seed */
+    int value_size;           /* E: value columns; the tag is columns E and E + 1 */
+
+    /* h_c(w): keyword w's candidate row in table c, ((mix(mix(w ^ seed) ^ (c + 1) * golden) >> 32) * m) >> 32.
+     * The product is below 2^63 because m <= 2^31. */
+    DPF_HD uint64_t row(int c, uint64_t w) const
+    {
+        const uint64_t z = batchcode_mix(batchcode_mix(w ^ seed) ^ ((uint64_t)(c + 1) * 0x9E3779B97F4A7C15ull));
+        return ((z >> 32) * m) >> 32;
+    }
+};
+
 /* One traversal phase of a launch: which subtrees the work items are, where an item starts and
  * which ticket counters hand the items out. */
 struct PhaseParams {
@@ -577,5 +598,29 @@ cudaError_t launch_batchcode_scatter(const int32_t *src, uint64_t first, uint64_
                                      const RowPlacement *place, int32_t *table, int cols, int stride, cudaStream_t stream);
 cudaError_t launch_batchcode_plan(const BatchCodeLayout &L, const int64_t *wanted, int64_t nq, int k, int64_t *alphas,
                                   int32_t *slots, cudaStream_t stream);
+
+/* Keyword-PIR contexts (dpf_kwpir.cu); every launch is enqueued on `stream` with no host synchronisation.
+ *   check  : radix-sort keys [n] into sorted and set *flags to KWPIR_DUPLICATE and/or KWPIR_RESERVED when two keywords
+ *            are equal or one is 2^64 - 1; temp holds kwpir_check_temp_bytes(n) bytes.
+ *   round  : round `round` (>= 1) of the placement: the count items of homeless (null: items 0..count-1) bid for slot
+ *            choice[i] * m + h_choice[i](keys[i]) (bid words (round << 32) | ~i, atomicMax: the smallest index wins);
+ *            each winner takes its slot in owner, and each loser and evicted owner advances its choice and is
+ *            appended to next, counted in *next_count (zero before the launch).
+ *   scatter: items [first, first + count), values holding their rows [count][L.value_size]: item i's value and tag go
+ *            to device row place[choice[i]].first + h_choice[i](keys[i]) of a stride-int32 row.  One warp per item.
+ *   plan   : rows3[q][c] = h_c(keywords[q]) for nq queries, one thread each.
+ *   find   : bins[j], rows[j] = the table and row whose tag is keywords[j] + 1, or -1, -1; one thread per keyword. */
+enum { KWPIR_DUPLICATE = 1, KWPIR_RESERVED = 2 };
+cudaError_t kwpir_check_temp_bytes(uint64_t n, size_t *bytes);
+cudaError_t launch_kwpir_check(const uint64_t *keys, uint64_t n, uint64_t *sorted, void *temp, size_t temp_bytes, uint32_t *flags,
+                               cudaStream_t stream);
+cudaError_t launch_kwpir_round(const KeywordLayout &L, const uint64_t *keys, const uint32_t *homeless, uint32_t count,
+                               uint32_t round, uint8_t *choice, unsigned long long *bid, int32_t *owner, uint32_t *next,
+                               uint32_t *next_count, cudaStream_t stream);
+cudaError_t launch_kwpir_scatter(const int32_t *values, uint64_t first, uint64_t count, const uint64_t *keys, const uint8_t *choice,
+                                 const KeywordLayout &L, const RowPlacement *place, int32_t *table, int stride, cudaStream_t stream);
+cudaError_t launch_kwpir_plan(const KeywordLayout &L, const uint64_t *keywords, int64_t nq, int64_t *rows3, cudaStream_t stream);
+cudaError_t launch_kwpir_find(const KeywordLayout &L, const uint64_t *keywords, int64_t count, const RowPlacement *place,
+                              const int32_t *table, int stride, int32_t *bins, int64_t *rows, cudaStream_t stream);
 
 }  // namespace b200dpf

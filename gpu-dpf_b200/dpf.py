@@ -750,6 +750,151 @@ class BatchCodeDPF(BinnedDPF):
             self.n, self.nbins, self.table_effective_entry_size, self.prf_method_string)
 
 
+class KeywordDPF(BinnedDPF):
+    """A value by its 64-bit keyword in one query (include/b200dpf.h, b200dpf_kwpir_create): the server places each
+    (keyword, value) item in one of three cuckoo hash tables of m slots, the client sends one key per table for its
+    keyword's three candidate rows, and the answer whose stored keyword matches is the value; an absent keyword comes
+    back zero with found False.  Every kind of key (early_termination, xor).
+
+        d = KeywordDPF(DPF.PRF_AES128, 0)
+        d.eval_init(keywords, values)                        # uint64 [n], int32 [n, E]
+        qa, qb = d.gen_queries(query_keywords)               # keys int32 [Q, 3, 524]
+        vals, found = d.reconstruct(d.eval_queries_device(qa.cuda()), d.eval_queries_device(qb.cuda()), query_keywords)
+
+    m = ceil(expansion * n / 3) slots per table.  `seed` is the public layout seed (None: random); when a placement
+    does not finish, eval_init retries seed + 1, seed + 2, ... (TRIES seeds in all) and `seed` is the one it ended
+    with.  Keywords are uint64 (numpy arrays or Python ints) or int64 tensors holding their bits; keyword 2^64 - 1 is
+    reserved.  The bins have value_size + 2 columns (the tag), so eval_queries_device returns [Q, 3, value_size + 2]."""
+
+    TRIES = 8
+
+    def __init__(self, prf=None, device=0, seed=None, expansion=1.3, early_termination=False, xor=False):
+        if not expansion >= 1.0:
+            raise Exception("KeywordDPF needs expansion >= 1 (3m slots for n items; 1.3 by default)")
+        DPF.__init__(self, prf, device, early_termination=early_termination, xor=xor, trim=True)
+        self.seed = int.from_bytes(os.urandom(8), "little") if seed is None else int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.expansion = float(expansion)
+        self.n = self.m = self.value_size = None
+
+    def use_layout(self, n, m, seed):
+        """Locate keywords for a table of n items in 3 tables of m slots under `seed` without holding it: a client
+        knows (n, m, seed), not the items.  eval_init does this too."""
+        self.n, self.m, self.seed = int(n), int(m), int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.bin_sizes = [self.m] * 3
+
+    def eval_init(self, keywords, values):
+        if self.buffers is not None:
+            dpf_cpp.eval_free(self.buffers)
+            self.buffers = None
+        kw = _keyword_tensor(keywords, "KeywordDPF.eval_init")
+        values = torch.as_tensor(values)
+        if values.dim() != 2 or values.shape[0] != kw.shape[0]:
+            raise Exception("KeywordDPF.eval_init: values must be [n, value_size] with one row per keyword")
+        n = int(kw.shape[0])
+        m = max(-(-n // 3), int(np.ceil(self.expansion * n / 3)))
+        for t in range(self.TRIES):
+            seed = (self.seed + t) & 0xFFFFFFFFFFFFFFFF
+            buffers = dpf_cpp.kwpir_init(kw, values, m, seed, self.device, self.kind.id)
+            if buffers:
+                break
+        else:
+            raise Exception("KeywordDPF.eval_init: the placement of %d items in 3 x %d slots did not finish for seeds %d..%d; "
+                            "use a larger expansion" % (n, m, self.seed, seed))
+        self.buffers = buffers
+        self.use_layout(n, m, seed)
+        self.value_size = int(values.shape[1])
+        self.table = None
+        self.table_num_entries = 3 * m
+        self.table_effective_entry_size = self.value_size + 2
+
+    def _need_layout(self, name):
+        if self.m is None:
+            raise Exception("KeywordDPF.%s: must call `eval_init` (or `use_layout`) first" % name)
+
+    def plan(self, keywords):
+        """The in-bin rows int64 [Q, 3] to query for keywords [Q] (b200dpf_kwpir_locate): row c is h_c(keyword)."""
+        self._need_layout("plan")
+        return dpf_cpp.kwpir_locate(self.m, self.seed, _keyword_tensor(keywords, "KeywordDPF.plan").cpu().contiguous())
+
+    def gen_queries(self, keywords, seeds=None):
+        """The host client: both servers' queries for keywords [Q], as int32 [Q, 3, 524] wire-format keys (key c of
+        query q for bin c, made by the kind's ChaCha20-DRBG keygen for trimmed_alpha(h_c(keyword), m)).  seeds: 44
+        bytes per key, 3Q keys in query-major order (None: os.urandom)."""
+        alphas = self.plan(keywords)
+        nq = alphas.shape[0]
+        if seeds is None:
+            seeds = os.urandom(44 * 3 * nq)
+        if not isinstance(seeds, (bytes, bytearray)) or len(seeds) != 44 * 3 * nq:
+            raise Exception("KeywordDPF.gen_queries: seeds must be bytes, 44 per key (%d keys)" % (3 * nq))
+        idx = torch.as_tensor([dpf_cpp.trimmed_alpha(int(a), self.m, self.kind.id) for a in alphas.reshape(-1).tolist()],
+                              dtype=torch.int64)
+        ka, kb = self.kind.gen_batch(idx, dpf_cpp.trimmed_domain(self.m, self.kind.id), bytes(seeds), self.prf_method, 0)
+        return ka.reshape(nq, 3, 524), kb.reshape(nq, 3, 524)
+
+    def gen_queries_device(self, keywords_dev, seeds_dev=None, compact=True):
+        """The device client for load generators: the rows of keywords_dev (an int64 [Q] CUDA tensor of the keywords'
+        bits) on the GPU (b200dpf_kwpir_plan_device), then the keys on the GPU (BinnedDPF.gen_queries_device), all
+        enqueued on the current torch stream.  Returns (qa, qb), the two servers' queries in the format of `compact`."""
+        name = "KeywordDPF.gen_queries_device"
+        if self.buffers is None:
+            raise Exception("%s: must call `eval_init` first" % name)
+        if not (isinstance(keywords_dev, torch.Tensor) and keywords_dev.is_cuda and keywords_dev.dtype in (torch.int64, torch.uint64)
+                and keywords_dev.is_contiguous() and keywords_dev.dim() == 1 and keywords_dev.device.index == self.device):
+            raise Exception("%s: keywords_dev must be a contiguous int64 [Q] tensor on cuda:%d" % (name, self.device))
+        nq = keywords_dev.shape[0]
+        alphas = torch.empty((nq, 3), dtype=torch.int64, device=keywords_dev.device)
+        stream = torch.cuda.current_stream(keywords_dev.device).cuda_stream
+        dpf_cpp.kwpir_plan_device(keywords_dev.data_ptr(), nq, self.buffers, alphas.data_ptr(), stream)
+        return BinnedDPF.gen_queries_device(self, alphas, seeds_dev, compact)
+
+    def reconstruct(self, out_a, out_b, keywords):
+        """The values of keywords [Q] from both servers' answers (int32 [Q, 3, value_size + 2], as eval_queries_device
+        returns them): (values int32 [Q, value_size], found bool [Q]).  A bin's row is a - b mod 2^32 (XOR-shared keys:
+        a ^ b); the value is that of the bin whose tag is keyword + 1, and zero with found False when none is."""
+        self._need_layout("reconstruct")
+        e = self.value_size if self.value_size is not None else out_a.shape[-1] - 2
+        kw = _keyword_tensor(keywords, "KeywordDPF.reconstruct").to(out_a.device)
+        if out_a.dim() != 3 or out_a.shape != out_b.shape or tuple(out_a.shape[1:]) != (3, e + 2) or kw.shape[0] != out_a.shape[0]:
+            raise Exception("KeywordDPF.reconstruct: answers must be [Q, 3, %d] and keywords [Q]" % (e + 2))
+        rows = out_a ^ out_b if self.xor else out_a - out_b          # int32 wraps: the difference mod 2^32
+        tag = kw.unsqueeze(1) + 1                                     # int64 wraps: keyword 2^64 - 1 has tag 0, never found
+        lo = rows[..., e].to(torch.int64) & 0xFFFFFFFF
+        hi = rows[..., e + 1].to(torch.int64) & 0xFFFFFFFF
+        match = (lo == (tag & 0xFFFFFFFF)) & (hi == ((tag >> 32) & 0xFFFFFFFF)) & (tag != 0)
+        values = torch.where(match.unsqueeze(-1), rows[..., :e], 0).sum(dim=1).to(torch.int32)
+        return values, match.any(dim=1)
+
+    def update(self, keywords, values):
+        """Replace the values of present keywords: the value of keywords[j] := values[j] (last occurrence wins);
+        synchronous.  A keyword that is not in the table raises, and nothing is applied."""
+        if self.buffers is None:
+            raise Exception("Must call `eval_init` before `update`")
+        kw = _keyword_tensor(keywords, "KeywordDPF.update")
+        values = torch.as_tensor(values)
+        if values.dim() != 2 or values.shape[0] != kw.shape[0] or values.shape[1] != self.value_size:
+            raise Exception("KeywordDPF.update: values must be [%d, %d] (one value per keyword)" % (kw.shape[0], self.value_size))
+        dpf_cpp.kwpir_update(kw.cpu().contiguous(), values.to(torch.int32).cpu().contiguous(), self.buffers)
+
+    def __repr__(self):
+        if self.buffers is None:
+            return "KeywordDPF(_uninitialized_, prf_method=%s)" % self.prf_method_string
+        return "KeywordDPF(items=%d, m=%d, value_size=%d, prf_method=%s)" % (self.n, self.m, self.value_size, self.prf_method_string)
+
+
+def _keyword_tensor(keywords, name):
+    """keywords as a 1-D int64 tensor holding the uint64 keywords' bits (a tensor stays on its device)"""
+    if isinstance(keywords, torch.Tensor):
+        if keywords.dim() != 1 or keywords.is_floating_point() or keywords.is_complex() or keywords.dtype == torch.bool:
+            raise Exception("%s: keywords must be a 1-D integer tensor or array of uint64 keywords" % name)
+        return keywords.view(torch.int64) if keywords.dtype == torch.uint64 else keywords.to(torch.int64)
+    a = keywords if isinstance(keywords, np.ndarray) else np.asarray(keywords, dtype=object)   # Python ints stay exact
+    if a.dtype == object and a.ndim == 1 and all(isinstance(x, (int, np.integer)) for x in a):
+        a = np.array([int(x) & 0xFFFFFFFFFFFFFFFF for x in a], np.uint64)
+    if a.ndim != 1 or a.dtype.kind not in "iu":
+        raise Exception("%s: keywords must be a 1-D integer tensor or array of uint64 keywords" % name)
+    return torch.from_numpy(np.ascontiguousarray(a.astype(np.uint64).view(np.int64)))
+
+
 def _next_pow2(n):
     return 1 << max(1, (n - 1).bit_length())
 

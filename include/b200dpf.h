@@ -64,7 +64,8 @@ enum {
     B200DPF_EINVAL = -1,   /* bad argument (shape, power of two, prf id, ...)   */
     B200DPF_ECUDA = -2,    /* CUDA runtime error or no usable device            */
     B200DPF_ENOMEM = -3,
-    B200DPF_ESTATE = -4    /* call out of order (e.g. eval before table upload) */
+    B200DPF_ESTATE = -4,   /* call out of order (e.g. eval before table upload) */
+    B200DPF_EFULL = -5     /* a keyword-PIR placement did not finish (b200dpf_kwpir_create) */
 };
 
 typedef struct b200dpf_ctx b200dpf_ctx;
@@ -414,7 +415,8 @@ int b200dpf_update_rows_device(b200dpf_ctx *ctx, const int64_t *indices_dev, con
 
 /* Grouped (batch-PIR) context: row indices[j] of bin bins[j] := rows[j].  Host buffers, synchronous.  A
  * bin id outside [0, nbins) or an index >= n[bin] is EINVAL, and nothing is applied.  ESTATE on a batch-code
- * context (b200dpf_batchcode_create), whose rows change in all three copies at once (b200dpf_batchcode_update_rows). */
+ * context (b200dpf_batchcode_create), whose rows change in all three copies at once (b200dpf_batchcode_update_rows),
+ * and on a keyword-PIR context (b200dpf_kwpir_create), whose tags must not change (b200dpf_kwpir_update). */
 int b200dpf_group_update_rows(b200dpf_ctx *ctx, const int32_t *bins, const int64_t *indices, const int32_t *rows,
                               int64_t count);
 
@@ -792,6 +794,85 @@ int b200dpf_batchcode_plan_device(b200dpf_ctx *ctx, const int64_t *wanted_dev, i
  * path, three entries per row).  An index outside [0, n), a negative count or more than (2^31 - 1) / 3 rows is EINVAL
  * before anything is applied; ESTATE on any other context. */
 int b200dpf_batchcode_update_rows(b200dpf_ctx *ctx, const int64_t *indices, const int32_t *rows, int64_t count);
+
+/* ------------------------------------------------------------------------------------------- */
+/* Keyword PIR: a value by its 64-bit keyword in one query (DESIGN.md section 14).              */
+/* ------------------------------------------------------------------------------------------- */
+/*
+ * A cuckoo hash table of n (keyword, value) items in three tables of m slots: the server places each item in one of
+ * its keyword's three candidate slots; a client computes the three slots from public parameters, sends one key per
+ * table, and keeps the answer whose stored keyword matches.  The server evaluates 3m rows per query.
+ *
+ * Layout.  Parameters: n items (1 <= n <= 2^30), m slots per table (ceil(n / 3) <= m <= 2^31), a public 64-bit
+ * layout_seed and E value columns (1 <= E <= 4094).  All arithmetic is mod 2^64.
+ *   mix(z)       the SplitMix64 finalizer of the batch-code layout above.
+ *   h_c(w)       for c = 0, 1, 2: ((mix(mix(w ^ layout_seed) ^ ((c + 1) * 0x9E3779B97F4A7C15)) >> 32) * m) >> 32, a row
+ *                in [0, m) (the product is below 2^63 because m <= 2^31).
+ *   context      a trimmed grouped context (b200dpf_group_create_trimmed) of 3 bins of m rows, entry size E + 2.
+ *   row format   item (w, value) sits in bin c at row h_c(w) for one c: columns [0, E) are value, column E the low and
+ *                column E + 1 the high 32 bits of the tag w + 1.  An empty slot is all zeros, so tag 0 means empty
+ *                and keyword 2^64 - 1 is refused.  The tag is the whole keyword: "found" is exact.
+ * Keywords wider than 64 bits must be hashed down by the caller; two that hash to the same 64 bits are one keyword.
+ * E = 14 keeps the context at 16 columns, the best-shaped evaluation; E = 16 makes 18 columns, which take the wide-entry
+ * path.
+ *
+ * Placement.  A pure function of the keywords in caller order, m and layout_seed: item i is its position in the
+ * caller's arrays; choice[i] in {0, 1, 2} starts at 0 and every item starts homeless.  Each round, every homeless item
+ * i bids for slot (choice[i], h_choice[i](w_i)); each slot bid on goes to its smallest bidding index, whose bid takes
+ * it; the slot's previous owner, if any, and every losing bidder advance choice by 1 mod 3 and are homeless in the next
+ * round.  The placement ends when no item is homeless.  A round's outcome depends only on the set of homeless items,
+ * so it does not depend on thread scheduling, device or stream.  After 1024 rounds with items still homeless the
+ * create fails with B200DPF_EFULL and creates nothing; another layout_seed or a larger m is the remedy (the Python
+ * layer retries layout_seed + 1, + 2, ..., 8 seeds in all).  DESIGN.md section 14 gives the rounds a build takes;
+ * m = ceil(1.3 n / 3), the Python default, stays far below the cap.
+ *
+ * Privacy.  Every query carries exactly one key for each of the three bins, whether or not its keyword is present.
+ * The layout and its seed are public and depend on no query.  The client learns the full rows of its three candidate
+ * slots, which may hold other keywords' items; like index PIR, this does not hide the database from the client.
+ */
+
+/* A keyword-PIR context of `kind` (B200DPF_KIND_*) on `device`, laid out as above.  keywords: uint64 [n], values: int32
+ * [n][value_size], each in host or device memory; keywords and values on the context's device are read in place, host
+ * values go up in chunks of at most 64 MiB.  Duplicate keywords and keyword 2^64 - 1 are EINVAL (found by a radix
+ * sort on the device, before placement).  The placement runs on the GPU, one bid and one resolve kernel per round;
+ * its O(n + m) scratch is freed before the call returns.  Synchronous.  B200DPF_EFULL when the placement does not
+ * finish (above).  b200dpf_group_eval, _group_eval_device, _group_eval_device_bins, _group_eval_queries_device,
+ * _group_gen_queries_device, _group_query_bytes, the option setters, timing and introspection work on it as on any
+ * trimmed grouped context of the kind; b200dpf_group_update_rows returns ESTATE on it (use b200dpf_kwpir_update). */
+int b200dpf_kwpir_create(b200dpf_ctx **ctx, const uint64_t *keywords, const int32_t *values, int64_t n, int value_size, int64_t m,
+                         uint64_t layout_seed, int device, int kind);
+
+/* The public parameters of a keyword-PIR context, which a client needs: n, m, layout_seed and value_size (E).  ESTATE
+ * on any other context. */
+int b200dpf_kwpir_layout(const b200dpf_ctx *ctx, int64_t *n, int64_t *m, uint64_t *layout_seed, int *value_size);
+
+/* The rounds the context's placement took, and their time on the device by CUDA events (the per-round host reads of
+ * the homeless count included, the duplicate check and the row scatter not).  ESTATE on any other context. */
+int b200dpf_kwpir_build_stats(const b200dpf_ctx *ctx, int *rounds, double *place_ms);
+
+/* Host only, no context: rows3[j][c] = h_c(keywords[j]), the in-bin row to query in bin c, for count keywords.
+ * EINVAL for m outside [1, 2^31], a negative count, a null buffer or keyword 2^64 - 1. */
+int b200dpf_kwpir_locate(int64_t m, uint64_t layout_seed, const uint64_t *keywords, int64_t count, int64_t *rows3);
+
+/* The same rows on the context's GPU for load generators, one thread per query: keywords_dev uint64 [nqueries] into
+ * alphas_dev int64 [nqueries][3] (both 8-byte aligned), which feeds b200dpf_group_gen_queries_device unchanged.
+ * Keyword 2^64 - 1 gets its rows like any other (it is never found).  Enqueued on cuda_stream with no host wait; it
+ * writes only the caller's buffers and does not join the context's one-operation-in-flight chain.  ESTATE on any other
+ * context; EINVAL for a null or misaligned buffer or nqueries outside [1, 2^24 / 3]. */
+int b200dpf_kwpir_plan_device(b200dpf_ctx *ctx, const uint64_t *keywords_dev, int64_t nqueries, int64_t *alphas_dev,
+                              void *cuda_stream);
+
+/* Value updates of a keyword-PIR context: the value of keywords[j] := values[j] (int32 [count][value_size]), the last
+ * occurrence of a keyword winning.  Host buffers, synchronous.  A kernel finds each keyword's slot from the tags of its
+ * three candidate rows; a keyword that is not in the table (or 2^64 - 1), a negative count or one of 2^31 or more is
+ * EINVAL before anything is applied.  The rows then take the path of b200dpf_group_update_rows, ordered against
+ * evaluations as it is.  Keywords cannot be inserted or deleted: that needs a new context.  ESTATE on any other
+ * context. */
+int b200dpf_kwpir_update(b200dpf_ctx *ctx, const uint64_t *keywords, const int32_t *values, int64_t count);
+
+/* Introspection: tags[c][r] (uint64 [3][m], host memory) receives the tag stored in row r of bin c, w + 1 for the item
+ * of keyword w placed there or 0 for an empty slot.  Synchronous.  ESTATE on any other context. */
+int b200dpf_kwpir_tags(const b200dpf_ctx *ctx, uint64_t *tags);
 
 /* Rows of the context's device table, padding included (on a grouped context all bins together; on a
  * multi-device context one device's); -1 for null.  A context that is not trimmed pads nothing: n (a
