@@ -1238,45 +1238,55 @@ int wait_source(const b200dpf_ctx *c, const void *src, bool *on_device, int *src
     return B200DPF_OK;
 }
 
-/* Fill the device rows of placement P from `src`, the caller's table of P.n rows in host or device memory, and wait
- * (the stage is then free for the next table): stage P's own rows in natural order (a shard gathers its leaves
- * own_val + k * 2^shift, k = 0, 1, ...), then place them in d_table, padded to 64-byte rows.  dpf_wrapper.cu:103-115
- * does the analogous reorder on the host with one ATen call per element. */
-int upload_table(b200dpf_ctx *c, const int32_t *src, const RowPlacement &P, DeviceBuffer<int32_t> *stage)
+/* Bytes of the device stage that carries a caller's rows to their context when they cannot be read in place */
+constexpr size_t kStageBytes = (size_t)64 << 20;
+
+/* Write the caller's rows into c's device table and wait; any stream may read the table on return.  `src` holds `rows`
+ * rows of `cols` int32 in host or device memory, of which c owns all, or with own.shift > 0 those of one shard: the leaves
+ * own.own_val + k * 2^own.shift, 2^own.lane_bits rows each.  scatter(chunk, first, count) enqueues on c->stream the
+ * kernel that places own rows [first, first + count), which chunk holds as [count][cols].  A contiguous source on c's
+ * device is read in place; any other goes through one device stage of at most kStageBytes, a whole number of leaves at
+ * a time.  A caller that writes several tables passes `keep`, the stage they share, so that it is allocated once. */
+template <class Scatter>
+int write_rows(b200dpf_ctx *c, const int32_t *src, uint64_t rows, int cols, const RowPlacement &own, Scatter scatter,
+               DeviceBuffer<int32_t> *keep = nullptr)
 {
     bool on_device;
     int src_device;
     int rc = wait_source(c, src, &on_device, &src_device);
     if (rc) return rc;
-    const size_t row_bytes = (size_t)c->entry_size * sizeof(int32_t);
-    const int64_t rows = (int64_t)P.n >> P.shift;
-    const size_t stage_bytes = (size_t)rows * row_bytes;
-    rc = stage->reserve(stage_bytes);
-    if (rc) return rc;
-    cudaError_t e = cudaSuccess;
-    if (P.shift == 0) {
-        e = cudaMemcpyAsync(stage->ptr, src, stage_bytes, cudaMemcpyDefault, c->stream);
+    const uint64_t own_rows = rows >> own.shift;
+    DeviceBuffer<int32_t> local;
+    DeviceBuffer<int32_t> &stage = keep ? *keep : local;
+    if (own.shift == 0 && on_device && src_device == c->device) {
+        CUDA_TRY(scatter(src, 0, own_rows));
     } else {
-        const int shards = 1 << P.shift;
-        const size_t leaf_bytes = row_bytes << P.lane_bits;
-        const int64_t leaves = rows >> P.lane_bits;
-        const int32_t *own = src + ((size_t)P.own_val << P.lane_bits) * c->entry_size;
-        if (on_device) {
-            e = cudaMemcpy2DAsync(stage->ptr, leaf_bytes, own, leaf_bytes * shards, leaf_bytes, (size_t)leaves, cudaMemcpyDefault,
-                                  c->stream);
-        } else {
-            std::vector<int32_t> gathered((size_t)rows * c->entry_size);
-            const size_t leaf_words = (size_t)c->entry_size << P.lane_bits;
-            for (int64_t j = 0; j < leaves; j++)
-                std::memcpy(gathered.data() + (size_t)j * leaf_words, own + (size_t)j * shards * leaf_words, leaf_bytes);
-            e = cudaMemcpyAsync(stage->ptr, gathered.data(), stage_bytes, cudaMemcpyHostToDevice, c->stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        const size_t row_bytes = (size_t)cols * sizeof(int32_t), leaf_bytes = row_bytes << own.lane_bits;
+        const uint64_t chunk = std::min<uint64_t>(own_rows, std::max<size_t>(1, kStageBytes / leaf_bytes) << own.lane_bits);
+        rc = stage.reserve((size_t)chunk * row_bytes);
+        if (rc) return rc;
+        for (uint64_t r0 = 0; r0 < own_rows; r0 += chunk) {     /* one stream: a chunk's copy waits for the previous scatter */
+            const uint64_t count = std::min<uint64_t>(chunk, own_rows - r0);
+            if (own.shift == 0) {
+                CUDA_TRY(cudaMemcpyAsync(stage.ptr, src + r0 * (uint64_t)cols, (size_t)count * row_bytes, cudaMemcpyDefault, c->stream));
+            } else {   /* own row r0 starts natural row (r0 << shift) + (own_val << lane_bits) */
+                const int32_t *from = src + ((r0 << own.shift) + ((uint64_t)own.own_val << own.lane_bits)) * (uint64_t)cols;
+                CUDA_TRY(cudaMemcpy2DAsync(stage.ptr, leaf_bytes, from, leaf_bytes << own.shift, leaf_bytes,
+                                           (size_t)(count >> own.lane_bits), cudaMemcpyDefault, c->stream));
+            }
+            CUDA_TRY(scatter(stage.ptr, r0, count));
         }
     }
-    CUDA_TRY(e);
-    CUDA_TRY(launch_fill_table(stage->ptr, c->d_table.ptr, P, c->entry_size, c->entry_pad, c->sm_count, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));     /* before the stage is freed */
     return B200DPF_OK;
+}
+
+/* Write the rows of placement P from `src`, the caller's table of P.n rows, padded to 64-byte rows */
+int fill_table(b200dpf_ctx *c, const int32_t *src, const RowPlacement &P, DeviceBuffer<int32_t> *keep = nullptr)
+{
+    return write_rows(c, src, P.n, c->entry_size, P, [&](const int32_t *chunk, uint64_t first, uint64_t count) {
+        return launch_fill_table(chunk, first, count, c->d_table.ptr, P, c->entry_size, c->entry_pad, c->sm_count, c->stream);
+    }, keep);
 }
 
 /* Run gen_one(i) for every i < count on `nthreads` threads (0: one per hardware thread); false when any
@@ -1609,10 +1619,8 @@ static int create_impl(b200dpf_ctx **out, const int32_t *table, int64_t n, int e
     rc = c->d_table.reserve(table_bytes);
     if (rc) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_table.ptr, 0, table_bytes, c->stream));
-    DeviceBuffer<int32_t> d_stage;
-    rc = upload_table(c.get(), table, c->place, &d_stage);
+    rc = fill_table(c.get(), table, c->place);
     if (rc) return rc;
-    d_stage.release();
 
     /* Like the reference's eval_init (dpf_wrapper.cu:120-129), set up everything a default batch
      * (512 keys) needs now, so the first evaluation pays neither allocations nor lazy module
@@ -2217,14 +2225,11 @@ static int group_create_impl(b200dpf_ctx **out, const int32_t *const *tables, co
     std::unique_ptr<b200dpf_ctx> c;
     int rc = group_open(tables, n, nbins, entry_size, device, kind, trimmed, &guard, &c);
     if (rc) return rc;
-    DeviceBuffer<int32_t> d_stage;     /* every bin's: the largest one's */
-    rc = d_stage.reserve((size_t)c->shape.n * entry_size * sizeof(int32_t));
-    if (rc) return rc;
+    DeviceBuffer<int32_t> stage;
     for (int g = 0; g < nbins; g++) {
-        rc = upload_table(c.get(), tables[g], place_of(c->bins->shape[(size_t)g], c->lane_bits(), trimmed, 0, 0), &d_stage);
+        rc = fill_table(c.get(), tables[g], place_of(c->bins->shape[(size_t)g], c->lane_bits(), trimmed, 0, 0), &stage);
         if (rc) return rc;
     }
-    CUDA_TRY(cudaStreamSynchronize(c->stream));    /* any stream may read the per-bin tables once the context is returned */
     *out = c.release();
     return B200DPF_OK;
 }
@@ -2670,36 +2675,6 @@ static int check_plan_args(const BatchCodeLayout &L, bool bufs, int64_t nqueries
     return B200DPF_OK;
 }
 
-/* Write the copies of rows [0, n) of `table` into the bins of c (placements already on the device), from the caller's
- * buffer if it is on c's device, else through a bounded stage in chunks, and wait. */
-static int batchcode_fill(b200dpf_ctx *c, const int32_t *table, const BatchCodeLayout &L)
-{
-    bool on_device;
-    int src_device;
-    int rc = wait_source(c, table, &on_device, &src_device);
-    if (rc) return rc;
-    const size_t row_bytes = (size_t)c->entry_size * sizeof(int32_t);
-    DeviceBuffer<int32_t> stage;
-    if (on_device && src_device == c->device) {
-        CUDA_TRY(launch_batchcode_scatter(table, 0, L.n, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_size, c->entry_pad,
-                                          c->stream));
-    } else {
-        constexpr size_t kStageBytes = (size_t)64 << 20;
-        const uint64_t chunk = std::min<uint64_t>(L.n, std::max<size_t>(1, kStageBytes / row_bytes));
-        rc = stage.reserve((size_t)chunk * row_bytes);
-        if (rc) return rc;
-        for (uint64_t r0 = 0; r0 < L.n; r0 += chunk) {     /* one stream: a chunk's copy waits for the previous scatter */
-            const uint64_t rows = std::min<uint64_t>(chunk, L.n - r0);
-            CUDA_TRY(cudaMemcpyAsync(stage.ptr, table + r0 * (uint64_t)c->entry_size, (size_t)rows * row_bytes, cudaMemcpyDefault,
-                                     c->stream));
-            CUDA_TRY(launch_batchcode_scatter(stage.ptr, r0, rows, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_size,
-                                              c->entry_pad, c->stream));
-        }
-    }
-    CUDA_TRY(cudaStreamSynchronize(c->stream));       /* before the stage is freed; any stream may read the table after */
-    return B200DPF_OK;
-}
-
 int b200dpf_batchcode_create(b200dpf_ctx **out, const int32_t *table, int64_t n, int entry_size, int nbins, uint64_t layout_seed,
                              int device, int kind)
 {
@@ -2714,7 +2689,12 @@ int b200dpf_batchcode_create(b200dpf_ctx **out, const int32_t *table, int64_t n,
     std::optional<DeviceGuard> guard;
     std::unique_ptr<b200dpf_ctx> c;
     rc = group_open(nullptr, rows.data(), nbins, entry_size, device, kind, true, &guard, &c);
-    if (!rc) rc = batchcode_fill(c.get(), table, L);
+    if (rc) return rc;
+    /* each row to its three copies in the bins (placements already on the device) */
+    rc = write_rows(c.get(), table, L.n, entry_size, RowPlacement{}, [&](const int32_t *chunk, uint64_t first, uint64_t count) {
+        return launch_batchcode_scatter(chunk, first, count, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_size, c->entry_pad,
+                                        c->stream);
+    });
     if (rc) return rc;
     c->bins->batch = L;
     *out = c.release();
@@ -3058,10 +3038,9 @@ static int kwpir_build(b200dpf_ctx *c, const uint64_t *keywords, const int32_t *
 {
     const cudaStream_t st = c->stream;
     const uint64_t n = L.n, slots = KWPIR_TABLES * L.m;
-    bool kw_on_device, val_on_device;
-    int kw_device, val_device;
+    bool kw_on_device;
+    int kw_device;
     int rc = wait_source(c, keywords, &kw_on_device, &kw_device);
-    if (!rc) rc = wait_source(c, values, &val_on_device, &val_device);
     if (rc) return rc;
     DeviceBuffer<uint64_t> d_keys, d_sorted;
     DeviceBuffer<char> d_temp;
@@ -3132,24 +3111,11 @@ static int kwpir_build(b200dpf_ctx *c, const uint64_t *keywords, const int32_t *
     d_list[0].release();
     d_list[1].release();
 
-    const size_t row_bytes = (size_t)L.value_size * sizeof(int32_t);
-    if (val_on_device && val_device == c->device) {
-        CUDA_TRY(launch_kwpir_scatter(values, 0, n, keys, d_choice.ptr, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_pad, st));
-    } else {
-        constexpr size_t kStageBytes = (size_t)64 << 20;
-        const uint64_t chunk = std::min<uint64_t>(n, std::max<size_t>(1, kStageBytes / row_bytes));
-        DeviceBuffer<int32_t> stage;
-        rc = stage.reserve((size_t)chunk * row_bytes);
-        if (rc) return rc;
-        for (uint64_t i0 = 0; i0 < n; i0 += chunk) {     /* one stream: a chunk's copy waits for the previous scatter */
-            const uint64_t items = std::min<uint64_t>(chunk, n - i0);
-            CUDA_TRY(cudaMemcpyAsync(stage.ptr, values + i0 * (uint64_t)L.value_size, (size_t)items * row_bytes, cudaMemcpyDefault, st));
-            CUDA_TRY(launch_kwpir_scatter(stage.ptr, i0, items, keys, d_choice.ptr, L, c->bins->d_place.ptr, c->d_table.ptr,
-                                          c->entry_pad, st));
-        }
-        CUDA_TRY(cudaStreamSynchronize(st));          /* before the stage is freed */
-    }
-    CUDA_TRY(cudaStreamSynchronize(st));              /* before the scratch is freed; any stream may read the table after */
+    /* write_rows waits: the scratch is free after it */
+    rc = write_rows(c, values, n, L.value_size, RowPlacement{}, [&](const int32_t *chunk, uint64_t first, uint64_t count) {
+        return launch_kwpir_scatter(chunk, first, count, keys, d_choice.ptr, L, c->bins->d_place.ptr, c->d_table.ptr, c->entry_pad, st);
+    });
+    if (rc) return rc;
     *K = GroupBins::Keyword{L, round, ms};
     return B200DPF_OK;
 }

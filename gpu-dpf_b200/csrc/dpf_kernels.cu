@@ -988,20 +988,20 @@ __global__ void probe_smem_kernel(uint32_t *out)
     if (threadIdx.x == 0) *out = (uint32_t)__cvta_generic_to_shared(g_dyn_smem);
 }
 
-/* table[P.first + q][c] = the stage's copy of natural row P.natural_row(q), for q < rows, c < cols.  The stage holds
- * P's own rows in natural order, a shard's leaf v at stage leaf v >> P.shift. */
-__global__ void fill_table_kernel(const int32_t *__restrict__ stage, int32_t *__restrict__ table, const RowPlacement P,
-                                  uint64_t rows, int cols, int stride)
+/* table[P.device_row(r)][c] = chunk[q][c] for q < count, c < cols, where r is the natural row of own row j = first + q:
+ * own leaf j >> lane_bits is natural leaf ((j >> lane_bits) << shift) | own_val. */
+__global__ void fill_table_kernel(const int32_t *__restrict__ chunk, uint64_t first, uint64_t count, int32_t *__restrict__ table,
+                                  const RowPlacement P, int cols, int stride)
 {
-    const uint64_t total = rows * (uint64_t)cols;
+    const uint64_t total = count * (uint64_t)cols;
     const uint64_t lane_mask = (1u << P.lane_bits) - 1u;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t q = i / (uint64_t)cols;
         const int c = (int)(i - q * (uint64_t)cols);
-        const uint64_t r = (uint64_t)P.natural_row(q);
-        const uint64_t src = ((r >> (P.lane_bits + P.shift)) << P.lane_bits) | (r & lane_mask);
-        table[(P.first + q) * (uint64_t)stride + c] = stage[src * (uint64_t)cols + c];
+        const uint64_t j = first + q;
+        const uint64_t r = ((((j >> P.lane_bits) << P.shift) | P.own_val) << P.lane_bits) | (j & lane_mask);
+        table[P.device_row((int64_t)r) * (uint64_t)stride + c] = chunk[i];
     }
 }
 
@@ -1219,15 +1219,14 @@ cudaError_t launch_sum_partials(uint32_t *dst, const PeerParts &parts, size_t wo
     return cudaGetLastError();
 }
 
-cudaError_t launch_fill_table(const int32_t *stage, int32_t *table, const RowPlacement &P, int cols, int stride,
-                              int sm_count, cudaStream_t stream)
+cudaError_t launch_fill_table(const int32_t *chunk, uint64_t first, uint64_t count, int32_t *table, const RowPlacement &P,
+                              int cols, int stride, int sm_count, cudaStream_t stream)
 {
-    const uint64_t rows = (uint64_t)P.n >> P.shift;   /* the rows P owns: n, or n / 2^shift of a shard */
-    const uint64_t total = rows * (uint64_t)cols;
+    const uint64_t total = count * (uint64_t)cols;
     const uint64_t cap = (uint64_t)std::max(sm_count, 1) * 16;
     int grid = (int)std::min<uint64_t>((total + 255) / 256, cap);
     if (grid < 1) grid = 1;
-    fill_table_kernel<<<grid, 256, 0, stream>>>(stage, table, P, rows, cols, stride);
+    fill_table_kernel<<<grid, 256, 0, stream>>>(chunk, first, count, table, P, cols, stride);
     return cudaGetLastError();
 }
 

@@ -488,12 +488,13 @@ static_assert(eval_block_shape(PRF_AES128, 4, MODE_GROUPED_DEV).threads == eval_
 /* Maximum dynamic shared memory the evaluation kernel may be given. */
 cudaError_t eval_max_smem(int prf, int nv, int mode, int *bytes);
 
-/* Table creation: device row P.device_row(i) of `table` := stage row i for every row i that P owns, the stage
- * holding P's own rows, [rows][cols], in natural order (a shard's leaf v at stage leaf v >> P.shift).  Padded columns
- * [cols, stride) are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM count to cap their
- * grids at a few waves. */
-cudaError_t launch_fill_table(const int32_t *stage, int32_t *table, const RowPlacement &P, int cols, int stride,
-                              int sm_count, cudaStream_t stream);
+/* Table creation, one chunk of P's own rows: the rows of P, or of its shard the leaves own_val + k * 2^shift, in natural
+ * order.  Own row j = first + q, held at chunk[q][0, cols), goes to device row P.device_row of its natural row
+ * ((((j >> lane_bits) << shift) | own_val) << lane_bits) | (j & (2^lane_bits - 1)).  Padded columns [cols, stride) and
+ * padding rows are left untouched (pre-zeroed).  The grid-stride helpers take the device's SM count to cap their grids
+ * at a few waves. */
+cudaError_t launch_fill_table(const int32_t *chunk, uint64_t first, uint64_t count, int32_t *table, const RowPlacement &P,
+                              int cols, int stride, int sm_count, cudaStream_t stream);
 
 /* Device-resident grouped evaluation (dpf_group_io.cu), one warp per key, no host synchronisation.
  * order[pos] = (the caller's index of the key at bin-sorted position pos, the depth of its bin).
