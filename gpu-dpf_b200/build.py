@@ -21,10 +21,11 @@ INCLUDE = os.path.join(ROOT, "include")
 LIB = os.path.join(HERE, "libb200dpf.so")
 EXT = os.path.join(HERE, "dpf_cpp" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 
-LIB_SOURCES = ["dpf_kernels.cu", "dpf_capi.cu", "dpf_keygen.cu", "dpf_group_io.cu", "dpf_group_plan.cu", "dpf_batchcode.cu",
-               "dpf_kwpir.cu", "dpf_host.cpp"]
+LIB_SOURCES = ["dpf_kernels.cu", "dpf_capi.cu", "dpf_plan.cu", "dpf_capi_keys.cu", "dpf_capi_multi.cu", "dpf_capi_group.cu",
+               "dpf_capi_update.cu", "dpf_capi_batchcode.cu", "dpf_capi_kwpir.cu", "dpf_keygen.cu", "dpf_group_io.cu",
+               "dpf_group_plan.cu", "dpf_batchcode.cu", "dpf_kwpir.cu", "dpf_host.cpp"]
 # this script is a dependency too: its flags (the target architecture among them) shape both binaries
-LIB_DEPS = LIB_SOURCES + ["dpf_core.cuh", "dpf_kernels.cuh", "dpf_host.h", os.path.join(INCLUDE, "b200dpf.h"),
+LIB_DEPS = LIB_SOURCES + ["dpf_core.cuh", "dpf_kernels.cuh", "dpf_host.h", "dpf_ctx.h", os.path.join(INCLUDE, "b200dpf.h"),
                           os.path.abspath(__file__)]
 EXT_SOURCES = ["dpf_cpp_ext.cpp"]
 

@@ -380,7 +380,7 @@ def churn_worker(name, iterations=12, seed=0):
 
 # The three ChaCha20 workers launch one kernel, dpf_eval_kernel<ChaCha20, 4, MODE_FUSED> (standard keys,
 # 16 columns, 256 threads: level_bytes = 4096), each with its own dynamic shared memory.  With the frontier off
-# there is no tree-top stack, so (dpf_capi.cu smem_layout / smem_bytes)
+# there is no tree-top stack, so (dpf_plan.cu smem_layout / smem_bytes)
 #     smem = off_lo + (s - 1) * 4096,   off_lo = 2048 * depth + 1040   (correction words, level-0 words, roots)
 # and s is subtree_log2 (below depth and s_max):
 #     n = 2^10, s = 2:  20480 + 1040 +  4096 = 25616 bytes
