@@ -1,5 +1,6 @@
 """The keyword-PIR layout restated in numpy from include/b200dpf.h (b200dpf_kwpir_*): the hash h_c, the round-based
-cuckoo placement and the tags it leaves in the three bins.  Shared by the host and the GPU tests."""
+cuckoo placement, the tags it leaves in the three bins and the bins' whole contents.  Shared by the host and the GPU
+tests."""
 import numpy as np
 
 M64 = (1 << 64) - 1
@@ -59,6 +60,24 @@ def tags(keywords, owner, m):
     with np.errstate(over="ignore"):
         out[full] = keywords[owner[full]] + np.uint64(1)
     return out.reshape(3, m)
+
+
+def bins(keywords, values, m, seed):
+    """The contents of the three bins: int32 [m, E + 2] each.  The slot of an item holds its value in columns 0 .. E-1
+    and its tag w + 1 in columns E (low 32 bits) and E + 1 (high 32 bits); an empty slot is all zeros.  The slots are
+    those of place(); a placement that does not finish raises."""
+    values = np.asarray(values, np.int32)
+    rounds, owner = place(keywords, m, seed)
+    if rounds is None:
+        raise ValueError("the placement of %d items in 3 x %d slots does not finish under seed %d" % (len(values), m, seed))
+    e = values.shape[1]
+    out = np.zeros((3 * m, e + 2), np.int32)
+    full = owner >= 0
+    out[full, :e] = values[owner[full]]
+    tag = tags(keywords, owner, m).reshape(-1)
+    out[:, e] = (tag & np.uint64(0xFFFFFFFF)).astype(np.uint32).view(np.int32)
+    out[:, e + 1] = (tag >> np.uint64(32)).astype(np.uint32).view(np.int32)
+    return [out[c * m:(c + 1) * m] for c in range(3)]
 
 
 def default_m(n, expansion=1.3):

@@ -16,56 +16,11 @@ for p in (HERE, os.path.join(ROOT, "gpu-dpf_b200")):
         sys.path.insert(0, p)
 
 import b200dpf as B  # noqa: E402
+from batchcode_ref import locate, per_copy, perm  # noqa: E402  (the layout, restated from include/b200dpf.h)
 
 EINVAL, ECUDA, ESTATE = -1, -2, -4
 M64 = (1 << 64) - 1
 SEEDS = (0, 1, 0x0123456789ABCDEF, M64)
-
-
-# ---- the layout, restated from include/b200dpf.h ----------------------------------------------------------------
-
-def mix(z):
-    """the SplitMix64 finalizer on a uint64 array"""
-    z = np.asarray(z, np.uint64)
-    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xbf58476d1ce4e5b9)
-    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94d049bb133111eb)
-    return z ^ (z >> np.uint64(31))
-
-
-def half_bits(n):
-    h = 1
-    while (1 << (2 * h)) < n:
-        h += 1
-    return h
-
-
-def feistel(seed, c, x, h):
-    mask = np.uint64((1 << h) - 1)
-    l, r = x >> np.uint64(h), x & mask
-    for i in range(4):
-        f = mix(np.uint64(seed) ^ mix((np.uint64(c * 8 + i) << np.uint64(32)) | r)) & mask
-        l, r = r, l ^ f
-    return (l << np.uint64(h)) | r
-
-
-def perm(n, seed, c, rows):
-    """pi_c of every row in `rows`: the Feistel network, cycle-walked below n"""
-    h = half_bits(n)
-    x = feistel(seed, c, np.asarray(rows, np.uint64), h)
-    while True:
-        out = x >= np.uint64(n)
-        if not out.any():
-            return x.astype(np.int64)
-        x[out] = feistel(seed, c, x[out], h)
-
-
-def per_copy(n, nbins, j):
-    return (n - j + nbins - 1) // nbins
-
-
-def locate(n, nbins, seed, row):
-    bins, rows = B.batchcode_locate(n, nbins, seed, row)
-    return [int(b) for b in bins], [int(r) for r in rows]
 
 
 # ---- the plan, restated: Kuhn's augmenting paths, rows in order, copies 0, 1, 2 ------------------------------------
